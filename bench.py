@@ -14,6 +14,8 @@ timed region.  Extra blocks on the same JSON line: `roofline`, `cpu_baseline`, `
 (image 0 of the timed batch against the oracle), `latency` (the reference's own call pattern:
 one image through `api_utils.unmold_detections`), `packed` (extension layout), `gather`
 (N > 1) and `config4` (BASELINE.json configs[3], sharded over the N ranks).
+
+--dump-outputs DIR writes what the last timed step computed (see dump_outputs()) as .npy files.
 """
 from __future__ import annotations
 
@@ -35,6 +37,7 @@ WORKLOAD = "BASELINE.json configs[1]: batch 32 images 1024x1024, 100 instances e
 BATCH, HW, N_INST, CLASSES = 32, (1024, 1024), 100, 81
 SEED = 20260921
 C4_BATCH, C4_HW, C4_INST = 128, (2160, 3840), 50     # BASELINE.json configs[3]
+DUMP_PIXELS = 2048          # --dump-outputs: sampled pixels per image (all R instance planes each)
 
 
 def make_bench_images(rank, count=BATCH):
@@ -98,9 +101,8 @@ def host_cores():
 
 def default_procs(cores):
     """Worker processes for the CPU legs.  The reference's path is memory-bound (one fresh
-    H x W canvas per instance, then np.stack(axis=-1)).  Measured on this pool's 128-thread
-    Xeon 8562Y+ host (masks/s at 16/32/64/128 processes: 1067 / 851 / 604 / 396), more
-    processes only make it slower, so the CPU legs use 16."""
+    H x W canvas per instance, then np.stack(axis=-1)): past a few tens of processes more of
+    them only make it slower, so the CPU legs use at most 16."""
     return max(1, min(cores, 16))
 
 
@@ -191,7 +193,7 @@ def run_reference(args, rank, world):
 
 # ----------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi clock / throttle sampling during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clock / throttle sampling during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -255,18 +257,39 @@ def load_peak():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except (OSError, KeyError, ValueError):
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
-def load_traffic():
-    """DRAM bytes per launch of the dominant kernel from the committed ncu summary."""
-    path = os.path.join(ROOT, "profiles", "mask_expand_ncu_summary.json")
-    try:
-        with open(path) as f:
-            j = json.load(f)
-        return j.get("dram_bytes_per_launch"), j.get("source")
-    except (OSError, ValueError):
-        return None, None
+def dump_outputs(out_dir, eng, counts, n_images):
+    """What the timed path hands its caller, from the last timed step: per image the kept count,
+    boxes, class ids, scores (rows past the count are zero) and the [H,W,N] masks.  The masks are
+    sampled: DUMP_PIXELS fixed pixels per image (seeded, independent of the outputs), all R
+    instance planes of each (planes past the count are zero)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    R = eng.R
+    keep = np.arange(R)[None, :] < counts[:n_images, None]                 # [B, R]
+    boxes = eng.d_boxes[:n_images].cpu().numpy().astype(np.float64) * keep[..., None]
+    class_ids = eng.d_class_ids[:n_images].cpu().numpy().astype(np.float64) * keep
+    scores = eng.d_scores[:n_images].cpu().numpy().astype(np.float32) * keep
+    rng = np.random.default_rng(SEED)
+    yx = np.empty((n_images, DUMP_PIXELS, 2), dtype=np.int64)
+    masks = np.zeros((n_images, DUMP_PIXELS, R), dtype=np.float32)
+    for b in range(n_images):
+        H, W = int(eng._geom_host[b][0]), int(eng._geom_host[b][1])
+        yx[b, :, 0] = rng.integers(0, H, DUMP_PIXELS)
+        yx[b, :, 1] = rng.integers(0, W, DUMP_PIXELS)
+        k = int(counts[b])
+        if k:
+            pix = torch.from_numpy(yx[b, :, 0] * W + yx[b, :, 1]).to(eng.device)
+            rows = eng.canvas_view(b, k).reshape(H * W, k).index_select(0, pix)
+            masks[b, :, :k] = rows.cpu().numpy()
+    arrays = {"counts": counts[:n_images].astype(np.float64), "boxes": boxes,
+              "class_ids": class_ids, "scores": scores, "mask_sample": masks,
+              "mask_sample_yx": yx.astype(np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 class Ctx:
@@ -540,6 +563,8 @@ def run_ours(args, rank, world, local_rank):
     algo_bytes = out_bytes + masks_per_step * (28 * 28 * 4 + 24)   # SURVEY.md 8d per-instance figure
 
     # ---- timed region: exactly K steps, device-timed, expand kernel timed per launch
+    if args.steps < 1:
+        raise SystemExit("--steps must be >= 1")
     sampler = ClockSampler(local_rank)
     ev0 = torch.cuda.Event(enable_timing=True)
     ev1 = torch.cuda.Event(enable_timing=True)
@@ -555,29 +580,33 @@ def run_ours(args, rank, world, local_rank):
     # --load-ms first (clocks settle, nvidia-smi gets samples), keep sampling through the
     # timed region
     sampler.start()
-    t_load = time.perf_counter()
-    while (time.perf_counter() - t_load) * 1e3 < args.load_ms:
-        for _ in range(10):
-            eng.enqueue(d_det, d_msk, stream)
+    try:
+        t_load = time.perf_counter()
+        while (time.perf_counter() - t_load) * 1e3 < args.load_ms:
+            for _ in range(10):
+                eng.enqueue(d_det, d_msk, stream)
+            torch.cuda.synchronize()
+        barrier()
+        ev0.record(stream)
+        for s in range(args.steps):
+            N.check(lib.mrx_unmold_prepare(P(d_det), N.MRX_F32, P(d_msk), N.MRX_F32, BATCH, N_INST,
+                                           28, 28, CLASSES, P(eng.d_geom), P(eng.d_boxes),
+                                           P(eng.d_class_ids), P(eng.d_scores), P(eng.d_src_index),
+                                           P(eng.d_counts), P(eng.d_status),
+                                           P(eng.d_tiles), P(eng.d_sched), st), "prepare")
+            kev[s][0].record(stream)
+            N.check(lib.mrx_mask_expand(P(eng.d_tiles), P(eng.d_src_index), P(eng.d_boxes),
+                                        P(eng.d_counts), P(eng.d_geom),
+                                        P(eng.d_canvas_off), P(eng.d_canvas), BATCH, N_INST, 28, 28,
+                                        eng.chunk_bytes, eng.ctas_per_sm, P(eng.d_sched), st),
+                    "expand")
+            kev[s][1].record(stream)
+        ev1.record(stream)
         torch.cuda.synchronize()
-    barrier()
-    ev0.record(stream)
-    for s in range(args.steps):
-        N.check(lib.mrx_unmold_prepare(P(d_det), N.MRX_F32, P(d_msk), N.MRX_F32, BATCH, N_INST, 28,
-                                       28, CLASSES, P(eng.d_geom), P(eng.d_boxes),
-                                       P(eng.d_class_ids), P(eng.d_scores), P(eng.d_src_index),
-                                       P(eng.d_counts), P(eng.d_status),
-                                       P(eng.d_tiles), P(eng.d_sched), st), "prepare")
-        kev[s][0].record(stream)
-        N.check(lib.mrx_mask_expand(P(eng.d_tiles), P(eng.d_src_index), P(eng.d_boxes),
-                                    P(eng.d_counts), P(eng.d_geom),
-                                    P(eng.d_canvas_off), P(eng.d_canvas), BATCH, N_INST, 28, 28,
-                                    eng.chunk_bytes, eng.ctas_per_sm, P(eng.d_sched), st),
-                "expand")
-        kev[s][1].record(stream)
-    ev1.record(stream)
-    torch.cuda.synchronize()
-    clocks = sampler.stop()
+    finally:
+        clocks = sampler.stop()       # never leave nvidia-smi running
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, eng.d_counts[:BATCH].cpu().numpy(), BATCH)
     elapsed_ms = ev0.elapsed_time(ev1)
     expand_ms = [a.elapsed_time(b) for a, b in kev]
     max_ms = ctx.max_over_ranks(elapsed_ms)
@@ -732,7 +761,6 @@ def run_ours(args, rank, world, local_rank):
 
     if rank == 0:
         peak, peak_src = load_peak()
-        traffic, traffic_src = load_traffic()
         k_ms = float(np.mean(expand_ms))
         achieved = algo_bytes / (k_ms * 1e-3) / 1e9
         line = {
@@ -745,7 +773,7 @@ def run_ours(args, rank, world, local_rank):
                        "num_classes": CLASSES, "mask_tile": "28x28 f32", "layout": "[H,W,N] bool",
                        "sharding": f"images over {world} rank(s), no data-path collective",
                        "l2": "per-step working set (813 MB in + 3.36 GB out per GPU) exceeds the "
-                             "126 MB L2; no explicit flush",
+                             "50 MB L2; no explicit flush",
                        "tile_buffer_bytes": eng.chunk_bytes or "auto", "seed": SEED,
                        "numa": numa},
             "clocks": clocks,
@@ -757,10 +785,10 @@ def run_ours(args, rank, world, local_rank):
                             "masks are waited for on the host"},
             "gpu_launches": 2 * args.steps,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic, "kernel": "mask_expand_team_kernel",
+                         "frac": achieved / peak, "kernel": "mask_expand_team_kernel",
                          "kernel_ms": k_ms, "kernel_ms_min": float(np.min(expand_ms)),
                          "algorithmic_bytes_per_launch": int(algo_bytes),
-                         "peak_source": peak_src, "traffic_source": traffic_src},
+                         "peak_source": peak_src},
             "cpu_baseline": cpu_block,
             "parity": parity,
             "latency": latency,
@@ -794,6 +822,8 @@ def main():
     ap.add_argument("--no-config4", action="store_true")
     ap.add_argument("--no-numa-bind", action="store_true")
     ap.add_argument("--cpu-procs", type=int, default=0, help="worker processes of the CPU legs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (sampled masks) as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))

@@ -1,5 +1,5 @@
-"""`from api.helpers import utils as api_utils` (/root/reference/serve.py:21) resolved to the
-B200 implementation.  Put the `dropin/` directory on PYTHONPATH ahead of the original app."""
+"""`from api.helpers import utils as api_utils` (serve.py:21) resolved to the
+H100 implementation.  Put the `dropin/` directory on PYTHONPATH ahead of the original app."""
 import os
 import sys
 

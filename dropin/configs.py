@@ -1,4 +1,4 @@
-"""`import configs as cf` (/root/reference/serve.py:22): stand-in deployment constants."""
+"""`import configs as cf` (serve.py:22): stand-in deployment constants."""
 import os
 import sys
 

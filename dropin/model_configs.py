@@ -1,4 +1,4 @@
-"""`from model_configs import mconfig as mcf` (/root/reference/serve.py:23)."""
+"""`from model_configs import mconfig as mcf` (serve.py:23)."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 /*
- * mrx.h -- C ABI of the B200 (sm_100a) Mask R-CNN serving hot path.
+ * mrx.h -- C ABI of the H100 (sm_90a) Mask R-CNN serving hot path.
  *
  * The reference (huyhoang17/matterport-maskrcnn-with-tensorflow-serving) has NO
  * FFI / plugin interface: its boundary is three plain Python call sites in

@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) implementation of the CPU-side serving hot path of
+"""H100-native (sm_90a) implementation of the CPU-side serving hot path of
 huyhoang17/matterport-maskrcnn-with-tensorflow-serving: `api_utils.get_anchors`,
 `api_utils.unmold_detections` and the `preprocess_input` mold step, behind the
 reference's own Python signatures.  See DESIGN.md / INTEGRATION.md.

@@ -1,6 +1,6 @@
 """Drop-in for the reference's `api.helpers.utils` (imported as `api_utils`,
-/root/reference/serve.py:21): same function names, positional arguments, return tuples and
-NumPy value semantics, computed by the sm_100a kernels in libmrx.so.
+serve.py:21): same function names, positional arguments, return tuples and
+NumPy value semantics, computed by the sm_90a kernels in libmrx.so.
 
     get_anchors(image_shape)                                         serve.py:105
     unmold_detections(detections, mrcnn_mask, original_image_shape,

@@ -1,5 +1,5 @@
 """Stand-in for the reference's absent `configs` module (`import configs as cf`,
-/root/reference/serve.py:22).  Attribute names are exactly the ones serve.py reads
+serve.py:22).  Attribute names are exactly the ones serve.py reads
 (serve.py:78,114,120-136,165); values are deployment placeholders."""
 
 HOST = "127.0.0.1"

@@ -1,4 +1,4 @@
-// anchors.cu -- api_utils.get_anchors (/root/reference/serve.py:105): the FPN pyramid
+// anchors.cu -- api_utils.get_anchors (serve.py:105): the FPN pyramid
 // anchors of upstream utils.generate_pyramid_anchors + norm_boxes, one thread per anchor.
 //
 // Output [A,4] float32, order: level-major, then y, x, ratio innermost
@@ -117,8 +117,11 @@ extern "C" int mrx_anchors(float *d_out, int img_h, int img_w, const double *sca
     return rc;
   const long long total = p.level_off[n_levels];
   if (total == 0) return MRX_OK;
+  DevInfo dev;
+  if (int rc = current_device_info(&dev)) return rc;
   long long blocks = (total + kAnchorThreads - 1) / kAnchorThreads;
-  if (blocks > 148LL * 16) blocks = 148LL * 16;   // grid-stride over a multiple of the SM count
+  const long long cap = 16LL * dev.sms;   // grid-stride over a multiple of the SM count
+  if (blocks > cap) blocks = cap;
   anchors_kernel<<<static_cast<unsigned>(blocks), kAnchorThreads, 0,
                    static_cast<cudaStream_t>(stream)>>>(p, reinterpret_cast<float4 *>(d_out));
   MRX_LAUNCH_CHECK("anchors_kernel");

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the sm_100a kernels behind include/mrx.h.
+// common.cuh -- shared helpers for the sm_90a kernels behind include/mrx.h.
 #pragma once
 
 #include <cuda_runtime.h>

@@ -1,5 +1,5 @@
 // composite.cu -- mask compositing of visualize.display_instances
-// (/root/reference/serve.py:160-169; SURVEY.md 8f rank 2: the consumer right behind
+// (serve.py:160-169; SURVEY.md 8f rank 2: the consumer right behind
 // unmold_detections).  The reference hands the [H,W,N] bool masks to matplotlib code whose
 // mask part is, per instance in order,
 //     for c in 0..2:  image[:,:,c] = where(mask == 1, image[:,:,c]*(1-alpha) + alpha*color[c]*255,
@@ -8,13 +8,12 @@
 // Doing that on the device canvas mrx_mask_expand just wrote removes the 105 MB per image
 // device -> host copy of the masks for callers that only want the overlay.
 //
-// Alternatives measured this round and removed again (profiles/README.md): tabulating the blend
-// per (instance, channel, value) instead of evaluating it in fp64 per pixel (0.884 vs 0.885 ms),
-// restricting every block of pixels to the instances whose box meets it (0.947 ms: slower), and
-// persistent CTAs with a two-stage bulk-copy ring (0.96 ms: four resident CTAs per SM are too
-// few threads for the divergent walk; time went as 1/CTAs).  What did pay: replacing the
-// load-and-store staging loop by ONE bulk copy per block (0.886 -> 0.653 ms), and the blend
-// constants' load loop by a second one (-> 0.623 ms).
+// Alternatives tried and removed again: tabulating the blend per (instance, channel, value)
+// instead of evaluating it in fp64 per pixel (no gain), restricting every block of pixels to the
+// instances whose box meets it (slower), and persistent CTAs with a two-stage bulk-copy ring
+// (slower: four resident CTAs per SM are too few threads for the divergent walk; time went as
+// 1/CTAs).  What did pay: replacing the load-and-store staging loop by ONE bulk copy per block,
+// and the blend constants' load loop by a second one.
 //
 // HBM-read bound: N bytes of canvas per pixel (3.36 GB per config-2 batch) + 3 B in + 3 B out.
 // One CTA = 256 consecutive pixels of one image: their 256*N canvas bytes are contiguous
@@ -28,7 +27,7 @@
 
 namespace mrx {
 
-constexpr int kCompThreads = 256;   // 128: 0.688 ms, 384/512: 0.667 ms, 256: 0.653 ms
+constexpr int kCompThreads = 256;   // faster than 128, 384 or 512 threads per CTA
 
 __global__ void __launch_bounds__(kCompThreads)
 composite_masks_kernel(const unsigned char *__restrict__ canvas,

@@ -1,6 +1,6 @@
 // expand_bits.cu -- mask expand with BIT-PACKED output (SURVEY.md 8f rank 4: compact masks).
 //
-// EXTENSION, not the reference layout: unmold_detections (/root/reference/serve.py:147-154)
+// EXTENSION, not the reference layout: unmold_detections (serve.py:147-154)
 // returns bool [H,W,N], one byte per element, and that is what mrx_mask_expand writes and what
 // the headline benchmark measures.  This kernel computes the SAME samples (same exact integer
 // source coordinates, same fp32 weights, same two fused multiply-adds in the same order as

@@ -2,8 +2,8 @@
 // TEAMS of warps, one role per warp and three named barriers per tile.
 //
 // Why: the store pattern alone (shared memory -> HBM bulk copies of k x 3200 B, no box work)
-// writes a B200 at ~7.4 TB/s (tools/store_ceiling.cu); a warp-specialised producer / consumer /
-// store-warp design over mbarrier rings (round 1, removed) reached 4.6 TB/s: its producer warps
+// runs at the HBM write rate (tools/store_ceiling.cu); a warp-specialised producer / consumer /
+// store-warp design over mbarrier rings (an earlier version, removed) fell well short: its producer warps
 // -- one dependent instruction stream listing (box,row) entries and issuing a TMA load per
 // entry -- were the critical path.  Here a tile is kTileRows canvas rows high, so a
 // box meets a tile once (not once per row); the horizontal source coordinate of a 32-column
@@ -126,7 +126,8 @@ __device__ __forceinline__ int tiles_of(int H, int W, int N, int rowcap, int til
 // ---- phase profile (build with -DMRX_TEAM_PROFILE): per-warp cycle totals of the six phases
 // of a team's tile loop, read back with mrx_debug_team_profile()
 #ifdef MRX_TEAM_PROFILE
-__device__ long long g_team_prof[148 * 32 * 12];
+constexpr int kProfCtas = 256;   // CTAs (= SMs) the profile has room for
+__device__ long long g_team_prof[kProfCtas * 32 * 12];
 #define PROF_DECL long long prof_t = clock64(), prof_acc[12] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
 #define PROF_ADD(k, v) prof_acc[k] += (v);
 #define PROF_NOW clock64()
@@ -137,7 +138,7 @@ __device__ long long g_team_prof[148 * 32 * 12];
     prof_t = now_;                           \
   }
 #define PROF_FLUSH                                                                   \
-  if (lane == 0 && blockIdx.x < 148 && warp < 32) {                                  \
+  if (lane == 0 && blockIdx.x < kProfCtas && warp < 32) {                            \
     for (int k_ = 0; k_ < 12; ++k_)                                                  \
       g_team_prof[(blockIdx.x * 32 + warp) * 12 + k_] = prof_acc[k_];                \
   }
@@ -760,7 +761,7 @@ extern "C" int mrx_debug_team_profile(long long *host_dst, int count) {
 }
 #endif
 
-// The shipped shape: 6 teams x 5 warps, 10-row tiles (profiles/README.md has the sweeps).
+// The shipped shape: 6 teams x 5 warps, 10-row tiles (tools/kernel_sweep.py compares the others).
 int launch_expand_team(const ExpandParams &prm, const DevInfo &dev, int want_buf, cudaStream_t st) {
   if (prm.mw > 30) return MRX_E_UNSUPPORTED;   // caller falls back to the generic kernel
   if (prm.values != nullptr) return launch_team_cfg<6, 5, 10, true>(prm, dev, want_buf, st);

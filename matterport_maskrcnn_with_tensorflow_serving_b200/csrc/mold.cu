@@ -1,5 +1,5 @@
 // mold.cu -- the pre-processing half of the path, preprocess_input
-// (/root/reference/serve.py:83-107):
+// (serve.py:83-107):
 //   cv2_resize_kernel   cv2.resize(img, (S, S))                      serve.py:88-89
 //   mold_image_kernel   utils.resize_image(square) + mold_image      serve.py:91-98
 //
@@ -161,9 +161,9 @@ mold_image_kernel(const unsigned char *__restrict__ src, int sh, int sw, int new
   }
 }
 
-static unsigned grid_for(long long total, int threads) {
+static unsigned grid_for(long long total, int threads, int sms) {
   long long blocks = (total + threads - 1) / threads;
-  const long long cap = 148LL * 32;
+  const long long cap = 32LL * sms;   // grid-stride over a multiple of the SM count
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   return static_cast<unsigned>(blocks);
@@ -176,8 +176,10 @@ using namespace mrx;
 static int cv2_resize_launch(const unsigned char *d_src, const long long *d_src_off,
                              const int *d_src_hw, int src_h, int src_w, unsigned char *d_dst,
                              int B, int dst_h, int dst_w, void *stream) {
+  DevInfo dev;
+  if (int rc = current_device_info(&dev)) return rc;
   const long long total = static_cast<long long>(dst_h) * dst_w;
-  dim3 grid(grid_for(total, kMoldThreads), B);
+  dim3 grid(grid_for(total, kMoldThreads, dev.sms), B);
   cv2_resize_kernel<<<grid, kMoldThreads, 0, static_cast<cudaStream_t>(stream)>>>(
       d_src, d_src_off, d_src_hw, src_h, src_w, d_dst, dst_h, dst_w);
   MRX_LAUNCH_CHECK("cv2_resize_kernel");
@@ -219,9 +221,11 @@ static int mold_launch(const unsigned char *d_src, int B, int src_h, int src_w, 
   // scipy.ndimage.zoom(grid_mode=True): zoom = in / out per axis (float64)
   const double zoom_y = static_cast<double>(src_h) / new_h;
   const double zoom_x = static_cast<double>(src_w) / new_w;
+  DevInfo dev;
+  if (int rc = current_device_info(&dev)) return rc;
   const long long total = static_cast<long long>(out_h) * out_w;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  dim3 grid(grid_for(total, kMoldThreads), B);
+  dim3 grid(grid_for(total, kMoldThreads, dev.sms), B);
   if (out_dtype == MRX_F64) {
     mold_image_kernel<double><<<grid, kMoldThreads, 0, st>>>(
         d_src, src_h, src_w, new_h, new_w, top, left, out_h, out_w, zoom_y, zoom_x,

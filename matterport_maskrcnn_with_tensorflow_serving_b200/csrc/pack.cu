@@ -16,14 +16,13 @@
 // into one output byte per (8 pixels, instance), transposed with eight byte permutes into one
 // 32-bit word per instance plane and stored.  Two forms, chosen per image:
 //   staged (up to ~220 instance slots): the CTA's 256 pixels arrive as eight 1-D bulk copies
-//     (TMA) and the loads are conflict-free shared-memory loads -- 0.545 ms on the config-2
-//     batch, 6.9 TB/s of reads + writes (above the measured COPY peak: the kernel reads 8 bytes
-//     for each it writes);
+//     (TMA) and the loads are conflict-free shared-memory loads (the kernel reads 8 bytes for
+//     each it writes, so it can beat a copy's rate);
 //   direct (more slots than that): the loads go to global memory, lanes laid out 4 pixel runs x
-//     8 quads so that every load instruction reads four fully used 32-byte sectors -- 0.76 ms on
-//     the same batch (5.9 sectors per request: latency of many small loads).
-// (Round 1 staged with ordinary loads and stores: 2 x 25.6 KB of shared-memory traffic per
-// 25.6 KB of canvas put it at the shared-memory bandwidth, 0.42 of the HBM roofline.)
+//     8 quads so that every load instruction reads four fully used 32-byte sectors -- slower
+//     (latency of many small loads).
+// (Staging with ordinary loads and stores costs 2 x 25.6 KB of shared-memory traffic per
+// 25.6 KB of canvas and runs at the shared-memory bandwidth, well below the HBM roofline.)
 //
 // pack_bytes_kernel (any N, any alignment; ragged instance counts): 256 consecutive pixels of a
 // row staged in shared memory at their global address mod 16 (one bulk copy), then one instance

@@ -1,5 +1,5 @@
 // rle.cu -- COCO run-length masks straight from the 28x28 tiles (SURVEY.md 8f rank 4: the second
-// compact format it names; the output of /root/reference/serve.py:147 re-encoded).
+// compact format it names; the output of serve.py:147 re-encoded).
 //
 // EXTENSION, not the reference layout.  For every kept instance the result is the
 // "uncompressed RLE" of pycocotools, {'size': [H, W], 'counts': [...]}: the [H, W] mask read in

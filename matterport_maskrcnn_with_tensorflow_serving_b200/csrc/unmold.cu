@@ -1,5 +1,5 @@
 // unmold.cu -- the serving post-processing path of the reference,
-// api_utils.unmold_detections (/root/reference/serve.py:147-154), as sm_100a kernels.
+// api_utils.unmold_detections (serve.py:147-154), as sm_90a kernels.
 //
 //   unmold_prologue_kernel   steps 1-6 of the upstream body (trim, class ids, window
 //                            normalisation, box affine + denorm, zero-area compaction)

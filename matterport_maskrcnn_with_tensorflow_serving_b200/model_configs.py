@@ -1,5 +1,5 @@
 """Stand-in for the reference's absent `model_configs` module
-(`from model_configs import mconfig as mcf`, /root/reference/serve.py:23).
+(`from model_configs import mconfig as mcf`, serve.py:23).
 
 serve.py reads IMAGE_MIN_DIM, IMAGE_MIN_SCALE, IMAGE_MAX_DIM, IMAGE_RESIZE_MODE
 (serve.py:93-96), NUM_CLASSES (:102) and, through `mold_image(..., mcf)` (:98),

@@ -1,7 +1,7 @@
 """Multi-GPU plumbing: images are independent units, so a batch shards by image with no
 collective on the data path; the only exchange is the final gather of per-image mask
 canvases to rank 0 (BASELINE.json north_star; the reference itself is single-image,
-single-process: /root/reference/serve.py:48).
+single-process: serve.py:48).
 
 Two gathers, both into ONE receive buffer on rank 0 that is allocated once and holds the whole
 batch in image order (rank 0's own shard is written there by its kernels, never copied):

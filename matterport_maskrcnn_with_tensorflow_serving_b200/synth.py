@@ -1,7 +1,7 @@
 """Seeded synthetic detections in the shape TF-Serving returns them to serve.py.
 
 The reference decodes `mrcnn_detection` [R,6] and `mrcnn_mask` [R,28,28,C] from the
-PredictResponse (/root/reference/serve.py:131-136) and hands them to
+PredictResponse (serve.py:131-136) and hands them to
 `unmold_detections` together with the molded-image shape and window produced by
 `preprocess_input` (serve.py:83-107, :147-154).  This module fabricates exactly those
 arrays (SURVEY.md section 8d) so tests, smoke() and bench.py feed the oracle and the

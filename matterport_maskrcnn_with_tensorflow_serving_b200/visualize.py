@@ -1,4 +1,4 @@
-"""Mask overlay of `visualize.display_instances` (reference: /root/reference/serve.py:160-169,
+"""Mask overlay of `visualize.display_instances` (reference: serve.py:160-169,
 `mrcnn.visualize` is un-vendored there) on the device.
 
 The reference passes the `[H, W, N]` bool masks `unmold_detections` returned to matplotlib

@@ -1,5 +1,5 @@
 """Response decode / request encode of the TF-Serving call without the Python list detour
-(SURVEY.md 8f rank 1; reference: /root/reference/serve.py:49-76 and :131-136).
+(SURVEY.md 8f rank 1; reference: serve.py:49-76 and :131-136).
 
 The reference turns `result.outputs[name].float_val` -- a protobuf repeated field -- into an
 ndarray with `np.array(...)`: every float becomes a Python object first.  For the mask tensor

@@ -4,7 +4,7 @@ This package is a NumPy/SciPy restatement of the algorithm that the reference's
 `serve.py` reaches through `api_utils.get_anchors` (serve.py:105),
 `api_utils.unmold_detections` (serve.py:147-154) and the body of
 `preprocess_input` (serve.py:83-107).  Those function bodies are not vendored in
-/root/reference (serve.py:17-23 import them from un-vendored, un-pinned packages:
+the reference repository (serve.py:17-23 import them from un-vendored, un-pinned packages:
 a fork of matterport/Mask_RCNN, scikit-image, scipy), so:
 
     *** PARITY UNPINNED ***  The reference ships no tests, golden vectors or

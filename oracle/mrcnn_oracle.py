@@ -1,7 +1,7 @@
 """NumPy/SciPy restatement of the reference's CPU serving path.  TEST INFRASTRUCTURE.
 
 PARITY UNPINNED: see oracle/__init__.py.  Every function names the reference call
-site it serves ([REF] = /root/reference/serve.py:line) and the public upstream
+site it serves ([REF] = serve.py:line) and the public upstream
 function whose published algorithm it restates ([UPSTREAM] = matterport/Mask_RCNN,
 no line numbers because no copy is on disk to check them against).
 

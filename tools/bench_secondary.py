@@ -1,6 +1,6 @@
 """Secondary workloads of BASELINE.json (configs[2], [3] per-GPU shard, [4]) and the mold step,
 device-timed with CUDA events.  Not the contract bench (bench.py measures configs[1]); the
-numbers go into profiles/README.md.  One JSON line per workload on stdout.
+numbers go into README.md.  One JSON line per workload on stdout.
 
   python tools/bench_secondary.py [--iters 20] [--cpu]     (--cpu also times the oracle)
 """

@@ -1,10 +1,10 @@
-// store_ceiling.cu -- developer microbenchmark (not part of the product): how fast can a B200
+// store_ceiling.cu -- developer microbenchmark (not part of the product): how fast can the GPU
 // be WRITTEN with the store pattern of mask_expand (shared memory -> HBM bulk copies), without
 // any of the kernel's box work?  Gives the practical ceiling for the kernel's roofline and
 // compares job geometries (one contiguous chunk vs. k row segments of a 2-D tile).
 //
-//   nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -o /tmp/store_ceiling tools/store_ceiling.cu
-//   ./store_ceiling            (prints one line per pattern)
+//   mkdir -p build && nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o build/store_ceiling tools/store_ceiling.cu
+//   build/store_ceiling        (prints one line per pattern)
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

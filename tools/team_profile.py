@@ -27,11 +27,13 @@ for _ in range(3):
     eng.enqueue(d_det, d_msk)
 torch.cuda.synchronize()
 lib = _native.load()
-buf = np.zeros(148 * 32 * 12, dtype=np.int64)
+SLOTS = 256   # kProfCtas of csrc/expand_team.cu
+sms = torch.cuda.get_device_properties(0).multi_processor_count
+buf = np.zeros(SLOTS * 32 * 12, dtype=np.int64)
 rc = lib.mrx_debug_team_profile(buf.ctypes.data_as(ctypes.c_void_p), buf.size)
 assert rc == 0
-a = buf.reshape(148, 32, 12)[:, :teams * warps].reshape(148, teams, warps, 12).astype(np.float64)
-tiles_per_team = 32 * (1024 // rows + (1 if 1024 % rows else 0)) * 32 / (148 * teams)
+a = buf.reshape(SLOTS, 32, 12)[:sms, :teams * warps].reshape(sms, teams, warps, 12).astype(np.float64)
+tiles_per_team = 32 * (1024 // rows + (1 if 1024 % rows else 0)) * 32 / (sms * teams)
 if COCO:
     tiles_per_team = 1.0   # (tile count depends on every image's N: totals per team instead)
 names = ["B2 wait", "zero", "B3 wait", "items", "fence+B1 wait", "post-B1 (cull | store+decode+drain)", "w0: store issue", "w0: decode"]
@@ -45,4 +47,4 @@ tot = a[:, :, :, :6].sum(axis=3).mean() / tiles_per_team
 print("  total per tile: %.0f cycles" % tot)
 items = a[..., 10].sum(); rows = a[..., 11].sum()
 print("  fast-path items: %.0f (%.2f per tile), rows/item %.1f, setup cycles/item %.0f, row-loop cycles/item %.0f (%.1f per row)" % (
-    items, items / (tiles_per_team * 148 * teams), rows / items, a[..., 8].sum() / items, a[..., 9].sum() / items, a[..., 9].sum() / rows))
+    items, items / (tiles_per_team * sms * teams), rows / items, a[..., 8].sum() / items, a[..., 9].sum() / items, a[..., 9].sum() / rows))
