@@ -48,8 +48,10 @@ extern "C" {
 #define MRX_F64 1
 
 /* per-image status bits written by mrx_unmold_prepare into d_status[b] */
-#define MRX_ST_CLASS_RANGE  1   /* class id outside [-C, C): numpy would raise IndexError */
-#define MRX_ST_BOX_RANGE    2   /* kept box outside the canvas: numpy paste would raise   */
+#define MRX_ST_CLASS_RANGE  1   /* class id outside [-C, C) or NaN: numpy would raise IndexError */
+/* kept box outside the canvas: numpy's paste would raise, or wrap a box that lies entirely at
+ * negative coordinates to the far edge; we raise for both */
+#define MRX_ST_BOX_RANGE    2
 
 /* limits (compile-time properties of the kernels) */
 #define MRX_MAX_LEVELS   8
@@ -99,7 +101,8 @@ int mrx_anchors(float *d_out, int img_h, int img_w,
  * C = number of classes in mrcnn_mask's last axis (for the class-range check).
  * d_sched (may be NULL): the scheduler words of the expand kernels (MRX_SCHED_WORDS x uint32),
  * zeroed here as well.  The class tiles are stored by ORIGINAL detection row,
- *   d_tiles[b][t] = float32(mrcnn_mask[b, t, :, :, class_id of row t])      (rows with class 0: untouched)
+ *   d_tiles[b][t] = float32(mrcnn_mask[b, t, :, :, class_id of row t])
+ *   (rows whose class_id is exactly 0: untouched; 0.5 truncates to class 0 and is gathered)
  * which needs nothing from steps 1-6, so both run side by side in the same grid.  The expand
  * entry points then take d_tile_index = d_src_index (kept instance k -> its row). */
 int mrx_unmold_prepare(const void *d_detections, int det_dtype, const void *d_mrcnn_mask,
@@ -133,8 +136,10 @@ int mrx_mask_expand(const float *d_tiles, const int *d_tile_index, const int *d_
  * stores every pre-threshold sample it evaluates: d_values is float32, indexed exactly like
  * d_canvas (element d_canvas_off[b] + (y*W_b + x)*N_b + n); only elements inside box n are
  * written.  The canvas is written as usual.  Tests compare these values with the float64
- * oracle (|diff| <= 1e-6).  Shapes the team kernel does not take (R > 200, mask tiles wider
- * than 30 columns) return MRX_E_UNSUPPORTED. */
+ * oracle (|diff| <= 1e-6).  Shapes the team kernel does not take return MRX_E_UNSUPPORTED
+ * before launching anything: mask tiles wider than 30 columns, and R whose tile row no longer
+ * fits a team's buffer (on an H100, R > 213 at B = 1; the limit drops slowly for large batches,
+ * whose scheduler table takes shared memory from the buffers). */
 int mrx_mask_expand_values(const float *d_tiles, const int *d_tile_index, const int *d_boxes,
                            const int *d_counts, const int *d_geom, const long long *d_canvas_off,
                            unsigned char *d_canvas, float *d_values, int B, int R, int mh, int mw,

@@ -120,8 +120,9 @@ __device__ __forceinline__ void prologue_body(const int b, const T *__restrict__
       score = row[5];
       // step 6: drop rows with (y2 - y1) * (x2 - x1) <= 0   (int32 arithmetic)
       keep = ((y2 - y1) * (x2 - x1)) > 0;
-      // numpy fancy indexing accepts class ids in [-C, C)
-      if (cls < -C || cls >= C) my_status |= MRX_ST_CLASS_RANGE;
+      // numpy fancy indexing accepts class ids in [-C, C); astype(int32) turns NaN into
+      // INT_MIN on the host, where the device conversion gives 0
+      if (cls < -C || cls >= C || isnan(row[4])) my_status |= MRX_ST_CLASS_RANGE;
       in_canvas = !(y1 < 0 || x1 < 0 || y2 > orig_h || x2 > orig_w || y2 <= y1 || x2 <= x1);
       if (keep && !in_canvas) my_status |= MRX_ST_BOX_RANGE;
     }
@@ -189,9 +190,10 @@ __device__ __forceinline__ void gather_strided(const T *__restrict__ in, int til
 
 // One launch for steps 1-6 AND the class-tile gather (the two do not depend on each other when
 // the tiles are stored by ORIGINAL detection row): grid (R + 1, B); CTA (t < R, b) copies the
-// tile of row t's own class -- rows with class_id == 0 can never be kept (the first of them ends
-// the list) and are skipped -- and CTA (R, b) runs the prologue of image b.  The expand kernels
-// then find instance k's tile through src_index[b][k].
+// tile of row t's own class -- rows whose class_id is exactly 0 can never be kept (the first of
+// them ends the list) and are skipped; a class_id such as 0.5 truncates to class 0 but does not
+// end the list, so its tile is gathered -- and CTA (R, b) runs the prologue of image b.  The
+// expand kernels then find instance k's tile through src_index[b][k].
 template <typename TD, typename TM>
 __global__ void __launch_bounds__(kPrepareThreads)
 unmold_prepare_kernel(const TD *__restrict__ det, const TM *__restrict__ mask, int R, int C,
@@ -207,10 +209,11 @@ unmold_prepare_kernel(const TD *__restrict__ det, const TM *__restrict__ mask, i
     return;
   }
   const int t = blockIdx.x;
-  int cls = static_cast<int>(det[(static_cast<size_t>(b) * R + t) * 6 + 4]);   // astype(int32)
-  if (cls == 0) return;
+  const TD class_id = det[(static_cast<size_t>(b) * R + t) * 6 + 4];
+  if (class_id == TD(0)) return;       // the trim's test, on the raw value
+  int cls = static_cast<int>(class_id);   // astype(int32)
   if (cls < 0) cls += C;
-  if (cls < 0 || cls >= C) cls = 0;    // flagged by the prologue; stay in bounds
+  if (cls < 0 || cls >= C) cls = 0;    // flagged by the prologue (NaN too); stay in bounds
   gather_strided(mask + (static_cast<size_t>(b) * R + t) * tile_elems * C + cls, tile_elems, C,
                  tiles + (static_cast<size_t>(b) * R + t) * tile_elems);
 }

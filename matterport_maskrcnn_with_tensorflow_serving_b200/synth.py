@@ -62,7 +62,7 @@ def make_image(rng, orig_hw, n_valid, num_classes=81, max_instances=100,
     way `norm_boxes` does, stored as float32 (the wire dtype, serve.py:131).  Rows
     past `n_valid` are all-zero padding (class_id 0 terminates, upstream semantics).
     `zero_area_rows` are indices (< n_valid) forced to x2 == x1 so that the
-    zero-area filter fires.
+    zero-area filter fires.  `mask_hw` is the tile side, or an (mh, mw) pair.
     """
     H, W = int(orig_hw[0]), int(orig_hw[1])
     if mold is None:
@@ -87,7 +87,8 @@ def make_image(rng, orig_hw, n_valid, num_classes=81, max_instances=100,
         det[:n, :4] = _norm_boxes_f32(boxes_px, image_shape[:2])
         det[:n, 4] = rng.integers(1, num_classes, size=n).astype(np.float32)
         det[:n, 5] = np.sort(rng.uniform(0.7, 1.0, size=n))[::-1].astype(np.float32)
-    masks = rng.random((R, mask_hw, mask_hw, num_classes), dtype=np.float32)
+    mh, mw = (mask_hw, mask_hw) if np.isscalar(mask_hw) else mask_hw
+    masks = rng.random((R, int(mh), int(mw), num_classes), dtype=np.float32)
     return SynthImage(det, masks, (H, W, 3), tuple(image_shape), tuple(window), n)
 
 

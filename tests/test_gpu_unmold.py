@@ -10,8 +10,8 @@ import oracle
 from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, synth
 from matterport_maskrcnn_with_tensorflow_serving_b200.engine import UnmoldEngine, make_geom
 
-from helpers import (MASK_VALUE_ATOL, compare_masks, item_of, mask_parity_stats, oracle_unmold,
-                     record_stats, value_parity_stats)
+from helpers import (MASK_VALUE_ATOL, check_values, compare_masks, item_of, oracle_unmold,
+                     run_with_values)
 
 pytestmark = pytest.mark.gpu
 
@@ -179,63 +179,6 @@ def test_chunk_size_independent(cuda_device, chunk):
         assert compare_masks(m, rm, rz, rb)[0] == 0
 
 
-def _run_with_values(ims, R, classes, dtype=np.float64):
-    """Batch through the PRODUCTION expand kernel's instrumented instantiation
-    (mrx_mask_expand_values: same template, same cull / hrow / walk code).  Returns per image
-    (boxes, class_ids, masks bool [H,W,N], values float32 [H,W,N])."""
-    import torch
-
-    eng = UnmoldEngine(len(ims), R, (28, 28), classes, det_dtype=dtype, mask_dtype=dtype)
-    eng.plan([make_geom(im.original_image_shape, im.image_shape, im.window) for im in ims])
-    d_det = torch.from_numpy(np.stack([im.detections.astype(dtype) for im in ims])).cuda()
-    d_msk = torch.from_numpy(np.stack([im.mrcnn_mask.astype(dtype) for im in ims])).cuda()
-    eng.enqueue(d_det, d_msk, expand=False)
-    total = int(eng._offsets[len(ims)])
-    d_values = torch.full((total,), float("nan"), dtype=torch.float32, device="cuda")
-    eng.enqueue_expand_values(d_values)
-    counts, boxes, cls, scores = eng.fetch_meta()
-    out = []
-    for b, im in enumerate(ims):
-        k = int(counts[b])
-        H, W = im.original_image_shape[:2]
-        o = int(eng._offsets[b])
-        m = eng.canvas_view(b, k).cpu().numpy().view(np.bool_)
-        v = d_values[o:o + H * W * k].view(H, W, k).cpu().numpy()
-        out.append((boxes[b, :k].copy(), cls[b, :k].copy(), m, v))
-    # the instrumented launch must leave the same canvas as the plain one
-    eng.enqueue_expand()
-    for b, im in enumerate(ims):
-        assert np.array_equal(eng.canvas_view(b, out[b][0].shape[0]).cpu().numpy().view(np.bool_),
-                              out[b][2])
-    return out
-
-
-def _check_values(name, ims, R, classes, dtype=np.float64):
-    """Pre-threshold samples of the production kernel vs the float64 oracle, every instance of
-    every image: |gpu - oracle| <= 1e-6; masks equal outside the band; stats recorded."""
-    got = _run_with_values(ims, R, classes, dtype)
-    tot = {"max_abs_err": 0.0, "samples": 0, "flips_outside_band": 0, "flips_inside_band": 0,
-           "band_pixels": 0, "pixels": 0, "images": len(ims), "instances": 0}
-    for im, (b, c, m, v) in zip(ims, got):
-        rb, rc, rs, rm, rz = oracle_unmold(im, dtype, return_resized=True)
-        np.testing.assert_array_equal(b, rb)
-        np.testing.assert_array_equal(c, rc)
-        vs = value_parity_stats(v, rz, rb)
-        ms = mask_parity_stats(m, rm, rz, rb)
-        tot["max_abs_err"] = max(tot["max_abs_err"], vs["max_abs_err"])
-        tot["samples"] += vs["samples"]
-        tot["instances"] += int(rb.shape[0])
-        for k in ("flips_outside_band", "flips_inside_band", "band_pixels", "pixels"):
-            tot[k] += ms[k]
-        # every in-box sample was stored (the buffer was NaN-filled)
-        for i, (y1, x1, y2, x2) in enumerate(rb):
-            assert not np.isnan(v[y1:y2, x1:x2, i]).any()
-    record_stats(name, tot)
-    assert tot["max_abs_err"] <= MASK_VALUE_ATOL, tot
-    assert tot["flips_outside_band"] == 0, tot
-    return tot
-
-
 @pytest.mark.parametrize("name,hw,n,R,classes,kw", [
     ("small_mixed", (96, 128), 12, 16, 5, {}),
     ("tiny_boxes_downscale", (150, 150), 30, 32, 3, dict(min_box=1, max_box_frac=0.1)),
@@ -250,7 +193,7 @@ def test_production_kernel_values_within_tolerance(cuda_device, name, hw, n, R, 
     rng = np.random.default_rng(909)
     ims = [synth.make_image(rng, hw, n, num_classes=classes, max_instances=R, **kw)
            for _ in range(2)]
-    _check_values("values/" + name, ims, R, classes)
+    check_values("values/" + name, ims, R, classes)
 
 
 def test_identity_resize_is_exact(cuda_device):
@@ -258,7 +201,7 @@ def test_identity_resize_is_exact(cuda_device):
     rng = np.random.default_rng(4)
     im = synth.make_image(rng, (64, 64), 6, num_classes=3, max_instances=8, min_box=28,
                           max_box_frac=28 / 64, mold=((64, 64, 3), (0, 0, 64, 64)))
-    (b, c, m, v), = _run_with_values([im], 8, 3)
+    (b, c, m, v), = run_with_values([im], 8, 3)
     assert ((b[:, 2] - b[:, 0]) == 28).all() and ((b[:, 3] - b[:, 1]) == 28).all()
     for i, (y1, x1, y2, x2) in enumerate(b):
         assert np.array_equal(v[y1:y2, x1:x2, i], im.mrcnn_mask[i, :, :, int(c[i])])
@@ -268,14 +211,14 @@ def test_exhaustive_config2_values_and_masks(cuda_device):
     """BASELINE.json configs[1] shape, EVERY instance of two images (1024x1024, 100 instances):
     values within 1e-6, masks equal outside the band; max error / band / flip counts recorded."""
     ims = synth.make_batch(77, 2, (1024, 1024), 100)
-    tot = _check_values("exhaustive/config2_2x1024x1024x100", ims, 100, 81)
+    tot = check_values("exhaustive/config2_2x1024x1024x100", ims, 100, 81)
     assert tot["instances"] == 200
 
 
 def test_exhaustive_config4_4k(cuda_device):
     """BASELINE.json configs[3] shape, every instance of one 2160x3840 image (50 instances)."""
     ims = synth.make_batch(55, 1, (2160, 3840), 50, max_instances=50)
-    tot = _check_values("exhaustive/config4_1x2160x3840x50", ims, 50, 81)
+    tot = check_values("exhaustive/config4_1x2160x3840x50", ims, 50, 81)
     assert tot["instances"] == 50
 
 
@@ -284,7 +227,7 @@ def test_exhaustive_first_image_of_the_bench_batch(cuda_device):
     import bench
 
     im = bench.make_bench_images(0, 1)[0]
-    tot = _check_values("exhaustive/bench_image0", [im], bench.N_INST, bench.CLASSES)
+    tot = check_values("exhaustive/bench_image0", [im], bench.N_INST, bench.CLASSES)
     assert tot["instances"] == bench.N_INST
 
 
