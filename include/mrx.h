@@ -16,6 +16,7 @@
  *   mrx_pack_masks         (extension: bit-packed transport of the masks of serve.py:147)
  *   mrx_mask_expand_packed (extension: the expand step writing that packed layout directly)
  *   mrx_rle_count / _write (extension: the same masks as COCO run-length encodings)
+ *   mrx_contours_count / _write <- visualize.display_instances (contour polygons) serve.py:160-169
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
  *
  * Conventions
@@ -37,7 +38,7 @@
 extern "C" {
 #endif
 
-#define MRX_ABI_VERSION 6
+#define MRX_ABI_VERSION 7
 
 #define MRX_OK              0
 #define MRX_E_INVALID      -1   /* bad argument (null pointer, size out of range) */
@@ -240,6 +241,43 @@ int mrx_rle_write(const float *d_tiles, const int *d_tile_index, const int *d_bo
                   const int *d_counts, const int *d_geom, int *d_col_count,
                   long long *d_inst_off, unsigned int *d_positions, unsigned int *d_run_lengths,
                   int B, int R, int mh, int mw, int max_w, void *stream);
+
+/* EXTENSION: mask outlines as polygons, the contour loop of visualize.display_instances
+ * (serve.py:160-169): for each instance, skimage.measure.find_contours(padded, 0.5) of the mask
+ * padded with one pixel of zeros on every side (fully_connected and positive_orientation 'low'),
+ * vertices as (x, y) image coordinates = np.fliplr(v) - 1 (contours.cu).  Input: the packed planes
+ * of mrx_pack_masks / mrx_mask_expand_packed (d_packed, d_packed_off as written there; d_counts,
+ * d_geom as for them).  d_regions [B,R,4] int32 (y1, x1, y2, x2), required: instance k is traced
+ * only inside that pixel rectangle (clamped to the image; pixels outside it count as 0; an empty
+ * rectangle gives no contour), e.g. the d_boxes of mrx_unmold_prepare, outside which the plane is
+ * zero.  Two calls around one host read:
+ *   mrx_contours_count:  d_row_off [B,R,max_h+1] int32 scratch; d_inst_off [B*R+1] int64: on
+ *                        return (stream-ordered) d_inst_off[i] = number of segments of all
+ *                        instances before i = b*R + k, d_inst_off[B*R] = their total S.  The
+ *                        caller reads them and allocates, from S alone:
+ *                          d_scratch          MRX_CONTOUR_SCRATCH_BYTES(S) bytes
+ *                          d_vertices         float32 [S + S/4, 2]   (every contour has >= 4 segments)
+ *                          d_contour_off      int64 [S/4 + 1]
+ *                          d_inst_contour_off int64 [B*R + 1]
+ *   mrx_contours_write:  total_segments = S, max_inst_segments = the largest d_inst_off[i+1] -
+ *                        d_inst_off[i] (it sets the number of pointer-jumping rounds).  Instance i's
+ *                        contours are c in [d_inst_contour_off[i], d_inst_contour_off[i+1]), in
+ *                        find_contours' order; contour c's vertices are
+ *                        d_vertices[d_contour_off[c] .. d_contour_off[c+1]) as (x, y) pairs, the
+ *                        first repeated at the end.  The values are exact (integers and halves).
+ * S above MRX_MAX_CONTOUR_SEGMENTS: MRX_E_UNSUPPORTED (split the batch). */
+#define MRX_MAX_CONTOUR_SEGMENTS (1 << 30)
+#define MRX_CONTOUR_SCRATCH_BYTES(S) (48LL * (S) + 256)
+int mrx_contours_count(const unsigned char *d_packed, const long long *d_packed_off,
+                       const int *d_counts, const int *d_geom, const int *d_regions,
+                       int *d_row_off, long long *d_inst_off, int B, int R, int max_h,
+                       void *stream);
+int mrx_contours_write(const unsigned char *d_packed, const long long *d_packed_off,
+                       const int *d_counts, const int *d_geom, const int *d_regions,
+                       const int *d_row_off, const long long *d_inst_off, long long total_segments,
+                       long long max_inst_segments, void *d_scratch, float *d_vertices,
+                       long long *d_contour_off, long long *d_inst_contour_off, int B, int R,
+                       int max_h, void *stream);
 
 /* ---------------------------------------------------------------- multi-GPU gather (8e) */
 /* Peer-memory plumbing for the final gather of the canvases to rank 0 (one process per GPU).

@@ -9,7 +9,7 @@ NumPy value semantics, computed by the sm_90a kernels in libmrx.so.
 
 Plus batched entry points the reference lacks (it is hard-wired to one image per call,
 serve.py:48): `unmold_detections_batch`, `unmold_detections_packed_batch`,
-`unmold_detections_rle_batch`, `unmold_overlay_batch`.
+`unmold_detections_rle_batch`, `unmold_detections_contours_batch`, `unmold_overlay_batch`.
 
 Numerical contract (checked by tests/ against the float64 oracle): N, boxes, class ids and
 scores are bit-exact.  The mask resize runs in float32 on exact integer source coordinates;
@@ -362,6 +362,28 @@ def unmold_detections_rle_batch(items):
                          "counts": runs[int(off[i]) + i:int(off[i + 1]) + i + 1].copy()})
         out.append(metas[b] + (rles,))
     return out
+
+
+def unmold_detections_contours_batch(items):
+    """EXTENSION: like `unmold_detections_batch` but every instance comes back as the contour
+    polygons `visualize.display_instances` draws for it -- a list of float64 [V, 2] (x, y) arrays
+    equal to `np.fliplr(v) - 1` of `skimage.measure.find_contours(padded_mask, 0.5)` -- traced on
+    the device from the packed masks; only the vertices travel to the host.  Masks with tiles up
+    to 30 columns are expanded straight into bits (`mrx_mask_expand_packed`), wider ones through
+    the byte canvas and `mrx_pack_masks`.  Returns a list of (boxes, class_ids, scores, contours)."""
+    if len(items) == 0:
+        return []
+    with _Staged(items, canvas=False) as st:
+        eng = st.eng
+        if eng.mw <= 30:
+            eng.enqueue_packed(st.d_det, st.d_msk)
+        else:
+            eng.plan(st.geoms, canvas=True)
+            eng.enqueue(st.d_det, st.d_msk)
+            eng.pack_masks()
+        counts, metas = st.meta()
+        contours = eng.enqueue_contours()
+    return [metas[b] + (contours[b],) for b in range(st.n)]
 
 
 def unmold_overlay_batch(items, images, colors=None, alpha=0.5):

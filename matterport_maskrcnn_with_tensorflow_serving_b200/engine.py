@@ -104,15 +104,17 @@ class UnmoldEngine:
         self._geom_host = None
         self._offsets = None
         self._n_images = 0
+        self._contour_bufs = {}     # work and output buffers of trace_contours, grown as needed
         self.lock = threading.RLock()
         # pinned staging for fetch_meta (one D2H batch + one synchronisation per call)
         self._h_meta = None
 
     def release(self):
-        """Free the canvas and the packed-output buffer (the work buffers stay)."""
+        """Free the canvas, the packed-output and the contour buffers (the work buffers stay)."""
         with self.lock:
             self.d_canvas = None
             self.d_packed = None
+            self._contour_bufs = {}
             self._geom_host = None
             self._offsets = None
             self._packed_off_host = None
@@ -306,6 +308,30 @@ class UnmoldEngine:
                                        self.mw, max_w, st), "mrx_rle_write")
         return d_runs, off
 
+    def trace_contours(self, stream=None):
+        """EXTENSION: the contour polygons of `visualize.display_instances` for every kept
+        instance of the planned batch, traced on the device from the packed planes (after
+        `enqueue_expand_packed` or `pack_masks`) inside each instance's box.  Synchronises to size
+        the output.  Returns (d_vertices float32 [V, 2] device tensor, d_contour_off int64 device
+        tensor [C + 1], inst_contour_off int64 ndarray [n*R + 1]); see `contours_to_lists`."""
+        n = self._n_images
+        if n == 0 or self.d_packed is None:
+            raise RuntimeError("trace_contours needs the packed planes: call enqueue_expand_packed "
+                               "or pack_masks first")
+        return trace_packed_contours(self.lib, self.device, self.d_packed, self.d_packed_off,
+                                     self.d_counts, self.d_geom, self.d_boxes, n, self.R,
+                                     int(self._geom_host[:, 0].max()), stream, self._contour_bufs)
+
+    def enqueue_contours(self, stream=None):
+        """`trace_contours` with the result on the host: per planned image, per kept instance, the
+        list of float64 [V, 2] (x, y) polygons `display_instances` draws for it."""
+        d_vert, d_coff, icoff = self.trace_contours(stream)
+        n = self._n_images
+        with _stream_ctx(stream):
+            counts = self.d_counts[:n].cpu().numpy()
+            verts, coff = _download_contours(d_vert, d_coff)
+        return contours_to_lists(verts, coff, icoff, counts, self.R)
+
     def pack_masks(self, stream=None):
         """EXTENSION: bit-pack the byte canvases already written for the planned batch
         (mrx_pack_masks; same output layout as `enqueue_expand_packed`).  Returns
@@ -350,6 +376,83 @@ class UnmoldEngine:
             raise ValueError(f"image {b}: a detection box falls outside the original image; "
                              "the reference's mask paste cannot broadcast it")
         return counts, hb[:n].numpy(), hk[:n].numpy(), hsc[:n].numpy()
+
+
+def _buffer(bufs, name, numel, dtype, device):
+    """A device tensor of at least `numel` elements kept in `bufs` (reallocated only to grow)."""
+    t = bufs.get(name)
+    if t is None or t.numel() < numel:
+        bufs[name] = None
+        t = bufs[name] = _torch().empty((max(int(numel), 1),), dtype=dtype, device=device)
+    return t
+
+
+def trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom, d_regions, n, R,
+                          max_h, stream=None, bufs=None):
+    """mrx_contours_count, one host read of the segment counts, mrx_contours_write.  Planes and
+    geometry as mrx_pack_masks writes / reads them; d_regions [n,R,4] int32 pixel rectangles.
+    `bufs`: a dict that keeps the work and output buffers between calls.  Returns
+    (d_vertices [V,2] float32, d_contour_off [C+1] int64, inst_contour_off int64 ndarray [n*R+1])."""
+    with _stream_ctx(stream):
+        return _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom,
+                                      d_regions, n, R, max_h, stream,
+                                      {} if bufs is None else bufs)
+
+
+def _stream_ctx(stream):
+    """Make `stream` current (host reads then wait for the work queued on it)."""
+    import contextlib
+
+    return contextlib.nullcontext() if stream is None else _torch().cuda.stream(stream)
+
+
+def _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom, d_regions, n, R,
+                           max_h, stream, bufs):
+    torch = _torch()
+    st = N.stream_ptr(stream)
+    ni = n * R
+    d_rows = _buffer(bufs, "rows", ni * (max_h + 1), torch.int32, device)
+    d_inst = _buffer(bufs, "inst", ni + 1, torch.int64, device)
+    args = (_ptr(d_packed), _ptr(d_packed_off), _ptr(d_counts), _ptr(d_geom), _ptr(d_regions),
+            _ptr(d_rows), _ptr(d_inst))
+    N.check(lib.mrx_contours_count(*args, n, R, max_h, st), "mrx_contours_count")
+    seg_off = d_inst[:ni + 1].cpu().numpy()     # how many segments: sizes every output
+    S = int(seg_off[-1])
+    smax = int(np.diff(seg_off).max()) if ni else 0
+    if S > N.MRX_MAX_CONTOUR_SEGMENTS:
+        raise N.MrxError(f"{S} contour segments in one batch (limit {N.MRX_MAX_CONTOUR_SEGMENTS}); "
+                         "split the batch")
+    d_scr = _buffer(bufs, "scratch", N.contour_scratch_bytes(S), torch.uint8, device)
+    d_vert = _buffer(bufs, "vertices", 2 * (S + S // 4), torch.float32, device)
+    d_coff = _buffer(bufs, "contour_off", S // 4 + 1, torch.int64, device)
+    d_icoff = _buffer(bufs, "inst_contour_off", ni + 1, torch.int64, device)
+    N.check(lib.mrx_contours_write(*args, C.c_longlong(S), C.c_longlong(smax), _ptr(d_scr),
+                                   _ptr(d_vert), _ptr(d_coff), _ptr(d_icoff), n, R, max_h, st),
+            "mrx_contours_write")
+    icoff = d_icoff[:ni + 1].cpu().numpy()
+    n_contours = int(icoff[-1])
+    # every contour repeats its first vertex: V = S + C
+    return d_vert[:2 * (S + n_contours)].view(-1, 2), d_coff[:n_contours + 1], icoff
+
+
+def _download_contours(d_vert, d_coff):
+    """Host copies (float64 vertices [V, 2], int64 contour offsets) of a trace's output."""
+    return d_vert.cpu().numpy().astype(np.float64), d_coff.cpu().numpy()
+
+
+def contours_to_lists(verts, contour_off, inst_contour_off, counts, R):
+    """Per image b, per kept instance k < counts[b], the list of float64 [V, 2] polygons: contour
+    c of instance i = b*R + k for c in [inst_contour_off[i], inst_contour_off[i+1]) has the
+    vertices verts[contour_off[c]:contour_off[c+1]]."""
+    polys = np.split(verts, contour_off[1:-1]) if len(contour_off) > 1 else []
+    out = []
+    for b, k_n in enumerate(counts):
+        per = []
+        for k in range(int(k_n)):
+            i = b * R + k
+            per.append(polys[int(inst_contour_off[i]):int(inst_contour_off[i + 1])])
+        out.append(per)
+    return out
 
 
 class AnchorGenerator:

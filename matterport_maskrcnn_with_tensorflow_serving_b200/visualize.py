@@ -8,8 +8,9 @@ This module does the blending part -- the only part that touches every mask byte
 `mrx_composite_masks`, either on masks the caller holds as NumPy arrays (`apply_masks`,
 `display_instances`) or directly on the device canvas of an `UnmoldEngine`
 (`composite_batch`), which avoids the 105 MB per image device -> host copy of the masks
-when only the overlay is wanted.  Boxes, captions and contours are NOT drawn (matplotlib
-rendering is out of scope, DESIGN.md section 7).
+when only the overlay is wanted.  `mask_contours` computes the contour polygons upstream draws
+(`find_contours` of each padded mask, traced on the device, DESIGN.md section 3.11).  Boxes,
+captions and contours are NOT drawn (matplotlib rendering is out of scope, DESIGN.md section 7).
 """
 from __future__ import annotations
 
@@ -144,6 +145,47 @@ def apply_masks(image, boxes, masks, colors, alpha=0.5):
         _ptr(d_off), _ptr(d_tab), C.c_double(1 - alpha), _ptr(d_out), 1, n,
         C.c_longlong(H * W), N.stream_ptr(None)), "mrx_composite_masks")
     return d_out.cpu().numpy()
+
+
+def mask_contours(boxes, masks):
+    """NumPy in, NumPy out: the contour loop of `display_instances` for one image, traced on the
+    device.  boxes [N,4]; masks bool [H,W,N].  Returns, per instance, the list of float64 [V, 2]
+    (x, y) polygons upstream draws: `np.fliplr(v) - 1` for v in
+    `skimage.measure.find_contours(padded_mask, 0.5)`, the mask padded with one pixel of zeros on
+    every side; no polygon for an instance whose box is all zeros."""
+    import torch
+
+    from .engine import _download_contours, contours_to_lists, trace_packed_contours
+
+    N.require_cuda()
+    lib = N.load()
+    boxes = np.asarray(boxes)
+    H, W = masks.shape[:2]
+    n = int(boxes.shape[0])
+    if masks.ndim != 3 or masks.shape[-1] != n:
+        raise ValueError("masks must be [H, W, N] for N boxes")
+    if n == 0:
+        return []
+    dev = torch.device("cuda", torch.cuda.current_device())
+    total = H * W * n
+    d_canvas = torch.zeros((total + 15) // 16 * 16, dtype=torch.uint8, device=dev)
+    d_canvas[:total].copy_(torch.from_numpy(
+        np.ascontiguousarray(masks).astype(np.bool_, copy=False).view(np.uint8).reshape(-1)))
+    d_off = torch.zeros(1, dtype=torch.int64, device=dev)
+    d_counts = torch.tensor([n], dtype=torch.int32, device=dev)
+    d_geom = torch.tensor([[H, W, H, W, 0, 0, H, W]], dtype=torch.int32, device=dev)
+    d_packed = torch.empty(n * H * ((W + 7) // 8), dtype=torch.uint8, device=dev)
+    N.check(lib.mrx_pack_masks(_ptr(d_canvas), _ptr(d_off), _ptr(d_counts), _ptr(d_geom),
+                               _ptr(d_packed), _ptr(d_off), 1, n, H, W, N.stream_ptr(None)),
+            "mrx_pack_masks")
+    # the whole image, or nothing for an all-zero box (display_instances skips those)
+    regions = np.zeros((n, 4), dtype=np.int32)
+    regions[boxes.reshape(n, -1).any(axis=1)] = (0, 0, H, W)
+    d_regions = torch.from_numpy(regions).to(dev)
+    d_vert, d_coff, icoff = trace_packed_contours(lib, dev, d_packed, d_off, d_counts, d_geom,
+                                                  d_regions, 1, n, H)
+    verts, coff = _download_contours(d_vert, d_coff)
+    return contours_to_lists(verts, coff, icoff, [n], n)[0]
 
 
 def display_instances(image, boxes, masks, class_ids=None, class_names=None, scores=None,

@@ -60,6 +60,15 @@ def unmold_case(name, batch, hw, n, classes, R, iters, base_images=4, seed=7, co
     rle_ms, _ = time_ms(lambda: eng.enqueue_rle(), max(3, iters // 4))
     d_runs, off = eng.enqueue_rle()
     rle_bytes = int(d_runs.numel()) * 4
+    # contour polygons from the packed planes (count pass, one host read of the segment counts,
+    # write pass, and the read of the contour counts): on planes already written, and with the
+    # packed expand before it
+    eng.enqueue_expand_packed()
+    ct_ms, _ = time_ms(lambda: eng.trace_contours(), max(3, iters // 4))
+    pct_ms, _ = time_ms(lambda: (eng.enqueue_expand_packed(), eng.trace_contours()), max(3, iters // 4))
+    d_vert, d_coff, icoff = eng.trace_contours()
+    n_vert, n_contours = int(d_vert.shape[0]), int(icoff[-1])
+    contour_bytes = n_vert * 8 + (n_contours + 1) * 8 + icoff.size * 8
     if composite:
         import random
 
@@ -83,6 +92,10 @@ def unmold_case(name, batch, hw, n, classes, R, iters, base_images=4, seed=7, co
                       "expand_packed_ms": round(pk_ms, 4),
                       "expand_packed_Mmasks_per_s": round(masks / pk_ms / 1e3, 2),
                       "rle_ms_incl_host_read": round(rle_ms, 4), "rle_output_MB": round(rle_bytes / 1e6, 2),
+                      "contours_ms_incl_host_read": round(ct_ms, 4),
+                      "expand_packed_plus_contours_ms": round(pct_ms, 4),
+                      "contour_segments": n_vert - n_contours, "contours": n_contours,
+                      "contour_vertices": n_vert, "contour_output_MB": round(contour_bytes / 1e6, 2),
                       "pack_kernel_ms": round(pack_ms, 4),
                       "pack_kernel_canvas_read_GBps": round(out_bytes / pack_ms / 1e6, 1)}), flush=True)
     del eng, d_det, d_msk
