@@ -1,4 +1,5 @@
-// capi.cu -- ABI housekeeping for include/mrx.h: version, last-error string, device props.
+// capi.cu -- ABI housekeeping for include/mrx.h: version, last-error string, device props; and
+// the host helpers the other sources share (device info, shared-memory opt-in, offsets scan).
 #include <stdarg.h>
 #include <string.h>
 
@@ -55,6 +56,21 @@ int ensure_dynamic_smem(const void *func, SmemCache *cache, int device, int byte
     return MRX_E_CUDA;
   }
   cache->set[device] = bytes;
+  return MRX_OK;
+}
+
+// ---- the second half of every count-then-write pair (RLE, contours): counts -> offsets
+constexpr int kOffsetsScanThreads = 1024;
+
+__global__ void __launch_bounds__(kOffsetsScanThreads)
+offsets_scan_kernel(long long *v, int n) {
+  const long long total = block_scan_range<kOffsetsScanThreads>(v, 0, n);
+  if (threadIdx.x == 0) v[n] = total;
+}
+
+int launch_offsets_scan(long long *d_v, int n, cudaStream_t st) {
+  offsets_scan_kernel<<<1, kOffsetsScanThreads, 0, st>>>(d_v, n);
+  MRX_LAUNCH_CHECK("offsets_scan_kernel");
   return MRX_OK;
 }
 

@@ -63,6 +63,9 @@ struct SmemCache {
 };
 int ensure_dynamic_smem(const void *func, SmemCache *cache, int device, int bytes);
 
+// Exclusive scan of d_v[0, n) in place on `st`, with their sum stored at d_v[n] (one CTA).
+int launch_offsets_scan(long long *d_v, int n, cudaStream_t st);
+
 // ---------------------------------------------------------------- device: PTX wrappers
 #if defined(__CUDACC__)
 
@@ -206,6 +209,62 @@ __device__ __forceinline__ void bulk_wait_all() {
 // make generic-proxy writes to shared memory visible to the async proxy (TMA)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+
+// ---------------------------------------------------------------- device: scans
+// inclusive scan of v over the lanes of a full warp
+template <typename T>
+__device__ __forceinline__ T warp_inclusive_scan(T v, int lane) {
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const T u = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v += u;
+  }
+  return v;
+}
+
+// sum of v over a full warp, in every lane
+template <typename T>
+__device__ __forceinline__ T warp_sum(T v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// Exclusive scan of v over the CTA (every thread calls it); total = the CTA's sum.
+template <typename T, int kThreads>
+__device__ __forceinline__ T block_exclusive_scan(T v, T *s_warp, T &total) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const T incl = warp_inclusive_scan(v, lane);
+  if (lane == 31) s_warp[warp] = incl;
+  __syncthreads();
+  T before = 0, sum = 0;
+#pragma unroll 4
+  for (int w = 0; w < kThreads / 32; ++w) {
+    const T x = s_warp[w];
+    if (w < warp) before += x;
+    sum += x;
+  }
+  __syncthreads();   // s_warp may be reused
+  total = sum;
+  return before + incl - v;
+}
+
+// Exclusive scan of a[lo, hi) in place by one CTA of kThreads (every thread calls it), kThreads
+// elements per pass in T with a 64-bit carry between passes; returns the sum of the range.
+template <int kThreads, typename T>
+__device__ __forceinline__ long long block_scan_range(T *a, int lo, int hi) {
+  __shared__ T s_warp[kThreads / 32];
+  long long carry = 0;
+  for (int base = lo; base < hi; base += kThreads) {
+    const int i = base + threadIdx.x;
+    const T v = i < hi ? a[i] : T(0);
+    T tot;
+    const T ex = block_exclusive_scan<T, kThreads>(v, s_warp, tot);
+    if (i < hi) a[i] = static_cast<T>(carry + ex);
+    carry += tot;
+  }
+  return carry;
 }
 
 #endif  // __CUDACC__

@@ -20,14 +20,16 @@
 //
 //   contour_count_kernel  warp per (instance, cell row): 34 cells per lane from two pixel rows with
 //                         bit operations, segments per row
-//   contour_row_scan_kernel / contour_inst_scan_kernel   row offsets per instance, instance offsets
+//   contour_row_scan_kernel / offsets_scan_kernel (capi.cu)   row offsets per instance, instance
+//                         offsets
 //   --- one host read of the total S and of the longest instance ---
 //   contour_link_kernel   the same walk over three cell rows: each segment's raster number, its
 //                         to-vertex, and its successor's number (row offset + popcount prefix)
 //   contour_jump_kernel   ceil(log2(max S_i)) rounds of pointer jumping: each segment learns the
 //                         smallest and largest number of its cycle and its distance to the largest
 //   contour_head / scan / write kernels   contour lengths, an exclusive scan over the segments
-//                         (contours and vertices before each cycle head), the vertex stores
+//                         (contours and vertices before each cycle head; the tile sums by
+//                         offsets_scan_kernel), the vertex stores
 //
 // Pointer jumping reads one 16-byte record per segment and round at a random address: the cost is
 // about ceil(log2(max S_i)) x 48 bytes of traffic per segment, far above the counting walk.
@@ -160,45 +162,6 @@ __device__ __forceinline__ CellRow cell_row(const Inst &in, int r, int c0) {
   return cr;
 }
 
-__device__ __forceinline__ int warp_sum(int v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-__device__ __forceinline__ int warp_incl_scan(int v, int lane) {
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int u = __shfl_up_sync(0xffffffffu, v, o);
-    if (lane >= o) v += u;
-  }
-  return v;
-}
-
-// Exclusive scan of v over the CTA (every thread calls it); total = the CTA's sum.
-template <typename T, int kThreads>
-__device__ __forceinline__ T block_exclusive_scan(T v, T *s_warp, T &total) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  T incl = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const T u = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += u;
-  }
-  if (lane == 31) s_warp[warp] = incl;
-  __syncthreads();
-  T before = 0, sum = 0;
-#pragma unroll 4
-  for (int w = 0; w < kThreads / 32; ++w) {
-    const T x = s_warp[w];
-    if (w < warp) before += x;
-    sum += x;
-  }
-  __syncthreads();   // s_warp may be reused
-  total = sum;
-  return before + incl - v;
-}
-
 // One warp per (instance, cell row): segments of the row, lanes on 32-cell words.
 __global__ void __launch_bounds__(kRowWarps * 32)
 contour_count_kernel(const Params p) {
@@ -214,40 +177,13 @@ contour_count_kernel(const Params p) {
   if (lane == 0) p.row_off[(static_cast<size_t>(b) * p.R + k) * p.row_pitch + j] = n;
 }
 
-// One CTA per instance: exclusive scan of its row counts (in place), instance total out.
+// One CTA per instance: exclusive scan of its cell rows' counts (in place), instance total out.
 __global__ void __launch_bounds__(256)
 contour_row_scan_kernel(const Params p) {
-  __shared__ long long s_warp[8];
   const int k = blockIdx.x, b = blockIdx.y;
   const size_t inst = static_cast<size_t>(b) * p.R + k;
-  const Inst in = inst_of(p, b, k);
-  int *ro = p.row_off + inst * p.row_pitch;
-  long long carry = 0;
-  for (int base = 0; base < in.nrows; base += 256) {
-    const int j = base + threadIdx.x;
-    const long long v = j < in.nrows ? ro[j] : 0;
-    long long tot;
-    const long long ex = block_exclusive_scan<long long, 256>(v, s_warp, tot);
-    if (j < in.nrows) ro[j] = static_cast<int>(carry + ex);
-    carry += tot;
-  }
-  if (threadIdx.x == 0) p.inst_off[inst] = carry;
-}
-
-// Exclusive scan of the n instance totals in place, inst_off[n] = their sum.  One CTA.
-__global__ void __launch_bounds__(1024)
-contour_inst_scan_kernel(long long *inst_off, int n) {
-  __shared__ long long s_warp[32];
-  long long carry = 0;
-  for (int base = 0; base < n; base += 1024) {
-    const int i = base + threadIdx.x;
-    const long long v = i < n ? inst_off[i] : 0;
-    long long tot;
-    const long long ex = block_exclusive_scan<long long, 1024>(v, s_warp, tot);
-    if (i < n) inst_off[i] = carry + ex;
-    carry += tot;
-  }
-  if (threadIdx.x == 0) inst_off[n] = carry;
+  const long long total = block_scan_range<256>(p.row_off + inst * p.row_pitch, 0, inst_of(p, b, k).nrows);
+  if (threadIdx.x == 0) p.inst_off[inst] = total;
 }
 
 // The count walk again over the rows above, at and below: every segment of the row gets its
@@ -278,8 +214,8 @@ contour_link_kernel(const Params p) {
       dn = cell_row(in, r + 1, c0);
     }
     const int nu = up.own_count(), nc = cr.own_count(), nd = dn.own_count();
-    const int iu = warp_incl_scan(nu, lane), ic = warp_incl_scan(nc, lane),
-              id = warp_incl_scan(nd, lane);
+    const int iu = warp_inclusive_scan(nu, lane), ic = warp_inclusive_scan(nc, lane),
+              id = warp_inclusive_scan(nd, lane);
     // first segment number of this word's own cells in each row
     const int wu = base_u + iu - nu, wc = base_c + ic - nc, wd = base_d + id - nd;
     base_u += __shfl_sync(0xffffffffu, iu, 31);
@@ -371,7 +307,7 @@ contour_head_kernel(const int4 *__restrict__ f, const int *__restrict__ succ,
 }
 
 // exclusive scan of the packed (contours, vertices) pairs: tile sums, scan of the tile sums (total
-// at bsum[ntiles]), tile scans
+// at bsum[ntiles], launch_offsets_scan), tile scans
 __global__ void __launch_bounds__(kScanThreads)
 contour_scan_reduce_kernel(const unsigned long long *__restrict__ v, unsigned long long *bsum, int S) {
   __shared__ unsigned long long s_warp[kScanThreads / 32];
@@ -383,21 +319,6 @@ contour_scan_reduce_kernel(const unsigned long long *__restrict__ v, unsigned lo
   unsigned long long tot;
   block_exclusive_scan<unsigned long long, kScanThreads>(x, s_warp, tot);
   if (threadIdx.x == 0) bsum[blockIdx.x] = tot;
-}
-
-__global__ void __launch_bounds__(kScanThreads)
-contour_scan_tiles_kernel(unsigned long long *bsum, int n) {
-  __shared__ unsigned long long s_warp[kScanThreads / 32];
-  unsigned long long carry = 0ull;
-  for (int base = 0; base < n; base += kScanThreads) {
-    const int i = base + threadIdx.x;
-    const unsigned long long x = i < n ? bsum[i] : 0ull;
-    unsigned long long tot;
-    const unsigned long long ex = block_exclusive_scan<unsigned long long, kScanThreads>(x, s_warp, tot);
-    if (i < n) bsum[i] = carry + ex;
-    carry += tot;
-  }
-  if (threadIdx.x == 0) bsum[n] = carry;
 }
 
 __global__ void __launch_bounds__(kScanThreads)
@@ -499,9 +420,7 @@ extern "C" int mrx_contours_count(const unsigned char *d_packed, const long long
   MRX_LAUNCH_CHECK("contour_count_kernel");
   contours::contour_row_scan_kernel<<<dim3(R, B), 256, 0, st>>>(prm);
   MRX_LAUNCH_CHECK("contour_row_scan_kernel");
-  contours::contour_inst_scan_kernel<<<1, 1024, 0, st>>>(d_inst_off, B * R);
-  MRX_LAUNCH_CHECK("contour_inst_scan_kernel");
-  return MRX_OK;
+  return launch_offsets_scan(d_inst_off, B * R, st);
 }
 
 extern "C" int mrx_contours_write(const unsigned char *d_packed, const long long *d_packed_off,
@@ -556,8 +475,10 @@ extern "C" int mrx_contours_write(const unsigned char *d_packed, const long long
     MRX_LAUNCH_CHECK("contour_head_kernel");
     contour_scan_reduce_kernel<<<ntiles, kScanThreads, 0, st>>>(scan, bsum, S);
     MRX_LAUNCH_CHECK("contour_scan_reduce_kernel");
-    contour_scan_tiles_kernel<<<1, kScanThreads, 0, st>>>(bsum, ntiles);
-    MRX_LAUNCH_CHECK("contour_scan_tiles_kernel");
+    // The tile sums are (contours << 32) | vertices pairs.  Every partial sum stays below 2^61 and
+    // the low half never carries (V = S + C < 2^32 at MRX_MAX_CONTOUR_SEGMENTS), so the signed
+    // 64-bit scan gives the same bits as an unsigned one.
+    if (int rc = launch_offsets_scan(reinterpret_cast<long long *>(bsum), ntiles, st)) return rc;
     contour_scan_apply_kernel<<<ntiles, kScanThreads, 0, st>>>(scan, bsum, S);
     MRX_LAUNCH_CHECK("contour_scan_apply_kernel");
     contour_write_kernel<<<grid, 256, 0, st>>>(jump[cur], len, scan, prm.to,

@@ -92,6 +92,39 @@ __device__ __forceinline__ float hrow(float rv, int idx, float wx) {
   const float hi = __shfl_sync(0xffffffffu, rv, idx + 1);
   return lerp(wx, lo, hi);
 }
+
+// ---- the scheduler of the persistent kernels.  Workers draw tickets 0, 1, ... from words[0]
+// of their scheduler pair; ticket j names the j-th work item of the batch, image by image.
+// Work table, on warp 0: s_prefix[b] = the work items of the images before b (b in [0, B]),
+// *s_total = all of them; work_of_b(b) = the items of image b.  The caller synchronises.
+// (Callers capture by value: a lambda holding a reference to the kernel's parameter struct
+// changes how the rest of the kernel is optimised.)
+template <typename WorkOf>
+__device__ __forceinline__ void image_work_table(int B, WorkOf work_of_b, int *s_prefix, int *s_total) {
+  const int lane = threadIdx.x & 31;
+  int carry = 0;
+  for (int base = 0; base < B; base += 32) {
+    const int b = base + lane;
+    const int incl = warp_inclusive_scan(b < B ? work_of_b(b) : 0, lane);
+    if (b < B) s_prefix[b + 1] = carry + incl;
+    carry += __shfl_sync(0xffffffffu, incl, 31);
+  }
+  if (lane == 0) {
+    s_prefix[0] = 0;
+    *s_total = carry;
+  }
+}
+
+// One thread of a worker that is done: counts it in words[1], and the last of the grid's
+// gridDim.x * workers_per_cta workers (CTAs, teams or warps) leaves both words at zero for the
+// next launch (no memset between launches).
+__device__ __forceinline__ void retire_worker(unsigned int *words, unsigned workers_per_cta) {
+  __threadfence();
+  if (atomicAdd(words + 1, 1u) == gridDim.x * workers_per_cta - 1u) {
+    words[0] = 0u;
+    words[1] = 0u;
+  }
+}
 #endif  // __CUDACC__
 
 struct ExpandParams {

@@ -97,28 +97,11 @@ mask_expand_bits_kernel(const BitsParams p) {
   for (int i = tid; i < (ubuf >> 4); i += kWarps * 32)
     reinterpret_cast<uint4 *>(s_zero)[i] = make_uint4(0u, 0u, 0u, 0u);
   if (warp == 0) {
-    int carry = 0;
-    for (int base = 0; base < p.B; base += 32) {
-      const int b = base + lane;
-      int v = 0;
-      if (b < p.B) {
-        const int H = p.geom[b * MRX_GEOM_INTS + 0], W = p.geom[b * MRX_GEOM_INTS + 1];
-        const int rb = unit_rows((W + 7) >> 3, ubuf);
-        v = p.counts[b] * ((H + rb - 1) / rb);
-      }
-      int incl = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += u;
-      }
-      if (b < p.B) s_prefix[b + 1] = carry + incl;
-      carry += __shfl_sync(0xffffffffu, incl, 31);
-    }
-    if (lane == 0) {
-      s_prefix[0] = 0;
-      s_total = carry;
-    }
+    image_work_table(p.B, [=](int b) {
+      const int H = p.geom[b * MRX_GEOM_INTS + 0], W = p.geom[b * MRX_GEOM_INTS + 1];
+      const int rb = unit_rows((W + 7) >> 3, ubuf);
+      return p.counts[b] * ((H + rb - 1) / rb);
+    }, s_prefix, &s_total);
   }
   fence_proxy_async_smem();   // the zero page is read by bulk copies only
   __syncthreads();
@@ -276,15 +259,10 @@ mask_expand_bits_kernel(const BitsParams p) {
       store_unit(g, buf + a, len, lane);
     }
   }
-  // ---- drain this warp's copies, then retire; the last warp of the grid leaves the scheduler
-  // words at zero for the next launch
+  // ---- drain this warp's copies, then retire (the workers are the warps)
   if (lane == 0) {
     bulk_wait_all<0>();
-    __threadfence();
-    if (atomicAdd(p.sched + 3, 1u) == gridDim.x * kWarps - 1u) {
-      p.sched[2] = 0u;
-      p.sched[3] = 0u;
-    }
+    retire_worker(p.sched + 2, kWarps);
   }
 }
 

@@ -210,25 +210,9 @@ mask_expand_team_kernel(const ExpandParams p, const int buf_bytes) {
 
   // ---- tiles per image -> prefix sums (first warp)
   if (warp == 0) {
-    int carry = 0;
-    for (int base = 0; base < p.B; base += 32) {
-      const int b = base + lane;
-      int v = 0;
-      if (b < p.B)
-        v = tiles_of(p.geom[b * MRX_GEOM_INTS + 0], p.geom[b * MRX_GEOM_INTS + 1], p.counts[b], rowcap, kTileRows);
-      int incl = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += u;
-      }
-      if (b < p.B) s_prefix[b + 1] = carry + incl;
-      carry += __shfl_sync(0xffffffffu, incl, 31);
-    }
-    if (lane == 0) {
-      s_prefix[0] = 0;
-      s_total = carry;
-    }
+    image_work_table(p.B, [=](int b) {
+      return tiles_of(p.geom[b * MRX_GEOM_INTS + 0], p.geom[b * MRX_GEOM_INTS + 1], p.counts[b], rowcap, kTileRows);
+    }, s_prefix, &s_total);
   }
   __syncthreads();
   const int total = s_total;
@@ -354,20 +338,9 @@ mask_expand_team_kernel(const ExpandParams p, const int buf_bytes) {
     if (ticket == 0xffffffffu) p.job_counter[0] = 0u;   // (never true) all three tickets are drawn: see the end
   }
   team_bar(bar_id, kTeamThreads);
-  // a team that is done says so; the last one of the grid leaves both scheduler words at zero
-  // for the next launch (no memset between launches)
-  auto retire = [&]() {
-    if (tt == 0) {
-      __threadfence();
-      const unsigned done = atomicAdd(p.job_counter + 1, 1u);
-      if (done == gridDim.x * kTeams - 1u) {
-        p.job_counter[0] = 0u;
-        p.job_counter[1] = 0u;
-      }
-    }
-  };
+  // the workers are the teams
   if (!s_job[0].valid) {   // fewer tiles than teams: nothing for this team
-    retire();
+    if (tt == 0) retire_worker(p.job_counter, kTeams);
     return;
   }
   cull(s_job[0], 0, 0, wt, kTeamWarps);
@@ -667,7 +640,7 @@ mask_expand_team_kernel(const ExpandParams p, const int buf_bytes) {
   // of the grid zeroes the counter): reading its value waits for it
   if (ticket == 0xffffffffu) p.job_counter[0] = 0u;   // (never true: not a ticket in either format)
   team_bar(bar_id, kTeamThreads);
-  retire();
+  if (tt == 0) retire_worker(p.job_counter, kTeams);
   PROF_MARK(5)
   PROF_FLUSH
 }

@@ -115,9 +115,7 @@ pack_quads_kernel(const unsigned char *__restrict__ canvas, const long long *__r
       // padding (every slot starts 16-byte aligned and holds whole words, see mrx.h), never
       // unmapped memory
       const unsigned bytes = npx_r ? (static_cast<unsigned>(a + npx_r * N) + 15u) & ~15u : 0u;
-      unsigned total = bytes;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+      const unsigned total = warp_sum(bytes);
       if (r == 0) mbar_arrive_expect_tx(&s_bar, total);
       __syncwarp();
       if (bytes)

@@ -12,7 +12,7 @@
 //
 //   rle_walk_kernel<false>   per (instance, 32-column block): number of transitions per column
 //   rle_scan_kernel          per instance: exclusive scan over its columns, instance total
-//   rle_offsets_kernel       exclusive scan of the instance totals (one CTA)
+//   offsets_scan_kernel      exclusive scan of the instance totals (capi.cu, one CTA)
 //   rle_walk_kernel<true>    the same walk again, now writing each transition's flat position
 //                            x*H + y at (instance base + column offset + running index)
 //   rle_counts_kernel        positions -> run lengths (differences, closing run to H*W)
@@ -148,73 +148,22 @@ rle_walk_kernel(const RleParams p) {
   if (!kWrite && colvalid) p.col_count[(static_cast<size_t>(b) * p.R + k) * p.max_w + x] = n;
 }
 
-// One CTA per instance: exclusive scan of its columns' transition counts (in place), total out.
+// One CTA per instance: exclusive scan of its box columns' transition counts (in place), total out.
 __global__ void __launch_bounds__(256)
 rle_scan_kernel(const RleParams p) {
   const int k = blockIdx.x, b = blockIdx.y;
   const size_t inst = static_cast<size_t>(b) * p.R + k;
-  __shared__ int s_warp[8];
-  __shared__ int s_carry;
-  if (k >= p.counts[b]) {
-    if (threadIdx.x == 0) p.inst_off[inst] = 0;
-    return;
-  }
-  const int H = p.geom[b * MRX_GEOM_INTS + 0], W = p.geom[b * MRX_GEOM_INTS + 1];
-  const int4 bx = p.boxes[inst];
-  const bool sane = box_in_canvas(bx, H, W);
-  const int x1 = sane ? bx.y : 0, x2 = sane ? bx.w : 0;
-  int *cc = p.col_count + inst * p.max_w;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) s_carry = 0;
-  __syncthreads();
-  for (int base = x1; base < x2; base += 256) {
-    const int x = base + threadIdx.x;
-    const int v = x < x2 ? cc[x] : 0;
-    int incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int u = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += u;
+  int x1 = 0, x2 = 0;   // no columns: not a kept instance, or its box is outside the canvas
+  if (k < p.counts[b]) {
+    const int H = p.geom[b * MRX_GEOM_INTS + 0], W = p.geom[b * MRX_GEOM_INTS + 1];
+    const int4 bx = p.boxes[inst];
+    if (box_in_canvas(bx, H, W)) {
+      x1 = bx.y;
+      x2 = bx.w;
     }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    int before = s_carry;
-    for (int w = 0; w < warp; ++w) before += s_warp[w];
-    if (x < x2) cc[x] = before + incl - v;
-    __syncthreads();
-    if (threadIdx.x == 255) s_carry = before + incl;
-    __syncthreads();
   }
-  if (threadIdx.x == 0) p.inst_off[inst] = s_carry;
-}
-
-// Exclusive scan of the n instance totals in place; inst_off[n] = grand total.  One CTA.
-__global__ void __launch_bounds__(1024)
-rle_offsets_kernel(long long *inst_off, int n) {
-  __shared__ long long s_warp[32];
-  __shared__ long long s_carry;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (threadIdx.x == 0) s_carry = 0;
-  __syncthreads();
-  for (int base = 0; base < n; base += 1024) {
-    const int i = base + threadIdx.x;
-    const long long v = i < n ? inst_off[i] : 0;
-    long long incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const long long u = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += u;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    long long before = s_carry;
-    for (int w = 0; w < warp; ++w) before += s_warp[w];
-    if (i < n) inst_off[i] = before + incl - v;
-    __syncthreads();
-    if (threadIdx.x == 1023) s_carry = before + incl;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) inst_off[n] = s_carry;
+  const long long total = block_scan_range<256>(p.col_count + inst * p.max_w, x1, x2);
+  if (threadIdx.x == 0) p.inst_off[inst] = total;
 }
 
 // positions -> run lengths.  Instance i has T = inst_off[i+1] - inst_off[i] transitions and
@@ -288,9 +237,7 @@ extern "C" int mrx_rle_count(const float *d_tiles, const int *d_tile_index, cons
   MRX_LAUNCH_CHECK("rle_walk_kernel<count>");
   rle::rle_scan_kernel<<<dim3(R, B), 256, 0, st>>>(prm);
   MRX_LAUNCH_CHECK("rle_scan_kernel");
-  rle::rle_offsets_kernel<<<1, 1024, 0, st>>>(d_inst_off, B * R);
-  MRX_LAUNCH_CHECK("rle_offsets_kernel");
-  return MRX_OK;
+  return launch_offsets_scan(d_inst_off, B * R, st);
 }
 
 extern "C" int mrx_rle_write(const float *d_tiles, const int *d_tile_index, const int *d_boxes,

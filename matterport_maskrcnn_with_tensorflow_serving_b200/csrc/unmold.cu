@@ -321,28 +321,11 @@ mask_expand_kernel(const ExpandParams p) {
 
   // ---- job table: jobs_b = ceil(H*W*N_b / chunk); exclusive prefix in s_jobs
   if (warp == 0) {
-    int carry = 0;
-    for (int base = 0; base < p.B; base += 32) {
-      const int b = base + lane;
-      int v = 0;
-      if (b < p.B) {
-        const long long bytes = static_cast<long long>(p.geom[b * MRX_GEOM_INTS + 0]) *
-                                p.geom[b * MRX_GEOM_INTS + 1] * p.counts[b];
-        v = static_cast<int>((bytes + p.chunk_bytes - 1) / p.chunk_bytes);
-      }
-      int incl = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += u;
-      }
-      if (b < p.B) s_jobs[b + 1] = carry + incl;
-      carry += __shfl_sync(0xffffffffu, incl, 31);
-    }
-    if (lane == 0) {
-      s_jobs[0] = 0;
-      s_total = carry;
-    }
+    image_work_table(p.B, [=](int b) {
+      const long long bytes = static_cast<long long>(p.geom[b * MRX_GEOM_INTS + 0]) *
+                              p.geom[b * MRX_GEOM_INTS + 1] * p.counts[b];
+      return static_cast<int>((bytes + p.chunk_bytes - 1) / p.chunk_bytes);
+    }, s_jobs, &s_total);
   }
   if (tid == 0) {
     mbar_init(&s_bar, 1);
@@ -513,12 +496,7 @@ mask_expand_kernel(const ExpandParams p) {
   }
   if (tid == 0) {
     bulk_wait_all<0>();
-    // the last CTA to retire leaves both scheduler words at zero for the next launch
-    __threadfence();
-    if (atomicAdd(p.job_counter + 1, 1u) == gridDim.x - 1u) {
-      p.job_counter[0] = 0u;
-      p.job_counter[1] = 0u;
-    }
+    retire_worker(p.job_counter, 1u);   // the workers are the CTAs
   }
 }
 

@@ -11,9 +11,10 @@ import random
 import numpy as np
 import pytest
 
+import contour_oracle as co
 import oracle
 from matterport_maskrcnn_with_tensorflow_serving_b200 import _native as N
-from matterport_maskrcnn_with_tensorflow_serving_b200 import synth, visualize
+from matterport_maskrcnn_with_tensorflow_serving_b200 import sharding, synth, visualize
 
 from helpers import (canvas_masks, check_values, compare_masks, oracle_unmold, pad_rows,
                      prepared_engine, record_stats)
@@ -153,6 +154,22 @@ def mixed_batch():
 
 
 @pytest.mark.parametrize("R", [100, GENERIC_R], ids=["team", "generic"])
+def test_expand_launches_after_one_prepare(cuda_device, mixed_batch, R):
+    """Every expand launch leaves its scheduler words at zero for the next one (mrx.h,
+    MRX_SCHED_WORDS): after one prepare, expanding the batch in image ranges, one launch each,
+    writes the bytes of a single launch.  One range holds only the image without instances."""
+    ims, _ = mixed_batch
+    whole, counts = _expand(ims, R, 4)
+    eng = prepared_engine([pad_rows(im, R) for im in ims], R, 4, np.float32)
+    eng.d_canvas.fill_(7)
+    bounds = sharding.chunk_bounds(len(ims), 3)
+    assert len(bounds) == 3 and (2, 3) in bounds and counts[2] == 0
+    for b0, b1 in bounds:
+        eng.enqueue_expand(images=(b0, b1))
+    _assert_same_canvas(whole, eng, counts, f"launches over {bounds}")
+
+
+@pytest.mark.parametrize("R", [100, GENERIC_R], ids=["team", "generic"])
 def test_mixed_geometries_in_one_launch(cuda_device, mixed_batch, R):
     ims, refs = mixed_batch
     eng, counts = _expand(ims, R, 4)
@@ -182,6 +199,17 @@ def test_mixed_geometries_in_one_launch(cuda_device, mixed_batch, R):
     check_packed(d_packed, off, "mrx_mask_expand_packed")
     d_packed.fill_(0xAA)
     check_packed(*eng.pack_masks(), "mrx_pack_masks")
+
+    # contours of those planes; B * R > 1024 for the generic R, so the instance offsets are
+    # scanned in more than one pass of the one-CTA scan
+    polys = eng.enqueue_contours()
+    for b in range(len(ims)):
+        k = int(counts[b])
+        want = co.mask_polygons(boxes[b, :k], masks[b])
+        assert len(polys[b]) == k == len(want), f"contours: image {b}"
+        for n, (got, ref) in enumerate(zip(polys[b], want)):
+            assert len(got) == len(ref) and all(np.array_equal(g, r) for g, r in zip(got, ref)), \
+                f"contours: image {b}, instance {n}"
 
     d_runs, off = eng.enqueue_rle()
     runs = d_runs.cpu().numpy().view(np.uint32)
