@@ -18,6 +18,7 @@
  *   mrx_rle_count / _write (extension: the same masks as COCO run-length encodings)
  *   mrx_contours_count / _write <- visualize.display_instances (contour polygons) serve.py:160-169
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
+ *   mrx_device_alloc/_free (the canvas allocation: compressible device memory where offered)
  *
  * Conventions
  *   - every pointer named d_* is DEVICE memory owned by the caller (the Python
@@ -38,7 +39,7 @@
 extern "C" {
 #endif
 
-#define MRX_ABI_VERSION 7
+#define MRX_ABI_VERSION 8
 
 #define MRX_OK              0
 #define MRX_E_INVALID      -1   /* bad argument (null pointer, size out of range) */
@@ -295,6 +296,17 @@ int mrx_peer_open(const unsigned char *handle64, void **d_ptr);
 int mrx_peer_close(void *d_ptr);
 int mrx_peer_signal(unsigned int *d_flag, unsigned int value, void *stream);
 int mrx_peer_wait(const unsigned int *d_flags, int n_flags, unsigned int value, void *stream);
+
+/* ---------------------------------------------------------------- canvas memory */
+/* Device memory on the current device for the mask canvas, requested as compressible (Hopper's
+ * compute data compression: mostly-zero lines take fewer DRAM bytes, reads and writes are
+ * unchanged) when the device reports CU_DEVICE_ATTRIBUTE_GENERIC_COMPRESSION_SUPPORTED, plain
+ * otherwise or when the compressible request is refused.  The size is rounded up to the
+ * allocation granularity.  *compressed = 1 when the driver granted compression, else 0.
+ * mrx_device_free takes the pointer and the byte count given to mrx_device_alloc; it synchronises
+ * the device first (as cudaFree does). */
+int mrx_device_alloc(unsigned long long bytes, void **d_ptr, int *compressed);
+int mrx_device_free(void *d_ptr, unsigned long long bytes);
 
 #ifdef __cplusplus
 }

@@ -23,7 +23,7 @@ MRX_ST_CLASS_RANGE = 1
 MRX_ST_BOX_RANGE = 2
 MRX_GEOM_INTS = 8
 MRX_MAX_BATCH = 4096
-ABI_VERSION = 7
+ABI_VERSION = 8
 MRX_SCHED_WORDS = 4
 MRX_PEER_HANDLE_BYTES = 64
 MRX_MAX_CONTOUR_SEGMENTS = 1 << 30
@@ -61,6 +61,8 @@ SIGNATURES = {
     "mrx_contours_count": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "mrx_contours_write": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_longlong, C.c_longlong,
                                 _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "mrx_device_alloc": (_i, [C.c_ulonglong, C.POINTER(C.c_void_p), _ip]),
+    "mrx_device_free": (_i, [_vp, C.c_ulonglong]),
     "mrx_peer_alloc": (_i, [C.c_ulonglong, C.POINTER(C.c_void_p)]),
     "mrx_peer_free": (_i, [_vp]),
     "mrx_peer_export": (_i, [_vp, C.c_char_p]),
@@ -144,6 +146,16 @@ def stream_ptr(stream):
     if stream is None:
         stream = torch.cuda.current_stream()
     return C.c_void_p(stream.cuda_stream)
+
+
+class DeviceBytes:
+    """`__cuda_array_interface__` view of raw device memory, so that torch can wrap memory it did
+    not allocate (peer memory, the canvas of mrx_device_alloc); torch keeps the object alive for
+    as long as the tensor's storage lives."""
+
+    def __init__(self, ptr, nbytes):
+        self.__cuda_array_interface__ = {"shape": (int(nbytes),), "typestr": "|u1",
+                                         "data": (int(ptr), False), "version": 2}
 
 
 def require_cuda():

@@ -13,6 +13,7 @@ from __future__ import annotations
 
 import ctypes as C
 import threading
+import weakref
 
 import numpy as np
 
@@ -57,7 +58,9 @@ class UnmoldEngine:
     Work buffers for up to `max_batch` images of up to `max_instances` detection rows are
     allocated once; the canvas (bool [H,W,N] per image, N innermost) lives in one device
     buffer with a fixed-capacity slot per image (capacity H*W*R rounded up to 256 B) so
-    that nothing on the path depends on a host read of the kept counts.
+    that nothing on the path depends on a host read of the kept counts.  The canvas comes from
+    mrx_device_alloc: compressible memory where the GPU grants it (`canvas_compressed`), so its
+    mostly-zero lines cost fewer DRAM bytes than they hold.
 
     Thread safety: an engine is a set of device buffers plus the plan of the last batch; a
     plan -> enqueue -> fetch sequence must not interleave with another thread's.  Callers
@@ -98,6 +101,7 @@ class UnmoldEngine:
         # scheduler words of the expand kernels: zeroed once here, left zeroed by every launch
         self.d_sched = torch.zeros((N.MRX_SCHED_WORDS,), dtype=i32, device=dev)
         self.d_canvas = None
+        self.canvas_compressed = False
         self.d_packed = None
         self.d_packed_off = None
         self._packed_off_host = None
@@ -146,7 +150,7 @@ class UnmoldEngine:
         total = int(off[-1])
         if canvas and (self.d_canvas is None or self.d_canvas.numel() < total):
             self.d_canvas = None
-            self.d_canvas = torch.empty((total,), dtype=torch.uint8, device=self.device)
+            self.d_canvas, self.canvas_compressed = _device_bytes(self.lib, total, self.device)
         self.d_geom[:n].copy_(torch.from_numpy(g))
         self.d_canvas_off[:n].copy_(torch.from_numpy(off[:n].copy()))
         self._geom_host = g
@@ -376,6 +380,26 @@ class UnmoldEngine:
             raise ValueError(f"image {b}: a detection box falls outside the original image; "
                              "the reference's mask paste cannot broadcast it")
         return counts, hb[:n].numpy(), hk[:n].numpy(), hsc[:n].numpy()
+
+
+def _device_bytes(lib, nbytes, device):
+    """(uint8 tensor of `nbytes`, compressed) over memory from mrx_device_alloc on `device`.  The
+    memory is freed when the last view of the tensor dies."""
+    torch = _torch()
+    ptr, compressed = C.c_void_p(0), C.c_int(0)
+    with torch.cuda.device(device):
+        N.check(lib.mrx_device_alloc(C.c_ulonglong(nbytes), C.byref(ptr), C.byref(compressed)),
+                "mrx_device_alloc")
+    owner = N.DeviceBytes(ptr.value, nbytes)
+    # torch holds `owner` for as long as any view of the tensor lives; at interpreter exit the
+    # driver reclaims the memory itself
+    weakref.finalize(owner, _free_device_bytes, lib, ptr.value, nbytes, device).atexit = False
+    return torch.as_tensor(owner, device=device), bool(compressed.value)
+
+
+def _free_device_bytes(lib, ptr, nbytes, device):
+    with _torch().cuda.device(device):
+        N.check(lib.mrx_device_free(C.c_void_p(ptr), C.c_ulonglong(nbytes)), "mrx_device_free")
 
 
 def _buffer(bufs, name, numel, dtype, device):

@@ -191,14 +191,6 @@ class RootGather:
         self._reqs = []
 
 
-class _DeviceBytes:
-    """`__cuda_array_interface__` view of raw device memory (so torch can wrap peer memory)."""
-
-    def __init__(self, ptr, nbytes):
-        self.__cuda_array_interface__ = {"shape": (int(nbytes),), "typestr": "|u1",
-                                         "data": (int(ptr), False), "version": 2}
-
-
 class PeerGather:
     """Fused compute + gather: rank `dst` owns one receive buffer, every rank's expand kernels
     write their output straight into it (their own range of it) over NVLink.
@@ -266,7 +258,7 @@ class PeerGather:
             self._release_local()
             raise RuntimeError(f"peer memory unavailable on at least one rank ({err})")
         if self._owner:
-            self._all = torch.as_tensor(_DeviceBytes(self.base, self.total), device=device)
+            self._all = torch.as_tensor(N.DeviceBytes(self.base, self.total), device=device)
             self._all[:self.HEADER].zero_()
             self.recv = self._all[self.HEADER:]
             torch.cuda.synchronize()
