@@ -60,6 +60,7 @@ extern "C" {
 #define MRX_MAX_RATIOS   8
 #define MRX_MAX_BATCH    4096    /* images per mrx_mask_expand launch */
 #define MRX_MAX_MASK_DIM 64      /* mask tile side (28 upstream); width must be a multiple of 4 */
+#define MRX_MAX_LANE_MASK_W 30   /* tile width of the lane kernels: mw + 2 lanes per warp */
 
 int         mrx_abi_version(void);
 const char *mrx_last_error(void);
@@ -113,10 +114,25 @@ int mrx_unmold_prepare(const void *d_detections, int det_dtype, const void *d_mr
                        int *d_src_index, int *d_counts, int *d_status,
                        float *d_tiles, unsigned int *d_sched, void *stream);
 
+/* Tile batch: the inputs of every entry point that reads the class tiles (mrx_mask_expand,
+ * mrx_mask_expand_values, mrx_mask_expand_packed, mrx_rle_count, mrx_rle_write), as
+ * mrx_unmold_prepare leaves them:
+ *   d_tiles [B,R,mh,mw] float32   d_boxes [B,R,4] int32   d_counts [B] int32   d_geom [B,8] int32
+ *   d_tile_index [B,R] int32, required: kept instance k of image b resizes
+ *   d_tiles[b][d_tile_index[b][k]] (d_src_index for the layout mrx_unmold_prepare writes).
+ * Each of them checks these first, in this order, before anything reaches the device:
+ *   - d_tiles, d_boxes, d_counts or d_geom null: MRX_E_INVALID;
+ *   - B outside [0, MRX_MAX_BATCH] or R outside [1, 65534]: MRX_E_INVALID;
+ *   - mh outside [2, MRX_MAX_MASK_DIM], or mw outside [4, max_mw] or not a multiple of 4:
+ *     MRX_E_UNSUPPORTED.  max_mw is MRX_MAX_MASK_DIM for mrx_mask_expand and MRX_MAX_LANE_MASK_W
+ *     for the others, the lane kernels, which keep a tile row in one warp's lanes;
+ *   - d_tile_index null: MRX_E_INVALID.
+ * Then it checks its own arguments, and B = 0 returns MRX_OK without launching anything. */
+
 /* The hot kernel.  For every image b writes the bool canvas [H_b, W_b, N_b]
  * (N innermost, 1 byte per element, values 0/1) at d_canvas + d_canvas_off[b]:
  * zero fill, zero-border half-pixel bilinear resize of each tile to its box,
- * >= 0.5 threshold and paste, fused so each output byte is written once.
+ * >= 0.5 threshold and paste, fused so each output byte is written once.  Inputs: a tile batch.
  *   d_canvas_off [B] int64, each a multiple of 16; slot b must hold at least
  *   round_up(H_b*W_b*N_b, 16) bytes (bytes past H_b*W_b*N_b may or may not be written).
  *   chunk_bytes: upper bound, in bytes, of the canvas tile a team of warps builds in
@@ -124,9 +140,7 @@ int mrx_unmold_prepare(const void *d_detections, int det_dtype, const void *d_mr
  *   10 rows x N instances; it is raised to the minimum that holds 16 pixels of R
  *   instances per row); multiple of 16, >= 1024; 0 = as large as fits (library default).
  *   ctas_per_sm: used by the generic kernel only (R too large for the tile buffers, or
- *   mask tiles wider than 30 columns); 0 = as many as fit.
- *   d_tile_index [B,R] int32, required: kept instance k of image b resizes
- *   d_tiles[b][d_tile_index[b][k]] (d_src_index for the layout mrx_unmold_prepare writes). */
+ *   mask tiles wider than MRX_MAX_LANE_MASK_W); 0 = as many as fit. */
 int mrx_mask_expand(const float *d_tiles, const int *d_tile_index, const int *d_boxes,
                     const int *d_counts, const int *d_geom, const long long *d_canvas_off,
                     unsigned char *d_canvas, int B, int R, int mh, int mw,
@@ -138,10 +152,10 @@ int mrx_mask_expand(const float *d_tiles, const int *d_tile_index, const int *d_
  * stores every pre-threshold sample it evaluates: d_values is float32, indexed exactly like
  * d_canvas (element d_canvas_off[b] + (y*W_b + x)*N_b + n); only elements inside box n are
  * written.  The canvas is written as usual.  Tests compare these values with the float64
- * oracle (|diff| <= 1e-6).  Shapes the team kernel does not take return MRX_E_UNSUPPORTED
- * before launching anything: mask tiles wider than 30 columns, and R whose tile row no longer
- * fits a team's buffer (on an H100, R > 213 at B = 1; the limit drops slowly for large batches,
- * whose scheduler table takes shared memory from the buffers). */
+ * oracle (|diff| <= 1e-6).  Inputs: a tile batch, as a lane kernel.  R whose tile row no longer
+ * fits a team's buffer returns MRX_E_UNSUPPORTED before launching anything (on an H100, R > 213
+ * at B = 1; the limit drops slowly for large batches, whose scheduler table takes shared memory
+ * from the buffers). */
 int mrx_mask_expand_values(const float *d_tiles, const int *d_tile_index, const int *d_boxes,
                            const int *d_counts, const int *d_geom, const long long *d_canvas_off,
                            unsigned char *d_canvas, float *d_values, int B, int R, int mh, int mw,
@@ -210,14 +224,13 @@ int mrx_pack_masks(const unsigned char *d_canvas, const long long *d_canvas_off,
                    void *stream);
 
 /* EXTENSION: the expand step with bit-packed output, without ever writing the byte canvas
- * (expand_bits.cu).  Same inputs as mrx_mask_expand (tiles, tile index, boxes, counts, geometry as
- * left by mrx_unmold_prepare); output layout exactly that of mrx_pack_masks:
+ * (expand_bits.cu).  Inputs: a tile batch, as a lane kernel (wider tiles take mrx_mask_expand +
+ * mrx_pack_masks).  Output layout exactly that of mrx_pack_masks:
  * image b at d_packed + d_packed_off[b] as uint8 [N_b, H_b, ceil(W_b/8)] (slot capacity
  * R * H_b * ceil(W_b/8)); planes n >= N_b are not written.  The samples are computed with the
  * same arithmetic as mrx_mask_expand, so  packed == np.packbits(canvas)  bit for bit.
  * d_packed may be memory of ANOTHER GPU mapped with mrx_peer_open (fused compute + gather).
- * max_w: widest W_b of the batch.  Mask tiles wider than 30 columns: MRX_E_UNSUPPORTED
- * (use mrx_mask_expand + mrx_pack_masks). */
+ * max_w: widest W_b of the batch. */
 int mrx_mask_expand_packed(const float *d_tiles, const int *d_tile_index, const int *d_boxes,
                            const int *d_counts,
                            const int *d_geom, const long long *d_packed_off,
@@ -234,7 +247,7 @@ int mrx_mask_expand_packed(const float *d_tiles, const int *d_tile_index, const 
  *                   allocates d_positions [T] and d_run_lengths [T + B*R] (uint32).
  *   mrx_rle_write:  instance i's runs are d_run_lengths[d_inst_off[i] + i ...], one more than
  *                   its value changes (d_inst_off[i+1] - d_inst_off[i] + 1); they sum to H*W.
- * Inputs as for mrx_mask_expand_packed.  Mask tiles wider than 30 columns: MRX_E_UNSUPPORTED. */
+ * Inputs: a tile batch, as a lane kernel; max_w as for mrx_mask_expand_packed. */
 int mrx_rle_count(const float *d_tiles, const int *d_tile_index, const int *d_boxes,
                   const int *d_counts, const int *d_geom, int *d_col_count,
                   long long *d_inst_off, int B, int R, int mh, int mw, int max_w, void *stream);

@@ -23,6 +23,8 @@ MRX_ST_CLASS_RANGE = 1
 MRX_ST_BOX_RANGE = 2
 MRX_GEOM_INTS = 8
 MRX_MAX_BATCH = 4096
+MRX_MAX_MASK_DIM = 64
+MRX_MAX_LANE_MASK_W = 30    # tile width of the lane kernels: mw + 2 lanes per warp
 ABI_VERSION = 8
 MRX_SCHED_WORDS = 4
 MRX_PEER_HANDLE_BYTES = 64

@@ -308,17 +308,12 @@ def unmold_detections_packed_batch(items, direct=True):
 
     direct=True: the expand kernel writes the bits itself (`mrx_mask_expand_packed`; the byte
     canvas is never materialised).  direct=False: byte canvas first, then `mrx_pack_masks`
-    (also what mask tiles wider than 30 columns take).  Both give identical bytes."""
+    (also what mask tiles wider than `MRX_MAX_LANE_MASK_W` columns take).  Both give identical
+    bytes."""
     if len(items) == 0:
         return []
     with _Staged(items, canvas=not direct) as st:
-        eng = st.eng
-        if direct and eng.mw <= 30:
-            d_packed, off = eng.enqueue_packed(st.d_det, st.d_msk)
-        else:
-            eng.plan(st.geoms, canvas=True)
-            eng.enqueue(st.d_det, st.d_msk)
-            d_packed, off = eng.pack_masks()
+        d_packed, off = st.eng.enqueue_packed(st.d_det, st.d_msk, direct=direct)
         counts, metas = st.meta()
         parts = []
         for b in range(st.n):
@@ -369,20 +364,15 @@ def unmold_detections_contours_batch(items):
     polygons `visualize.display_instances` draws for it -- a list of float64 [V, 2] (x, y) arrays
     equal to `np.fliplr(v) - 1` of `skimage.measure.find_contours(padded_mask, 0.5)` -- traced on
     the device from the packed masks; only the vertices travel to the host.  Masks with tiles up
-    to 30 columns are expanded straight into bits (`mrx_mask_expand_packed`), wider ones through
-    the byte canvas and `mrx_pack_masks`.  Returns a list of (boxes, class_ids, scores, contours)."""
+    to `MRX_MAX_LANE_MASK_W` columns are expanded straight into bits (`mrx_mask_expand_packed`),
+    wider ones through the byte canvas and `mrx_pack_masks`.  Returns a list of (boxes,
+    class_ids, scores, contours)."""
     if len(items) == 0:
         return []
     with _Staged(items, canvas=False) as st:
-        eng = st.eng
-        if eng.mw <= 30:
-            eng.enqueue_packed(st.d_det, st.d_msk)
-        else:
-            eng.plan(st.geoms, canvas=True)
-            eng.enqueue(st.d_det, st.d_msk)
-            eng.pack_masks()
+        st.eng.enqueue_packed(st.d_det, st.d_msk)
         counts, metas = st.meta()
-        contours = eng.enqueue_contours()
+        contours = st.eng.enqueue_contours()
     return [metas[b] + (contours[b],) for b in range(st.n)]
 
 

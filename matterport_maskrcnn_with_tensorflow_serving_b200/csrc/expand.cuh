@@ -127,24 +127,36 @@ __device__ __forceinline__ void retire_worker(unsigned int *words, unsigned work
 }
 #endif  // __CUDACC__
 
-struct ExpandParams {
+// The batch mrx_unmold_prepare leaves on the device, as every kernel that reads the class tiles
+// takes it (mrx.h, "Tile batch").
+struct TileBatch {
   const float *tiles;           // [B,R,mh,mw]
   const int *tile_index;        // [B,R] tile of kept instance k = tiles[b][tile_index[b][k]]
   const int4 *boxes;            // [B,R] (y1,x1,y2,x2)
   const int *counts;            // [B]
   const int *geom;              // [B,8]
+  int B, R, mh, mw;
+};
+
+// The one host check of a tile batch (unmold.cu): pointers, sizes, then the tile shape against
+// max_mw (MRX_MAX_MASK_DIM, or MRX_MAX_LANE_MASK_W for the kernels that keep a tile row in one
+// warp's lanes).  Returns MRX_OK or the error code, with mrx_last_error() naming `fn`.
+int check_tile_batch(const char *fn, const TileBatch &t, int max_mw);
+
+struct ExpandParams {
+  TileBatch t;
   const long long *canvas_off;  // [B]
   unsigned char *canvas;
   unsigned int *job_counter;    // [0] tile ticket, [1] teams / CTAs retired; zero between launches
   float *values;                // test instantiation only: pre-threshold samples, indexed like canvas
-  int B, R, mh, mw, chunk_bytes;
-  int flags;                    // development switches (MRX_EXPAND_FLAGS; -DMRX_DEV builds only)
+  int chunk_bytes;
+  int flags;                    // team kernel development switches (MRX_EXPAND_FLAGS; -DMRX_DEV only)
 };
 
 // The default kernel: teams of warps build 2-D tiles (one persistent CTA per SM).  want_buf =
 // upper bound of a team's tile buffer in bytes (0 = as large as fits).  Returns MRX_OK, an
 // error code with mrx_last_error() set, or MRX_E_UNSUPPORTED when R does not fit a buffer or
-// mw > 30 (the caller then takes the generic kernel).
+// mw > MRX_MAX_LANE_MASK_W (the caller then takes the generic kernel).
 int launch_expand_team(const ExpandParams &prm, const DevInfo &dev, int want_buf, cudaStream_t st);
 
 }  // namespace mrx

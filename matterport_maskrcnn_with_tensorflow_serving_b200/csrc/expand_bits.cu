@@ -45,15 +45,10 @@ namespace bits {
 constexpr int kGroup = 4;   // column blocks a warp walks side by side (independent chains)
 
 struct BitsParams {
-  const float *tiles;            // [B,R,mh,mw]
-  const int *tile_index;         // [B,R] (see ExpandParams)
-  const int4 *boxes;             // [B,R]
-  const int *counts;             // [B]
-  const int *geom;               // [B,8]
+  TileBatch t;
   const long long *packed_off;   // [B]
   unsigned char *packed;
   unsigned int *sched;           // [2] unit ticket, [3] warps retired (MRX_SCHED_WORDS)
-  int B, R, mh, mw;
   int ubuf;                      // bytes of one unit buffer (multiple of 16, incl. 16 B of slack)
 };
 
@@ -85,7 +80,7 @@ mask_expand_bits_kernel(const BitsParams p) {
   const int tid = threadIdx.x;
   const int lane = tid & 31;
   const int warp = tid >> 5;
-  const int mh = p.mh, mw = p.mw;
+  const int mh = p.t.mh, mw = p.t.mw;
   const int ubuf = p.ubuf;
 
   // ---- shared memory: [zero page][2 buffers per warp][unit prefix per image]
@@ -97,10 +92,10 @@ mask_expand_bits_kernel(const BitsParams p) {
   for (int i = tid; i < (ubuf >> 4); i += kWarps * 32)
     reinterpret_cast<uint4 *>(s_zero)[i] = make_uint4(0u, 0u, 0u, 0u);
   if (warp == 0) {
-    image_work_table(p.B, [=](int b) {
-      const int H = p.geom[b * MRX_GEOM_INTS + 0], W = p.geom[b * MRX_GEOM_INTS + 1];
+    image_work_table(p.t.B, [=](int b) {
+      const int H = p.t.geom[b * MRX_GEOM_INTS + 0], W = p.t.geom[b * MRX_GEOM_INTS + 1];
       const int rb = unit_rows((W + 7) >> 3, ubuf);
-      return p.counts[b] * ((H + rb - 1) / rb);
+      return p.t.counts[b] * ((H + rb - 1) / rb);
     }, s_prefix, &s_total);
   }
   fence_proxy_async_smem();   // the zero page is read by bulk copies only
@@ -130,14 +125,14 @@ mask_expand_bits_kernel(const BitsParams p) {
       while (u >= s_prefix[cur_b + 1]) ++cur_b;
       if (cur_b != cached_b) {
         cached_b = cur_b;
-        H = p.geom[cur_b * MRX_GEOM_INTS + 0];
-        W = p.geom[cur_b * MRX_GEOM_INTS + 1];
+        H = p.t.geom[cur_b * MRX_GEOM_INTS + 0];
+        W = p.t.geom[cur_b * MRX_GEOM_INTS + 1];
         WB = (W + 7) >> 3;
         rb = unit_rows(WB, ubuf);
         nbands = (H + rb - 1) / rb;
-        tiles_b = p.tiles + static_cast<size_t>(cur_b) * p.R * mh * mw;
-        boxes_b = p.boxes + static_cast<size_t>(cur_b) * p.R;
-        tidx_b = p.tile_index + static_cast<size_t>(cur_b) * p.R;
+        tiles_b = p.t.tiles + static_cast<size_t>(cur_b) * p.t.R * mh * mw;
+        boxes_b = p.t.boxes + static_cast<size_t>(cur_b) * p.t.R;
+        tidx_b = p.t.tile_index + static_cast<size_t>(cur_b) * p.t.R;
         out_b = p.packed + p.packed_off[cur_b];
       }
       const int local = u - s_prefix[cur_b];
@@ -275,14 +270,14 @@ using namespace mrx;
 template <int kWarps>
 static int launch_bits(mrx::bits::BitsParams prm, const DevInfo &dev, int max_w, cudaStream_t st) {
   using namespace mrx::bits;
-  const size_t fixed = static_cast<size_t>(prm.B + 1) * sizeof(int) + 1024;   // prefix + static + slack
+  const size_t fixed = static_cast<size_t>(prm.t.B + 1) * sizeof(int) + 1024;   // prefix + static + slack
   int ubuf = static_cast<int>((static_cast<size_t>(dev.max_smem_optin) - fixed) / (1 + 2 * kWarps)) & ~127;
   if (ubuf > 8192) ubuf = 8192;
   const int wb = (max_w + 7) >> 3;
   MRX_CHECK_SUPPORTED(wb + 16 <= ubuf, "mrx_mask_expand_packed: image %d pixels wide does not fit a "
                       "unit buffer of %d bytes", max_w, ubuf);
   prm.ubuf = ubuf;
-  const size_t smem = static_cast<size_t>(ubuf) * (1 + 2 * kWarps) + static_cast<size_t>(prm.B + 1) * sizeof(int);
+  const size_t smem = static_cast<size_t>(ubuf) * (1 + 2 * kWarps) + static_cast<size_t>(prm.t.B + 1) * sizeof(int);
   static SmemCache cache;
   if (int rc = ensure_dynamic_smem(reinterpret_cast<const void *>(mask_expand_bits_kernel<kWarps>), &cache,
                                    dev.device, static_cast<int>(smem)))
@@ -298,31 +293,15 @@ extern "C" int mrx_mask_expand_packed(const float *d_tiles, const int *d_tile_in
                                       unsigned char *d_packed, int B, int R, int mh, int mw,
                                       int max_w, unsigned int *d_sched, void *stream) {
   using namespace mrx::bits;
-  MRX_CHECK_ARG(d_tiles && d_boxes && d_counts && d_geom && d_packed_off && d_packed && d_sched,
-                "mrx_mask_expand_packed: null pointer");
-  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH && R >= 1 && max_w >= 1,
-                "mrx_mask_expand_packed: bad sizes B=%d R=%d max_w=%d", B, R, max_w);
-  MRX_CHECK_SUPPORTED(mh >= 2 && mh <= MRX_MAX_MASK_DIM && mw >= 4 && mw <= 30,
-                      "mrx_mask_expand_packed: mask tile %dx%d unsupported (2<=mh<=%d, 4<=mw<=30)",
-                      mh, mw, MRX_MAX_MASK_DIM);
-  MRX_CHECK_ARG(d_tile_index, "mrx_mask_expand_packed: null tile index");
+  const TileBatch t{d_tiles, d_tile_index, reinterpret_cast<const int4 *>(d_boxes), d_counts,
+                    d_geom, B, R, mh, mw};
+  if (int rc = check_tile_batch("mrx_mask_expand_packed", t, MRX_MAX_LANE_MASK_W)) return rc;
+  MRX_CHECK_ARG(d_packed_off && d_packed && d_sched, "mrx_mask_expand_packed: null pointer");
+  MRX_CHECK_ARG(max_w >= 1, "mrx_mask_expand_packed: bad max_w %d", max_w);
   if (B == 0) return MRX_OK;
   DevInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  BitsParams prm;
-  prm.tiles = d_tiles;
-  prm.tile_index = d_tile_index;
-  prm.boxes = reinterpret_cast<const int4 *>(d_boxes);
-  prm.counts = d_counts;
-  prm.geom = d_geom;
-  prm.packed_off = d_packed_off;
-  prm.packed = d_packed;
-  prm.sched = d_sched;
-  prm.B = B;
-  prm.R = R;
-  prm.mh = mh;
-  prm.mw = mw;
-  prm.ubuf = 0;
+  const BitsParams prm{t, d_packed_off, d_packed, d_sched, 0};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #ifdef MRX_DEV
   if (const char *e = getenv("MRX_BITS_WARPS")) {

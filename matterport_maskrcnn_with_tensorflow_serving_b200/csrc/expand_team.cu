@@ -193,7 +193,7 @@ mask_expand_team_kernel(const ExpandParams p, const int buf_bytes) {
   const int tm = warp / kTeamWarps;            // team
   const int wt = warp - tm * kTeamWarps;       // warp within the team
   const int tt = tid - tm * kTeamThreads;      // thread within the team
-  const int mh = p.mh, mw = p.mw;
+  const int mh = p.t.mh, mw = p.t.mw;
   const int rowcap = (buf_bytes / kTileRows) & ~15;
 
   // ---- carve shared memory: [team buffers][team entry lists][team job descriptors][prefix]
@@ -210,8 +210,8 @@ mask_expand_team_kernel(const ExpandParams p, const int buf_bytes) {
 
   // ---- tiles per image -> prefix sums (first warp)
   if (warp == 0) {
-    image_work_table(p.B, [=](int b) {
-      return tiles_of(p.geom[b * MRX_GEOM_INTS + 0], p.geom[b * MRX_GEOM_INTS + 1], p.counts[b], rowcap, kTileRows);
+    image_work_table(p.t.B, [=](int b) {
+      return tiles_of(p.t.geom[b * MRX_GEOM_INTS + 0], p.t.geom[b * MRX_GEOM_INTS + 1], p.t.counts[b], rowcap, kTileRows);
     }, s_prefix, &s_total);
   }
   __syncthreads();
@@ -236,9 +236,9 @@ mask_expand_team_kernel(const ExpandParams p, const int buf_bytes) {
     const int b = cur_b;
     if (b != dc.b) {   // per-image constants (divisions), kept by the decoding thread
       dc.b = b;
-      dc.H = p.geom[b * MRX_GEOM_INTS + 0];
-      dc.W = p.geom[b * MRX_GEOM_INTS + 1];
-      dc.N = p.counts[b];
+      dc.H = p.t.geom[b * MRX_GEOM_INTS + 0];
+      dc.W = p.t.geom[b * MRX_GEOM_INTS + 1];
+      dc.N = p.t.counts[b];
       int P_, pitch_;
       tile_geom(dc.W, dc.N, rowcap, P_, pitch_);
       dc.P = P_;
@@ -246,15 +246,15 @@ mask_expand_team_kernel(const ExpandParams p, const int buf_bytes) {
       dc.tx = (dc.W + P_ - 1) / P_;
       dc.canvas = p.canvas + p.canvas_off[b];
       // kept rows are in increasing order: no row was dropped iff the last one kept its index
-      dc.ident = dc.N == 0 || p.tile_index[static_cast<size_t>(b) * p.R + dc.N - 1] == dc.N - 1;
+      dc.ident = dc.N == 0 || p.t.tile_index[static_cast<size_t>(b) * p.t.R + dc.N - 1] == dc.N - 1;
     }
     const int H = dc.H, W = dc.W, N = dc.N, P = dc.P, pitch = dc.pitch, tiles_x = dc.tx;
     const int local = j - s_prefix[b];
     const int band = local / tiles_x;
     const int tx = local - band * tiles_x;
     const unsigned RW = static_cast<unsigned>(W) * N;
-    out->tiles_b = p.tiles + static_cast<size_t>(b) * p.R * mh * mw;
-    out->boxes_b = p.boxes + static_cast<size_t>(b) * p.R;
+    out->tiles_b = p.t.tiles + static_cast<size_t>(b) * p.t.R * mh * mw;
+    out->boxes_b = p.t.boxes + static_cast<size_t>(b) * p.t.R;
     out->x0 = tx * P;
     out->pw = min(P, W - tx * P);
     out->y0 = band * kTileRows;
@@ -304,7 +304,7 @@ mask_expand_team_kernel(const ExpandParams p, const int buf_bytes) {
       TEntry e;
       e.x1 = bx.y;
       e.x2 = bx.w;
-      const int tile = jb.ident ? n : __ldg(p.tile_index + (jb.boxes_b - p.boxes) + n);
+      const int tile = jb.ident ? n : __ldg(p.t.tile_index + (jb.boxes_b - p.t.boxes) + n);
       e.npk = n | (tile << 8) | (ra << 16) | (rb << 22);
       e.invD = __fdiv_rn(1.0f, static_cast<float>(2 * (bx.w - bx.y)));
       e.Dy = 2 * bh;
@@ -654,17 +654,17 @@ static int launch_team_cfg(const ExpandParams &prm, const DevInfo &dev, int want
   constexpr size_t kStatic = 256 + static_cast<size_t>(kTeams) * (kCand + 48);   // static __shared__ of the kernel
   const size_t fixed = static_cast<size_t>(kTeams) * kCand * sizeof(TEntry) +
                        static_cast<size_t>(kTeams) * 2 * sizeof(TJob) +
-                       static_cast<size_t>(prm.B + 1) * sizeof(int) + kStatic;
+                       static_cast<size_t>(prm.t.B + 1) * sizeof(int) + kStatic;
   MRX_CHECK_SUPPORTED(fixed + static_cast<size_t>(kTeams) * 2048 <= static_cast<size_t>(max_optin),
-                      "mrx_mask_expand: batch of %d images does not fit the scheduler table", prm.B);
+                      "mrx_mask_expand: batch of %d images does not fit the scheduler table", prm.t.B);
   // (the kernel's zero fill is unrolled for tile buffers of up to this size)
   constexpr int kMaxBuf = (232448 - kTeams * (kCand * static_cast<int>(sizeof(TEntry)) +
                                               2 * static_cast<int>(sizeof(TJob)))) / kTeams;
   const int avail = min(static_cast<int>((static_cast<size_t>(max_optin) - fixed) / kTeams), kMaxBuf) & ~127;
   // a tile row must hold 16 pixels of R instances (aligned shapes) / one pixel + alignment shift
-  const int need = (max(16 * prm.R, prm.R + 48) * kTileRows + 127) & ~127;
+  const int need = (max(16 * prm.t.R, prm.t.R + 48) * kTileRows + 127) & ~127;
   // (an entry packs the instance and its tile index into 8 bits each)
-  if (need > avail || prm.R > 256) return MRX_E_UNSUPPORTED;   // caller falls back to the generic kernel
+  if (need > avail || prm.t.R > 256) return MRX_E_UNSUPPORTED;   // caller falls back to the generic kernel
   int buf = avail;
   if (want_buf > 0 && want_buf < buf) buf = want_buf & ~127;
   if (buf < need) buf = need;
@@ -691,7 +691,7 @@ extern "C" int mrx_debug_team_profile(long long *host_dst, int count) {
 
 // The shipped shape: 6 teams x 5 warps, 10-row tiles (tools/kernel_sweep.py compares the others).
 int launch_expand_team(const ExpandParams &prm, const DevInfo &dev, int want_buf, cudaStream_t st) {
-  if (prm.mw > 30) return MRX_E_UNSUPPORTED;   // caller falls back to the generic kernel
+  if (prm.t.mw > MRX_MAX_LANE_MASK_W) return MRX_E_UNSUPPORTED;   // caller falls back to the generic kernel
   if (prm.values != nullptr) return launch_team_cfg<6, 5, 10, true>(prm, dev, want_buf, st);
 #ifdef MRX_DEV
   // development sweep: MRX_EXPAND_TEAMS="<teams>x<warps>x<rows>"

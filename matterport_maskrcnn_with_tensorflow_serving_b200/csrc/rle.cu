@@ -33,15 +33,11 @@ namespace rle {
 constexpr int kWalkWarps = 8;
 
 struct RleParams {
-  const float *tiles;         // [B,R,mh,mw]
-  const int *tile_index;      // [B,R]
-  const int4 *boxes;          // [B,R]
-  const int *counts;          // [B]
-  const int *geom;            // [B,8]
+  TileBatch t;
   int *col_count;             // [B,R,max_w]: transitions per column -> exclusive offsets (scan)
   long long *inst_off;        // [B*R + 1]: totals -> exclusive offsets of the instances
   unsigned int *positions;    // [total] flat positions of the transitions (write pass)
-  int B, R, mh, mw, max_w;
+  int max_w;
 };
 
 // One warp: instance k of image b, columns [32*cb, 32*cb + 32).
@@ -51,19 +47,19 @@ rle_walk_kernel(const RleParams p) {
   const int lane = threadIdx.x & 31;
   const int cb = blockIdx.x * kWalkWarps + (threadIdx.x >> 5);
   const int k = blockIdx.y, b = blockIdx.z;
-  if (k >= p.counts[b]) return;
-  const int H = p.geom[b * MRX_GEOM_INTS + 0], W = p.geom[b * MRX_GEOM_INTS + 1];
-  const int4 bx = __ldg(p.boxes + static_cast<size_t>(b) * p.R + k);   // (y1, x1, y2, x2)
+  if (k >= p.t.counts[b]) return;
+  const int H = p.t.geom[b * MRX_GEOM_INTS + 0], W = p.t.geom[b * MRX_GEOM_INTS + 1];
+  const int4 bx = __ldg(p.t.boxes + static_cast<size_t>(b) * p.t.R + k);   // (y1, x1, y2, x2)
   if (!box_in_canvas(bx, H, W) || (cb << 5) >= bx.w || (cb << 5) + 32 <= bx.y) return;
-  const int mh = p.mh, mw = p.mw;
+  const int mh = p.t.mh, mw = p.t.mw;
   const int bh = bx.z - bx.x, bw = bx.w - bx.y;
   const int D = 2 * bw, Dy = 2 * bh;
   const float invD = __fdiv_rn(1.0f, static_cast<float>(D));
   const float invDy = __fdiv_rn(1.0f, static_cast<float>(Dy));
-  const int tile = __ldg(p.tile_index + static_cast<size_t>(b) * p.R + k);
+  const int tile = __ldg(p.t.tile_index + static_cast<size_t>(b) * p.t.R + k);
   const bool lanecol = lane >= 1 && lane <= mw;      // lane l holds tile column l - 1
   const int lcol = min(max(lane - 1, 0), mw - 1);
-  const LaneRows raw{p.tiles + (static_cast<size_t>(b) * p.R + tile) * mh * mw + lcol, mh, mw, lanecol};
+  const LaneRows raw{p.t.tiles + (static_cast<size_t>(b) * p.t.R + tile) * mh * mw + lcol, mh, mw, lanecol};
   // horizontal source coordinate of column x: taps idx, idx + 1 of the zero-padded tile row
   auto hcoord = [&](int x, int &idx, float &wx) {
     const SrcPos s = src_floor(src_num(mw, x, bx.y, bw), D, invD);
@@ -84,7 +80,7 @@ rle_walk_kernel(const RleParams p) {
   const bool full = bx.x == 0 && bx.z == H;          // column seams carry the previous column's bit
   unsigned int *out = nullptr;
   if (kWrite) {
-    const size_t inst = static_cast<size_t>(b) * p.R + k;
+    const size_t inst = static_cast<size_t>(b) * p.t.R + k;
     out = p.positions + p.inst_off[inst] + (colvalid ? p.col_count[inst * p.max_w + x] : 0);
   }
   const unsigned base = static_cast<unsigned>(x) * static_cast<unsigned>(H);
@@ -145,18 +141,18 @@ rle_walk_kernel(const RleParams p) {
       ++n;
     }
   }
-  if (!kWrite && colvalid) p.col_count[(static_cast<size_t>(b) * p.R + k) * p.max_w + x] = n;
+  if (!kWrite && colvalid) p.col_count[(static_cast<size_t>(b) * p.t.R + k) * p.max_w + x] = n;
 }
 
 // One CTA per instance: exclusive scan of its box columns' transition counts (in place), total out.
 __global__ void __launch_bounds__(256)
 rle_scan_kernel(const RleParams p) {
   const int k = blockIdx.x, b = blockIdx.y;
-  const size_t inst = static_cast<size_t>(b) * p.R + k;
+  const size_t inst = static_cast<size_t>(b) * p.t.R + k;
   int x1 = 0, x2 = 0;   // no columns: not a kept instance, or its box is outside the canvas
-  if (k < p.counts[b]) {
-    const int H = p.geom[b * MRX_GEOM_INTS + 0], W = p.geom[b * MRX_GEOM_INTS + 1];
-    const int4 bx = p.boxes[inst];
+  if (k < p.t.counts[b]) {
+    const int H = p.t.geom[b * MRX_GEOM_INTS + 0], W = p.t.geom[b * MRX_GEOM_INTS + 1];
+    const int4 bx = p.t.boxes[inst];
     if (box_in_canvas(bx, H, W)) {
       x1 = bx.y;
       x2 = bx.w;
@@ -193,43 +189,17 @@ rle_counts_kernel(const unsigned int *__restrict__ positions, const long long *_
 
 using namespace mrx;
 
-static int fill_rle_params(rle::RleParams &prm, const float *d_tiles, const int *d_tile_index,
-                           const int *d_boxes, const int *d_counts, const int *d_geom,
-                           int *d_col_count, long long *d_inst_off, unsigned int *d_positions,
-                           int B, int R, int mh, int mw, int max_w) {
-  MRX_CHECK_ARG(d_tiles && d_boxes && d_counts && d_geom && d_col_count && d_inst_off,
-                "mrx_rle: null pointer");
-  MRX_CHECK_ARG(B >= 1 && B <= 65535 && R >= 1 && R <= 65535 && max_w >= 1,
-                "mrx_rle: bad sizes B=%d R=%d max_w=%d", B, R, max_w);
-  MRX_CHECK_SUPPORTED(mh >= 2 && mh <= MRX_MAX_MASK_DIM && mw >= 4 && mw <= 30,
-                      "mrx_rle: mask tile %dx%d unsupported (2<=mh<=%d, 4<=mw<=30)", mh, mw,
-                      MRX_MAX_MASK_DIM);
-  MRX_CHECK_ARG(d_tile_index, "mrx_rle: null tile index");
-  prm.tiles = d_tiles;
-  prm.tile_index = d_tile_index;
-  prm.boxes = reinterpret_cast<const int4 *>(d_boxes);
-  prm.counts = d_counts;
-  prm.geom = d_geom;
-  prm.col_count = d_col_count;
-  prm.inst_off = d_inst_off;
-  prm.positions = d_positions;
-  prm.B = B;
-  prm.R = R;
-  prm.mh = mh;
-  prm.mw = mw;
-  prm.max_w = max_w;
-  return MRX_OK;
-}
-
 extern "C" int mrx_rle_count(const float *d_tiles, const int *d_tile_index, const int *d_boxes,
                              const int *d_counts, const int *d_geom, int *d_col_count,
                              long long *d_inst_off, int B, int R, int mh, int mw, int max_w,
                              void *stream) {
+  const TileBatch t{d_tiles, d_tile_index, reinterpret_cast<const int4 *>(d_boxes), d_counts,
+                    d_geom, B, R, mh, mw};
+  if (int rc = check_tile_batch("mrx_rle_count", t, MRX_MAX_LANE_MASK_W)) return rc;
+  MRX_CHECK_ARG(d_col_count && d_inst_off && max_w >= 1,
+                "mrx_rle_count: null pointer or max_w %d < 1", max_w);
   if (B == 0) return MRX_OK;
-  rle::RleParams prm;
-  if (int rc = fill_rle_params(prm, d_tiles, d_tile_index, d_boxes, d_counts, d_geom, d_col_count,
-                               d_inst_off, nullptr, B, R, mh, mw, max_w))
-    return rc;
+  const rle::RleParams prm{t, d_col_count, d_inst_off, nullptr, max_w};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int cblocks = (max_w + 31) >> 5;
   dim3 grid((cblocks + rle::kWalkWarps - 1) / rle::kWalkWarps, R, B);
@@ -245,12 +215,13 @@ extern "C" int mrx_rle_write(const float *d_tiles, const int *d_tile_index, cons
                              long long *d_inst_off, unsigned int *d_positions,
                              unsigned int *d_run_lengths, int B, int R, int mh, int mw, int max_w,
                              void *stream) {
+  const TileBatch t{d_tiles, d_tile_index, reinterpret_cast<const int4 *>(d_boxes), d_counts,
+                    d_geom, B, R, mh, mw};
+  if (int rc = check_tile_batch("mrx_rle_write", t, MRX_MAX_LANE_MASK_W)) return rc;
+  MRX_CHECK_ARG(d_col_count && d_inst_off && d_positions && d_run_lengths && max_w >= 1,
+                "mrx_rle_write: null pointer or max_w %d < 1", max_w);
   if (B == 0) return MRX_OK;
-  MRX_CHECK_ARG(d_positions && d_run_lengths, "mrx_rle_write: null pointer");
-  rle::RleParams prm;
-  if (int rc = fill_rle_params(prm, d_tiles, d_tile_index, d_boxes, d_counts, d_geom, d_col_count,
-                               d_inst_off, d_positions, B, R, mh, mw, max_w))
-    return rc;
+  const rle::RleParams prm{t, d_col_count, d_inst_off, d_positions, max_w};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int cblocks = (max_w + 31) >> 5;
   dim3 grid((cblocks + rle::kWalkWarps - 1) / rle::kWalkWarps, R, B);

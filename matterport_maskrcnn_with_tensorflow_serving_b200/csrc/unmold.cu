@@ -14,7 +14,6 @@
 //   tiles [B,R,mh,mw] f32 (selected class only, 3136 B per instance at 28x28)
 //   canvas: image b at canvas + canvas_off[b], bytes [H_b, W_b, N_b] (N innermost)
 #include <stdlib.h>
-#include <string.h>
 
 #include "expand.cuh"
 
@@ -236,7 +235,6 @@ unmold_prepare_kernel(const TD *__restrict__ det, const TM *__restrict__ mask, i
 // Job descriptors are computed by one thread a job ahead (double-buffered in smem) so
 // the 32-bit divisions are off the critical path of the other warps.
 constexpr int kExpandThreads = 256;
-constexpr int kExpandWarps = kExpandThreads / 32;
 constexpr int kEMax = 64;  // entries per pass == pairs tested per pass
 
 struct __align__(16) Entry {
@@ -249,7 +247,6 @@ struct __align__(16) Entry {
   float wy;     // vertical weight of the lower source row
   int otop;     // float offset of the upper source row inside the staging slot, -1 = outside
   int obot;     // same for the lower source row
-  int src_off;  // float offset of the staged rows inside this image's tiles
 };
 
 struct __align__(16) JobInfo {
@@ -272,9 +269,9 @@ __device__ __forceinline__ void make_job(const ExpandParams &p, const int *s_job
   }
   while (job >= s_jobs[cur_b + 1]) ++cur_b;
   const int b = cur_b;
-  const int H = p.geom[b * MRX_GEOM_INTS + 0];
-  const int W = p.geom[b * MRX_GEOM_INTS + 1];
-  const int N = p.counts[b];
+  const int H = p.t.geom[b * MRX_GEOM_INTS + 0];
+  const int W = p.t.geom[b * MRX_GEOM_INTS + 1];
+  const int N = p.t.counts[b];
   const unsigned L = static_cast<unsigned>(H) * W * N;         // host guarantees < 2^31
   const unsigned c0 = static_cast<unsigned>(job - s_jobs[b]) * p.chunk_bytes;
   const int len = static_cast<int>(min(static_cast<unsigned>(p.chunk_bytes), L - c0));
@@ -282,8 +279,8 @@ __device__ __forceinline__ void make_job(const ExpandParams &p, const int *s_job
   const int g1 = static_cast<int>((c0 + len - 1) / N);   // last pixel touched
   const int r0 = g0 / W;
   const int r1 = g1 / W;
-  out->tiles_b = p.tiles + static_cast<size_t>(b) * p.R * p.mh * p.mw;
-  out->boxes_b = p.boxes + static_cast<size_t>(b) * p.R;
+  out->tiles_b = p.t.tiles + static_cast<size_t>(b) * p.t.R * p.t.mh * p.t.mw;
+  out->boxes_b = p.t.boxes + static_cast<size_t>(b) * p.t.R;
   out->dst = p.canvas + p.canvas_off[b] + c0;
   out->H = H;
   out->W = W;
@@ -304,7 +301,7 @@ mask_expand_kernel(const ExpandParams p) {
   const int tid = threadIdx.x;
   const int lane = tid & 31;
   const int warp = tid >> 5;
-  const int mh = p.mh, mw = p.mw;
+  const int mh = p.t.mh, mw = p.t.mw;
   const int slot_floats = 2 * mw;             // two tile rows
   const uint32_t slot_bytes = slot_floats * 4;
 
@@ -321,9 +318,9 @@ mask_expand_kernel(const ExpandParams p) {
 
   // ---- job table: jobs_b = ceil(H*W*N_b / chunk); exclusive prefix in s_jobs
   if (warp == 0) {
-    image_work_table(p.B, [=](int b) {
-      const long long bytes = static_cast<long long>(p.geom[b * MRX_GEOM_INTS + 0]) *
-                              p.geom[b * MRX_GEOM_INTS + 1] * p.counts[b];
+    image_work_table(p.t.B, [=](int b) {
+      const long long bytes = static_cast<long long>(p.t.geom[b * MRX_GEOM_INTS + 0]) *
+                              p.t.geom[b * MRX_GEOM_INTS + 1] * p.t.counts[b];
       return static_cast<int>((bytes + p.chunk_bytes - 1) / p.chunk_bytes);
     }, s_jobs, &s_total);
   }
@@ -380,7 +377,7 @@ mask_expand_kernel(const ExpandParams p) {
           n = pr - dr * J.N;
           const int row = J.r0 + dr;
           const int4 bx = __ldg(J.boxes_b + n);   // (y1, x1, y2, x2)
-          tile = __ldg(p.tile_index + (J.boxes_b - p.boxes) + n);
+          tile = __ldg(p.t.tile_index + (J.boxes_b - p.t.boxes) + n);
           const int xlo = max(0, J.g0 - row * J.W);
           const int xhi = min(J.W, J.g1 + 1 - row * J.W);
           const int xa = max(xlo, bx.y);
@@ -402,7 +399,6 @@ mask_expand_kernel(const ExpandParams p) {
             e.wy = src_weight(sy.rem, invDy);
             e.otop = (sy.i < 0) ? -1 : (sy.i - jc) * mw;
             e.obot = (sy.i + 1 > mh - 1) ? -1 : (sy.i + 1 - jc) * mw;
-            e.src_off = (tile * mh + jc) * mw;
           }
         }
         const unsigned bal = __ballot_sync(0xffffffffu, valid);
@@ -413,9 +409,8 @@ mask_expand_kernel(const ExpandParams p) {
           const int slot = base + __popc(bal & ((1u << lane) - 1u));
           s_entry[slot] = e;
           // ---- 2a. stage tile rows jc, jc+1
-          if (!(p.flags & 1))
-            bulk_g2s(s_stage + slot * slot_floats,
-                     J.tiles_b + (static_cast<size_t>(tile) * mh + jc) * mw, slot_bytes, &s_bar);
+          bulk_g2s(s_stage + slot * slot_floats,
+                   J.tiles_b + (static_cast<size_t>(tile) * mh + jc) * mw, slot_bytes, &s_bar);
         }
       }
       if (tid == 0) s_next = 0;
@@ -423,7 +418,7 @@ mask_expand_kernel(const ExpandParams p) {
       const int E = s_count[pass_parity];
       if (tid == 0) {
         s_count[pass_parity ^ 1] = 0;
-        if (E > 0 && !(p.flags & 1)) mbar_arrive_expect_tx(&s_bar, E * slot_bytes);
+        if (E > 0) mbar_arrive_expect_tx(&s_bar, E * slot_bytes);
         if (p0 == 0) {
           // describe the next job while the tile rows are in flight
           make_job(p, s_jobs, total_jobs, next_job, cur_b, &s_job[(k + 1) & 1]);
@@ -433,17 +428,8 @@ mask_expand_kernel(const ExpandParams p) {
       pass_parity ^= 1;
       if (E == 0) continue;
       wrote = true;
-      if (!(p.flags & 1)) {
-        mbar_wait(&s_bar, bar_parity);
-        bar_parity ^= 1;
-      } else {
-        for (int ei = warp; ei < E; ei += kExpandWarps) {
-          const int so = s_entry[ei].src_off;
-          for (int i = lane; i < slot_floats; i += 32)
-            s_stage[ei * slot_floats + i] = __ldg(J.tiles_b + so + i);
-        }
-        __syncthreads();
-      }
+      mbar_wait(&s_bar, bar_parity);
+      bar_parity ^= 1;
 
       // ---- 3. warps grab entries and walk their x-spans
       while (true) {
@@ -481,16 +467,9 @@ mask_expand_kernel(const ExpandParams p) {
     // ---- 4. hand the chunk to the TMA
     fence_proxy_async_smem();
     __syncthreads();   // (S3)
-    if (!(p.flags & 2)) {
-      if (tid == 0) {
-        bulk_s2g(J.dst, s_out, static_cast<uint32_t>(J.len16));
-        bulk_commit();
-      }
-    } else {
-      const uint4 *s4 = reinterpret_cast<const uint4 *>(s_out);
-      uint4 *d4 = reinterpret_cast<uint4 *>(J.dst);
-      const int n16 = J.len16 >> 4;
-      for (int i = tid; i < n16; i += kExpandThreads) __stcs(d4 + i, s4[i]);
+    if (tid == 0) {
+      bulk_s2g(J.dst, s_out, static_cast<uint32_t>(J.len16));
+      bulk_commit();
     }
     if (wrote) clean = 0;
   }
@@ -507,11 +486,16 @@ mask_expand_kernel(const ExpandParams p) {
 // =====================================================================================
 using namespace mrx;
 
-static int check_mask_dims(int mh, int mw) {
-  MRX_CHECK_SUPPORTED(mh >= 2 && mh <= MRX_MAX_MASK_DIM && mw >= 4 && mw <= MRX_MAX_MASK_DIM &&
-                          (mw % 4) == 0,
-                      "mask tile %dx%d unsupported (need 2<=mh<=%d, 4<=mw<=%d, mw%%4==0)", mh,
-                      mw, MRX_MAX_MASK_DIM, MRX_MAX_MASK_DIM);
+int mrx::check_tile_batch(const char *fn, const TileBatch &t, int max_mw) {
+  MRX_CHECK_ARG(t.tiles && t.boxes && t.counts && t.geom, "%s: null pointer", fn);
+  MRX_CHECK_ARG(t.B >= 0 && t.B <= MRX_MAX_BATCH && t.R >= 1 && t.R <= 65534,
+                "%s: bad sizes B=%d R=%d (need 0<=B<=%d, 1<=R<=65534)", fn, t.B, t.R, MRX_MAX_BATCH);
+  MRX_CHECK_SUPPORTED(t.mh >= 2 && t.mh <= MRX_MAX_MASK_DIM && t.mw >= 4 && t.mw <= max_mw &&
+                          (t.mw % 4) == 0,
+                      "%s: mask tile %dx%d unsupported (need 2<=mh<=%d, 4<=mw<=%d, mw%%4==0)", fn,
+                      t.mh, t.mw, MRX_MAX_MASK_DIM, max_mw);
+  // (after the shape checks: a shape no kernel takes is reported as such)
+  MRX_CHECK_ARG(t.tile_index, "%s: null tile index", fn);
   return MRX_OK;
 }
 
@@ -546,66 +530,36 @@ extern "C" int mrx_unmold_prepare(const void *d_detections, int det_dtype, const
   return MRX_OK;
 }
 
-static int mask_expand_impl(const float *d_tiles, const int *d_tile_index, const int *d_boxes,
-                            const int *d_counts, const int *d_geom, const long long *d_canvas_off,
-                            unsigned char *d_canvas, float *d_values, int B, int R, int mh, int mw,
-                            int chunk_bytes, int ctas_per_sm, unsigned int *d_sched,
-                            void *stream) {
-  MRX_CHECK_ARG(d_tiles && d_boxes && d_counts && d_geom && d_canvas_off &&
-                    d_canvas && d_sched,
-                "mrx_mask_expand: null pointer");
-  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH && R >= 1, "mrx_mask_expand: bad sizes B=%d R=%d",
-                B, R);
-  if (int rc = check_mask_dims(mh, mw)) return rc;
-  // (after the shape checks: a shape no kernel takes is reported as such)
-  MRX_CHECK_ARG(d_tile_index, "mrx_mask_expand: null tile index");
+// mrx_mask_expand and mrx_mask_expand_values, after check_tile_batch
+static int mask_expand_impl(const TileBatch &t, const long long *d_canvas_off,
+                            unsigned char *d_canvas, float *d_values, int chunk_bytes,
+                            int ctas_per_sm, unsigned int *d_sched, void *stream) {
+  MRX_CHECK_ARG(d_canvas_off && d_canvas && d_sched, "mrx_mask_expand: null pointer");
   const int want_buf = chunk_bytes;   // team kernel: upper bound of a team's tile buffer, 0 = auto
   if (chunk_bytes == 0) chunk_bytes = 25600;
   MRX_CHECK_ARG(chunk_bytes >= 1024 && (chunk_bytes % 16) == 0,
                 "mrx_mask_expand: chunk_bytes %d must be a multiple of 16, >= 1024", chunk_bytes);
-  if (B == 0) return MRX_OK;
+  if (t.B == 0) return MRX_OK;
 
   DevInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
 
-  ExpandParams prm;
-  prm.tiles = d_tiles;
-  prm.tile_index = d_tile_index;
-  prm.boxes = reinterpret_cast<const int4 *>(d_boxes);
-  prm.counts = d_counts;
-  prm.geom = d_geom;
-  prm.canvas_off = d_canvas_off;
-  prm.canvas = d_canvas;
-  prm.job_counter = d_sched;
-  prm.values = d_values;
-  prm.B = B;
-  prm.R = R;
-  prm.mh = mh;
-  prm.mw = mw;
-  prm.chunk_bytes = chunk_bytes;
-  prm.flags = 0;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // the team kernel keeps a tile row in one warp's registers (mw + 2 <= 32 lanes); wider tiles
-  // and R too large for its tile buffers take the generic kernel
-  bool generic = mw > 30;
+  ExpandParams prm{t, d_canvas_off, d_canvas, d_sched, d_values, chunk_bytes, 0};
 #ifdef MRX_DEV
-  {
-    const char *f = getenv("MRX_EXPAND_FLAGS");
-    prm.flags = f ? atoi(f) : 0;
-    const char *impl = getenv("MRX_EXPAND_IMPL");
-    if (impl != nullptr && strcmp(impl, "generic") == 0) generic = true;
-  }
+  if (const char *f = getenv("MRX_EXPAND_FLAGS")) prm.flags = atoi(f);
 #endif
-  if (!generic) {
-    const int rc = launch_expand_team(prm, dev, want_buf, st);
-    if (rc != MRX_E_UNSUPPORTED) return rc;
-  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  // the team kernel refuses tiles wider than MRX_MAX_LANE_MASK_W and R too large for its tile
+  // buffers: those take the generic kernel
+  const int rc = launch_expand_team(prm, dev, want_buf, st);
+  if (rc != MRX_E_UNSUPPORTED) return rc;
   MRX_CHECK_SUPPORTED(d_values == nullptr,
-                      "mrx_mask_expand_values: shape outside the team kernel (R=%d, mw=%d)", R, mw);
+                      "mrx_mask_expand_values: shape outside the team kernel (R=%d, mw=%d)", t.R,
+                      t.mw);
   const size_t smem = static_cast<size_t>(chunk_bytes) +
-                      static_cast<size_t>(kEMax) * 2 * mw * sizeof(float) +
+                      static_cast<size_t>(kEMax) * 2 * t.mw * sizeof(float) +
                       static_cast<size_t>(kEMax) * sizeof(Entry) +
-                      static_cast<size_t>(B + 1) * sizeof(int);
+                      static_cast<size_t>(t.B + 1) * sizeof(int);
   MRX_CHECK_SUPPORTED(smem <= static_cast<size_t>(dev.max_smem_optin),
                       "mrx_mask_expand: %zu B shared memory > device limit %d (chunk_bytes too "
                       "large)",
@@ -629,8 +583,11 @@ extern "C" int mrx_mask_expand(const float *d_tiles, const int *d_tile_index, co
                                const long long *d_canvas_off, unsigned char *d_canvas, int B,
                                int R, int mh, int mw, int chunk_bytes, int ctas_per_sm,
                                unsigned int *d_sched, void *stream) {
-  return mask_expand_impl(d_tiles, d_tile_index, d_boxes, d_counts, d_geom, d_canvas_off,
-                          d_canvas, nullptr, B, R, mh, mw, chunk_bytes, ctas_per_sm, d_sched, stream);
+  const TileBatch t{d_tiles, d_tile_index, reinterpret_cast<const int4 *>(d_boxes), d_counts,
+                    d_geom, B, R, mh, mw};
+  if (int rc = check_tile_batch("mrx_mask_expand", t, MRX_MAX_MASK_DIM)) return rc;
+  return mask_expand_impl(t, d_canvas_off, d_canvas, nullptr, chunk_bytes, ctas_per_sm, d_sched,
+                          stream);
 }
 
 extern "C" int mrx_mask_expand_values(const float *d_tiles, const int *d_tile_index,
@@ -638,7 +595,9 @@ extern "C" int mrx_mask_expand_values(const float *d_tiles, const int *d_tile_in
                                       const int *d_geom, const long long *d_canvas_off,
                                       unsigned char *d_canvas, float *d_values, int B, int R,
                                       int mh, int mw, unsigned int *d_sched, void *stream) {
+  const TileBatch t{d_tiles, d_tile_index, reinterpret_cast<const int4 *>(d_boxes), d_counts,
+                    d_geom, B, R, mh, mw};
+  if (int rc = check_tile_batch("mrx_mask_expand_values", t, MRX_MAX_LANE_MASK_W)) return rc;
   MRX_CHECK_ARG(d_values != nullptr, "mrx_mask_expand_values: null pointer");
-  return mask_expand_impl(d_tiles, d_tile_index, d_boxes, d_counts, d_geom, d_canvas_off,
-                          d_canvas, d_values, B, R, mh, mw, 0, 0, d_sched, stream);
+  return mask_expand_impl(t, d_canvas_off, d_canvas, d_values, 0, 0, d_sched, stream);
 }

@@ -269,10 +269,19 @@ class UnmoldEngine:
                 "mrx_mask_expand_packed")
         return self.d_packed, off
 
-    def enqueue_packed(self, d_detections, d_mrcnn_mask, stream=None):
-        """prologue -> class-tile gather -> packed expand (no byte canvas is written)."""
-        self.enqueue(d_detections, d_mrcnn_mask, stream, expand=False)
-        return self.enqueue_expand_packed(stream)
+    def enqueue_packed(self, d_detections, d_mrcnn_mask, stream=None, direct=True):
+        """prologue -> class-tile gather -> packed masks.  Returns (d_packed, offsets).
+        direct=True: the expand kernel writes the bits itself (mrx_mask_expand_packed, no byte
+        canvas is written) when the tiles are at most MRX_MAX_LANE_MASK_W columns wide.
+        Otherwise, and for direct=False: byte canvas, then mrx_pack_masks.  Both give identical
+        bytes."""
+        if direct and self.mw <= N.MRX_MAX_LANE_MASK_W:
+            self.enqueue(d_detections, d_mrcnn_mask, stream, expand=False)
+            return self.enqueue_expand_packed(stream)
+        if self._n_images:      # (a plan made with canvas=False has no canvas)
+            self.plan(self._geom_host, canvas=True)
+        self.enqueue(d_detections, d_mrcnn_mask, stream)
+        return self.pack_masks(stream)
 
     # ------------------------------------------------------------------ results
     def canvas_bytes(self, counts):

@@ -1,7 +1,7 @@
 """The expand kernels over the mask-tile shapes the C ABI accepts (2 <= mh <= 64, 4 <= mw <= 64,
 mw % 4 == 0; square or not), not only the 28x28 tiles of the model.
 
-Tiles up to 30 columns wide take the team kernel, whose fast and general paths, six-row queue and
+Tiles up to MRX_MAX_LANE_MASK_W (30) columns wide take the team kernel, whose fast and general paths, six-row queue and
 lane-column clamps all depend on mh and mw; the bit-packed and RLE kernels compute the same
 sample.  Wider tiles take the generic kernel, which stages two tile rows per canvas row.  Every
 shape runs boxes of every size relative to the tile: 1 px, smaller than the tile (downscale),
@@ -119,9 +119,13 @@ def test_generic_kernel_tile_shape(cuda_device, mask_hw):
 
 @pytest.mark.parametrize("mask_hw", [(1, 28), (28, 6)], ids=["mh1", "mw6"])
 def test_tile_shape_no_kernel_takes_raises(cuda_device, mask_hw):
-    """mrx_unmold_prepare gathers tiles of any shape, but no expand kernel takes these: the call
-    must fail rather than return masks."""
+    """mrx_unmold_prepare gathers tiles of any shape, but no expand kernel takes these: every
+    call must fail rather than return masks."""
     rng = np.random.default_rng(7)
     im = synth.make_image(rng, (64, 80), 5, num_classes=CLASSES, max_instances=8, mask_hw=mask_hw)
     with pytest.raises(N.MrxError, match=r"mrx_mask_expand failed \(status -2\)"):
         api_utils.unmold_detections(*item_of(im))
+    with pytest.raises(N.MrxError, match=r"mrx_mask_expand_packed failed \(status -2\)"):
+        api_utils.unmold_detections_packed_batch([item_of(im)])
+    with pytest.raises(N.MrxError, match=r"mrx_rle_count failed \(status -2\)"):
+        api_utils.unmold_detections_rle_batch([item_of(im)])

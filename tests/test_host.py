@@ -45,14 +45,58 @@ def test_host_side_argument_validation():
     assert lib.mrx_mask_expand_values(None, None, None, None, None, None, None, None, 1, 100,
                                       28, 28, None, None) == -1
     p16 = C.c_void_p(16)
-    assert lib.mrx_mask_expand_packed(p16, None, p16, p16, p16, p16, p16, 1, 100, 28, 32, 1024,
-                                      p16, None) == -2      # mask tiles wider than 30 columns
-    assert b"30" in lib.mrx_last_error()
-    assert lib.mrx_mask_expand_packed(p16, None, p16, p16, p16, p16, p16, 1, 100, 28, 28, 1024,
-                                      p16, None) == -1      # the tile index is required
     assert lib.mrx_unmold_prepare(p16, 0, p16, 3, 1, 100, 28, 28, 81, p16, p16, p16, p16, p16,
                                   p16, p16, p16, p16, None) == -1      # bad mask dtype
     assert lib.mrx_peer_export(None, None) == -1 and lib.mrx_peer_wait(None, 1, 1, None) == -1
+
+
+# The entry points that read a tile batch, as (tile_index, B, R, mh, mw) -> status; every other
+# argument is a non-null placeholder.  The lane kernels keep a tile row in one warp's lanes.
+def _tile_batch_entry_points(lib):
+    p = C.c_void_p(16)
+    return {
+        "mrx_mask_expand": lambda ti, B, R, mh, mw: lib.mrx_mask_expand(
+            p, ti, p, p, p, p, p, B, R, mh, mw, 0, 0, p, None),
+        "mrx_mask_expand_values": lambda ti, B, R, mh, mw: lib.mrx_mask_expand_values(
+            p, ti, p, p, p, p, p, p, B, R, mh, mw, p, None),
+        "mrx_mask_expand_packed": lambda ti, B, R, mh, mw: lib.mrx_mask_expand_packed(
+            p, ti, p, p, p, p, p, B, R, mh, mw, 1024, p, None),
+        "mrx_rle_count": lambda ti, B, R, mh, mw: lib.mrx_rle_count(
+            p, ti, p, p, p, p, p, B, R, mh, mw, 1024, None),
+        "mrx_rle_write": lambda ti, B, R, mh, mw: lib.mrx_rle_write(
+            p, ti, p, p, p, p, p, p, p, B, R, mh, mw, 1024, None),
+    }
+
+
+# (what is wrong, null tile index, B, R, mh, mw, status, lane kernels only)
+BAD_TILE_BATCHES = [
+    ("B > MRX_MAX_BATCH", False, N.MRX_MAX_BATCH + 1, 100, 28, 28, -1, False),
+    ("R = 0", False, 1, 0, 28, 28, -1, False),
+    ("R = 65535", False, 1, 65535, 28, 28, -1, False),
+    ("mh = 1", False, 1, 100, 1, 28, -2, False),
+    ("mw % 4 != 0", False, 1, 100, 28, 6, -2, False),
+    ("mw > MRX_MAX_LANE_MASK_W", False, 1, 100, 28, 32, -2, True),
+    ("null tile index", True, 1, 100, 28, 28, -1, False),
+]
+
+
+@pytest.mark.parametrize("fn", ["mrx_mask_expand", "mrx_mask_expand_values",
+                                "mrx_mask_expand_packed", "mrx_rle_count", "mrx_rle_write"])
+def test_tile_batch_checks_agree(fn):
+    """Every entry point that reads the tile batch refuses the same bad inputs with the same
+    status, names itself in the message, and returns before touching the device."""
+    lib = N.load()
+    call = _tile_batch_entry_points(lib)[fn]
+    lane = fn != "mrx_mask_expand"
+    for what, null_index, B, R, mh, mw, status, lane_only in BAD_TILE_BATCHES:
+        if lane_only and not lane:
+            continue
+        assert call(None if null_index else C.c_void_p(16), B, R, mh, mw) == status, what
+        msg = lib.mrx_last_error().decode()
+        assert msg.startswith(fn + ":"), (what, msg)
+        if status == -2:
+            limit = N.MRX_MAX_LANE_MASK_W if lane else N.MRX_MAX_MASK_DIM
+            assert f"mw<={limit}" in msg, (what, msg)
 
 
 def test_product_path_has_no_cpu_fallback():
