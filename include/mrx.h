@@ -16,6 +16,7 @@
  *   mrx_pack_masks         (extension: bit-packed transport of the masks of serve.py:147)
  *   mrx_mask_expand_packed (extension: the expand step writing that packed layout directly)
  *   mrx_rle_count / _write (extension: the same masks as COCO run-length encodings)
+ *   mrx_rle_strings        (extension: those encodings as COCO compressed RLE strings)
  *   mrx_contours_count / _write <- visualize.display_instances (contour polygons) serve.py:160-169
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
  *   mrx_device_alloc/_free (the canvas allocation: compressible device memory where offered)
@@ -39,7 +40,7 @@
 extern "C" {
 #endif
 
-#define MRX_ABI_VERSION 8
+#define MRX_ABI_VERSION 9
 
 #define MRX_OK              0
 #define MRX_E_INVALID      -1   /* bad argument (null pointer, size out of range) */
@@ -255,6 +256,21 @@ int mrx_rle_write(const float *d_tiles, const int *d_tile_index, const int *d_bo
                   const int *d_counts, const int *d_geom, int *d_col_count,
                   long long *d_inst_off, unsigned int *d_positions, unsigned int *d_run_lengths,
                   int B, int R, int mh, int mw, int max_w, void *stream);
+
+/* EXTENSION: pycocotools' compressed RLE ("counts" string of mask.encode) of every kept instance,
+ * from the output of mrx_rle_write (d_run_lengths, d_inst_off as written there; d_counts and R as
+ * given there).  d_str_off [B*R+1] int64: exclusive byte offsets of the instances' strings, total
+ * at [B*R] (instances k >= counts[b] get empty strings).  d_str: at least
+ * MRX_RLE_STRING_BOUND(T, B*R) bytes, T = d_inst_off[B*R] (every count takes at most 7
+ * characters).  Strings are not NUL-terminated.  Run j of an instance is written as
+ * x = cnts[j] - cnts[j-2] (cnts[j] for j <= 2) in little-endian 5-bit groups, character
+ * '0' + group, 0x20 added to every group but the last, whose bit 0x10 is the sign.  Checks: null
+ * pointers, B outside [0, MRX_MAX_BATCH] or R outside [1, 65534]: MRX_E_INVALID; B = 0 returns
+ * MRX_OK without launching anything. */
+#define MRX_RLE_STRING_BOUND(T, n) (7LL * ((T) + (n)))
+int mrx_rle_strings(const unsigned int *d_run_lengths, const long long *d_inst_off,
+                    const int *d_counts, int B, int R, long long *d_str_off,
+                    unsigned char *d_str, void *stream);
 
 /* EXTENSION: mask outlines as polygons, the contour loop of visualize.display_instances
  * (serve.py:160-169): for each instance, skimage.measure.find_contours(padded, 0.5) of the mask

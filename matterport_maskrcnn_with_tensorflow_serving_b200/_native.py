@@ -25,7 +25,7 @@ MRX_GEOM_INTS = 8
 MRX_MAX_BATCH = 4096
 MRX_MAX_MASK_DIM = 64
 MRX_MAX_LANE_MASK_W = 30    # tile width of the lane kernels: mw + 2 lanes per warp
-ABI_VERSION = 8
+ABI_VERSION = 9
 MRX_SCHED_WORDS = 4
 MRX_PEER_HANDLE_BYTES = 64
 MRX_MAX_CONTOUR_SEGMENTS = 1 << 30
@@ -34,6 +34,12 @@ MRX_MAX_CONTOUR_SEGMENTS = 1 << 30
 def contour_scratch_bytes(total_segments):
     """MRX_CONTOUR_SCRATCH_BYTES(S): device scratch of mrx_contours_write for S segments."""
     return 48 * int(total_segments) + 256
+
+
+def rle_string_bound(total_changes, n_instances):
+    """MRX_RLE_STRING_BOUND(T, n): bytes of mrx_rle_strings' output for T value changes (runs
+    T + n) over n instances; every count takes at most 7 characters."""
+    return 7 * (int(total_changes) + int(n_instances))
 
 
 class MrxError(RuntimeError):
@@ -60,6 +66,7 @@ SIGNATURES = {
                                     _vp]),
     "mrx_rle_count": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
     "mrx_rle_write": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
+    "mrx_rle_strings": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
     "mrx_contours_count": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "mrx_contours_write": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_longlong, C.c_longlong,
                                 _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),

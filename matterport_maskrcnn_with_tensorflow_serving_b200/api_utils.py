@@ -9,7 +9,8 @@ NumPy value semantics, computed by the sm_90a kernels in libmrx.so.
 
 Plus batched entry points the reference lacks (it is hard-wired to one image per call,
 serve.py:48): `unmold_detections_batch`, `unmold_detections_packed_batch`,
-`unmold_detections_rle_batch`, `unmold_detections_contours_batch`, `unmold_overlay_batch`.
+`unmold_detections_rle_batch`, `unmold_detections_contours_batch`, `unmold_overlay_batch`,
+and `unmold_coco_results_batch` (upstream's `build_coco_results` of the unmolded detections).
 
 Numerical contract (checked by tests/ against the float64 oracle): N, boxes, class ids and
 scores are bit-exact.  The mask resize runs in float32 on exact integer source coordinates;
@@ -332,15 +333,22 @@ def unmold_detections_packed_batch(items, direct=True):
     return out
 
 
-def unmold_detections_rle_batch(items):
+def unmold_detections_rle_batch(items, compressed=False):
     """EXTENSION (not the reference layout): like `unmold_detections_batch` but every mask comes
     back as a COCO run-length encoding -- pycocotools' "uncompressed RLE" dict
     {'size': [H, W], 'counts': uint32 array} (column-major runs starting with zeros) -- computed
     on the device straight from the 28x28 tiles; the [H,W,N] masks are never materialised and
     only the run lengths (a few KB per mask) travel to the host.  Decoding a result gives exactly
-    the mask `unmold_detections` returns.  Returns a list of (boxes, class_ids, scores, rles)."""
+    the mask `unmold_detections` returns.  Returns a list of (boxes, class_ids, scores, rles).
+
+    compressed=True: every dict is {'size': [H, W], 'counts': bytes}, pycocotools' compressed RLE,
+    byte for byte what `pycocotools.mask.encode(np.asfortranarray(mask))` returns for that mask.
+    The strings are made on the device (`mrx_rle_strings`); only they and their offsets travel to
+    the host.  `counts.decode("ascii")` makes a dict JSON can hold."""
     if len(items) == 0:
         return []
+    if compressed:
+        return _rle_strings_batch(items)
     with _Staged(items, canvas=False) as st:
         eng = st.eng
         eng.enqueue(st.d_det, st.d_msk, expand=False)
@@ -356,6 +364,56 @@ def unmold_detections_rle_batch(items):
             rles.append({"size": [H, W],
                          "counts": runs[int(off[i]) + i:int(off[i + 1]) + i + 1].copy()})
         out.append(metas[b] + (rles,))
+    return out
+
+
+def _rle_strings_batch(items):
+    with _Staged(items, canvas=False) as st:
+        eng = st.eng
+        eng.enqueue(st.d_det, st.d_msk, expand=False)
+        d_str, d_str_off = eng.enqueue_rle_strings()
+        counts, metas = st.meta()
+        soff = d_str_off.cpu().numpy()
+        blob = d_str[:int(soff[-1])].cpu().numpy().tobytes()
+    out = []
+    for b in range(st.n):
+        H, W = int(st.geoms[b][0]), int(st.geoms[b][1])
+        rles = []
+        for k in range(int(counts[b])):
+            i = b * eng.R + k
+            rles.append({"size": [H, W], "counts": blob[int(soff[i]):int(soff[i + 1])]})
+        out.append(metas[b] + (rles,))
+    return out
+
+
+def unmold_coco_results_batch(items, image_ids, category_ids=None):
+    """`unmold_detections` followed by upstream's `build_coco_results` (Matterport
+    samples/coco/coco.py) in one device pass: a flat list with one dict per kept instance, images
+    in order,
+
+        {"image_id": image_ids[b], "category_id": int(category_ids[class_id]),
+         "bbox": [x1, y1, x2 - x1, y2 - y1], "score": float(score),
+         "segmentation": {"size": [H, W], "counts": bytes}}
+
+    the values upstream builds: `bbox` from the kept boxes as Python ints, `segmentation` the
+    compressed RLE of `unmold_detections_rle_batch(items, compressed=True)`.  `category_ids` maps
+    class ids to dataset category ids, as upstream's `dataset.get_source_class_id` does; None keeps
+    the class id.  items as for `unmold_detections_batch`, one image id per item.  (Upstream takes
+    one image's detections and repeats them for every id in its `image_ids`; here each item has its
+    own id.)"""
+    if len(image_ids) != len(items):
+        raise ValueError(f"{len(items)} items but {len(image_ids)} image ids")
+    out = []
+    for image_id, (rois, class_ids, scores, rles) in zip(
+            image_ids, unmold_detections_rle_batch(items, compressed=True)):
+        for i in range(rois.shape[0]):
+            y1, x1, y2, x2 = (int(v) for v in rois[i])
+            cid = int(class_ids[i])
+            out.append({"image_id": image_id,
+                        "category_id": cid if category_ids is None else int(category_ids[cid]),
+                        "bbox": [x1, y1, x2 - x1, y2 - y1],
+                        "score": float(scores[i]),
+                        "segmentation": rles[i]})
     return out
 
 

@@ -17,6 +17,12 @@
 //                            x*H + y at (instance base + column offset + running index)
 //   rle_counts_kernel        positions -> run lengths (differences, closing run to H*W)
 //
+// mrx_rle_strings turns those run lengths into pycocotools' compressed RLE ("counts" string of
+// mask.encode, its rleToString) on the device:
+//   rle_string_count_kernel  per instance: characters of its string
+//   offsets_scan_kernel      exclusive scan of the instance lengths (capi.cu, one CTA)
+//   rle_string_write_kernel  per instance: the characters, a CTA-wide scan per chunk of runs
+//
 // Column seams: column x continues at (x+1, 0) after (x, H-1).  Outside its box an instance is
 // zero, so a column starts after a zero unless the box spans the full height (then it starts
 // after the previous column's last pixel), and a run still open at the last box row is closed
@@ -183,6 +189,88 @@ rle_counts_kernel(const unsigned int *__restrict__ positions, const long long *_
   }
 }
 
+// ---- compressed strings.  Run j of an instance is stored as the signed delta
+// x = cnts[j] - cnts[j-2] (cnts[j] itself for j <= 2) in little-endian 5-bit groups, each written
+// as the character '0' + group, with 0x20 added to every group but the last; the last group's bit
+// 0x10 is the sign.  x needs bits(x ^ (x >> 63)) + 1 bits in two's complement, so
+// (bits + 5) / 5 characters: 1 to 7 for run lengths below 2^32.
+constexpr int kStrThreads = 256;
+
+__device__ __forceinline__ long long run_delta(const unsigned int *cnts, long long j) {
+  long long x = cnts[j];
+  if (j > 2) x -= cnts[j - 2];
+  return x;
+}
+
+__device__ __forceinline__ int delta_chars(long long x) {
+  return (64 - __clzll(x ^ (x >> 63)) + 5) / 5;
+}
+
+// kept instance k of image b: its runs (cnts, m of them), as rle_counts_kernel wrote them
+struct InstRuns {
+  const unsigned int *cnts;
+  long long m;
+};
+
+__device__ __forceinline__ InstRuns inst_runs(const unsigned int *runs, const long long *inst_off,
+                                              size_t inst) {
+  const long long lo = inst_off[inst];
+  return {runs + lo + inst, inst_off[inst + 1] - lo + 1};
+}
+
+// One CTA per instance: length of its string (0 for k >= counts[b]).
+__global__ void __launch_bounds__(kStrThreads)
+rle_string_count_kernel(const unsigned int *__restrict__ runs,
+                        const long long *__restrict__ inst_off,
+                        const int *__restrict__ counts_per_image, int R,
+                        long long *__restrict__ str_len) {
+  __shared__ long long s_warp[kStrThreads / 32];
+  const int k = blockIdx.x, b = blockIdx.y;
+  const size_t inst = static_cast<size_t>(b) * R + k;
+  if (k >= counts_per_image[b]) {
+    if (threadIdx.x == 0) str_len[inst] = 0;
+    return;
+  }
+  const InstRuns r = inst_runs(runs, inst_off, inst);
+  long long n = 0;
+  for (long long j = threadIdx.x; j < r.m; j += kStrThreads) n += delta_chars(run_delta(r.cnts, j));
+  long long total;
+  block_exclusive_scan<long long, kStrThreads>(n, s_warp, total);
+  if (threadIdx.x == 0) str_len[inst] = total;
+}
+
+// One CTA per instance, kStrThreads runs per pass: a scan of the pass's character counts places
+// every run's characters after those of the runs before it.
+__global__ void __launch_bounds__(kStrThreads)
+rle_string_write_kernel(const unsigned int *__restrict__ runs,
+                        const long long *__restrict__ inst_off,
+                        const int *__restrict__ counts_per_image, int R,
+                        const long long *__restrict__ str_off, unsigned char *__restrict__ str) {
+  __shared__ int s_warp[kStrThreads / 32];
+  const int k = blockIdx.x, b = blockIdx.y;
+  if (k >= counts_per_image[b]) return;
+  const size_t inst = static_cast<size_t>(b) * R + k;
+  const InstRuns r = inst_runs(runs, inst_off, inst);
+  unsigned char *o = str + str_off[inst];
+  for (long long base = 0; base < r.m; base += kStrThreads) {
+    const long long j = base + threadIdx.x;
+    long long x = 0;
+    int n = 0;
+    if (j < r.m) {
+      x = run_delta(r.cnts, j);
+      n = delta_chars(x);
+    }
+    int pass;
+    const int at = block_exclusive_scan<int, kStrThreads>(n, s_warp, pass);
+    for (int c = 0; c < n; ++c) {
+      const int g = static_cast<int>(x & 0x1f);
+      x >>= 5;
+      o[at + c] = static_cast<unsigned char>('0' + (c + 1 < n ? g | 0x20 : g));
+    }
+    o += pass;
+  }
+}
+
 }  // namespace rle
 
 }  // namespace mrx
@@ -230,5 +318,25 @@ extern "C" int mrx_rle_write(const float *d_tiles, const int *d_tile_index, cons
   rle::rle_counts_kernel<<<dim3(R, B), 256, 0, st>>>(d_positions, d_inst_off, d_counts, d_geom, R,
                                                      d_run_lengths);
   MRX_LAUNCH_CHECK("rle_counts_kernel");
+  return MRX_OK;
+}
+
+extern "C" int mrx_rle_strings(const unsigned int *d_run_lengths, const long long *d_inst_off,
+                               const int *d_counts, int B, int R, long long *d_str_off,
+                               unsigned char *d_str, void *stream) {
+  MRX_CHECK_ARG(d_run_lengths && d_inst_off && d_counts && d_str_off && d_str,
+                "mrx_rle_strings: null pointer");
+  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH && R >= 1 && R <= 65534,
+                "mrx_rle_strings: bad sizes B=%d R=%d (need 0<=B<=%d, 1<=R<=65534)", B, R,
+                MRX_MAX_BATCH);
+  if (B == 0) return MRX_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  rle::rle_string_count_kernel<<<dim3(R, B), rle::kStrThreads, 0, st>>>(
+      d_run_lengths, d_inst_off, d_counts, R, d_str_off);
+  MRX_LAUNCH_CHECK("rle_string_count_kernel");
+  if (int rc = launch_offsets_scan(d_str_off, B * R, st)) return rc;
+  rle::rle_string_write_kernel<<<dim3(R, B), rle::kStrThreads, 0, st>>>(
+      d_run_lengths, d_inst_off, d_counts, R, d_str_off, d_str);
+  MRX_LAUNCH_CHECK("rle_string_write_kernel");
   return MRX_OK;
 }

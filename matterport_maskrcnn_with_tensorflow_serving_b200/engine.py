@@ -301,6 +301,13 @@ class UnmoldEngine:
         (after `enqueue(..., expand=False)`; no mask is materialised).  Synchronises once to
         size the output.  Returns (d_run_lengths uint32 tensor, inst_off int64 ndarray [n*R+1]):
         instance i = b*R + k owns d_run_lengths[inst_off[i] + i : inst_off[i+1] + i + 1]."""
+        with _stream_ctx(stream):
+            d_runs, _, off = self._enqueue_rle()
+        return d_runs, off
+
+    def _enqueue_rle(self):
+        """`enqueue_rle` on the current stream, also returning the device copy of inst_off:
+        (d_runs, d_off, off)."""
         torch = _torch()
         n = self._n_images
         g = self._geom_host
@@ -308,7 +315,7 @@ class UnmoldEngine:
         dev = self.device
         d_col = torch.empty((n * self.R * max_w,), dtype=torch.int32, device=dev)
         d_off = torch.empty((n * self.R + 1,), dtype=torch.int64, device=dev)
-        st = N.stream_ptr(stream)
+        st = N.stream_ptr(None)
         args = (_ptr(self.d_tiles), _ptr(self.d_src_index), _ptr(self.d_boxes), _ptr(self.d_counts),
                 _ptr(self.d_geom), _ptr(d_col), _ptr(d_off))
         N.check(self.lib.mrx_rle_count(*args, n, self.R, self.mh, self.mw, max_w, st),
@@ -319,7 +326,25 @@ class UnmoldEngine:
         d_runs = torch.empty((total + n * self.R,), dtype=torch.int32, device=dev)
         N.check(self.lib.mrx_rle_write(*args, _ptr(d_pos), _ptr(d_runs), n, self.R, self.mh,
                                        self.mw, max_w, st), "mrx_rle_write")
-        return d_runs, off
+        return d_runs, d_off, off
+
+    def enqueue_rle_strings(self, stream=None):
+        """EXTENSION: pycocotools' compressed RLE (the "counts" string of `mask.encode`) of every
+        mask of the planned batch: `enqueue_rle` (and its one synchronisation), then
+        mrx_rle_strings, on `stream`.  Returns (d_str uint8, d_str_off int64 [n*R+1]) device
+        tensors: instance i = b*R + k's string is d_str[d_str_off[i]:d_str_off[i+1]] (empty for
+        k >= N_b), d_str_off[n*R] the total."""
+        torch = _torch()
+        ni = self._n_images * self.R
+        with _stream_ctx(stream):
+            d_runs, d_off, off = self._enqueue_rle()
+            d_str = torch.empty((max(N.rle_string_bound(off[-1], ni), 1),), dtype=torch.uint8,
+                                device=self.device)
+            d_str_off = torch.empty((ni + 1,), dtype=torch.int64, device=self.device)
+            N.check(self.lib.mrx_rle_strings(_ptr(d_runs), _ptr(d_off), _ptr(self.d_counts),
+                                             self._n_images, self.R, _ptr(d_str_off), _ptr(d_str),
+                                             N.stream_ptr(None)), "mrx_rle_strings")
+        return d_str, d_str_off
 
     def trace_contours(self, stream=None):
         """EXTENSION: the contour polygons of `visualize.display_instances` for every kept

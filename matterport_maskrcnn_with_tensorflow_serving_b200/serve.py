@@ -6,8 +6,9 @@
 
 plus the batched surface the reference lacks (it is hard-wired to one image per request,
 serve.py:48,53,63,74): `preprocess_input_batch`, `grpc_inference_batch`, `do_inference_batch`,
-and `do_inference_unmolded` for callers that want the (rois, class_ids, scores, masks) tuple
-of serve.py:147 instead of the picture.
+`do_inference_unmolded` for callers that want the (rois, class_ids, scores, masks) tuple
+of serve.py:147 instead of the picture, and `do_inference_coco_batch` for callers that want COCO
+result dicts (compressed RLE masks) to answer with JSON.
 
 The TensorFlow-Serving RPC itself (serve.py:26-80) is out of scope and is injected:
 `set_predict_fn(fn)` installs `fn(molded_image_f32, image_meta_f32, anchors_f32) ->
@@ -212,3 +213,20 @@ def do_inference_batch(imgs, colors=None, media_dir=None):
         print(">>> Save image: {}".format(paths[-1]))
     print(">>> Complete!")
     return paths
+
+
+def do_inference_coco_batch(imgs, image_ids, category_ids=None):
+    """The answer of a JSON endpoint instead of a PNG: batched pre-processing, one RPC per image
+    (`grpc_inference_batch`), then `api_utils.unmold_coco_results_batch` -- one COCO result dict
+    per detected instance, its mask as a compressed RLE made on the device.  image_ids: one per
+    image; category_ids: class id -> dataset category id (None: the class id itself).  Decode each
+    `segmentation["counts"]` with `.decode("ascii")` before `json.dumps`."""
+    imgs = [_check_image(im) for im in imgs]
+    if len(image_ids) != len(imgs):
+        raise ValueError(f"{len(imgs)} images but {len(image_ids)} image ids")
+    if len(imgs) == 0:
+        return []
+    res = grpc_inference_batch(imgs)
+    items = [(det, msk, img.shape, mshape, window)
+             for (det, msk, mshape, window), img in zip(res, imgs)]
+    return api_utils.unmold_coco_results_batch(items, image_ids, category_ids)

@@ -1,12 +1,15 @@
 """Secondary workloads of BASELINE.json (configs[2], [3] per-GPU shard, [4]) and the mold step,
 device-timed with CUDA events.  Not the contract bench (bench.py measures configs[1]); the
-numbers go into README.md.  One JSON line per workload on stdout.
+numbers go into README.md.  One JSON line per workload on stdout; the COCO compressed-RLE line of
+each unmold workload also names the GPU and its power limit.
 
   python tools/bench_secondary.py [--iters 20] [--cpu]     (--cpu also times the oracle)
 """
 import argparse
+import ctypes as C
 import json
 import os
+import subprocess
 import sys
 import time
 
@@ -14,7 +17,7 @@ import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from matterport_maskrcnn_with_tensorflow_serving_b200 import synth  # noqa: E402
+from matterport_maskrcnn_with_tensorflow_serving_b200 import _native as N, synth  # noqa: E402
 from matterport_maskrcnn_with_tensorflow_serving_b200.engine import (  # noqa: E402
     AnchorGenerator, Molder, UnmoldEngine, make_geom)
 from matterport_maskrcnn_with_tensorflow_serving_b200.model_configs import MaskRCNNServingConfig  # noqa: E402
@@ -60,6 +63,7 @@ def unmold_case(name, batch, hw, n, classes, R, iters, base_images=4, seed=7, co
     rle_ms, _ = time_ms(lambda: eng.enqueue_rle(), max(3, iters // 4))
     d_runs, off = eng.enqueue_rle()
     rle_bytes = int(d_runs.numel()) * 4
+    strings = rle_strings_record(eng, d_runs, off, masks, iters)
     # contour polygons from the packed planes (count pass, one host read of the segment counts,
     # write pass, and the read of the contour counts): on planes already written, and with the
     # packed expand before it
@@ -98,8 +102,51 @@ def unmold_case(name, batch, hw, n, classes, R, iters, base_images=4, seed=7, co
                       "contour_vertices": n_vert, "contour_output_MB": round(contour_bytes / 1e6, 2),
                       "pack_kernel_ms": round(pack_ms, 4),
                       "pack_kernel_canvas_read_GBps": round(out_bytes / pack_ms / 1e6, 1)}), flush=True)
+    print(json.dumps({"workload": name + " -> COCO compressed RLE strings", **strings, **card()}),
+          flush=True)
     del eng, d_det, d_msk
     torch.cuda.empty_cache()
+
+
+def card():
+    """Name and power limit of the GPU the numbers come from (read-only nvidia-smi query)."""
+    idx = (os.environ.get("CUDA_VISIBLE_DEVICES") or "0").split(",")[0]
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits",
+                              "-i", idx], capture_output=True, text=True, timeout=60).stdout
+        limit = float(out.strip())
+    except (OSError, ValueError, subprocess.SubprocessError):
+        limit = None
+    return {"gpu": torch.cuda.get_device_name(0), "power_limit_W": limit}
+
+
+def rle_strings_record(eng, d_runs, off, masks, iters):
+    """mrx_rle_strings alone on the runs of the planned batch, and enqueue_rle_strings with the
+    download of the strings; string bytes against the bytes of the kept instances' uint32 runs."""
+    ni = eng._n_images * eng.R
+    d_inst_off = torch.from_numpy(off).to(eng.device)
+    d_str = torch.empty((N.rle_string_bound(off[-1], ni),), dtype=torch.uint8, device=eng.device)
+    d_str_off = torch.empty((ni + 1,), dtype=torch.int64, device=eng.device)
+    args = [C.c_void_p(t.data_ptr()) for t in (d_runs, d_inst_off, eng.d_counts)]
+
+    def strings():
+        N.check(eng.lib.mrx_rle_strings(*args, eng._n_images, eng.R, C.c_void_p(d_str_off.data_ptr()),
+                                        C.c_void_p(d_str.data_ptr()), N.stream_ptr(None)),
+                "mrx_rle_strings")
+
+    def strings_downloaded():
+        s, s_off = eng.enqueue_rle_strings()
+        h_off = s_off.cpu().numpy()
+        return s[:int(h_off[-1])].cpu().numpy()
+
+    k_ms, _ = time_ms(strings, iters)
+    e2e_ms, _ = time_ms(strings_downloaded, max(3, iters // 4))
+    str_bytes = int(strings_downloaded().size)
+    run_bytes = 4 * (int(off[-1]) + masks)      # T value changes -> T + masks runs
+    return {"rle_strings_kernel_ms": round(k_ms, 4),
+            "enqueue_rle_strings_ms_incl_download": round(e2e_ms, 4),
+            "string_MB": round(str_bytes / 1e6, 3), "uncompressed_runs_MB": round(run_bytes / 1e6, 3),
+            "string_over_runs": round(str_bytes / run_bytes, 4)}
 
 
 def anchors_sweep(iters, cpu):
