@@ -1,8 +1,9 @@
-"""Repeat-launch stress of the warp-specialised expand kernel: its producers, consumers and
-store warps synchronise only through mbarriers and ticket counters, so a protocol bug shows up
-as a rare hang or as a byte that differs between launches.  Runs a few hundred launches over
-mixed shapes and checks every result against the first one (the output is a pure function of
-the inputs: consumers only ever store 1s into zeroed chunks)."""
+"""Repeat-launch stress of the team expand kernel: its teams of warps synchronise through named
+barriers, hand out tiles from a global ticket counter and drain each tile buffer with bulk copies
+before re-zeroing it, so a protocol bug shows up as a rare hang or as a byte that differs between
+launches.  Runs a few hundred launches over mixed shapes and checks every result against the
+first one (the output is a pure function of the inputs: a team only ever stores 1s into a tile
+buffer it has zeroed)."""
 import numpy as np
 import pytest
 
