@@ -198,7 +198,6 @@ class _Staged:
                     m.dtype != m0.dtype:
                 raise ValueError("all images of a batch must share shapes and dtypes")
         self.n = n = len(items)
-        self.geoms = geoms
         R, (mh, mw, Cc) = d0.shape[0], m0.shape[1:]
         self.eng = eng = _engine_for(n, R, mh, mw, Cc, d0.dtype, m0.dtype)
         eng.lock.acquire()
@@ -246,21 +245,23 @@ def _as_tensor(arr):
         return torch.from_numpy(arr)
 
 
-def _download(parts):
-    """parts: list of (device uint8 tensor 1-D, nbytes).  One pinned buffer per part from the
-    pool, async copies, one synchronisation; returns uint8 ndarrays."""
+def _download(views):
+    """views: contiguous device uint8 tensors.  One pinned buffer per view from the pool, async
+    copies, one synchronisation; returns uint8 ndarrays of the views' shapes."""
     import torch
 
     taken = []
-    for d_t, nbytes in parts:
+    for v in views:
+        nbytes = v.numel()
         if nbytes == 0:
             taken.append(None)
             continue
         t, size = _pool.take(nbytes)
-        t[:nbytes].copy_(d_t[:nbytes], non_blocking=True)
+        t[:nbytes].copy_(v.view(-1), non_blocking=True)
         taken.append((t, size, nbytes))
     torch.cuda.current_stream().synchronize()
-    return [None if x is None else _pool.as_array(*x) for x in taken]
+    return [np.empty(tuple(v.shape), np.uint8) if x is None else
+            _pool.as_array(*x).reshape(tuple(v.shape)) for v, x in zip(views, taken)]
 
 
 # ----------------------------------------------------------------------------- entry points
@@ -275,23 +276,10 @@ def unmold_detections_batch(items):
         eng = st.eng
         eng.enqueue(st.d_det, st.d_msk)
         counts, metas = st.meta()
-        parts = []
-        for b in range(st.n):
-            k = int(counts[b])
-            H, W = st.geoms[b][0], st.geoms[b][1]
-            o = int(eng._offsets[b])
-            parts.append((eng.d_canvas[o:o + H * W * k], H * W * k))
-        arrays = _download(parts)
-    out = []
-    for b in range(st.n):
-        k = int(counts[b])
-        H, W = st.geoms[b][0], st.geoms[b][1]
-        if k == 0:
-            full = np.empty((H, W, 0))            # upstream: np.empty(shape[:2] + (0,))
-        else:
-            full = arrays[b].reshape(H, W, k).view(np.bool_)
-        out.append(metas[b] + (full,))
-    return out
+        arrays = _download([eng.canvas_view(b, counts[b]) for b in range(st.n)])
+    # upstream returns np.empty(shape[:2] + (0,)) for no instances
+    return [metas[b] + (a.view(np.bool_) if a.shape[2] else np.empty(a.shape),)
+            for b, a in enumerate(arrays)]
 
 
 def unpack_masks(packed, width):
@@ -314,23 +302,10 @@ def unmold_detections_packed_batch(items, direct=True):
     if len(items) == 0:
         return []
     with _Staged(items, canvas=not direct) as st:
-        d_packed, off = st.eng.enqueue_packed(st.d_det, st.d_msk, direct=direct)
+        st.eng.enqueue_packed(st.d_det, st.d_msk, direct=direct)
         counts, metas = st.meta()
-        parts = []
-        for b in range(st.n):
-            k = int(counts[b])
-            H, W = int(st.geoms[b][0]), int(st.geoms[b][1])
-            wb = (W + 7) // 8
-            parts.append((d_packed[int(off[b]):int(off[b]) + k * H * wb], k * H * wb))
-        arrays = _download(parts)
-    out = []
-    for b in range(st.n):
-        k = int(counts[b])
-        H, W = int(st.geoms[b][0]), int(st.geoms[b][1])
-        wb = (W + 7) // 8
-        pk = np.empty((0, H, wb), np.uint8) if k == 0 else arrays[b].reshape(k, H, wb)
-        out.append(metas[b] + (pk,))
-    return out
+        arrays = _download([st.eng.packed_view(b, counts[b]) for b in range(st.n)])
+    return [metas[b] + (a,) for b, a in enumerate(arrays)]
 
 
 def unmold_detections_rle_batch(items, compressed=False):
@@ -347,43 +322,25 @@ def unmold_detections_rle_batch(items, compressed=False):
     the host.  `counts.decode("ascii")` makes a dict JSON can hold."""
     if len(items) == 0:
         return []
-    if compressed:
-        return _rle_strings_batch(items)
     with _Staged(items, canvas=False) as st:
         eng = st.eng
+        layout = eng.layout
         eng.enqueue(st.d_det, st.d_msk, expand=False)
-        d_runs, off = eng.enqueue_rle()
-        counts, metas = st.meta()
-        runs = d_runs.cpu().numpy().view(np.uint32)
-    out = []
-    for b in range(st.n):
-        H, W = int(st.geoms[b][0]), int(st.geoms[b][1])
-        rles = []
-        for k in range(int(counts[b])):
-            i = b * eng.R + k
-            rles.append({"size": [H, W],
-                         "counts": runs[int(off[i]) + i:int(off[i + 1]) + i + 1].copy()})
-        out.append(metas[b] + (rles,))
-    return out
-
-
-def _rle_strings_batch(items):
-    with _Staged(items, canvas=False) as st:
-        eng = st.eng
-        eng.enqueue(st.d_det, st.d_msk, expand=False)
-        d_str, d_str_off = eng.enqueue_rle_strings()
-        counts, metas = st.meta()
-        soff = d_str_off.cpu().numpy()
-        blob = d_str[:int(soff[-1])].cpu().numpy().tobytes()
-    out = []
-    for b in range(st.n):
-        H, W = int(st.geoms[b][0]), int(st.geoms[b][1])
-        rles = []
-        for k in range(int(counts[b])):
-            i = b * eng.R + k
-            rles.append({"size": [H, W], "counts": blob[int(soff[i]):int(soff[i + 1])]})
-        out.append(metas[b] + (rles,))
-    return out
+        if compressed:
+            d_str, d_str_off = eng.enqueue_rle_strings()
+            counts, metas = st.meta()
+            soff = d_str_off.cpu().numpy()
+            blob = d_str[:int(soff[-1])].cpu().numpy().tobytes()
+            encoding = lambda i: blob[int(soff[i]):int(soff[i + 1])]  # noqa: E731
+        else:
+            d_runs, off = eng.enqueue_rle()
+            counts, metas = st.meta()
+            runs = d_runs.cpu().numpy().view(np.uint32)
+            encoding = lambda i: runs[int(off[i]) + i:int(off[i + 1]) + i + 1].copy()  # noqa: E731
+    rles = [[] for _ in range(st.n)]
+    for b, _, i in layout.kept_instances(counts):
+        rles[b].append({"size": list(layout.hw(b)), "counts": encoding(i)})
+    return [metas[b] + (rles[b],) for b in range(st.n)]
 
 
 def unmold_coco_results_batch(items, image_ids, category_ids=None):

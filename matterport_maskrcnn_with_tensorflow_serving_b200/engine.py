@@ -52,15 +52,75 @@ def make_geom(original_image_shape, image_shape, window):
     return [oh, ow, ih, iw, wy1, wx1, wy2, wx2]
 
 
+def _slot_offsets(sizes, align):
+    """int64 [n+1]: where each slot of `sizes` bytes rounded up to `align` starts; [n] the total."""
+    off = np.zeros(len(sizes) + 1, dtype=np.int64)
+    np.cumsum((sizes + align - 1) // align * align, out=off[1:])
+    return off
+
+
+class BatchLayout:
+    """Where the outputs of n images ([n, 8] geometry, see make_geom) with R detection rows each
+    live; host only.  Byte canvas: image b owns H*W*R bytes rounded up to 256 from canvas_off[b],
+    its k kept masks bool [H, W, k] first.  Packed planes: R*H*ceil(W/8) bytes rounded up to 16
+    from packed_off[b], its k planes uint8 [k, H, ceil(W/8)] first.  Instance i = b*R + k indexes
+    the per-instance outputs (RLE runs and strings, contours).  limits=True refuses (ValueError)
+    what the expand kernels do not take: a refused batch never becomes a layout."""
+
+    def __init__(self, geoms, R, limits=True):
+        g = np.ascontiguousarray(np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS))
+        self._pixels = hw = g[:, 0].astype(np.int64) * g[:, 1]
+        if limits:
+            if (g[:, :4] < 2).any():
+                raise ValueError("image sides must be >= 2")
+            if (hw > (1 << 30)).any():
+                raise ValueError("canvas larger than 2^30 pixels is not supported")
+            if (hw * R >= (1 << 31) - (1 << 20)).any():
+                raise ValueError("a canvas of H*W*R >= 2^31 bytes is not supported "
+                                 "(32-bit chunk math)")
+        self.geom, self.R, self.n = g, int(R), g.shape[0]
+        self.canvas_off = _slot_offsets(hw * R, 256)
+        self.packed_off = _slot_offsets(g[:, 0].astype(np.int64) * ((g[:, 1] + 7) // 8) * R, 16)
+        self.max_h, self.max_w = int(g[:, 0].max(initial=0)), int(g[:, 1].max(initial=0))
+
+    def hw(self, b):
+        return int(self.geom[b, 0]), int(self.geom[b, 1])
+
+    def canvas_span(self, b, k):
+        """[start, end) of image b's [H, W, k] masks in the byte canvas."""
+        H, W = self.hw(b)
+        o = int(self.canvas_off[b])
+        return o, o + H * W * int(k)
+
+    def packed_shape(self, b, k):
+        H, W = self.hw(b)
+        return int(k), H, (W + 7) // 8
+
+    def packed_span(self, b, k):
+        """[start, end) of image b's [k, H, ceil(W/8)] planes in the packed output."""
+        k, H, wb = self.packed_shape(b, k)
+        o = int(self.packed_off[b])
+        return o, o + k * H * wb
+
+    def canvas_bytes(self, counts):
+        """Algorithmic canvas bytes for kept counts (sum H*W*N)."""
+        return int((self._pixels * np.asarray(counts, np.int64)).sum())
+
+    def kept_instances(self, counts):
+        """(b, k, i = b*R + k) of every kept instance k < counts[b], in image order."""
+        for b, n_kept in enumerate(counts):
+            for k in range(int(n_kept)):
+                yield b, k, b * self.R + k
+
+
 class UnmoldEngine:
     """Batched, device-resident `unmold_detections`.
 
     Work buffers for up to `max_batch` images of up to `max_instances` detection rows are
-    allocated once; the canvas (bool [H,W,N] per image, N innermost) lives in one device
-    buffer with a fixed-capacity slot per image (capacity H*W*R rounded up to 256 B) so
-    that nothing on the path depends on a host read of the kept counts.  The canvas comes from
-    mrx_device_alloc: compressible memory where the GPU grants it (`canvas_compressed`), so its
-    mostly-zero lines cost fewer DRAM bytes than they hold.
+    allocated once; the canvas lives in one device buffer with a fixed-capacity slot per image
+    (`layout`, a BatchLayout) so that nothing on the path depends on a host read of the kept
+    counts.  It comes from mrx_device_alloc: compressible memory where the GPU grants it
+    (`canvas_compressed`), so its mostly-zero lines cost fewer DRAM bytes than they hold.
 
     Thread safety: an engine is a set of device buffers plus the plan of the last batch; a
     plan -> enqueue -> fetch sequence must not interleave with another thread's.  Callers
@@ -104,10 +164,8 @@ class UnmoldEngine:
         self.canvas_compressed = False
         self.d_packed = None
         self.d_packed_off = None
-        self._packed_off_host = None
-        self._geom_host = None
-        self._offsets = None
-        self._n_images = 0
+        self._packed_off_layout = None  # the layout whose packed offsets d_packed_off holds
+        self.layout = None              # BatchLayout of the planned batch
         self._contour_bufs = {}     # work and output buffers of trace_contours, grown as needed
         self.lock = threading.RLock()
         # pinned staging for fetch_meta (one D2H batch + one synchronisation per call)
@@ -119,44 +177,35 @@ class UnmoldEngine:
             self.d_canvas = None
             self.d_packed = None
             self._contour_bufs = {}
-            self._geom_host = None
-            self._offsets = None
-            self._packed_off_host = None
-            self._n_images = 0
+            self.layout = None
+
+    # read-only views of the planned layout (the benchmark, tools and tests read them)
+    _geom_host = property(lambda self: None if self.layout is None else self.layout.geom)
+    _offsets = property(lambda self: None if self.layout is None else self.layout.canvas_off)
+    _n_images = property(lambda self: 0 if self.layout is None else self.layout.n)
 
     # ------------------------------------------------------------------ planning
     def plan(self, geoms, canvas=True):
         """Set the per-image geometry ([n,8] ints, see make_geom) and size the canvas
         (canvas=False: geometry only, for callers that want the packed output alone)."""
         torch = _torch()
-        g = np.ascontiguousarray(np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS))
+        g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
         n = g.shape[0]
         if n < 1 or n > self.B:
             raise ValueError(f"batch of {n} images does not fit max_batch={self.B}")
-        if self._geom_host is not None and self._geom_host.shape == g.shape and \
-                np.array_equal(self._geom_host, g) and \
-                (not canvas or (self.d_canvas is not None and
-                                self.d_canvas.numel() >= int(self._offsets[-1]))):
+        layout = self.layout
+        if layout is None or not np.array_equal(layout.geom, g):
+            layout = BatchLayout(g, self.R)     # (raises before anything here changes)
+        elif not canvas or (self.d_canvas is not None and
+                            self.d_canvas.numel() >= int(layout.canvas_off[-1])):
             return      # (a plan made with canvas=False may have left a smaller canvas behind)
-        if (g[:, :4] < 2).any():
-            raise ValueError("image sides must be >= 2")
-        if (g[:, 0].astype(np.int64) * g[:, 1] > (1 << 30)).any():
-            raise ValueError("canvas larger than 2^30 pixels is not supported")
-        if (g[:, 0].astype(np.int64) * g[:, 1] * self.R >= (1 << 31) - (1 << 20)).any():
-            raise ValueError("a canvas of H*W*R >= 2^31 bytes is not supported (32-bit chunk math)")
-        cap = (g[:, 0].astype(np.int64) * g[:, 1].astype(np.int64) * self.R + 255) // 256 * 256
-        off = np.zeros(n + 1, dtype=np.int64)
-        np.cumsum(cap, out=off[1:])
-        total = int(off[-1])
+        total = int(layout.canvas_off[-1])
         if canvas and (self.d_canvas is None or self.d_canvas.numel() < total):
             self.d_canvas = None
             self.d_canvas, self.canvas_compressed = _device_bytes(self.lib, total, self.device)
-        self.d_geom[:n].copy_(torch.from_numpy(g))
-        self.d_canvas_off[:n].copy_(torch.from_numpy(off[:n].copy()))
-        self._geom_host = g
-        self._offsets = off
-        self._n_images = n
-        self._packed_off_host = None
+        self.d_geom[:n].copy_(torch.from_numpy(layout.geom))
+        self.d_canvas_off[:n].copy_(torch.from_numpy(layout.canvas_off[:n].copy()))
+        self.layout = layout
 
     # ------------------------------------------------------------------ launch
     def enqueue(self, d_detections, d_mrcnn_mask, stream=None, expand=True):
@@ -214,7 +263,7 @@ class UnmoldEngine:
         """Parity instrumentation: the same kernel (second instantiation of its template) also
         stores every pre-threshold sample into d_values (float32, indexed like the canvas)."""
         n = self._n_images
-        if d_values.dtype != _torch().float32 or d_values.numel() < int(self._offsets[n]):
+        if d_values.dtype != _torch().float32 or d_values.numel() < int(self.layout.canvas_off[n]):
             raise ValueError("d_values must be float32 with one element per canvas byte")
         N.check(self.lib.mrx_mask_expand_values(
             _ptr(self.d_tiles), _ptr(self.d_src_index), _ptr(self.d_boxes), _ptr(self.d_counts),
@@ -224,20 +273,15 @@ class UnmoldEngine:
 
     # ------------------------------------------------------------------ packed output
     def packed_layout(self):
-        """(offsets int64 [n+1], total bytes) of the packed output of the planned batch: image b
-        occupies [off[b], off[b+1]) as uint8 [R, H_b, ceil(W_b/8)] (first N_b planes valid)."""
-        n = self._n_images
-        if n == 0:
+        """(layout.packed_off, total bytes) of the planned batch's packed output; d_packed_off is
+        uploaded once per plan, when a packed output is first wanted (not on every plan)."""
+        layout = self.layout
+        if layout is None:
             raise RuntimeError("plan() first")
-        if self._packed_off_host is None:
-            g = self._geom_host
-            wb = (g[:, 1].astype(np.int64) + 7) // 8
-            sizes = (g[:, 0].astype(np.int64) * wb * self.R + 15) // 16 * 16
-            off = np.zeros(n + 1, dtype=np.int64)
-            np.cumsum(sizes, out=off[1:])
-            self._packed_off_host = off
-            self.d_packed_off = _torch().from_numpy(off[:n].copy()).to(self.device)
-        return self._packed_off_host, int(self._packed_off_host[-1])
+        if self._packed_off_layout is not layout:
+            self.d_packed_off = _torch().from_numpy(layout.packed_off[:-1].copy()).to(self.device)
+            self._packed_off_layout = layout
+        return layout.packed_off, int(layout.packed_off[-1])
 
     def _packed_buffer(self):
         torch = _torch()
@@ -259,13 +303,12 @@ class UnmoldEngine:
         else:
             off, _ = self.packed_layout()
             base = C.c_void_p(int(packed_ptr))
-        g = self._geom_host
         if b1 > b0:
             N.check(self.lib.mrx_mask_expand_packed(
                 _ptr(self.d_tiles[b0:]), _ptr(self.d_src_index[b0:]), _ptr(self.d_boxes[b0:]),
                 _ptr(self.d_counts[b0:]),
                 _ptr(self.d_geom[b0:]), _ptr(self.d_packed_off[b0:]), base, b1 - b0, self.R,
-                self.mh, self.mw, int(g[:, 1].max()), _ptr(self.d_sched), N.stream_ptr(stream)),
+                self.mh, self.mw, self.layout.max_w, _ptr(self.d_sched), N.stream_ptr(stream)),
                 "mrx_mask_expand_packed")
         return self.d_packed, off
 
@@ -278,23 +321,24 @@ class UnmoldEngine:
         if direct and self.mw <= N.MRX_MAX_LANE_MASK_W:
             self.enqueue(d_detections, d_mrcnn_mask, stream, expand=False)
             return self.enqueue_expand_packed(stream)
-        if self._n_images:      # (a plan made with canvas=False has no canvas)
-            self.plan(self._geom_host, canvas=True)
+        if self.layout is not None:     # (a plan made with canvas=False has no canvas)
+            self.plan(self.layout.geom, canvas=True)
         self.enqueue(d_detections, d_mrcnn_mask, stream)
         return self.pack_masks(stream)
 
     # ------------------------------------------------------------------ results
     def canvas_bytes(self, counts):
-        """Algorithmic canvas bytes for kept counts (sum H*W*N)."""
-        g = self._geom_host
-        return int((g[:, 0].astype(np.int64) * g[:, 1] * np.asarray(counts, np.int64)).sum())
+        return self.layout.canvas_bytes(counts)
 
     def canvas_view(self, b, n_kept):
         """uint8 device view [H, W, n_kept] of image b's slot (values 0/1)."""
-        g = self._geom_host[b]
-        H, W = int(g[0]), int(g[1])
-        o = int(self._offsets[b])
-        return self.d_canvas[o:o + H * W * n_kept].view(H, W, n_kept)
+        lo, hi = self.layout.canvas_span(b, n_kept)
+        return self.d_canvas[lo:hi].view(*self.layout.hw(b), n_kept)
+
+    def packed_view(self, b, n_kept):
+        """uint8 device view [n_kept, H, ceil(W/8)] of image b's packed planes."""
+        lo, hi = self.layout.packed_span(b, n_kept)
+        return self.d_packed[lo:hi].view(self.layout.packed_shape(b, n_kept))
 
     def enqueue_rle(self, stream=None):
         """EXTENSION: COCO run-length encodings of the planned batch's masks, from the tiles
@@ -310,8 +354,7 @@ class UnmoldEngine:
         (d_runs, d_off, off)."""
         torch = _torch()
         n = self._n_images
-        g = self._geom_host
-        max_w = int(g[:, 1].max())
+        max_w = self.layout.max_w
         dev = self.device
         d_col = torch.empty((n * self.R * max_w,), dtype=torch.int32, device=dev)
         d_off = torch.empty((n * self.R + 1,), dtype=torch.int64, device=dev)
@@ -352,13 +395,12 @@ class UnmoldEngine:
         `enqueue_expand_packed` or `pack_masks`) inside each instance's box.  Synchronises to size
         the output.  Returns (d_vertices float32 [V, 2] device tensor, d_contour_off int64 device
         tensor [C + 1], inst_contour_off int64 ndarray [n*R + 1]); see `contours_to_lists`."""
-        n = self._n_images
-        if n == 0 or self.d_packed is None:
+        if self.layout is None or self.d_packed is None:
             raise RuntimeError("trace_contours needs the packed planes: call enqueue_expand_packed "
                                "or pack_masks first")
         return trace_packed_contours(self.lib, self.device, self.d_packed, self.d_packed_off,
-                                     self.d_counts, self.d_geom, self.d_boxes, n, self.R,
-                                     int(self._geom_host[:, 0].max()), stream, self._contour_bufs)
+                                     self.d_counts, self.d_geom, self.d_boxes, self.layout,
+                                     stream, self._contour_bufs)
 
     def enqueue_contours(self, stream=None):
         """`trace_contours` with the result on the host: per planned image, per kept instance, the
@@ -368,7 +410,7 @@ class UnmoldEngine:
         with _stream_ctx(stream):
             counts = self.d_counts[:n].cpu().numpy()
             verts, coff = _download_contours(d_vert, d_coff)
-        return contours_to_lists(verts, coff, icoff, counts, self.R)
+        return contours_to_lists(verts, coff, icoff, counts, self.layout)
 
     def pack_masks(self, stream=None):
         """EXTENSION: bit-pack the byte canvases already written for the planned batch
@@ -376,11 +418,10 @@ class UnmoldEngine:
         (d_packed, offsets)."""
         n = self._n_images
         off = self._packed_buffer()
-        g = self._geom_host
         N.check(self.lib.mrx_pack_masks(
             _ptr(self.d_canvas), _ptr(self.d_canvas_off), _ptr(self.d_counts), _ptr(self.d_geom),
             _ptr(self.d_packed), _ptr(self.d_packed_off), n, self.R,
-            int(g[:, 0].max()), int(g[:, 1].max()), N.stream_ptr(stream)), "mrx_pack_masks")
+            self.layout.max_h, self.layout.max_w, N.stream_ptr(stream)), "mrx_pack_masks")
         return self.d_packed, off
 
     def fetch_meta(self, stream=None):
@@ -445,16 +486,15 @@ def _buffer(bufs, name, numel, dtype, device):
     return t
 
 
-def trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom, d_regions, n, R,
-                          max_h, stream=None, bufs=None):
-    """mrx_contours_count, one host read of the segment counts, mrx_contours_write.  Planes and
-    geometry as mrx_pack_masks writes / reads them; d_regions [n,R,4] int32 pixel rectangles.
-    `bufs`: a dict that keeps the work and output buffers between calls.  Returns
-    (d_vertices [V,2] float32, d_contour_off [C+1] int64, inst_contour_off int64 ndarray [n*R+1])."""
+def trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom, d_regions, layout,
+                          stream=None, bufs=None):
+    """mrx_contours_count, one host read of the segment counts, mrx_contours_write, over the planes
+    of a BatchLayout as mrx_pack_masks writes them; d_regions [n,R,4] int32 pixel rectangles; `bufs`
+    keeps the work and output buffers between calls.  Returns (d_vertices [V,2] float32,
+    d_contour_off [C+1] int64, inst_contour_off int64 ndarray [n*R+1])."""
     with _stream_ctx(stream):
         return _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom,
-                                      d_regions, n, R, max_h, stream,
-                                      {} if bufs is None else bufs)
+                                      d_regions, layout, stream, {} if bufs is None else bufs)
 
 
 def _stream_ctx(stream):
@@ -464,10 +504,11 @@ def _stream_ctx(stream):
     return contextlib.nullcontext() if stream is None else _torch().cuda.stream(stream)
 
 
-def _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom, d_regions, n, R,
-                           max_h, stream, bufs):
+def _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom, d_regions,
+                           layout, stream, bufs):
     torch = _torch()
     st = N.stream_ptr(stream)
+    n, R, max_h = layout.n, layout.R, layout.max_h
     ni = n * R
     d_rows = _buffer(bufs, "rows", ni * (max_h + 1), torch.int32, device)
     d_inst = _buffer(bufs, "inst", ni + 1, torch.int64, device)
@@ -498,18 +539,14 @@ def _download_contours(d_vert, d_coff):
     return d_vert.cpu().numpy().astype(np.float64), d_coff.cpu().numpy()
 
 
-def contours_to_lists(verts, contour_off, inst_contour_off, counts, R):
+def contours_to_lists(verts, contour_off, inst_contour_off, counts, layout):
     """Per image b, per kept instance k < counts[b], the list of float64 [V, 2] polygons: contour
-    c of instance i = b*R + k for c in [inst_contour_off[i], inst_contour_off[i+1]) has the
-    vertices verts[contour_off[c]:contour_off[c+1]]."""
+    c of instance i (`layout.kept_instances`) for c in [inst_contour_off[i], inst_contour_off[i+1])
+    has the vertices verts[contour_off[c]:contour_off[c+1]]."""
     polys = np.split(verts, contour_off[1:-1]) if len(contour_off) > 1 else []
-    out = []
-    for b, k_n in enumerate(counts):
-        per = []
-        for k in range(int(k_n)):
-            i = b * R + k
-            per.append(polys[int(inst_contour_off[i]):int(inst_contour_off[i + 1])])
-        out.append(per)
+    out = [[] for _ in counts]
+    for b, _, i in layout.kept_instances(counts):
+        out[b].append(polys[int(inst_contour_off[i]):int(inst_contour_off[i + 1])])
     return out
 
 
@@ -718,15 +755,14 @@ class StreamingUnmolder:
         self.packed = bool(packed)
         self.zero_copy = mask_upload == "zero_copy"
         engine.plan(geoms, canvas=False)       # the outputs live here, double-buffered
-        n = engine._n_images
-        self.n = n
+        n = self.n = engine.layout.n
         dev = engine.device
         det_t, msk_t = _torch_dtype(engine.det_dtype), _torch_dtype(engine.mask_dtype)
         self.d_det = [torch.empty((n, engine.R, 6), dtype=det_t, device=dev) for _ in range(2)]
         self.d_msk = None if self.zero_copy else [
             torch.empty((n, engine.R, engine.mh, engine.mw, engine.C), dtype=msk_t, device=dev)
             for _ in range(2)]
-        self.total = engine.packed_layout()[1] if self.packed else int(engine._offsets[n])
+        self.total = engine.packed_layout()[1] if self.packed else int(engine.layout.canvas_off[-1])
         self.d_out = [torch.empty((self.total,), dtype=torch.uint8, device=dev) for _ in range(2)]
         self.h_out = [torch.empty((self.total,), dtype=torch.uint8).pin_memory() for _ in range(2)]
         self.h_counts = [torch.empty((n,), dtype=torch.int32).pin_memory() for _ in range(2)]

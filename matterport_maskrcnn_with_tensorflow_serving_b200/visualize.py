@@ -21,6 +21,7 @@ import random as _random
 import numpy as np
 
 from . import _native as N
+from .engine import BatchLayout, _download_contours, contours_to_lists, trace_packed_contours
 
 
 def random_colors(n, bright=True, rng=None):
@@ -61,13 +62,13 @@ class CompositeStage:
         N.require_cuda()
         self.lib = N.load()
         self.engine = engine
-        B = engine._n_images
+        self.layout = layout = engine.layout
+        B = 0 if layout is None else layout.n
         if B == 0 or len(images) != B:
             raise ValueError(f"{len(images)} images for a plan of {B}")
         dev = engine.device
-        geom = engine._geom_host
-        self.geom = geom
-        sizes = [int(geom[b][0]) * int(geom[b][1]) * 3 for b in range(B)]
+        hw = [layout.hw(b) for b in range(B)]
+        sizes = [H * W * 3 for H, W in hw]
         offs = np.zeros(B + 1, dtype=np.int64)
         np.cumsum(sizes, out=offs[1:])
         self.offs = offs
@@ -75,7 +76,7 @@ class CompositeStage:
         for b, img in enumerate(images):
             t = img if torch.is_tensor(img) else torch.from_numpy(np.ascontiguousarray(img))
             if t.dtype != torch.uint8 or t.numel() != sizes[b]:
-                raise ValueError(f"image {b}: expected uint8 {geom[b][0]}x{geom[b][1]}x3")
+                raise ValueError(f"image {b}: expected uint8 {hw[b][0]}x{hw[b][1]}x3")
             self.d_in[int(offs[b]):int(offs[b + 1])].copy_(t.reshape(-1), non_blocking=True)
         self.d_out = torch.empty_like(self.d_in)
         shared = len(colors) > 0 and _is_triple(colors[0])
@@ -86,19 +87,20 @@ class CompositeStage:
         self.alpha = alpha
         self.d_tab = torch.from_numpy(tab).to(dev)
         self.d_off = torch.from_numpy(offs[:B].copy()).to(dev)
-        self.max_px = max(int(geom[b][0]) * int(geom[b][1]) for b in range(B))
+        self.max_px = max(H * W for H, W in hw)
 
     def run(self, stream=None):
         eng = self.engine
+        B = eng.layout.n
         N.check(self.lib.mrx_composite_masks(
             _ptr(eng.d_canvas), _ptr(eng.d_canvas_off), _ptr(eng.d_counts),
             _ptr(eng.d_geom), _ptr(eng.d_boxes), _ptr(self.d_in), _ptr(self.d_off),
             _ptr(self.d_tab), C.c_double(1 - self.alpha),
-            _ptr(self.d_out), eng._n_images, eng.R, C.c_longlong(self.max_px),
+            _ptr(self.d_out), B, eng.R, C.c_longlong(self.max_px),
             N.stream_ptr(stream)), "mrx_composite_masks")
-        offs, geom = self.offs, self.geom
-        return [self.d_out[int(offs[b]):int(offs[b + 1])].view(int(geom[b][0]), int(geom[b][1]), 3)
-                for b in range(eng._n_images)]
+        offs = self.offs
+        return [self.d_out[int(offs[b]):int(offs[b + 1])].view(*self.layout.hw(b), 3)
+                for b in range(B)]
 
 
 def composite_batch(engine, images, colors, alpha=0.5, stream=None):
@@ -109,6 +111,24 @@ def composite_batch(engine, images, colors, alpha=0.5, stream=None):
     images, or one such list per image.  Returns a list of uint8 HxWx3 CUDA tensors.
     """
     return CompositeStage(engine, images, colors, alpha).run(stream)
+
+
+def _stage_masks(mask_bytes, H, W, n):
+    """Caller-held masks (`mask_bytes`, the uint8 bytes of [H, W, n]) as a one-image batch on the
+    current device: (layout, device, d_canvas, d_off, d_counts, d_geom); the canvas past the masks
+    is zero and d_off (one zero) serves every offset argument.  The plan's limits are the expand
+    kernels': the pack, contour and overlay kernels check their own and take 1-pixel sides."""
+    import torch
+
+    layout = BatchLayout([[H, W, H, W, 0, 0, H, W]], n, limits=False)
+    dev = torch.device("cuda", torch.cuda.current_device())
+    d_canvas = torch.zeros(int(layout.canvas_off[-1]), dtype=torch.uint8, device=dev)
+    lo, hi = layout.canvas_span(0, n)
+    d_canvas[lo:hi].copy_(torch.from_numpy(mask_bytes.reshape(-1)))
+    d_off = torch.zeros(1, dtype=torch.int64, device=dev)
+    d_counts = torch.tensor([n], dtype=torch.int32, device=dev)
+    d_geom = torch.from_numpy(layout.geom).to(dev)
+    return layout, dev, d_canvas, d_off, d_counts, d_geom
 
 
 def apply_masks(image, boxes, masks, colors, alpha=0.5):
@@ -128,14 +148,8 @@ def apply_masks(image, boxes, masks, colors, alpha=0.5):
         raise ValueError("masks must be [H, W, N] for N boxes")
     if n == 0:
         return image.astype(np.uint8).copy()
-    dev = torch.device("cuda", torch.cuda.current_device())
-    total = H * W * n
-    d_canvas = torch.zeros((total + 15) // 16 * 16, dtype=torch.uint8, device=dev)
-    d_canvas[:total].copy_(torch.from_numpy(
-        np.ascontiguousarray(masks).view(np.uint8).reshape(-1)))
-    d_off = torch.zeros(1, dtype=torch.int64, device=dev)
-    d_counts = torch.tensor([n], dtype=torch.int32, device=dev)
-    d_geom = torch.tensor([[H, W, H, W, 0, 0, H, W]], dtype=torch.int32, device=dev)
+    _, dev, d_canvas, d_off, d_counts, d_geom = _stage_masks(
+        np.ascontiguousarray(masks).view(np.uint8), H, W, n)
     d_boxes = torch.from_numpy(np.ascontiguousarray(boxes, dtype=np.int32)).to(dev)
     d_img = torch.from_numpy(image.astype(np.uint8, copy=False)).to(dev)
     d_out = torch.empty_like(d_img)
@@ -155,8 +169,6 @@ def mask_contours(boxes, masks):
     every side; no polygon for an instance whose box is all zeros."""
     import torch
 
-    from .engine import _download_contours, contours_to_lists, trace_packed_contours
-
     N.require_cuda()
     lib = N.load()
     boxes = np.asarray(boxes)
@@ -166,15 +178,9 @@ def mask_contours(boxes, masks):
         raise ValueError("masks must be [H, W, N] for N boxes")
     if n == 0:
         return []
-    dev = torch.device("cuda", torch.cuda.current_device())
-    total = H * W * n
-    d_canvas = torch.zeros((total + 15) // 16 * 16, dtype=torch.uint8, device=dev)
-    d_canvas[:total].copy_(torch.from_numpy(
-        np.ascontiguousarray(masks).astype(np.bool_, copy=False).view(np.uint8).reshape(-1)))
-    d_off = torch.zeros(1, dtype=torch.int64, device=dev)
-    d_counts = torch.tensor([n], dtype=torch.int32, device=dev)
-    d_geom = torch.tensor([[H, W, H, W, 0, 0, H, W]], dtype=torch.int32, device=dev)
-    d_packed = torch.empty(n * H * ((W + 7) // 8), dtype=torch.uint8, device=dev)
+    layout, dev, d_canvas, d_off, d_counts, d_geom = _stage_masks(
+        np.ascontiguousarray(masks).astype(np.bool_, copy=False).view(np.uint8), H, W, n)
+    d_packed = torch.empty(int(layout.packed_off[-1]), dtype=torch.uint8, device=dev)
     N.check(lib.mrx_pack_masks(_ptr(d_canvas), _ptr(d_off), _ptr(d_counts), _ptr(d_geom),
                                _ptr(d_packed), _ptr(d_off), 1, n, H, W, N.stream_ptr(None)),
             "mrx_pack_masks")
@@ -183,9 +189,9 @@ def mask_contours(boxes, masks):
     regions[boxes.reshape(n, -1).any(axis=1)] = (0, 0, H, W)
     d_regions = torch.from_numpy(regions).to(dev)
     d_vert, d_coff, icoff = trace_packed_contours(lib, dev, d_packed, d_off, d_counts, d_geom,
-                                                  d_regions, 1, n, H)
+                                                  d_regions, layout)
     verts, coff = _download_contours(d_vert, d_coff)
-    return contours_to_lists(verts, coff, icoff, [n], n)[0]
+    return contours_to_lists(verts, coff, icoff, [n], layout)[0]
 
 
 def display_instances(image, boxes, masks, class_ids=None, class_names=None, scores=None,
