@@ -130,12 +130,31 @@ int mrx_unmold_prepare(const void *d_detections, int det_dtype, const void *d_mr
  *   - d_tile_index null: MRX_E_INVALID.
  * Then it checks its own arguments, and B = 0 returns MRX_OK without launching anything. */
 
-/* The hot kernel.  For every image b writes the bool canvas [H_b, W_b, N_b]
- * (N innermost, 1 byte per element, values 0/1) at d_canvas + d_canvas_off[b]:
- * zero fill, zero-border half-pixel bilinear resize of each tile to its box,
- * >= 0.5 threshold and paste, fused so each output byte is written once.  Inputs: a tile batch.
- *   d_canvas_off [B] int64, each a multiple of 16; slot b must hold at least
- *   round_up(H_b*W_b*N_b, 16) bytes (bytes past H_b*W_b*N_b may or may not be written).
+/* Output slots: where the masks of a planned batch live (engine.BatchLayout states the same on
+ * the host), for every entry point that writes or reads them (mrx_mask_expand,
+ * mrx_mask_expand_values, mrx_mask_expand_packed, mrx_pack_masks, mrx_composite_masks,
+ * mrx_contours_count, mrx_contours_write).  N_b = d_counts[b], H_b, W_b = d_geom[b][0], [1].
+ *   Canvas slots: image b's bool masks [H_b, W_b, N_b] (N innermost, 1 byte per element, values
+ *     0/1) at d_canvas + d_canvas_off[b] (int64, each a multiple of 16).  Slot b holds at least
+ *     round_up(H_b*W_b*N_b, 16) bytes; bytes past H_b*W_b*N_b may be read, and written by the
+ *     expand kernels.
+ *   Packed slots: image b's planes uint8 [N_b, H_b, ceil(W_b/8)] at d_packed + d_packed_off[b]
+ *     (int64), packed[n, y, :] = np.packbits(masks[y, :, n]) (most significant bit first); slot b
+ *     holds R*H_b*ceil(W_b/8) bytes.  Planes n >= N_b are not written.
+ *   Extents for grid sizing: max_h, max_w and max_pixels are the largest H_b, W_b and H_b*W_b of
+ *     the batch (or more).  mrx_pack_masks and mrx_composite_masks take 0 as "no image has a
+ *     pixel" and return MRX_OK without launching; mrx_mask_expand_packed and mrx_contours_* need
+ *     at least 1 (contours writes its offsets even when there is nothing to trace).
+ * Each of them checks, in this order, before anything reaches the device (right after the tile
+ * batch, for the three that read one):
+ *   - the slot base (d_canvas or d_packed), its offsets, d_counts or d_geom null: MRX_E_INVALID;
+ *   - B outside [0, MRX_MAX_BATCH] or R outside [1, 65534]: MRX_E_INVALID;
+ *   - then its own extents and arguments, and B = 0 returns MRX_OK without launching anything.
+ * Every message of mrx_last_error() starts with the name of the function called. */
+
+/* The hot kernel.  For every image b writes its canvas slot (see "Output slots"): zero fill,
+ * zero-border half-pixel bilinear resize of each tile to its box, >= 0.5 threshold and paste,
+ * fused so each output byte is written once.  Inputs: a tile batch.
  *   chunk_bytes: upper bound, in bytes, of the canvas tile a team of warps builds in
  *   shared memory and stores with one bulk copy per tile row (a tile is P pixels x
  *   10 rows x N instances; it is raised to the minimum that holds 16 pixels of R
@@ -152,7 +171,7 @@ int mrx_mask_expand(const float *d_tiles, const int *d_tile_index, const int *d_
  * coordinates, interpolation and row walk -- a second instantiation of it), which in addition
  * stores every pre-threshold sample it evaluates: d_values is float32, indexed exactly like
  * d_canvas (element d_canvas_off[b] + (y*W_b + x)*N_b + n); only elements inside box n are
- * written.  The canvas is written as usual.  Tests compare these values with the float64
+ * written.  The canvas slots are written as usual.  Tests compare these values with the float64
  * oracle (|diff| <= 1e-6).  Inputs: a tile batch, as a lane kernel.  R whose tile row no longer
  * fits a team's buffer returns MRX_E_UNSUPPORTED before launching anything (on an H100, R > 213
  * at B = 1; the limit drops slowly for large batches, whose scheduler table takes shared memory
@@ -197,14 +216,14 @@ int mrx_mold_image_batch(const unsigned char *d_src, int B, int src_h, int src_w
 
 /* ---------------------------------------------------------------- compositing (8f) */
 /* Mask part of visualize.display_instances(img, boxes, masks, ...) (serve.py:160-169), on
- * the canvas mrx_mask_expand wrote: for every image b, per instance i in order (skipped when
+ * the canvas slots mrx_mask_expand wrote: for every image b, per instance i in order (skipped when
  * its box is all zeros), per channel c,
  *     v = uint32( float64(v) * one_minus_alpha + blend[b][i][c] )      where mask[.,.,i] == 1
  * starting from the uint8 image and ending with astype(uint8).
  *   d_images / d_out: uint8 H_b x W_b x 3 images of the batch, image b at byte offset
  *   d_image_off[b] (int64) in both;  d_blend [B,R,3] float64 = alpha * color[c] * 255,
  *   evaluated by the caller in float64 in that order;  d_boxes [B,R,4] as written by
- *   mrx_unmold_prepare;  max_pixels = max_b H_b * W_b (grid sizing). */
+ *   mrx_unmold_prepare;  max_pixels: the extent of "Output slots", below 2^31 - 257. */
 int mrx_composite_masks(const unsigned char *d_canvas, const long long *d_canvas_off,
                         const int *d_counts, const int *d_geom, const int *d_boxes,
                         const unsigned char *d_images, const long long *d_image_off,
@@ -213,12 +232,12 @@ int mrx_composite_masks(const unsigned char *d_canvas, const long long *d_canvas
                         void *stream);
 
 /* ---------------------------------------------------------------- packed masks (8f) */
-/* EXTENSION (not the reference layout): bit-packed copy of the canvases for transport.
- * For image b:  d_packed + d_packed_off[b]  holds  uint8 [N_b, H_b, ceil(W_b/8)]  with
- *     packed[n, y, :] = np.packbits(masks[y, :, n])          (most significant bit first)
- * so that np.unpackbits(packed, axis=-1, count=W).transpose(1, 2, 0) is the bool [H,W,N] array
- * unmold_detections returns.  Slot b must hold R * H_b * ceil(W_b/8) bytes; d_packed_off int64.
- * max_h / max_w: largest H_b / W_b of the batch (grid sizing). */
+/* EXTENSION (not the reference layout): bit-packed copy of the canvas slots into the packed
+ * slots, for transport (see "Output slots"): np.unpackbits(packed, axis=-1,
+ * count=W).transpose(1, 2, 0) is the bool [H,W,N] array unmold_detections returns.  max_h,
+ * max_w: the extents of "Output slots"; max_h above 65535: MRX_E_UNSUPPORTED.  R too large for
+ * the kernels' shared memory returns MRX_E_UNSUPPORTED before launching anything (on an H100,
+ * R > 907). */
 int mrx_pack_masks(const unsigned char *d_canvas, const long long *d_canvas_off,
                    const int *d_counts, const int *d_geom, unsigned char *d_packed,
                    const long long *d_packed_off, int B, int R, int max_h, int max_w,
@@ -226,12 +245,10 @@ int mrx_pack_masks(const unsigned char *d_canvas, const long long *d_canvas_off,
 
 /* EXTENSION: the expand step with bit-packed output, without ever writing the byte canvas
  * (expand_bits.cu).  Inputs: a tile batch, as a lane kernel (wider tiles take mrx_mask_expand +
- * mrx_pack_masks).  Output layout exactly that of mrx_pack_masks:
- * image b at d_packed + d_packed_off[b] as uint8 [N_b, H_b, ceil(W_b/8)] (slot capacity
- * R * H_b * ceil(W_b/8)); planes n >= N_b are not written.  The samples are computed with the
- * same arithmetic as mrx_mask_expand, so  packed == np.packbits(canvas)  bit for bit.
- * d_packed may be memory of ANOTHER GPU mapped with mrx_peer_open (fused compute + gather).
- * max_w: widest W_b of the batch. */
+ * mrx_pack_masks).  Output: the packed slots (see "Output slots"), exactly as mrx_pack_masks
+ * writes them.  The samples are computed with the same arithmetic as mrx_mask_expand, so
+ * packed == np.packbits(canvas)  bit for bit.  d_packed may be memory of ANOTHER GPU mapped with
+ * mrx_peer_open (fused compute + gather).  max_w: the extent of "Output slots". */
 int mrx_mask_expand_packed(const float *d_tiles, const int *d_tile_index, const int *d_boxes,
                            const int *d_counts,
                            const int *d_geom, const long long *d_packed_off,
@@ -275,9 +292,9 @@ int mrx_rle_strings(const unsigned int *d_run_lengths, const long long *d_inst_o
 /* EXTENSION: mask outlines as polygons, the contour loop of visualize.display_instances
  * (serve.py:160-169): for each instance, skimage.measure.find_contours(padded, 0.5) of the mask
  * padded with one pixel of zeros on every side (fully_connected and positive_orientation 'low'),
- * vertices as (x, y) image coordinates = np.fliplr(v) - 1 (contours.cu).  Input: the packed planes
- * of mrx_pack_masks / mrx_mask_expand_packed (d_packed, d_packed_off as written there; d_counts,
- * d_geom as for them).  d_regions [B,R,4] int32 (y1, x1, y2, x2), required: instance k is traced
+ * vertices as (x, y) image coordinates = np.fliplr(v) - 1 (contours.cu).  Input: the packed slots
+ * (see "Output slots") as mrx_pack_masks / mrx_mask_expand_packed write them; max_h: the extent
+ * of "Output slots", below 2^30.  d_regions [B,R,4] int32 (y1, x1, y2, x2), required: instance k is traced
  * only inside that pixel rectangle (clamped to the image; pixels outside it count as 0; an empty
  * rectangle gives no contour), e.g. the d_boxes of mrx_unmold_prepare, outside which the plane is
  * zero.  Two calls around one host read:

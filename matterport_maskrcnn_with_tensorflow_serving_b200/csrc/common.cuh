@@ -66,6 +66,22 @@ int ensure_dynamic_smem(const void *func, SmemCache *cache, int device, int byte
 // Exclusive scan of d_v[0, n) in place on `st`, with their sum stored at d_v[n] (one CTA).
 int launch_offsets_scan(long long *d_v, int n, cudaStream_t st);
 
+// ---------------------------------------------------------------- output slots
+// The byte canvas or the packed planes of a planned batch (mrx.h, "Output slots"): image b's
+// slot starts at base + off[b].  T is const for the kernels that only read the slots.  (Pointers
+// in a struct do not carry __restrict__ into a kernel: a kernel that relied on restrict-qualified
+// pointer parameters reads off[] with __ldg, or keeps those parameters.)
+template <typename T>
+struct Slots {
+  T *base;
+  const long long *off;   // [B] int64 byte offsets
+};
+
+// The one host check of a batch's output slots (unmold.cu): null pointers, then B and R.
+// Returns MRX_OK or MRX_E_INVALID, with mrx_last_error() naming `fn`.
+int check_slots(const char *fn, const void *base, const long long *off, const int *counts,
+                const int *geom, int B, int R);
+
 // ---------------------------------------------------------------- device: PTX wrappers
 #if defined(__CUDACC__)
 

@@ -30,10 +30,8 @@ namespace mrx {
 constexpr int kCompThreads = 256;   // faster than 128, 384 or 512 threads per CTA
 
 __global__ void __launch_bounds__(kCompThreads)
-composite_masks_kernel(const unsigned char *__restrict__ canvas,
-                       const long long *__restrict__ canvas_off,
-                       const int *__restrict__ counts, const int *__restrict__ geom,
-                       const int4 *__restrict__ boxes, const unsigned char *__restrict__ images,
+composite_masks_kernel(const Slots<const unsigned char> canvas, const int *__restrict__ counts,
+                       const int *__restrict__ geom, const int4 *__restrict__ boxes, const unsigned char *__restrict__ images,
                        const long long *__restrict__ image_off, const double *__restrict__ blend,
                        double one_minus_alpha, unsigned char *__restrict__ out, int R,
                        int blend_bulk) {
@@ -70,7 +68,7 @@ composite_masks_kernel(const unsigned char *__restrict__ canvas,
     const unsigned cbytes = blend_bulk ? (static_cast<unsigned>(N) * 24u + 15u) & ~15u : 0u;
     if (bytes + cbytes) {
       mbar_arrive_expect_tx(&s_bar, bytes + cbytes);
-      if (bytes) bulk_g2s(s_can, canvas + canvas_off[b] + static_cast<size_t>(p0) * N, bytes, &s_bar);
+      if (bytes) bulk_g2s(s_can, canvas.base + __ldg(canvas.off + b) + static_cast<size_t>(p0) * N, bytes, &s_bar);
       if (cbytes) bulk_g2s(s_blend, blend + static_cast<size_t>(b) * R * 3, cbytes, &s_bar);
     } else {
       mbar_arrive(&s_bar);
@@ -140,11 +138,10 @@ extern "C" int mrx_composite_masks(const unsigned char *d_canvas, const long lon
                                    unsigned char *d_out, int B, int R, long long max_pixels,
                                    void *stream) {
   using namespace mrx;
-  MRX_CHECK_ARG(d_canvas && d_canvas_off && d_counts && d_geom && d_boxes && d_images &&
-                    d_image_off && d_blend && d_out,
-                "mrx_composite_masks: null pointer");
-  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH && R >= 1 && max_pixels >= 0,
-                "mrx_composite_masks: bad sizes B=%d R=%d", B, R);
+  const char *fn = "mrx_composite_masks";
+  if (int rc = check_slots(fn, d_canvas, d_canvas_off, d_counts, d_geom, B, R)) return rc;
+  MRX_CHECK_ARG(d_boxes && d_images && d_image_off && d_blend && d_out, "%s: null pointer", fn);
+  MRX_CHECK_ARG(max_pixels >= 0, "%s: bad max_pixels %lld", fn, max_pixels);
   if (B == 0 || max_pixels == 0) return MRX_OK;
   DevInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
@@ -162,7 +159,8 @@ extern "C" int mrx_composite_masks(const unsigned char *d_canvas, const long lon
     return rc;
   dim3 grid(static_cast<unsigned>(blocks), static_cast<unsigned>(B));
   composite_masks_kernel<<<grid, kCompThreads, smem, static_cast<cudaStream_t>(stream)>>>(
-      d_canvas, d_canvas_off, d_counts, d_geom, reinterpret_cast<const int4 *>(d_boxes), d_images,
+      Slots<const unsigned char>{d_canvas, d_canvas_off}, d_counts, d_geom,
+      reinterpret_cast<const int4 *>(d_boxes), d_images,
       d_image_off, d_blend, one_minus_alpha, d_out, R,
       ((R & 1) == 0 && (reinterpret_cast<uintptr_t>(d_blend) & 15u) == 0u) ? 1 : 0);
   MRX_LAUNCH_CHECK("composite_masks_kernel");

@@ -69,8 +69,7 @@ constexpr uint64_t kWindow = (1ull << 34) - 1;
 constexpr uint64_t kOwn = kWindow & ~1ull & ~(1ull << 33);
 
 struct Params {
-  const unsigned char *packed;   // image b at packed + packed_off[b]: uint8 [R, H_b, wb_b]
-  const long long *packed_off;   // [B]
+  Slots<const unsigned char> packed;   // image b: uint8 [R, H_b, wb_b] (mrx.h, "Output slots")
   const int *counts;             // [B]
   const int *geom;               // [B, 8]
   const int4 *regions;           // [B, R] (y1, x1, y2, x2) pixels
@@ -98,7 +97,7 @@ __device__ __forceinline__ Inst inst_of(const Params &p, int b, int k) {
   Inst in;
   const int H = p.geom[b * MRX_GEOM_INTS + 0], W = p.geom[b * MRX_GEOM_INTS + 1];
   in.wb = (W + 7) >> 3;
-  in.plane = p.packed + p.packed_off[b] + static_cast<long long>(k) * H * in.wb;
+  in.plane = p.packed.base + p.packed.off[b] +static_cast<long long>(k) * H * in.wb;
   const int4 r = p.regions[static_cast<size_t>(b) * p.R + k];
   in.g = {max(r.x, 0), max(r.y, 0), min(r.z, H), min(r.w, W)};
   const bool empty = k >= p.counts[b] || in.g.y2 <= in.g.y1 || in.g.x2 <= in.g.x1;
@@ -383,15 +382,13 @@ static int fill_contour_params(contours::Params &prm, const char *fn, const unsi
                                const long long *d_packed_off, const int *d_counts,
                                const int *d_geom, const int *d_regions, const int *d_row_off,
                                const long long *d_inst_off, int B, int R, int max_h) {
-  MRX_CHECK_ARG(d_packed && d_packed_off && d_counts && d_geom && d_row_off && d_inst_off,
-                "%s: null pointer", fn);
+  if (int rc = check_slots(fn, d_packed, d_packed_off, d_counts, d_geom, B, R)) return rc;
+  MRX_CHECK_ARG(d_row_off && d_inst_off, "%s: null pointer", fn);
   MRX_CHECK_ARG(d_regions, "%s: the region argument d_regions is required", fn);
-  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH && R >= 1 && R <= 65535 && max_h >= 1 &&
-                    max_h < (1 << 30),
-                "%s: bad sizes B=%d R=%d max_h=%d", fn, B, R, max_h);
+  MRX_CHECK_ARG(max_h >= 1 && max_h < (1 << 30), "%s: bad max_h %d (need 1<=max_h<2^30)", fn,
+                max_h);
   prm = {};
-  prm.packed = d_packed;
-  prm.packed_off = d_packed_off;
+  prm.packed = {d_packed, d_packed_off};
   prm.counts = d_counts;
   prm.geom = d_geom;
   prm.regions = reinterpret_cast<const int4 *>(d_regions);

@@ -145,8 +145,7 @@ int check_tile_batch(const char *fn, const TileBatch &t, int max_mw);
 
 struct ExpandParams {
   TileBatch t;
-  const long long *canvas_off;  // [B]
-  unsigned char *canvas;
+  Slots<unsigned char> canvas;  // image b: bytes [H_b, W_b, N_b] (mrx.h, "Output slots")
   unsigned int *job_counter;    // [0] tile ticket, [1] teams / CTAs retired; zero between launches
   float *values;                // test instantiation only: pre-threshold samples, indexed like canvas
   int chunk_bytes;

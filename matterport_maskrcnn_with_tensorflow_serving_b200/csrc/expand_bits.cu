@@ -46,8 +46,7 @@ constexpr int kGroup = 4;   // column blocks a warp walks side by side (independ
 
 struct BitsParams {
   TileBatch t;
-  const long long *packed_off;   // [B]
-  unsigned char *packed;
+  Slots<unsigned char> packed;   // image b: uint8 [N_b, H_b, ceil(W_b/8)] (mrx.h, "Output slots")
   unsigned int *sched;           // [2] unit ticket, [3] warps retired (MRX_SCHED_WORDS)
   int ubuf;                      // bytes of one unit buffer (multiple of 16, incl. 16 B of slack)
 };
@@ -133,7 +132,7 @@ mask_expand_bits_kernel(const BitsParams p) {
         tiles_b = p.t.tiles + static_cast<size_t>(cur_b) * p.t.R * mh * mw;
         boxes_b = p.t.boxes + static_cast<size_t>(cur_b) * p.t.R;
         tidx_b = p.t.tile_index + static_cast<size_t>(cur_b) * p.t.R;
-        out_b = p.packed + p.packed_off[cur_b];
+        out_b = p.packed.base + p.packed.off[cur_b];
       }
       const int local = u - s_prefix[cur_b];
       const int n = local / nbands;
@@ -295,13 +294,15 @@ extern "C" int mrx_mask_expand_packed(const float *d_tiles, const int *d_tile_in
   using namespace mrx::bits;
   const TileBatch t{d_tiles, d_tile_index, reinterpret_cast<const int4 *>(d_boxes), d_counts,
                     d_geom, B, R, mh, mw};
-  if (int rc = check_tile_batch("mrx_mask_expand_packed", t, MRX_MAX_LANE_MASK_W)) return rc;
-  MRX_CHECK_ARG(d_packed_off && d_packed && d_sched, "mrx_mask_expand_packed: null pointer");
-  MRX_CHECK_ARG(max_w >= 1, "mrx_mask_expand_packed: bad max_w %d", max_w);
+  const char *fn = "mrx_mask_expand_packed";
+  if (int rc = check_tile_batch(fn, t, MRX_MAX_LANE_MASK_W)) return rc;
+  if (int rc = check_slots(fn, d_packed, d_packed_off, d_counts, d_geom, B, R)) return rc;
+  MRX_CHECK_ARG(d_sched, "%s: null pointer", fn);
+  MRX_CHECK_ARG(max_w >= 1, "%s: bad max_w %d", fn, max_w);
   if (B == 0) return MRX_OK;
   DevInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  const BitsParams prm{t, d_packed_off, d_packed, d_sched, 0};
+  const BitsParams prm{t, {d_packed, d_packed_off}, d_sched, 0};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 #ifdef MRX_DEV
   if (const char *e = getenv("MRX_BITS_WARPS")) {

@@ -244,7 +244,7 @@ mask_expand_team_kernel(const ExpandParams p, const int buf_bytes) {
       dc.P = P_;
       dc.pitch = pitch_;
       dc.tx = (dc.W + P_ - 1) / P_;
-      dc.canvas = p.canvas + p.canvas_off[b];
+      dc.canvas = p.canvas.base + p.canvas.off[b];
       // kept rows are in increasing order: no row was dropped iff the last one kept its index
       dc.ident = dc.N == 0 || p.t.tile_index[static_cast<size_t>(b) * p.t.R + dc.N - 1] == dc.N - 1;
     }
@@ -433,7 +433,7 @@ mask_expand_team_kernel(const ExpandParams p, const int buf_bytes) {
         // kValues: where the sample of (tile row ra, this lane's column, instance n) goes
         [[maybe_unused]] float *vout = nullptr;
         if (kValues)
-          vout = p.values + (g0 - p.canvas) + static_cast<size_t>(ra) * RW +
+          vout = p.values + (g0 - p.canvas.base) + static_cast<size_t>(ra) * RW +
                  static_cast<size_t>(x - x0) * N + n;
         int step = 2 * mh;
         // the byte every set sample stores: 1, derived from a value ptxas cannot fold (the sign

@@ -302,49 +302,51 @@ extern "C" int mrx_pack_masks(const unsigned char *d_canvas, const long long *d_
                               const long long *d_packed_off, int B, int R, int max_h, int max_w,
                               void *stream) {
   using namespace mrx;
-  MRX_CHECK_ARG(d_canvas && d_canvas_off && d_counts && d_geom && d_packed && d_packed_off,
-                "mrx_pack_masks: null pointer");
-  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH && R >= 1 && max_h >= 0 && max_w >= 0,
-                "mrx_pack_masks: bad sizes B=%d R=%d", B, R);
+  const char *fn = "mrx_pack_masks";
+  if (int rc = check_slots(fn, d_canvas, d_canvas_off, d_counts, d_geom, B, R)) return rc;
+  MRX_CHECK_ARG(d_packed && d_packed_off, "%s: null pointer", fn);
+  MRX_CHECK_ARG(max_h >= 0 && max_w >= 0, "%s: bad max_h %d / max_w %d", fn, max_h, max_w);
   if (B == 0 || max_h == 0 || max_w == 0) return MRX_OK;
-  MRX_CHECK_SUPPORTED(max_h <= 65535, "mrx_pack_masks: image taller than 65535 rows");
+  MRX_CHECK_SUPPORTED(max_h <= 65535, "%s: image taller than 65535 rows", fn);
   DevInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // pack_quads_kernel's staged form takes every image while eight runs of R instance slots fit
-  // the shared memory of a quarter of an SM (four or more CTAs resident); beyond that, its direct
-  // form packs the images with N % 4 == 0 and pack_bytes_kernel the others
+  // Everything is decided before the first launch, so that a batch either kernel cannot take
+  // leaves the packed output untouched.  pack_quads_kernel's staged form takes every image while
+  // eight runs of R instance slots fit the shared memory of a quarter of an SM (four or more CTAs
+  // resident); beyond that, its direct form packs the images with N % 4 == 0 and
+  // pack_bytes_kernel the others.
   int stage_bytes = kPackRuns * pack_max_run_pitch(R);
   if (stage_bytes + 1024 > dev.max_smem_optin / 4) stage_bytes = 0;
-  {
-    const int max_quads = (R + 3) >> 2;
-    const int warps_per_row = ((max_w + 127) >> 7) * ((max_quads + 7) >> 3);
-    // the grid covers both forms: one CTA per 256 pixels (staged) / per eight warps' worth of
-    // (pixel run, quad) blocks (direct)
-    const int direct_ctas = (warps_per_row + kPackThreads / 32 - 1) / (kPackThreads / 32);
-    const int staged_ctas = (max_w + kPackPixels - 1) / kPackPixels;
-    static SmemCache quads_cache;
-    if (int rc = ensure_dynamic_smem(reinterpret_cast<const void *>(pack_quads_kernel), &quads_cache,
-                                     dev.device, stage_bytes))
+  const size_t bytes_smem = stage_bytes ? 0 : static_cast<size_t>(kPackPixels) * R + 32;
+  MRX_CHECK_SUPPORTED(bytes_smem <= static_cast<size_t>(dev.max_smem_optin),
+                      "%s: R=%d needs %zu B of shared memory (limit %d)", fn, R, bytes_smem,
+                      dev.max_smem_optin);
+  static SmemCache quads_cache, bytes_cache;
+  if (int rc = ensure_dynamic_smem(reinterpret_cast<const void *>(pack_quads_kernel), &quads_cache,
+                                   dev.device, stage_bytes))
+    return rc;
+  int bytes_occ = 0;
+  if (bytes_smem) {
+    if (int rc = ensure_dynamic_smem(reinterpret_cast<const void *>(pack_bytes_kernel), &bytes_cache,
+                                     dev.device, static_cast<int>(bytes_smem)))
       return rc;
-    dim3 grid(stage_bytes ? staged_ctas : direct_ctas, max_h, B);
-    pack_quads_kernel<<<grid, kPackThreads, stage_bytes, st>>>(d_canvas, d_canvas_off, d_counts,
-                                                               d_geom, d_packed, d_packed_off,
-                                                               stage_bytes);
-    MRX_LAUNCH_CHECK("pack_quads_kernel");
+    MRX_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bytes_occ, pack_bytes_kernel,
+                                                           kPackThreads, bytes_smem));
   }
-  if (stage_bytes == 0) {
-    const size_t smem = static_cast<size_t>(kPackPixels) * R + 32;
-    MRX_CHECK_SUPPORTED(smem <= static_cast<size_t>(dev.max_smem_optin),
-                        "mrx_pack_masks: R=%d needs %zu B of shared memory (limit %d)", R, smem,
-                        dev.max_smem_optin);
-    static SmemCache cache;
-    if (int rc = ensure_dynamic_smem(reinterpret_cast<const void *>(pack_bytes_kernel), &cache,
-                                     dev.device, static_cast<int>(smem)))
-      return rc;
-    int occ = 0;
-    MRX_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, pack_bytes_kernel, kPackThreads, smem));
-    pack_bytes_kernel<<<dev.sms * max(occ, 1), kPackThreads, smem, st>>>(
+
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int max_quads = (R + 3) >> 2;
+  const int warps_per_row = ((max_w + 127) >> 7) * ((max_quads + 7) >> 3);
+  // the grid covers both forms: one CTA per 256 pixels (staged) / per eight warps' worth of
+  // (pixel run, quad) blocks (direct)
+  const int direct_ctas = (warps_per_row + kPackThreads / 32 - 1) / (kPackThreads / 32);
+  const int staged_ctas = (max_w + kPackPixels - 1) / kPackPixels;
+  dim3 grid(stage_bytes ? staged_ctas : direct_ctas, max_h, B);
+  pack_quads_kernel<<<grid, kPackThreads, stage_bytes, st>>>(
+      d_canvas, d_canvas_off, d_counts, d_geom, d_packed, d_packed_off, stage_bytes);
+  MRX_LAUNCH_CHECK("pack_quads_kernel");
+  if (bytes_smem) {
+    pack_bytes_kernel<<<dev.sms * max(bytes_occ, 1), kPackThreads, bytes_smem, st>>>(
         d_canvas, d_canvas_off, d_counts, d_geom, d_packed, d_packed_off, B, stage_bytes);
     MRX_LAUNCH_CHECK("pack_bytes_kernel");
   }

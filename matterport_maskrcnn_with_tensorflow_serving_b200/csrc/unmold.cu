@@ -281,7 +281,7 @@ __device__ __forceinline__ void make_job(const ExpandParams &p, const int *s_job
   const int r1 = g1 / W;
   out->tiles_b = p.t.tiles + static_cast<size_t>(b) * p.t.R * p.t.mh * p.t.mw;
   out->boxes_b = p.t.boxes + static_cast<size_t>(b) * p.t.R;
-  out->dst = p.canvas + p.canvas_off[b] + c0;
+  out->dst = p.canvas.base + p.canvas.off[b] + c0;
   out->H = H;
   out->W = W;
   out->N = N;
@@ -486,10 +486,22 @@ mask_expand_kernel(const ExpandParams p) {
 // =====================================================================================
 using namespace mrx;
 
+// the batch size limits shared by the tile batch and the output slots
+static int check_batch_sizes(const char *fn, int B, int R) {
+  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH && R >= 1 && R <= 65534,
+                "%s: bad sizes B=%d R=%d (need 0<=B<=%d, 1<=R<=65534)", fn, B, R, MRX_MAX_BATCH);
+  return MRX_OK;
+}
+
+int mrx::check_slots(const char *fn, const void *base, const long long *off, const int *counts,
+                     const int *geom, int B, int R) {
+  MRX_CHECK_ARG(base && off && counts && geom, "%s: null pointer", fn);
+  return check_batch_sizes(fn, B, R);
+}
+
 int mrx::check_tile_batch(const char *fn, const TileBatch &t, int max_mw) {
   MRX_CHECK_ARG(t.tiles && t.boxes && t.counts && t.geom, "%s: null pointer", fn);
-  MRX_CHECK_ARG(t.B >= 0 && t.B <= MRX_MAX_BATCH && t.R >= 1 && t.R <= 65534,
-                "%s: bad sizes B=%d R=%d (need 0<=B<=%d, 1<=R<=65534)", fn, t.B, t.R, MRX_MAX_BATCH);
+  if (int rc = check_batch_sizes(fn, t.B, t.R)) return rc;
   MRX_CHECK_SUPPORTED(t.mh >= 2 && t.mh <= MRX_MAX_MASK_DIM && t.mw >= 4 && t.mw <= max_mw &&
                           (t.mw % 4) == 0,
                       "%s: mask tile %dx%d unsupported (need 2<=mh<=%d, 4<=mw<=%d, mw%%4==0)", fn,
@@ -530,21 +542,21 @@ extern "C" int mrx_unmold_prepare(const void *d_detections, int det_dtype, const
   return MRX_OK;
 }
 
-// mrx_mask_expand and mrx_mask_expand_values, after check_tile_batch
-static int mask_expand_impl(const TileBatch &t, const long long *d_canvas_off,
-                            unsigned char *d_canvas, float *d_values, int chunk_bytes,
-                            int ctas_per_sm, unsigned int *d_sched, void *stream) {
-  MRX_CHECK_ARG(d_canvas_off && d_canvas && d_sched, "mrx_mask_expand: null pointer");
+// mrx_mask_expand and mrx_mask_expand_values (`fn`), after check_tile_batch and check_slots
+static int mask_expand_impl(const char *fn, const TileBatch &t, Slots<unsigned char> canvas,
+                            float *d_values, int chunk_bytes, int ctas_per_sm,
+                            unsigned int *d_sched, void *stream) {
+  MRX_CHECK_ARG(d_sched, "%s: null pointer", fn);
   const int want_buf = chunk_bytes;   // team kernel: upper bound of a team's tile buffer, 0 = auto
   if (chunk_bytes == 0) chunk_bytes = 25600;
   MRX_CHECK_ARG(chunk_bytes >= 1024 && (chunk_bytes % 16) == 0,
-                "mrx_mask_expand: chunk_bytes %d must be a multiple of 16, >= 1024", chunk_bytes);
+                "%s: chunk_bytes %d must be a multiple of 16, >= 1024", fn, chunk_bytes);
   if (t.B == 0) return MRX_OK;
 
   DevInfo dev;
   if (int rc = current_device_info(&dev)) return rc;
 
-  ExpandParams prm{t, d_canvas_off, d_canvas, d_sched, d_values, chunk_bytes, 0};
+  ExpandParams prm{t, canvas, d_sched, d_values, chunk_bytes, 0};
 #ifdef MRX_DEV
   if (const char *f = getenv("MRX_EXPAND_FLAGS")) prm.flags = atoi(f);
 #endif
@@ -585,9 +597,11 @@ extern "C" int mrx_mask_expand(const float *d_tiles, const int *d_tile_index, co
                                unsigned int *d_sched, void *stream) {
   const TileBatch t{d_tiles, d_tile_index, reinterpret_cast<const int4 *>(d_boxes), d_counts,
                     d_geom, B, R, mh, mw};
-  if (int rc = check_tile_batch("mrx_mask_expand", t, MRX_MAX_MASK_DIM)) return rc;
-  return mask_expand_impl(t, d_canvas_off, d_canvas, nullptr, chunk_bytes, ctas_per_sm, d_sched,
-                          stream);
+  const char *fn = "mrx_mask_expand";
+  if (int rc = check_tile_batch(fn, t, MRX_MAX_MASK_DIM)) return rc;
+  if (int rc = check_slots(fn, d_canvas, d_canvas_off, d_counts, d_geom, B, R)) return rc;
+  return mask_expand_impl(fn, t, {d_canvas, d_canvas_off}, nullptr, chunk_bytes, ctas_per_sm,
+                          d_sched, stream);
 }
 
 extern "C" int mrx_mask_expand_values(const float *d_tiles, const int *d_tile_index,
@@ -597,7 +611,9 @@ extern "C" int mrx_mask_expand_values(const float *d_tiles, const int *d_tile_in
                                       int mh, int mw, unsigned int *d_sched, void *stream) {
   const TileBatch t{d_tiles, d_tile_index, reinterpret_cast<const int4 *>(d_boxes), d_counts,
                     d_geom, B, R, mh, mw};
-  if (int rc = check_tile_batch("mrx_mask_expand_values", t, MRX_MAX_LANE_MASK_W)) return rc;
-  MRX_CHECK_ARG(d_values != nullptr, "mrx_mask_expand_values: null pointer");
-  return mask_expand_impl(t, d_canvas_off, d_canvas, d_values, 0, 0, d_sched, stream);
+  const char *fn = "mrx_mask_expand_values";
+  if (int rc = check_tile_batch(fn, t, MRX_MAX_LANE_MASK_W)) return rc;
+  if (int rc = check_slots(fn, d_canvas, d_canvas_off, d_counts, d_geom, B, R)) return rc;
+  MRX_CHECK_ARG(d_values != nullptr, "%s: null pointer", fn);
+  return mask_expand_impl(fn, t, {d_canvas, d_canvas_off}, d_values, 0, 0, d_sched, stream);
 }
