@@ -18,6 +18,8 @@
  *   mrx_rle_count / _write (extension: the same masks as COCO run-length encodings)
  *   mrx_rle_strings        (extension: those encodings as COCO compressed RLE strings)
  *   mrx_contours_count / _write <- visualize.display_instances (contour polygons) serve.py:160-169
+ *   mrx_mask_extents / _overlaps / _matches (extension: mrcnn.utils.compute_overlaps_masks and
+ *                             compute_matches, scoring the masks against ground truth)
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
  *   mrx_device_alloc/_free (the canvas allocation: compressible device memory where offered)
  *
@@ -40,7 +42,7 @@
 extern "C" {
 #endif
 
-#define MRX_ABI_VERSION 9
+#define MRX_ABI_VERSION 10
 
 #define MRX_OK              0
 #define MRX_E_INVALID      -1   /* bad argument (null pointer, size out of range) */
@@ -133,7 +135,7 @@ int mrx_unmold_prepare(const void *d_detections, int det_dtype, const void *d_mr
 /* Output slots: where the masks of a planned batch live (engine.BatchLayout states the same on
  * the host), for every entry point that writes or reads them (mrx_mask_expand,
  * mrx_mask_expand_values, mrx_mask_expand_packed, mrx_pack_masks, mrx_composite_masks,
- * mrx_contours_count, mrx_contours_write).  N_b = d_counts[b], H_b, W_b = d_geom[b][0], [1].
+ * mrx_contours_count, mrx_contours_write, mrx_mask_extents, mrx_mask_overlaps).  N_b = d_counts[b], H_b, W_b = d_geom[b][0], [1].
  *   Canvas slots: image b's bool masks [H_b, W_b, N_b] (N innermost, 1 byte per element, values
  *     0/1) at d_canvas + d_canvas_off[b] (int64, each a multiple of 16).  Slot b holds at least
  *     round_up(H_b*W_b*N_b, 16) bytes; bytes past H_b*W_b*N_b may be read, and written by the
@@ -325,6 +327,51 @@ int mrx_contours_write(const unsigned char *d_packed, const long long *d_packed_
                        long long max_inst_segments, void *d_scratch, float *d_vertices,
                        long long *d_contour_off, long long *d_inst_contour_off, int B, int R,
                        int max_h, void *stream);
+
+/* ---------------------------------------------------------------- mask IoU and matches */
+/* EXTENSION: upstream mrcnn.utils.compute_overlaps_masks and the matching loop of compute_matches
+ * on the packed slots (see "Output slots"), so that scoring predictions against ground truth
+ * needs no mask on the host (overlaps.cu).
+ *
+ * mrx_mask_extents: for every plane k < N_b, d_areas[b][k] (int64) = its set pixels and
+ *   d_extents[b][k] (int32 y1, x1, y2, x2, exclusive ends; all 0 for an empty plane) = their tight
+ *   bounding box, counted only inside d_regions[b][k] (int32 [B,R,4] y1, x1, y2, x2, required;
+ *   clamped to the image, pixels outside count as 0), e.g. the d_boxes of mrx_unmold_prepare,
+ *   outside which an expanded plane is zero, or (0, 0, H_b, W_b).
+ * mrx_mask_overlaps: two slot sets of one batch (R1 and R2 planes per slot) sharing d_geom, with
+ *   their areas and extents from mrx_mask_extents: d_overlaps [B,R1,R2] float32, element (b, i, j)
+ *   for i < N1_b, j < N2_b = IoU of plane i of set 1 and plane j of set 2 in NumPy's float32
+ *   order, i = f32(inter), u = (f32(a1) + f32(a2)) - i, i / u (NaN when both are empty); other
+ *   elements are not written.  d_packed1 and d_packed2 must be 4-byte aligned.
+ * mrx_mask_matches: per image b, its N_b = d_pred_counts[b] predictions (d_pred_class_ids [B,R1]
+ *   int32, d_scores [B,R1] of score_dtype) and M_b = d_gt_counts[b] ground-truth instances
+ *   (d_gt_class_ids [B,R2] int32), d_overlaps as above.  thresholds[T] (HOST, 1 <= T <=
+ *   MRX_MAX_IOU_THRESHOLDS) and score_threshold are compared with (double)IoU.  Writes
+ *     d_order [B,R1] int32: rank -> prediction, by score descending, NaN first, ties larger
+ *                           index first;
+ *     d_pred_match [T,B,R1] int32 by rank: the matched ground-truth index or -1;
+ *     d_gt_match   [T,B,R2] int32: the rank of the prediction that matched it or -1.
+ *   The prediction of rank r takes, among the ground truth still unmatched and of its class whose
+ *   IoU is NaN or >= both thresholds, the one with the largest IoU (NaN above every number, ties
+ *   the larger index): what compute_matches' loop picks.
+ * Checks: those of "Output slots" for each slot set (mrx_mask_extents, mrx_mask_overlaps), then
+ * null pointers; for mrx_mask_matches null pointers, B outside [0, MRX_MAX_BATCH], R1 or R2
+ * outside [1, 65534], T outside [1, MRX_MAX_IOU_THRESHOLDS] or a bad score_dtype: MRX_E_INVALID.
+ * B = 0 returns MRX_OK without launching anything. */
+#define MRX_MAX_IOU_THRESHOLDS 64
+int mrx_mask_extents(const unsigned char *d_packed, const long long *d_packed_off,
+                     const int *d_counts, const int *d_geom, const int *d_regions,
+                     long long *d_areas, int *d_extents, int B, int R, void *stream);
+int mrx_mask_overlaps(const unsigned char *d_packed1, const long long *d_packed_off1,
+                      const int *d_counts1, const long long *d_areas1, const int *d_extents1,
+                      int R1, const unsigned char *d_packed2, const long long *d_packed_off2,
+                      const int *d_counts2, const long long *d_areas2, const int *d_extents2,
+                      int R2, const int *d_geom, float *d_overlaps, int B, void *stream);
+int mrx_mask_matches(const float *d_overlaps, const int *d_pred_counts,
+                     const int *d_pred_class_ids, const void *d_scores, int score_dtype,
+                     const int *d_gt_counts, const int *d_gt_class_ids, const double *thresholds,
+                     int T, double score_threshold, int *d_order, int *d_pred_match,
+                     int *d_gt_match, int B, int R1, int R2, void *stream);
 
 /* ---------------------------------------------------------------- multi-GPU gather (8e) */
 /* Peer-memory plumbing for the final gather of the canvases to rank 0 (one process per GPU).

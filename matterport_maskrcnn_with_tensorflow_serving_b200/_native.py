@@ -17,6 +17,7 @@ LIB_PATH = os.path.join(_PKG_DIR, "lib", os.environ.get("MRX_LIB", "libmrx.so"))
 HEADER_PATH = os.path.join(os.path.dirname(_PKG_DIR), "include", "mrx.h")
 
 MRX_OK = 0
+MRX_E_UNSUPPORTED = -2
 MRX_F32 = 0
 MRX_F64 = 1
 MRX_ST_CLASS_RANGE = 1
@@ -25,10 +26,11 @@ MRX_GEOM_INTS = 8
 MRX_MAX_BATCH = 4096
 MRX_MAX_MASK_DIM = 64
 MRX_MAX_LANE_MASK_W = 30    # tile width of the lane kernels: mw + 2 lanes per warp
-ABI_VERSION = 9
+ABI_VERSION = 10
 MRX_SCHED_WORDS = 4
 MRX_PEER_HANDLE_BYTES = 64
 MRX_MAX_CONTOUR_SEGMENTS = 1 << 30
+MRX_MAX_IOU_THRESHOLDS = 64
 
 
 def contour_scratch_bytes(total_segments):
@@ -70,6 +72,11 @@ SIGNATURES = {
     "mrx_contours_count": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
     "mrx_contours_write": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_longlong, C.c_longlong,
                                 _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "mrx_mask_extents": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
+    "mrx_mask_overlaps": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp,
+                               _i, _vp]),
+    "mrx_mask_matches": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _dp, _i, C.c_double, _vp, _vp,
+                              _vp, _i, _i, _i, _vp]),
     "mrx_device_alloc": (_i, [C.c_ulonglong, C.POINTER(C.c_void_p), _ip]),
     "mrx_device_free": (_i, [_vp, C.c_ulonglong]),
     "mrx_peer_alloc": (_i, [C.c_ulonglong, C.POINTER(C.c_void_p)]),

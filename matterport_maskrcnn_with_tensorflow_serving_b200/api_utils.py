@@ -10,7 +10,8 @@ NumPy value semantics, computed by the sm_90a kernels in libmrx.so.
 Plus batched entry points the reference lacks (it is hard-wired to one image per call,
 serve.py:48): `unmold_detections_batch`, `unmold_detections_packed_batch`,
 `unmold_detections_rle_batch`, `unmold_detections_contours_batch`, `unmold_overlay_batch`,
-and `unmold_coco_results_batch` (upstream's `build_coco_results` of the unmolded detections).
+`unmold_coco_results_batch` (upstream's `build_coco_results` of the unmolded detections) and
+`unmold_compute_ap_batch` (upstream's `compute_ap` of them against ground truth).
 
 Numerical contract (checked by tests/ against the float64 oracle): N, boxes, class ids and
 scores are bit-exact.  The mask resize runs in float32 on exact integer source coordinates;
@@ -371,6 +372,53 @@ def unmold_coco_results_batch(items, image_ids, category_ids=None):
                         "bbox": [x1, y1, x2 - x1, y2 - y1],
                         "score": float(scores[i]),
                         "segmentation": rles[i]})
+    return out
+
+
+def unmold_compute_ap_batch(items, gts, iou_thresholds=(0.5,), score_threshold=0.0):
+    """`unmold_detections` scored against ground truth without the masks leaving the device:
+    for every image b and threshold t, upstream's
+    `compute_ap(*gts[b], *unmold_detections(*items[b]), t)` (Matterport `mrcnn.utils`, with
+    `score_threshold` passed on to its `compute_matches`).  gts[b] = (gt_boxes [M,4],
+    gt_class_ids [M], gt_masks [H,W,M]) in image b's original shape; gt_boxes are `trim_zeros`-ed
+    and the masks and class ids cut to the rows left, as upstream does.  The predicted masks are
+    bit-packed on the device, the ground truth is packed there too, and the IoUs and matches are
+    computed there (`evaluate` has the NumPy drop-ins and states the tie order).  Returns one dict
+    per image: `rois`, `class_ids`, `scores` (as `unmold_detections` returns them), `overlaps`
+    [N, M] (float32, rows in descending score order; float64 zeros when N or M is 0), and
+    `pred_match` [T, N], `gt_match` [T, M] (float64) and `ap` [T] for the T thresholds."""
+    from . import evaluate
+
+    if len(gts) != len(items):
+        raise ValueError(f"{len(items)} items but {len(gts)} ground-truth tuples")
+    if len(items) == 0:
+        return []
+    thresholds = list(iou_thresholds)
+    gt_cls, gt_masks = [], []
+    for boxes, cls, masks in gts:
+        m = evaluate.trim_zeros(np.asarray(boxes)).shape[0]
+        gt_cls.append(np.asarray(cls)[:m])
+        gt_masks.append(np.asarray(masks)[..., :m])
+    with _Staged(items, canvas=False) as st:
+        eng = st.eng
+        eng.enqueue_packed(st.d_det, st.d_msk)
+        gt = eng.ground_truth(gt_cls, gt_masks)
+        d_ov = eng.enqueue_overlaps(gt)
+        d_order, d_pm, d_gm = eng.enqueue_matches(gt, thresholds, score_threshold)
+        counts, metas = st.meta()
+        ov, order, pm, gm = (t.cpu().numpy() for t in (d_ov, d_order, d_pm, d_gm))
+    out = []
+    for b, (rois, class_ids, scores) in enumerate(metas):
+        n, m = int(counts[b]), int(gt.counts[b])
+        pred_match = pm[:, b, :n].astype(np.float64)
+        gt_match = gm[:, b, :m].astype(np.float64)
+        out.append({
+            "rois": rois, "class_ids": class_ids, "scores": scores,
+            "overlaps": ov[b, :n, :m][order[b, :n]] if n and m else np.zeros((n, m)),
+            "pred_match": pred_match, "gt_match": gt_match,
+            "ap": np.array([evaluate.ap_from_matches(pred_match[t], gt_match[t])[0]
+                            for t in range(len(thresholds))]),
+        })
     return out
 
 

@@ -1,0 +1,342 @@
+// overlaps.cu -- scoring predicted masks against ground truth on the packed planes: upstream's
+// compute_overlaps_masks (mask IoU) and the matching loop of compute_matches (mrcnn/utils.py).
+//
+// Input: bit-packed planes as mrx_pack_masks / mrx_mask_expand_packed write them (uint8 [N, H,
+// ceil(W/8)], most significant bit first).  Pixel x of a row is bit 7 - (x & 7) of byte x >> 3 in
+// every plane of an image, so the bytes of two planes line up column for column; only their
+// addresses differ in alignment (a plane is H * ceil(W/8) bytes).
+//
+//   mask_extents_kernel  CTA per plane: popcount area and tight extent inside a region, warps on
+//                        rows, lanes on bytes
+//   mask_overlaps_kernel CTA per (image, prediction), warp per ground-truth instance: a pair whose
+//                        extents do not meet (or with an empty mask) gets its IoU without a read;
+//                        the others AND and popcount the intersection rectangle, four bytes of a
+//                        row per lane, each realigned from aligned words with a funnel shift
+//   mask_rank_kernel     CTA per image: rank of every prediction by score (descending, NaN first,
+//                        ties larger index first), by counting
+//   mask_match_kernel    warp per (image, threshold): predictions in rank order, each takes the
+//                        best unmatched candidate of its class (an argmax over the warp)
+//
+// IoU arithmetic is NumPy's float32 order: i = f32(inter), u = (f32(a1) + f32(a2)) - i, i / u,
+// each rounded once (exact counts; bit-equal to NumPy while H*W <= 2^24).
+#include <climits>
+
+#include "common.cuh"
+
+namespace mrx {
+
+namespace overlaps {
+
+constexpr int kWarps = 8;
+
+struct Planes {
+  Slots<const unsigned char> packed;   // image b: uint8 [R, H_b, wb_b]
+  const int *counts;                   // [B]
+  const long long *areas;              // [B, R]
+  const int4 *extents;                 // [B, R] (y1, x1, y2, x2), exclusive ends
+  int R;
+};
+
+__device__ __forceinline__ const unsigned char *plane_of(const Slots<const unsigned char> &s,
+                                                         int b, int k, int H, int wb) {
+  return s.base + s.off[b] + static_cast<long long>(k) * H * wb;
+}
+
+// ---------------------------------------------------------------- extents
+__global__ void __launch_bounds__(kWarps * 32)
+mask_extents_kernel(Slots<const unsigned char> packed, const int *__restrict__ counts,
+                    const int *__restrict__ geom, const int4 *__restrict__ regions,
+                    long long *__restrict__ areas, int4 *__restrict__ extents, int R) {
+  const int k = blockIdx.x, b = blockIdx.y;
+  if (k >= counts[b]) return;
+  const int H = geom[b * MRX_GEOM_INTS + 0], W = geom[b * MRX_GEOM_INTS + 1];
+  const int wb = (W + 7) >> 3;
+  const int4 r = regions[static_cast<size_t>(b) * R + k];
+  const int y1 = max(r.x, 0), x1 = max(r.y, 0), y2 = min(r.z, H), x2 = min(r.w, W);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  long long area = 0;
+  int ymin = INT_MAX, xmin = INT_MAX, ymax = -1, xmax = -1;
+  if (y2 > y1 && x2 > x1) {
+    const unsigned char *plane = plane_of(packed, b, k, H, wb);
+    const int jb0 = x1 >> 3, jb1 = (x2 - 1) >> 3;
+    for (int y = y1 + warp; y < y2; y += kWarps) {
+      const unsigned char *row = plane + static_cast<long long>(y) * wb;
+      for (int j = jb0 + lane; j <= jb1; j += 32) {
+        // pixels [x1, x2) of byte j: bit 7 - t is pixel 8j + t
+        const int lo = max(x1 - 8 * j, 0), hi = min(x2 - 8 * j, 8);
+        const unsigned v = __ldg(row + j) & (0xFFu >> lo) & (0xFFu << (8 - hi));
+        if (v) {
+          area += __popc(v);
+          ymin = min(ymin, y);
+          ymax = max(ymax, y);
+          xmin = min(xmin, 8 * j + __clz(v) - 24);
+          xmax = max(xmax, 8 * j + 8 - __ffs(v));
+        }
+      }
+    }
+  }
+  area = warp_sum(area);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    ymin = min(ymin, __shfl_xor_sync(0xffffffffu, ymin, o));
+    xmin = min(xmin, __shfl_xor_sync(0xffffffffu, xmin, o));
+    ymax = max(ymax, __shfl_xor_sync(0xffffffffu, ymax, o));
+    xmax = max(xmax, __shfl_xor_sync(0xffffffffu, xmax, o));
+  }
+  __shared__ long long s_area[kWarps];
+  __shared__ int4 s_ext[kWarps];
+  if (lane == 0) {
+    s_area[warp] = area;
+    s_ext[warp] = make_int4(ymin, xmin, ymax, xmax);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    long long a = 0;
+    int4 e = make_int4(INT_MAX, INT_MAX, -1, -1);
+    for (int w = 0; w < kWarps; ++w) {
+      a += s_area[w];
+      e = make_int4(min(e.x, s_ext[w].x), min(e.y, s_ext[w].y), max(e.z, s_ext[w].z),
+                    max(e.w, s_ext[w].w));
+    }
+    const size_t i = static_cast<size_t>(b) * R + k;
+    areas[i] = a;
+    extents[i] = a ? make_int4(e.x, e.y, e.z + 1, e.w + 1) : make_int4(0, 0, 0, 0);
+  }
+}
+
+// ---------------------------------------------------------------- overlaps
+// The n (1..4) bytes at p as a little-endian word (byte p in bits 0-7), the rest zero, from the
+// aligned words that hold them (only those: never a word past the last byte wanted).
+__device__ __forceinline__ uint32_t load_bytes(const unsigned char *p, int n) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p);
+  const uint32_t *w = reinterpret_cast<const uint32_t *>(a & ~static_cast<uintptr_t>(3));
+  const int s = static_cast<int>(a & 3u);
+  const uint32_t lo = __ldg(w);
+  const uint32_t hi = s + n > 4 ? __ldg(w + 1) : 0u;
+  const uint32_t v = __funnelshift_r(lo, hi, 8 * s);
+  return n >= 4 ? v : v & ((1u << (8 * n)) - 1u);
+}
+
+// pixels of rows [y1, y2) x columns [x1, x2) set in both planes, summed over the warp
+__device__ __forceinline__ long long and_count(const unsigned char *p1, const unsigned char *p2,
+                                               int wb, int y1, int x1, int y2, int x2, int lane) {
+  const int jb0 = x1 >> 3, nbytes = ((x2 - 1) >> 3) - jb0 + 1;
+  const int nw = (nbytes + 3) >> 2;
+  // edge bytes: pixels from x1 in the first byte, up to x2 - 1 in the last
+  const uint32_t first = 0xFFu >> (x1 & 7), last = (0xFFu << (7 - ((x2 - 1) & 7))) & 0xFFu;
+  const int total = (y2 - y1) * nw;
+  long long n = 0;
+  for (int e = lane; e < total; e += 32) {
+    const int r = e / nw, c = e - r * nw;
+    const long long o = static_cast<long long>(y1 + r) * wb + jb0 + 4 * c;
+    const int nv = min(4, nbytes - 4 * c);
+    uint32_t m = load_bytes(p1 + o, nv) & load_bytes(p2 + o, nv);
+    if (c == 0) m &= first | 0xFFFFFF00u;
+    if (c == nw - 1) {
+      const int q = 8 * (nv - 1);
+      m &= ~(0xFFu << q) | (last << q);
+    }
+    n += __popc(m);
+  }
+  return warp_sum(n);
+}
+
+__global__ void __launch_bounds__(kWarps * 32)
+mask_overlaps_kernel(const Planes p1, const Planes p2, const int *__restrict__ geom,
+                     float *__restrict__ out) {
+  const int i = blockIdx.x, b = blockIdx.y;
+  const int N = p1.counts[b], M = p2.counts[b];
+  if (i >= N) return;
+  const int H = geom[b * MRX_GEOM_INTS + 0], W = geom[b * MRX_GEOM_INTS + 1];
+  const int wb = (W + 7) >> 3;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const size_t i1 = static_cast<size_t>(b) * p1.R + i;
+  const long long a1 = p1.areas[i1];
+  const int4 e1 = p1.extents[i1];
+  const unsigned char *plane1 = plane_of(p1.packed, b, i, H, wb);
+  float *row = out + i1 * p2.R;
+  for (int j = warp; j < M; j += kWarps) {
+    const size_t i2 = static_cast<size_t>(b) * p2.R + j;
+    const long long a2 = p2.areas[i2];
+    const int4 e2 = p2.extents[i2];
+    const int y1 = max(e1.x, e2.x), x1 = max(e1.y, e2.y), y2 = min(e1.z, e2.z), x2 = min(e1.w, e2.w);
+    long long inter = 0;
+    if (a1 && a2 && y2 > y1 && x2 > x1)
+      inter = and_count(plane1, plane_of(p2.packed, b, j, H, wb), wb, y1, x1, y2, x2, lane);
+    if (lane == 0) {
+      const float fi = __ll2float_rn(inter);
+      const float u = __fsub_rn(__fadd_rn(__ll2float_rn(a1), __ll2float_rn(a2)), fi);
+      row[j] = __fdiv_rn(fi, u);   // 0 / 0 = NaN: both masks empty
+    }
+  }
+}
+
+// ---------------------------------------------------------------- ranks and matches
+struct MatchParams {
+  const float *overlaps;      // [B, R1, R2]
+  const int *pred_counts;     // [B]
+  const int *pred_class;      // [B, R1]
+  const void *scores;         // [B, R1] f32 / f64
+  const int *gt_counts;       // [B]
+  const int *gt_class;        // [B, R2]
+  int *order;                 // [B, R1]
+  int *pred_match;            // [T, B, R1]
+  int *gt_match;              // [T, B, R2]
+  int B, R1, R2, score_f64;
+  double score_threshold;
+  double thresholds[MRX_MAX_IOU_THRESHOLDS];
+};
+
+__device__ __forceinline__ double score_at(const MatchParams &p, size_t i) {
+  return p.score_f64 ? static_cast<const double *>(p.scores)[i]
+                     : static_cast<double>(static_cast<const float *>(p.scores)[i]);
+}
+
+// rank of prediction i = the predictions before it: higher score, NaN above every number, equal
+// scores by larger index (np.argsort(kind="stable")[::-1])
+__global__ void __launch_bounds__(256) mask_rank_kernel(const MatchParams p) {
+  const int b = blockIdx.x;
+  const int N = p.pred_counts[b];
+  const size_t base = static_cast<size_t>(b) * p.R1;
+  for (int i = threadIdx.x; i < N; i += blockDim.x) {
+    const double si = score_at(p, base + i);
+    const bool ni = isnan(si);
+    int rank = 0;
+    for (int k = 0; k < N; ++k) {
+      const double sk = score_at(p, base + k);
+      const bool nk = isnan(sk);
+      const bool tie = (nk && ni) || sk == si;
+      rank += (nk && !ni) || (!nk && !ni && sk > si) || (tie && k > i);
+    }
+    p.order[base + rank] = i;
+  }
+}
+
+// Prediction i (rank order) matches the first ground-truth instance j of np.argsort(overlaps[i])
+// reversed (stable: NaN first, ties larger j first) that is unmatched, of i's class, and whose IoU
+// is NaN or at least both thresholds.  Lane j % 32 owns gt_match[j].
+__global__ void __launch_bounds__(32) mask_match_kernel(const MatchParams p) {
+  const int b = blockIdx.x, t = blockIdx.y, lane = threadIdx.x;
+  const int N = p.pred_counts[b], M = p.gt_counts[b];
+  const double thr = p.thresholds[t], sthr = p.score_threshold;
+  int *gm = p.gt_match + (static_cast<size_t>(t) * p.B + b) * p.R2;
+  int *pm = p.pred_match + (static_cast<size_t>(t) * p.B + b) * p.R1;
+  const int *gcls = p.gt_class + static_cast<size_t>(b) * p.R2;
+  for (int j = lane; j < M; j += 32) gm[j] = -1;
+  for (int r = 0; r < N; ++r) {
+    const int i = p.order[static_cast<size_t>(b) * p.R1 + r];
+    const int ci = p.pred_class[static_cast<size_t>(b) * p.R1 + i];
+    const float *row = p.overlaps + (static_cast<size_t>(b) * p.R1 + i) * p.R2;
+    // key: 2 = NaN above 1 = a number (its bits order like its value, IoU >= +0), then j
+    unsigned long long best = 0ull;
+    for (int j = lane; j < M; j += 32) {
+      if (gm[j] != -1 || gcls[j] != ci) continue;
+      const float v = row[j];
+      unsigned long long key = 0ull;
+      if (isnan(v))
+        key = (2ull << 62) | static_cast<unsigned>(j);
+      else if (static_cast<double>(v) >= thr && static_cast<double>(v) >= sthr)
+        key = (1ull << 62) | (static_cast<unsigned long long>(__float_as_uint(v)) << 16) |
+              static_cast<unsigned>(j);
+      best = key > best ? key : best;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long x = __shfl_xor_sync(0xffffffffu, best, o);
+      best = x > best ? x : best;
+    }
+    const int j = best ? static_cast<int>(best & 0xFFFFu) : -1;
+    if (j >= 0 && lane == (j & 31)) gm[j] = r;
+    if (lane == 0) pm[r] = j;
+  }
+}
+
+}  // namespace overlaps
+
+}  // namespace mrx
+
+using namespace mrx;
+
+extern "C" int mrx_mask_extents(const unsigned char *d_packed, const long long *d_packed_off,
+                                const int *d_counts, const int *d_geom, const int *d_regions,
+                                long long *d_areas, int *d_extents, int B, int R, void *stream) {
+  const char *fn = "mrx_mask_extents";
+  if (int rc = check_slots(fn, d_packed, d_packed_off, d_counts, d_geom, B, R)) return rc;
+  MRX_CHECK_ARG(d_regions, "%s: the region argument d_regions is required", fn);
+  MRX_CHECK_ARG(d_areas && d_extents, "%s: null pointer", fn);
+  if (B == 0) return MRX_OK;
+  overlaps::mask_extents_kernel<<<dim3(R, B), overlaps::kWarps * 32, 0,
+                                  static_cast<cudaStream_t>(stream)>>>(
+      {d_packed, d_packed_off}, d_counts, d_geom, reinterpret_cast<const int4 *>(d_regions),
+      d_areas, reinterpret_cast<int4 *>(d_extents), R);
+  MRX_LAUNCH_CHECK("mask_extents_kernel");
+  return MRX_OK;
+}
+
+extern "C" int mrx_mask_overlaps(const unsigned char *d_packed1, const long long *d_packed_off1,
+                                 const int *d_counts1, const long long *d_areas1,
+                                 const int *d_extents1, int R1,
+                                 const unsigned char *d_packed2, const long long *d_packed_off2,
+                                 const int *d_counts2, const long long *d_areas2,
+                                 const int *d_extents2, int R2, const int *d_geom,
+                                 float *d_overlaps, int B, void *stream) {
+  const char *fn = "mrx_mask_overlaps";
+  if (int rc = check_slots(fn, d_packed1, d_packed_off1, d_counts1, d_geom, B, R1)) return rc;
+  if (int rc = check_slots(fn, d_packed2, d_packed_off2, d_counts2, d_geom, B, R2)) return rc;
+  MRX_CHECK_ARG(d_areas1 && d_extents1 && d_areas2 && d_extents2, "%s: null areas or extents", fn);
+  MRX_CHECK_ARG(d_overlaps, "%s: null pointer", fn);
+  MRX_CHECK_ARG(((reinterpret_cast<uintptr_t>(d_packed1) | reinterpret_cast<uintptr_t>(d_packed2)) &
+                 3u) == 0u,
+                "%s: packed bases must be 4-byte aligned", fn);
+  if (B == 0) return MRX_OK;
+  const overlaps::Planes p1{{d_packed1, d_packed_off1}, d_counts1, d_areas1,
+                            reinterpret_cast<const int4 *>(d_extents1), R1};
+  const overlaps::Planes p2{{d_packed2, d_packed_off2}, d_counts2, d_areas2,
+                            reinterpret_cast<const int4 *>(d_extents2), R2};
+  overlaps::mask_overlaps_kernel<<<dim3(R1, B), overlaps::kWarps * 32, 0,
+                                   static_cast<cudaStream_t>(stream)>>>(p1, p2, d_geom, d_overlaps);
+  MRX_LAUNCH_CHECK("mask_overlaps_kernel");
+  return MRX_OK;
+}
+
+extern "C" int mrx_mask_matches(const float *d_overlaps, const int *d_pred_counts,
+                                const int *d_pred_class_ids, const void *d_scores, int score_dtype,
+                                const int *d_gt_counts, const int *d_gt_class_ids,
+                                const double *thresholds, int T, double score_threshold,
+                                int *d_order, int *d_pred_match, int *d_gt_match, int B, int R1,
+                                int R2, void *stream) {
+  const char *fn = "mrx_mask_matches";
+  MRX_CHECK_ARG(d_overlaps && d_pred_counts && d_pred_class_ids && d_scores && d_gt_counts &&
+                    d_gt_class_ids && thresholds && d_order && d_pred_match && d_gt_match,
+                "%s: null pointer", fn);
+  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH, "%s: bad B %d (need 0<=B<=%d)", fn, B, MRX_MAX_BATCH);
+  MRX_CHECK_ARG(R1 >= 1 && R1 <= 65534 && R2 >= 1 && R2 <= 65534,
+                "%s: bad R1 %d / R2 %d (need 1<=R<=65534)", fn, R1, R2);
+  MRX_CHECK_ARG(T >= 1 && T <= MRX_MAX_IOU_THRESHOLDS, "%s: bad T %d (need 1<=T<=%d)", fn, T,
+                MRX_MAX_IOU_THRESHOLDS);
+  MRX_CHECK_ARG(score_dtype == MRX_F32 || score_dtype == MRX_F64, "%s: bad score dtype %d", fn,
+                score_dtype);
+  if (B == 0) return MRX_OK;
+  overlaps::MatchParams p{};
+  p.overlaps = d_overlaps;
+  p.pred_counts = d_pred_counts;
+  p.pred_class = d_pred_class_ids;
+  p.scores = d_scores;
+  p.gt_counts = d_gt_counts;
+  p.gt_class = d_gt_class_ids;
+  p.order = d_order;
+  p.pred_match = d_pred_match;
+  p.gt_match = d_gt_match;
+  p.B = B;
+  p.R1 = R1;
+  p.R2 = R2;
+  p.score_f64 = score_dtype == MRX_F64;
+  p.score_threshold = score_threshold;
+  for (int t = 0; t < T; ++t) p.thresholds[t] = thresholds[t];
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  overlaps::mask_rank_kernel<<<B, 256, 0, st>>>(p);
+  MRX_LAUNCH_CHECK("mask_rank_kernel");
+  overlaps::mask_match_kernel<<<dim3(B, T), 32, 0, st>>>(p);
+  MRX_LAUNCH_CHECK("mask_match_kernel");
+  return MRX_OK;
+}

@@ -5,6 +5,8 @@ every computation on the path is a libmrx kernel launched through ctypes.
 
   UnmoldEngine     batched `unmold_detections` (serve.py:147-154): prologue -> class-tile
                    gather -> fused mask expand, all stream-ordered, no host sync
+  MaskBatch        caller-held masks (ground truth) as packed planes, scored against an
+                   engine's masks by `mask_overlaps` / `mask_matches`
   AnchorGenerator  `get_anchors` (serve.py:105)
   Molder           the body of `preprocess_input` (serve.py:83-107): cv2.resize + resize_image
                    + mold_image
@@ -14,6 +16,7 @@ from __future__ import annotations
 import ctypes as C
 import threading
 import weakref
+from typing import NamedTuple
 
 import numpy as np
 
@@ -167,16 +170,20 @@ class UnmoldEngine:
         self._packed_off_layout = None  # the layout whose packed offsets d_packed_off holds
         self.layout = None              # BatchLayout of the planned batch
         self._contour_bufs = {}     # work and output buffers of trace_contours, grown as needed
+        self._eval_bufs = {}        # prediction areas and extents of enqueue_overlaps
+        self._overlaps = None       # (ground truth, overlaps) of the last enqueue_overlaps
         self.lock = threading.RLock()
         # pinned staging for fetch_meta (one D2H batch + one synchronisation per call)
         self._h_meta = None
 
     def release(self):
-        """Free the canvas, the packed-output and the contour buffers (the work buffers stay)."""
+        """Free the canvas, the packed-output, contour and overlap buffers (the work buffers stay)."""
         with self.lock:
             self.d_canvas = None
             self.d_packed = None
             self._contour_bufs = {}
+            self._eval_bufs = {}
+            self._overlaps = None
             self.layout = None
 
     # read-only views of the planned layout (the benchmark, tools and tests read them)
@@ -412,6 +419,50 @@ class UnmoldEngine:
             verts, coff = _download_contours(d_vert, d_coff)
         return contours_to_lists(verts, coff, icoff, counts, self.layout)
 
+    # ------------------------------------------------------------------ scoring against ground truth
+    def ground_truth(self, class_ids, masks, stream=None):
+        """A `MaskBatch` of ground truth for the planned images: class_ids[b] [M_b] and bool
+        masks[b] [H_b, W_b, M_b] in the plan's image shapes."""
+        if self.layout is None:
+            raise RuntimeError("plan() first")
+        return MaskBatch(self.lib, self.device, self.layout.geom, class_ids, masks, stream)
+
+    def enqueue_overlaps(self, gt, stream=None):
+        """EXTENSION: upstream `compute_overlaps_masks(pred_masks, gt_masks)` of every planned image
+        against `gt` (a `MaskBatch` from `ground_truth`), on the packed planes (after
+        `enqueue_expand_packed` or `pack_masks`); each prediction is read only inside its box.
+        Returns the float32 device tensor [n, R, gt.R]: element (b, i, j) for i < N_b, j < M_b is
+        the IoU of kept instance i and ground-truth instance j."""
+        if self.layout is None or self.d_packed is None:
+            raise RuntimeError("enqueue_overlaps needs the packed planes: call "
+                               "enqueue_expand_packed or pack_masks first")
+        n = self._n_images
+        if gt.n != n or not np.array_equal(gt.geom, self.layout.geom):
+            raise ValueError("the ground truth was staged for another plan")
+        torch = _torch()
+        bufs = self._eval_bufs
+        d_areas = _buffer(bufs, "areas", n * self.R, torch.int64, self.device)
+        d_ext = _buffer(bufs, "extents", n * self.R * 4, torch.int32, self.device)
+        N.check(self.lib.mrx_mask_extents(
+            _ptr(self.d_packed), _ptr(self.d_packed_off), _ptr(self.d_counts), _ptr(self.d_geom),
+            _ptr(self.d_boxes), _ptr(d_areas), _ptr(d_ext), n, self.R, N.stream_ptr(stream)),
+            "mrx_mask_extents")
+        pred = Planes(self.d_packed, self.d_packed_off, self.d_counts, d_areas, d_ext, self.R)
+        self._overlaps = (gt, mask_overlaps(self.lib, pred, gt.planes, self.d_geom, n, stream))
+        return self._overlaps[1]
+
+    def enqueue_matches(self, gt, thresholds, score_threshold=0.0, stream=None):
+        """EXTENSION: the matching of upstream `compute_matches` for each IoU threshold, on the
+        overlaps of the last `enqueue_overlaps(gt)`.  Thresholds compare as upstream's do
+        (`comparison_threshold`).  Returns device tensors (order [n, R]: rank -> kept instance,
+        by score; pred_match [T, n, R] by rank: gt index or -1; gt_match [T, n, gt.R]: rank or
+        -1)."""
+        last = self._overlaps
+        if last is None or last[0] is not gt:
+            raise RuntimeError("enqueue_overlaps(gt) first")
+        return mask_matches(self.lib, last[1], self.d_counts, self.d_class_ids, self.d_scores,
+                            _dtype_code(self.det_dtype), gt, thresholds, score_threshold, stream)
+
     def pack_masks(self, stream=None):
         """EXTENSION: bit-pack the byte canvases already written for the planned batch
         (mrx_pack_masks; same output layout as `enqueue_expand_packed`).  Returns
@@ -484,6 +535,134 @@ def _buffer(bufs, name, numel, dtype, device):
         bufs[name] = None
         t = bufs[name] = _torch().empty((max(int(numel), 1),), dtype=dtype, device=device)
     return t
+
+
+class Planes(NamedTuple):
+    """One side of `mask_overlaps`: packed slots (d_packed, d_packed_off), counts [n], areas
+    [n, R] int64 and extents [n, R, 4] int32 of mrx_mask_extents, and the slot's R."""
+    d_packed: object
+    d_packed_off: object
+    d_counts: object
+    d_areas: object
+    d_extents: object
+    R: int
+
+
+class MaskBatch:
+    """Caller-held masks of a batch on the device as packed planes, with their areas, extents
+    and class ids: class_ids[b] [M_b] and masks[b] [H_b, W_b, M_b] (bool, or thresholded `> .5`
+    as upstream's compute_overlaps_masks does) for the images of `geoms` ([n, 8], see make_geom).
+    Each image's bytes pass through one staging canvas sized for the largest image and are packed
+    into its slot by mrx_pack_masks, so device memory holds one image's bytes plus the packed
+    planes.  M_b above what mrx_pack_masks takes raises ValueError."""
+
+    def __init__(self, lib, device, geoms, class_ids, masks, stream=None):
+        torch = _torch()
+        g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
+        n = self.n = g.shape[0]
+        if len(masks) != n or len(class_ids) != n:
+            raise ValueError(f"{len(masks)} masks and {len(class_ids)} class-id arrays for "
+                             f"{n} images")
+        staged, counts = [], np.zeros(n, dtype=np.int32)
+        for b, (cls, m) in enumerate(zip(class_ids, masks)):
+            m = np.asarray(m)
+            H, W = int(g[b, 0]), int(g[b, 1])
+            if m.ndim != 3 or m.shape[:2] != (H, W):
+                raise ValueError(f"image {b}: masks must be [{H}, {W}, M], got {m.shape}")
+            if np.shape(cls) != (m.shape[2],):
+                raise ValueError(f"image {b}: {np.shape(cls)} class ids for {m.shape[2]} masks")
+            m = m if m.dtype == np.bool_ else m > .5
+            staged.append(np.ascontiguousarray(m).view(np.uint8))
+            counts[b] = m.shape[2]
+        self.R = R = max(int(counts.max(initial=0)), 1)
+        layout = BatchLayout(g, R, limits=False)
+        self.geom, self.counts = layout.geom, counts
+        cls = np.zeros((n, R), dtype=np.int32)
+        for b, c in enumerate(class_ids):
+            c = np.asarray(c)
+            if c.size and (c.astype(np.int32) != c).any():
+                raise ValueError(f"image {b}: class ids must be integers within int32")
+            cls[b, :c.size] = c
+        st = N.stream_ptr(stream)
+        with _stream_ctx(stream):
+            self.d_geom = torch.from_numpy(layout.geom).to(device)
+            self.d_counts = torch.from_numpy(counts).to(device)
+            self.d_class_ids = torch.from_numpy(cls).to(device)
+            d_off = torch.from_numpy(layout.packed_off[:-1].copy()).to(device)
+            d_packed = torch.empty((max(int(layout.packed_off[-1]), 1),), dtype=torch.uint8,
+                                   device=device)
+            canvas = torch.empty((max(max(s.size for s in staged), 1) + 15) // 16 * 16,
+                                 dtype=torch.uint8, device=device)
+            d_zero = torch.zeros((1,), dtype=torch.int64, device=device)
+            for b, s in enumerate(staged):
+                if s.size == 0:
+                    continue
+                canvas[:s.size].copy_(torch.from_numpy(s.reshape(-1)))
+                H, W = layout.hw(b)
+                rc = lib.mrx_pack_masks(_ptr(canvas), _ptr(d_zero), _ptr(self.d_counts[b:]),
+                                        _ptr(self.d_geom[b:]), _ptr(d_packed), _ptr(d_off[b:]),
+                                        1, R, H, W, st)
+                if rc == N.MRX_E_UNSUPPORTED:
+                    raise ValueError(lib.mrx_last_error().decode())
+                N.check(rc, "mrx_pack_masks")
+            del canvas
+            regions = np.zeros((n, R, 4), dtype=np.int32)
+            regions[:, :, 2:] = layout.geom[:, None, :2]
+            d_regions = torch.from_numpy(regions).to(device)
+            d_areas = torch.empty((n, R), dtype=torch.int64, device=device)
+            d_ext = torch.empty((n, R, 4), dtype=torch.int32, device=device)
+            N.check(lib.mrx_mask_extents(_ptr(d_packed), _ptr(d_off), _ptr(self.d_counts),
+                                         _ptr(self.d_geom), _ptr(d_regions), _ptr(d_areas),
+                                         _ptr(d_ext), n, R, st), "mrx_mask_extents")
+        self.planes = Planes(d_packed, d_off, self.d_counts, d_areas, d_ext, R)
+
+
+def mask_overlaps(lib, p1, p2, d_geom, n, stream=None):
+    """mrx_mask_overlaps of two `Planes` of the same n images (d_geom [n, 8]): float32 device
+    tensor [n, p1.R, p2.R], element (b, i, j) the IoU of mask i of p1 and mask j of p2 for i, j
+    below the image's counts (the rest is not written)."""
+    d_out = _torch().empty((n, p1.R, p2.R), dtype=_torch().float32, device=d_geom.device)
+    N.check(lib.mrx_mask_overlaps(
+        _ptr(p1.d_packed), _ptr(p1.d_packed_off), _ptr(p1.d_counts), _ptr(p1.d_areas),
+        _ptr(p1.d_extents), p1.R, _ptr(p2.d_packed), _ptr(p2.d_packed_off), _ptr(p2.d_counts),
+        _ptr(p2.d_areas), _ptr(p2.d_extents), p2.R, _ptr(d_geom), _ptr(d_out), n,
+        N.stream_ptr(stream)), "mrx_mask_overlaps")
+    return d_out
+
+
+def comparison_threshold(t):
+    """The float64 value compute_matches effectively compares its float32 IoUs with: NumPy (NEP 50)
+    compares a Python float or int weakly, in float32, and a NumPy scalar strongly, in float64
+    (`float32(0.7) < 0.7` is False, `float32(0.7) < np.float64(0.7)` is True)."""
+    if isinstance(t, (np.generic, np.ndarray)):
+        return float(t)
+    if isinstance(t, (int, float)):
+        return float(np.float32(t))
+    raise TypeError(f"threshold must be a Python or NumPy real number, got {type(t).__name__}")
+
+
+def mask_matches(lib, d_overlaps, d_pred_counts, d_pred_class_ids, d_scores, score_code, gt,
+                 thresholds, score_threshold=0.0, stream=None):
+    """mrx_mask_matches on overlaps [n, R1, gt.R] (see `mask_overlaps`), thresholds in launches of
+    at most MRX_MAX_IOU_THRESHOLDS.  Returns device tensors (order [n, R1], pred_match
+    [T, n, R1], gt_match [T, n, gt.R]) int32."""
+    torch = _torch()
+    n, R1, R2 = (int(v) for v in d_overlaps.shape)
+    thr = [comparison_threshold(t) for t in thresholds]
+    if not thr:
+        raise ValueError("no IoU threshold given")
+    dev = d_overlaps.device
+    d_order = torch.empty((n, R1), dtype=torch.int32, device=dev)
+    d_pm = torch.empty((len(thr), n, R1), dtype=torch.int32, device=dev)
+    d_gm = torch.empty((len(thr), n, R2), dtype=torch.int32, device=dev)
+    for t0 in range(0, len(thr), N.MRX_MAX_IOU_THRESHOLDS):
+        chunk = thr[t0:t0 + N.MRX_MAX_IOU_THRESHOLDS]
+        N.check(lib.mrx_mask_matches(
+            _ptr(d_overlaps), _ptr(d_pred_counts), _ptr(d_pred_class_ids), _ptr(d_scores),
+            score_code, _ptr(gt.d_counts), _ptr(gt.d_class_ids), N.double_array(chunk), len(chunk),
+            C.c_double(comparison_threshold(score_threshold)), _ptr(d_order), _ptr(d_pm[t0]),
+            _ptr(d_gm[t0]), n, R1, R2, N.stream_ptr(stream)), "mrx_mask_matches")
+    return d_order, d_pm, d_gm
 
 
 def trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom, d_regions, layout,

@@ -107,6 +107,33 @@ def make_batch(seed, batch, orig_hw, n_valid, num_classes=81, max_instances=100,
     return out
 
 
+def jitter_ground_truth(im, rng, max_shift=8, class_flip_frac=0.1):
+    """The same synthetic image with every valid box moved by up to `max_shift` molded-image
+    pixels in y and in x (kept inside the window) and about `class_flip_frac` of the class ids
+    changed: unmolded, its masks overlap the original's with IoUs spread over (0, 1], which makes
+    ground truth with real matches and misses."""
+    det = im.detections.copy()
+    n = im.n_valid
+    if n:
+        shape = im.image_shape[:2]
+        h, w = shape
+        scale = np.array([h - 1, w - 1, h - 1, w - 1], dtype=np.float64)
+        shift = np.array([0, 0, 1, 1], dtype=np.float64)
+        px = np.around(det[:n, :4].astype(np.float64) * scale + shift)
+        wy1, wx1, wy2, wx2 = im.window
+        d = rng.integers(-max_shift, max_shift + 1, size=(n, 2))
+        px[:, [0, 2]] += d[:, :1]
+        px[:, [1, 3]] += d[:, 1:]
+        px[:, [0, 2]] = np.clip(px[:, [0, 2]], wy1, wy2)
+        px[:, [1, 3]] = np.clip(px[:, [1, 3]], wx1, wx2)
+        det[:n, :4] = _norm_boxes_f32(px, shape)
+        flip = rng.random(n) < class_flip_frac
+        C = im.mrcnn_mask.shape[-1]
+        det[:n, 4][flip] = (det[:n, 4][flip] + rng.integers(1, max(C - 1, 2), size=int(flip.sum()))
+                            - 1) % max(C - 1, 1) + 1
+    return SynthImage(det, im.mrcnn_mask, im.original_image_shape, im.image_shape, im.window, n)
+
+
 def synth_rgb_image(rng, h, w):
     """uint8 RGB image with smooth structure + noise (for the mold step)."""
     yy, xx = np.mgrid[0:h, 0:w]

@@ -149,6 +149,83 @@ def rle_strings_record(eng, d_runs, off, masks, iters):
             "string_over_runs": round(str_bytes / run_bytes, 4)}
 
 
+def eval_case(iters, cpu):
+    """configs[1] batch scored against ground truth: 32 x 1024x1024, 100 predictions against the
+    100 instances of the same image jittered (synth.jitter_ground_truth).  The three kernels
+    alone, and unmold_compute_ap_batch end to end (gt upload included) for one and for the ten
+    thresholds of compute_ap_range; --cpu: the oracle's compute_overlaps_masks per image."""
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils
+    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import mask_matches
+
+    batch, base_n = 32, 4
+    base = synth.make_batch(7, base_n, (1024, 1024), 100)
+    rng = np.random.default_rng(8)
+    base_gt = api_utils.unmold_detections_batch(
+        [(j.detections, j.mrcnn_mask, j.original_image_shape, j.image_shape, j.window)
+         for j in (synth.jitter_ground_truth(im, rng, 12, 0.1) for im in base)])
+    ims = [base[i % base_n] for i in range(batch)]
+    gts = [(g[0], g[1], g[3]) for g in (base_gt[i % base_n] for i in range(batch))]
+    items = [(im.detections, im.mrcnn_mask, im.original_image_shape, im.image_shape, im.window)
+             for im in ims]
+    eng = UnmoldEngine(batch, 100, (28, 28), 81)
+    eng.plan([make_geom(im.original_image_shape, im.image_shape, im.window) for im in ims], canvas=False)
+    d_det = torch.from_numpy(np.stack([im.detections for im in ims])).cuda()
+    d_msk = torch.from_numpy(np.stack([im.mrcnn_mask for im in ims])).cuda()
+    eng.enqueue_packed(d_det, d_msk)
+    gt = eng.ground_truth([g[1] for g in gts], [g[2] for g in gts])
+    d_ov = eng.enqueue_overlaps(gt)
+    lib, n, R = eng.lib, batch, eng.R
+    area_buf, ext_buf = eng._eval_bufs["areas"], eng._eval_bufs["extents"]
+
+    def extents():
+        N.check(lib.mrx_mask_extents(*(C.c_void_p(t.data_ptr()) for t in (
+            eng.d_packed, eng.d_packed_off, eng.d_counts, eng.d_geom, eng.d_boxes, area_buf,
+            ext_buf)), n, R, N.stream_ptr(None)), "mrx_mask_extents")
+
+    ext_ms, _ = time_ms(extents, iters)
+    ov_ms, _ = time_ms(lambda: eng.enqueue_overlaps(gt), iters)
+    m1_ms, _ = time_ms(lambda: mask_matches(lib, d_ov, eng.d_counts, eng.d_class_ids, eng.d_scores,
+                                            N.MRX_F32, gt, [0.5]), iters)
+    thr10 = np.arange(0.5, 1.0, 0.05)
+    m10_ms, _ = time_ms(lambda: mask_matches(lib, d_ov, eng.d_counts, eng.d_class_ids, eng.d_scores,
+                                             N.MRX_F32, gt, thr10), iters)
+    counts = eng.d_counts[:n].cpu().numpy()
+    ov = d_ov.cpu().numpy()
+    pairs = int(sum(int(counts[b]) * int(gt.counts[b]) for b in range(n)))
+    nonzero = int(sum(int((ov[b, :counts[b], :gt.counts[b]] > 0).sum()) for b in range(n)))
+    packed_pred = int(eng.packed_layout()[1])
+    e2e = {}
+    for name, thr in [("1", (0.5,)), ("10", thr10)]:
+        t0 = time.perf_counter()
+        reps = max(2, iters // 8)
+        for _ in range(reps):
+            res = api_utils.unmold_compute_ap_batch(items, gts, thr)
+        e2e[name] = (time.perf_counter() - t0) / reps * 1e3
+    matches = int(sum((r["pred_match"][0] > -1).sum() for r in res))
+    rec = {"workload": "configs[1] 32 x 1024x1024 x 100 predictions vs 100 jittered gt -> mask IoU, "
+                       "matches, AP", "pairs": pairs, "pairs_with_overlap": nonzero,
+           "matches_at_0.5": matches,
+           "pred_packed_MB": round(packed_pred / 1e6, 1),
+           "gt_packed_MB": round(int(gt.planes.d_packed.numel()) / 1e6, 1),
+           "extents_kernel_ms": round(ext_ms, 4), "overlaps_ms_incl_pred_extents": round(ov_ms, 4),
+           "matches_kernel_ms_1_threshold": round(m1_ms, 4),
+           "matches_kernel_ms_10_thresholds": round(m10_ms, 4),
+           "unmold_compute_ap_batch_ms_1_threshold": round(e2e["1"], 1),
+           "unmold_compute_ap_batch_ms_10_thresholds": round(e2e["10"], 1),
+           "note": "end to end: H2D of the inputs and of the bool gt masks (105 MB per image), "
+                   "unmold, pack, scoring, downloads and the host AP tail", **card()}
+    if cpu:
+        sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+        import eval_oracle
+        masks = api_utils.unmold_detections_batch(items[:1])[0][3]
+        t0 = time.perf_counter()
+        eval_oracle.compute_overlaps_masks(masks, gts[0][2])
+        rec["cpu_oracle_compute_overlaps_masks_ms_per_image"] = round((time.perf_counter() - t0) * 1e3, 1)
+    print(json.dumps(rec), flush=True)
+    del eng, d_det, d_msk, gt, d_ov
+    torch.cuda.empty_cache()
+
+
 def anchors_sweep(iters, cpu):
     import oracle
     gen = AnchorGenerator(MaskRCNNServingConfig)
@@ -199,8 +276,12 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--cpu", action="store_true")
+    ap.add_argument("--only-eval", action="store_true", help="only the mask IoU / AP record")
     args = ap.parse_args()
     torch.cuda.set_device(0)
+    eval_case(args.iters, args.cpu)
+    if args.only_eval:
+        return
     unmold_case("configs[1] 32 x 1024x1024 x 100", 32, (1024, 1024), 100, 81, 100, args.iters, composite=True)
     unmold_case("configs[2] 64 x 800x1333 (HxW) x U{1..100}", 64, (800, 1333), (1, 100), 81, 100,
                 args.iters, base_images=16)
