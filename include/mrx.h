@@ -20,6 +20,7 @@
  *   mrx_contours_count / _write <- visualize.display_instances (contour polygons) serve.py:160-169
  *   mrx_mask_extents / _overlaps / _matches (extension: mrcnn.utils.compute_overlaps_masks and
  *                             compute_matches, scoring the masks against ground truth)
+ *   mrx_rle_parse / _decode (extension: ground truth given as COCO RLE, decoded to packed planes)
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
  *   mrx_device_alloc/_free (the canvas allocation: compressible device memory where offered)
  *
@@ -42,7 +43,7 @@
 extern "C" {
 #endif
 
-#define MRX_ABI_VERSION 10
+#define MRX_ABI_VERSION 11
 
 #define MRX_OK              0
 #define MRX_E_INVALID      -1   /* bad argument (null pointer, size out of range) */
@@ -135,7 +136,8 @@ int mrx_unmold_prepare(const void *d_detections, int det_dtype, const void *d_mr
 /* Output slots: where the masks of a planned batch live (engine.BatchLayout states the same on
  * the host), for every entry point that writes or reads them (mrx_mask_expand,
  * mrx_mask_expand_values, mrx_mask_expand_packed, mrx_pack_masks, mrx_composite_masks,
- * mrx_contours_count, mrx_contours_write, mrx_mask_extents, mrx_mask_overlaps).  N_b = d_counts[b], H_b, W_b = d_geom[b][0], [1].
+ * mrx_contours_count, mrx_contours_write, mrx_mask_extents, mrx_mask_overlaps, mrx_rle_decode).
+ * N_b = d_counts[b], H_b, W_b = d_geom[b][0], [1].
  *   Canvas slots: image b's bool masks [H_b, W_b, N_b] (N innermost, 1 byte per element, values
  *     0/1) at d_canvas + d_canvas_off[b] (int64, each a multiple of 16).  Slot b holds at least
  *     round_up(H_b*W_b*N_b, 16) bytes; bytes past H_b*W_b*N_b may be read, and written by the
@@ -372,6 +374,42 @@ int mrx_mask_matches(const float *d_overlaps, const int *d_pred_counts,
                      const int *d_gt_counts, const int *d_gt_class_ids, const double *thresholds,
                      int T, double score_threshold, int *d_order, int *d_pred_match,
                      int *d_gt_match, int B, int R1, int R2, void *stream);
+
+/* ---------------------------------------------------------------- COCO RLE to packed planes */
+/* EXTENSION: the inverse of mrx_rle_strings / mrx_rle_write, for ground truth held as COCO RLE
+ * (pycocotools' compressed strings or uncompressed count lists; rle_decode.cu).  Instance
+ * i = b*R + k for k < N_b = d_counts[b]; others are not read or written.
+ *
+ * mrx_rle_parse: the "counts" strings of mask.encode, instance i's at
+ *   d_str[d_str_off[i] .. d_str_off[i+1]) (d_str_off [B*R+1] int64), in the format of
+ *   mrx_rle_strings.  A string of L characters holds at most L runs: they go to
+ *   d_runs + d_str_off[i] (uint32), their number to d_run_count[i], and the instance's status
+ *   word (MRX_RLE_ST_* bits of CHAR, TRUNC, RANGE) to d_status[i].  An instance with an empty
+ *   string is left alone (its runs, count and status are the caller's: how a batch mixes strings
+ *   with uploaded count lists).
+ * mrx_rle_decode: instance i's d_run_count[i] runs (column-major, starting with zeros) at
+ *   d_runs + d_run_off[i] (d_run_off [B*R] int64) into the packed slots (see "Output slots"):
+ *   every byte of planes k < N_b, pad bits included, is written, so no memset is needed.
+ *   d_run_end: int64 scratch indexed like d_runs (the run ends).  d_status [B*R]: as
+ *   mrx_rle_parse left it (or zeroed by the caller); MRX_RLE_ST_SUM is added when the runs do not
+ *   sum to H_b*W_b.  The plane of an instance with any status bit is unspecified; whatever its
+ *   runs say, nothing outside that plane is written.  max_h, max_w: the extents of
+ *   "Output slots", at least 1.
+ * Checks: mrx_rle_parse: null pointers, B outside [0, MRX_MAX_BATCH] or R outside [1, 65534]:
+ * MRX_E_INVALID.  mrx_rle_decode: those of "Output slots", then null pointers and the extents.
+ * B = 0 returns MRX_OK without launching anything.  Areas and extents: mrx_mask_extents with the
+ * whole image as region. */
+#define MRX_RLE_ST_CHAR   1   /* a character outside '0' .. '0' + 63 */
+#define MRX_RLE_ST_TRUNC  2   /* the string ends inside a value */
+#define MRX_RLE_ST_RANGE  4   /* a count negative or above 2^32 - 1 (or a value of > 7 groups) */
+#define MRX_RLE_ST_SUM    8   /* the counts do not sum to H*W */
+int mrx_rle_parse(const unsigned char *d_str, const long long *d_str_off, const int *d_counts,
+                  unsigned int *d_runs, int *d_run_count, int *d_status, int B, int R,
+                  void *stream);
+int mrx_rle_decode(const unsigned int *d_runs, const long long *d_run_off, const int *d_run_count,
+                   long long *d_run_end, int *d_status, const int *d_counts, const int *d_geom,
+                   const long long *d_packed_off, unsigned char *d_packed, int B, int R,
+                   int max_h, int max_w, void *stream);
 
 /* ---------------------------------------------------------------- multi-GPU gather (8e) */
 /* Peer-memory plumbing for the final gather of the canvases to rank 0 (one process per GPU).

@@ -386,7 +386,17 @@ def unmold_compute_ap_batch(items, gts, iou_thresholds=(0.5,), score_threshold=0
     computed there (`evaluate` has the NumPy drop-ins and states the tie order).  Returns one dict
     per image: `rois`, `class_ids`, `scores` (as `unmold_detections` returns them), `overlaps`
     [N, M] (float32, rows in descending score order; float64 zeros when N or M is 0), and
-    `pred_match` [T, N], `gt_match` [T, M] (float64) and `ap` [T] for the T thresholds."""
+    `pred_match` [T, N], `gt_match` [T, M] (float64) and `ap` [T] for the T thresholds.
+
+    COCO ground truth: gts[b] = (gt_boxes, gt_class_ids, gt_rles) with gt_rles a list of M RLE
+    dicts {'size': [H, W], 'counts': ...} -- compressed strings (`bytes` or `str`, what
+    `annToRLE` returns) or uncompressed count lists -- for every image of the batch.  They are
+    decoded on the device (`MaskBatch.from_rle`, which raises ValueError for malformed ones), so
+    only the strings and runs are uploaded; the results are the same as for the decoded bool
+    masks.  gt_boxes may be None: the boxes are then upstream's `extract_bboxes` of the decoded
+    masks (y1, x1, y2, x2, exclusive ends, zeros for an empty mask), read from the device with
+    one synchronisation, `trim_zeros`-ed and applied as above; that image's dict also has them
+    as `gt_rois` (int32 [M, 4])."""
     from . import evaluate
 
     if len(gts) != len(items):
@@ -394,15 +404,35 @@ def unmold_compute_ap_batch(items, gts, iou_thresholds=(0.5,), score_threshold=0
     if len(items) == 0:
         return []
     thresholds = list(iou_thresholds)
+    rle = [isinstance(g[2], (list, tuple)) and all(isinstance(r, dict) for r in g[2]) for g in gts]
+    if any(rle) and not all(rle):
+        raise ValueError("ground truth must be bool mask arrays for every image or RLE lists for "
+                         "every image")
+    rle = all(rle)
     gt_cls, gt_masks = [], []
     for boxes, cls, masks in gts:
+        if rle and boxes is None:
+            gt_cls.append(np.asarray(cls))
+            gt_masks.append(list(masks))
+            continue
         m = evaluate.trim_zeros(np.asarray(boxes)).shape[0]
         gt_cls.append(np.asarray(cls)[:m])
-        gt_masks.append(np.asarray(masks)[..., :m])
+        gt_masks.append(list(masks)[:m] if rle else np.asarray(masks)[..., :m])
+    gt_rois = {}
     with _Staged(items, canvas=False) as st:
         eng = st.eng
         eng.enqueue_packed(st.d_det, st.d_msk)
-        gt = eng.ground_truth(gt_cls, gt_masks)
+        if rle:
+            gt = eng.ground_truth_rle(gt_cls, gt_masks)
+            keep = gt.counts.copy()
+            for b, g in enumerate(gts):
+                if g[0] is None:
+                    gt_rois[b] = gt.extents[b, :keep[b]].copy()
+                    keep[b] = evaluate.trim_zeros(gt_rois[b]).shape[0]
+            if gt_rois:
+                gt.set_counts(keep)
+        else:
+            gt = eng.ground_truth(gt_cls, gt_masks)
         d_ov = eng.enqueue_overlaps(gt)
         d_order, d_pm, d_gm = eng.enqueue_matches(gt, thresholds, score_threshold)
         counts, metas = st.meta()
@@ -419,6 +449,8 @@ def unmold_compute_ap_batch(items, gts, iou_thresholds=(0.5,), score_threshold=0
             "ap": np.array([evaluate.ap_from_matches(pred_match[t], gt_match[t])[0]
                             for t in range(len(thresholds))]),
         })
+        if b in gt_rois:
+            out[-1]["gt_rois"] = gt_rois[b]
     return out
 
 

@@ -5,8 +5,8 @@ every computation on the path is a libmrx kernel launched through ctypes.
 
   UnmoldEngine     batched `unmold_detections` (serve.py:147-154): prologue -> class-tile
                    gather -> fused mask expand, all stream-ordered, no host sync
-  MaskBatch        caller-held masks (ground truth) as packed planes, scored against an
-                   engine's masks by `mask_overlaps` / `mask_matches`
+  MaskBatch        caller-held masks (ground truth) as packed planes, from bool arrays or COCO
+                   RLE, scored against an engine's masks by `mask_overlaps` / `mask_matches`
   AnchorGenerator  `get_anchors` (serve.py:105)
   Molder           the body of `preprocess_input` (serve.py:83-107): cv2.resize + resize_image
                    + mold_image
@@ -427,6 +427,14 @@ class UnmoldEngine:
             raise RuntimeError("plan() first")
         return MaskBatch(self.lib, self.device, self.layout.geom, class_ids, masks, stream)
 
+    def ground_truth_rle(self, class_ids, rles, stream=None):
+        """`ground_truth` from COCO RLE: class_ids[b] [M_b] and rles[b], a list of M_b dicts
+        {'size': [H_b, W_b], 'counts': ...} (see `MaskBatch.from_rle`, which also states what
+        raises), decoded on the device."""
+        if self.layout is None:
+            raise RuntimeError("plan() first")
+        return MaskBatch.from_rle(self.lib, self.device, self.layout.geom, class_ids, rles, stream)
+
     def enqueue_overlaps(self, gt, stream=None):
         """EXTENSION: upstream `compute_overlaps_masks(pred_masks, gt_masks)` of every planned image
         against `gt` (a `MaskBatch` from `ground_truth`), on the packed planes (after
@@ -577,12 +585,7 @@ class MaskBatch:
         self.R = R = max(int(counts.max(initial=0)), 1)
         layout = BatchLayout(g, R, limits=False)
         self.geom, self.counts = layout.geom, counts
-        cls = np.zeros((n, R), dtype=np.int32)
-        for b, c in enumerate(class_ids):
-            c = np.asarray(c)
-            if c.size and (c.astype(np.int32) != c).any():
-                raise ValueError(f"image {b}: class ids must be integers within int32")
-            cls[b, :c.size] = c
+        cls = _class_id_table(class_ids, n, R)
         st = N.stream_ptr(stream)
         with _stream_ctx(stream):
             self.d_geom = torch.from_numpy(layout.geom).to(device)
@@ -606,15 +609,204 @@ class MaskBatch:
                     raise ValueError(lib.mrx_last_error().decode())
                 N.check(rc, "mrx_pack_masks")
             del canvas
-            regions = np.zeros((n, R, 4), dtype=np.int32)
-            regions[:, :, 2:] = layout.geom[:, None, :2]
-            d_regions = torch.from_numpy(regions).to(device)
-            d_areas = torch.empty((n, R), dtype=torch.int64, device=device)
-            d_ext = torch.empty((n, R, 4), dtype=torch.int32, device=device)
-            N.check(lib.mrx_mask_extents(_ptr(d_packed), _ptr(d_off), _ptr(self.d_counts),
-                                         _ptr(self.d_geom), _ptr(d_regions), _ptr(d_areas),
-                                         _ptr(d_ext), n, R, st), "mrx_mask_extents")
+            d_regions = torch.from_numpy(_whole_image_regions(layout.geom, R)).to(device)
+            d_areas, d_ext = _whole_image_extents(lib, d_packed, d_off, self.d_counts, self.d_geom,
+                                                  d_regions, n, R, st)
         self.planes = Planes(d_packed, d_off, self.d_counts, d_areas, d_ext, R)
+
+    @classmethod
+    def from_rle(cls, lib, device, geoms, class_ids, rles, stream=None):
+        """The same batch from COCO RLE: rles[b] is a list of M_b dicts {'size': [H_b, W_b],
+        'counts': c} with c pycocotools' compressed string (`bytes`, or an ASCII `str`) or its
+        uncompressed runs (a 1-D sequence of integers in [0, 2^32), column-major, starting with
+        zeros), as `annToRLE` or `mask.encode` give them; kinds may mix.  The strings and runs
+        (`pack_rle`) are uploaded once and decoded on the device (mrx_rle_parse, mrx_rle_decode);
+        no mask exists on the host.  Then mrx_mask_extents, and one synchronisation to read the
+        status words and the extents (`extents`, int32 [n, R, 4]: what upstream's
+        `extract_bboxes` returns for each mask).
+
+        Raises ValueError naming the image and the instance for a size other than the image's, a
+        counts value of another type, an uncompressed count outside [0, 2^32) and a class-id count
+        other than M_b (all before anything is uploaded), and for a malformed string or runs
+        found on the device: a character outside '0'..'o', a string that ends inside a value, a
+        count that is negative or does not fit in uint32, or counts that do not sum to H*W.
+        pycocotools decodes such input without a check; this raises instead."""
+        torch = _torch()
+        self = cls.__new__(cls)
+        g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
+        n = self.n = g.shape[0]
+        pk = pack_rle(g, class_ids, rles)
+        counts, R = pk["counts"], pk["R"]
+        self.R = R
+        layout = BatchLayout(g, R, limits=False)
+        self.geom, self.counts = layout.geom, counts
+        S = pk["strings"].size
+        # one upload: every table, each at a multiple of 16 bytes (mrx_mask_extents reads the
+        # regions as int4), then the runs and the strings
+        parts = [pk["str_off"], pk["run_off"], layout.packed_off[:-1], pk["run_count"],
+                 np.zeros(n * R, np.int32), counts, _class_id_table(class_ids, n, R).reshape(-1),
+                 layout.geom.reshape(-1), _whole_image_regions(layout.geom, R).reshape(-1),
+                 pk["runs"], pk["strings"]]
+        sizes = [p.nbytes for p in parts]
+        starts = np.concatenate([[0], np.cumsum([(s + 15) // 16 * 16 for s in sizes])])
+        blob = np.zeros(int(starts[-1]), np.uint8)
+        for p, a, s in zip(parts, starts, sizes):
+            blob[a:a + s] = np.ascontiguousarray(p).view(np.uint8).reshape(-1)
+        st = N.stream_ptr(stream)
+        with _stream_ctx(stream):
+            d_blob = torch.from_numpy(blob).to(device)
+            views = [d_blob[a:a + s].view(_torch_of(p.dtype)) for p, a, s in zip(parts, starts, sizes)]
+            (d_str_off, d_run_off, d_off, d_run_count, d_status, self.d_counts, d_cls, d_geom,
+             d_regions, d_uploaded_runs, d_str) = views
+            self.d_class_ids = d_cls.view(n, R)
+            self.d_geom = d_geom.view(n, N.MRX_GEOM_INTS)
+            d_runs = torch.empty((max(S + pk["runs"].size, 1),), dtype=torch.int32, device=device)
+            d_runs[S:S + pk["runs"].size].copy_(d_uploaded_runs)
+            d_ends = torch.empty((d_runs.numel(),), dtype=torch.int64, device=device)
+            d_packed = torch.empty((max(int(layout.packed_off[-1]), 1),), dtype=torch.uint8,
+                                   device=device)
+            if S:
+                N.check(lib.mrx_rle_parse(_ptr(d_str), _ptr(d_str_off), _ptr(self.d_counts),
+                                          _ptr(d_runs), _ptr(d_run_count), _ptr(d_status), n, R,
+                                          st), "mrx_rle_parse")
+            N.check(lib.mrx_rle_decode(_ptr(d_runs), _ptr(d_run_off), _ptr(d_run_count),
+                                       _ptr(d_ends), _ptr(d_status), _ptr(self.d_counts),
+                                       _ptr(self.d_geom), _ptr(d_off), _ptr(d_packed), n, R,
+                                       max(layout.max_h, 1), max(layout.max_w, 1), st),
+                    "mrx_rle_decode")
+            d_areas, d_ext = _whole_image_extents(lib, d_packed, d_off, self.d_counts, self.d_geom,
+                                                  d_regions.view(n, R, 4), n, R, st)
+            status = d_status.cpu().numpy().reshape(n, R)     # the one synchronisation
+            self.extents = d_ext.cpu().numpy()
+        for b, k in zip(*np.nonzero(status)):
+            what = [msg for bit, msg in _RLE_STATUS if status[b, k] & bit]
+            H, W = layout.hw(b)
+            raise ValueError(f"image {b}, instance {k}: " + "; ".join(what).format(hw=H * W))
+        self.planes = Planes(d_packed, d_off, self.d_counts, d_areas, d_ext, R)
+        return self
+
+    def set_counts(self, counts, stream=None):
+        """Keep only the first counts[b] instances of each image (counts[b] <= M_b), as upstream
+        cuts the ground truth to the rows `trim_zeros` leaves of its boxes."""
+        counts = np.asarray(counts, dtype=np.int32).reshape(self.n)
+        if (counts < 0).any() or (counts > self.counts).any():
+            raise ValueError("counts must lie within the batch's instances")
+        with _stream_ctx(stream):
+            self.d_counts.copy_(_torch().from_numpy(counts))
+        self.counts = counts
+
+
+_RLE_STATUS = [
+    (N.MRX_RLE_ST_CHAR, "a counts character outside '0'..'o'"),
+    (N.MRX_RLE_ST_TRUNC, "the counts string ends inside a value"),
+    (N.MRX_RLE_ST_RANGE, "a count is negative or does not fit in uint32"),
+    (N.MRX_RLE_ST_SUM, "the counts do not sum to H*W = {hw}"),
+]
+
+
+def _torch_of(np_dtype):
+    torch = _torch()
+    return {np.dtype(np.int64): torch.int64, np.dtype(np.int32): torch.int32,
+            np.dtype(np.uint32): torch.int32, np.dtype(np.uint8): torch.uint8}[np.dtype(np_dtype)]
+
+
+def _class_id_table(class_ids, n, R):
+    """int32 [n, R]: image b's class ids first, zeros after them."""
+    cls = np.zeros((n, R), dtype=np.int32)
+    for b, c in enumerate(class_ids):
+        c = np.asarray(c)
+        if c.size and (c.astype(np.int32) != c).any():
+            raise ValueError(f"image {b}: class ids must be integers within int32")
+        cls[b, :c.size] = c
+    return cls
+
+
+def _whole_image_regions(geom, R):
+    """int32 [n, R, 4]: (0, 0, H_b, W_b) for every instance."""
+    regions = np.zeros((geom.shape[0], R, 4), dtype=np.int32)
+    regions[:, :, 2:] = geom[:, None, :2]
+    return regions
+
+
+def _whole_image_extents(lib, d_packed, d_off, d_counts, d_geom, d_regions, n, R, st):
+    torch = _torch()
+    d_areas = torch.empty((n, R), dtype=torch.int64, device=d_packed.device)
+    d_ext = torch.empty((n, R, 4), dtype=torch.int32, device=d_packed.device)
+    N.check(lib.mrx_mask_extents(_ptr(d_packed), _ptr(d_off), _ptr(d_counts), _ptr(d_geom),
+                                 _ptr(d_regions), _ptr(d_areas), _ptr(d_ext), n, R, st),
+            "mrx_mask_extents")
+    return d_areas, d_ext
+
+
+def pack_rle(geoms, class_ids, rles):
+    """The host side of `MaskBatch.from_rle`, NumPy only: checks every instance and packs the
+    batch into one byte buffer of strings and one uint32 array of uncompressed runs.  Instance
+    i = b*R + k (R = max(1, max M_b)).  Returns a dict:
+      counts     int32 [n]       M_b
+      R          int
+      strings    uint8 [S]       the compressed strings, instance i's at str_off[i]:str_off[i+1]
+                                 (empty for uncompressed instances and k >= M_b)
+      str_off    int64 [n*R+1]
+      runs       uint32 [C]      the uncompressed runs, one instance after another
+      run_off    int64 [n*R]     where instance i's runs are in the device buffer of
+                                 [S parsed slots | runs]: str_off[i] for a string, S + its
+                                 offset in `runs` for a list
+      run_count  int32 [n*R]     len(runs of i) for a list, 0 otherwise (the parse writes it)"""
+    g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
+    n = g.shape[0]
+    if len(rles) != n or len(class_ids) != n:
+        raise ValueError(f"{len(rles)} RLE lists and {len(class_ids)} class-id arrays for {n} "
+                         "images")
+    counts = np.zeros(n, dtype=np.int32)
+    for b, (cls, inst) in enumerate(zip(class_ids, rles)):
+        if np.shape(cls) != (len(inst),):
+            raise ValueError(f"image {b}: {np.shape(cls)} class ids for {len(inst)} RLE dicts")
+        counts[b] = len(inst)
+    R = max(int(counts.max(initial=0)), 1)
+    strings, runs = [], []
+    str_len = np.zeros(n * R, np.int64)
+    run_len = np.zeros(n * R, np.int64)
+    is_list = np.zeros(n * R, bool)
+    for b, inst in enumerate(rles):
+        hw = [int(g[b, 0]), int(g[b, 1])]
+        for k, rle in enumerate(inst):
+            i, where = b * R + k, f"image {b}, instance {k}"
+            try:
+                size, c = rle["size"], rle["counts"]
+            except (TypeError, KeyError):
+                raise ValueError(f"{where}: an RLE is a dict with 'size' and 'counts'") from None
+            got = [int(v) for v in np.ravel(size)]
+            if got != hw:
+                raise ValueError(f"{where}: size {got} is not the image's {hw}")
+            if isinstance(c, str):
+                try:
+                    c = c.encode("ascii")
+                except UnicodeEncodeError:
+                    raise ValueError(f"{where}: the counts string is not ASCII") from None
+            if isinstance(c, (bytes, bytearray)):
+                strings.append(np.frombuffer(bytes(c), np.uint8))
+                str_len[i] = len(c)
+                continue
+            a = np.asarray(c)
+            if a.ndim != 1 or not (a.dtype.kind in "iu" or (a.size == 0 and a.dtype.kind == "f")):
+                raise ValueError(f"{where}: counts must be bytes, str or a 1-D sequence of "
+                                 f"integers, got {type(c).__name__}")
+            if a.size and (a.min() < 0 or a.max() > 0xFFFFFFFF):
+                raise ValueError(f"{where}: an uncompressed count is negative or does not fit in "
+                                 "uint32")
+            runs.append(a.astype(np.uint32))
+            run_len[i] = a.size
+            is_list[i] = True
+    str_off = np.zeros(n * R + 1, np.int64)
+    np.cumsum(str_len, out=str_off[1:])
+    S = int(str_off[-1])
+    list_off = np.concatenate([[0], np.cumsum(run_len)[:-1]]) if n * R else np.zeros(0, np.int64)
+    run_off = np.where(is_list, S + list_off, str_off[:-1]).astype(np.int64)
+    return {"counts": counts, "R": R,
+            "strings": np.concatenate(strings) if strings else np.zeros(0, np.uint8),
+            "str_off": str_off,
+            "runs": np.concatenate(runs) if runs else np.zeros(0, np.uint32),
+            "run_off": run_off, "run_count": np.where(is_list, run_len, 0).astype(np.int32)}
 
 
 def mask_overlaps(lib, p1, p2, d_geom, n, stream=None):

@@ -153,16 +153,19 @@ def eval_case(iters, cpu):
     """configs[1] batch scored against ground truth: 32 x 1024x1024, 100 predictions against the
     100 instances of the same image jittered (synth.jitter_ground_truth).  The three kernels
     alone, and unmold_compute_ap_batch end to end (gt upload included) for one and for the ten
-    thresholds of compute_ap_range; --cpu: the oracle's compute_overlaps_masks per image."""
+    thresholds of compute_ap_range, with the ground truth as bool masks and as COCO compressed
+    strings (rle_gt_record); --cpu: the oracle's compute_overlaps_masks per image."""
     from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils
     from matterport_maskrcnn_with_tensorflow_serving_b200.engine import mask_matches
 
     batch, base_n = 32, 4
     base = synth.make_batch(7, base_n, (1024, 1024), 100)
     rng = np.random.default_rng(8)
-    base_gt = api_utils.unmold_detections_batch(
-        [(j.detections, j.mrcnn_mask, j.original_image_shape, j.image_shape, j.window)
-         for j in (synth.jitter_ground_truth(im, rng, 12, 0.1) for im in base)])
+    jittered = [(j.detections, j.mrcnn_mask, j.original_image_shape, j.image_shape, j.window)
+                for j in (synth.jitter_ground_truth(im, rng, 12, 0.1) for im in base)]
+    base_gt = api_utils.unmold_detections_batch(jittered)
+    # the same ground truth as COCO compressed strings, so that both paths score identical masks
+    base_rle = [r[3] for r in api_utils.unmold_detections_rle_batch(jittered, compressed=True)]
     ims = [base[i % base_n] for i in range(batch)]
     gts = [(g[0], g[1], g[3]) for g in (base_gt[i % base_n] for i in range(batch))]
     items = [(im.detections, im.mrcnn_mask, im.original_image_shape, im.image_shape, im.window)
@@ -202,7 +205,8 @@ def eval_case(iters, cpu):
             res = api_utils.unmold_compute_ap_batch(items, gts, thr)
         e2e[name] = (time.perf_counter() - t0) / reps * 1e3
     matches = int(sum((r["pred_match"][0] > -1).sum() for r in res))
-    rec = {"workload": "configs[1] 32 x 1024x1024 x 100 predictions vs 100 jittered gt -> mask IoU, "
+    rle = rle_gt_record(eng, gts, base_rle, base_n, items, thr10, iters)
+    rec = {"workload":"configs[1] 32 x 1024x1024 x 100 predictions vs 100 jittered gt -> mask IoU, "
                        "matches, AP", "pairs": pairs, "pairs_with_overlap": nonzero,
            "matches_at_0.5": matches,
            "pred_packed_MB": round(packed_pred / 1e6, 1),
@@ -213,7 +217,7 @@ def eval_case(iters, cpu):
            "unmold_compute_ap_batch_ms_1_threshold": round(e2e["1"], 1),
            "unmold_compute_ap_batch_ms_10_thresholds": round(e2e["10"], 1),
            "note": "end to end: H2D of the inputs and of the bool gt masks (105 MB per image), "
-                   "unmold, pack, scoring, downloads and the host AP tail", **card()}
+                   "unmold, pack, scoring, downloads and the host AP tail", **rle, **card()}
     if cpu:
         sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
         import eval_oracle
@@ -224,6 +228,80 @@ def eval_case(iters, cpu):
     print(json.dumps(rec), flush=True)
     del eng, d_det, d_msk, gt, d_ov
     torch.cuda.empty_cache()
+
+
+def rle_gt_record(eng, gts, base_rle, base_n, items, thr10, iters):
+    """The ground truth of eval_case as COCO compressed strings: mrx_rle_parse, mrx_rle_decode
+    and the whole-image mrx_mask_extents alone on the uploaded strings, and
+    unmold_compute_ap_batch end to end with them in place of the bool masks."""
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils
+    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import BatchLayout, pack_rle
+
+    n, lib = len(gts), eng.lib
+    rles = [base_rle[b % base_n] for b in range(n)]
+    cls = [g[1] for g in gts]
+    geom = eng.layout.geom
+    pk = pack_rle(geom, cls, rles)
+    R = pk["R"]
+    layout = BatchLayout(geom, R, limits=False)
+    dev = eng.device
+    up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)   # noqa: E731
+    d_str, d_str_off, d_run_off = up(pk["strings"]), up(pk["str_off"]), up(pk["run_off"])
+    d_counts, d_geom = up(pk["counts"]), up(geom)
+    d_run_count = up(pk["run_count"])
+    d_status = torch.zeros((n * R,), dtype=torch.int32, device=dev)
+    d_runs = torch.empty((pk["strings"].size,), dtype=torch.int32, device=dev)
+    d_ends = torch.empty((pk["strings"].size,), dtype=torch.int64, device=dev)
+    d_off = up(layout.packed_off[:-1])
+    d_packed = torch.empty((int(layout.packed_off[-1]),), dtype=torch.uint8, device=dev)
+    regions = np.zeros((n, R, 4), np.int32)
+    regions[:, :, 2:] = geom[:, None, :2]
+    d_regions = up(regions)
+    d_areas = torch.empty((n, R), dtype=torch.int64, device=dev)
+    d_ext = torch.empty((n, R, 4), dtype=torch.int32, device=dev)
+    p = lambda t: C.c_void_p(t.data_ptr())   # noqa: E731
+    st = N.stream_ptr(None)
+
+    def parse():
+        N.check(lib.mrx_rle_parse(p(d_str), p(d_str_off), p(d_counts), p(d_runs), p(d_run_count),
+                                  p(d_status), n, R, st), "mrx_rle_parse")
+
+    def decode():
+        N.check(lib.mrx_rle_decode(p(d_runs), p(d_run_off), p(d_run_count), p(d_ends), p(d_status),
+                                   p(d_counts), p(d_geom), p(d_off), p(d_packed), n, R,
+                                   layout.max_h, layout.max_w, st), "mrx_rle_decode")
+
+    def extents():
+        N.check(lib.mrx_mask_extents(p(d_packed), p(d_off), p(d_counts), p(d_geom), p(d_regions),
+                                     p(d_areas), p(d_ext), n, R, st), "mrx_mask_extents")
+
+    parse_ms, _ = time_ms(parse, iters)
+    decode_ms, _ = time_ms(decode, iters)
+    ext_ms, _ = time_ms(extents, iters)
+    assert not d_status.any().item(), "the benchmark's strings must decode cleanly"
+    rle_gts = [(g[0], g[1], r) for g, r in zip(gts, rles)]
+    e2e = {}
+    for name, thr in [("1", (0.5,)), ("10", thr10)]:
+        reps = max(2, iters // 8)
+        api_utils.unmold_compute_ap_batch(items, rle_gts, thr)
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            res = api_utils.unmold_compute_ap_batch(items, rle_gts, thr)
+        e2e[name] = (time.perf_counter() - t0) / reps * 1e3
+    want = api_utils.unmold_compute_ap_batch(items, gts, thr10)
+    same = all(np.array_equal(a["pred_match"], b["pred_match"]) and
+               np.array_equal(a["gt_match"], b["gt_match"]) for a, b in zip(res, want))
+    packed = int(sum(layout.packed_span(b, pk["counts"][b])[1] - layout.packed_span(b, 0)[0]
+                     for b in range(n)))
+    return {"rle_gt_string_MB": round(pk["strings"].size / 1e6, 2),
+            "rle_gt_instances": int(pk["counts"].sum()),
+            "rle_parse_kernel_ms": round(parse_ms, 4),
+            "rle_decode_kernels_ms": round(decode_ms, 4),
+            "rle_decode_packed_write_GBps": round(packed / decode_ms / 1e6, 1),
+            "rle_gt_extents_kernel_ms": round(ext_ms, 4),
+            "unmold_compute_ap_batch_ms_1_threshold_rle_gt": round(e2e["1"], 1),
+            "unmold_compute_ap_batch_ms_10_thresholds_rle_gt": round(e2e["10"], 1),
+            "rle_gt_results_equal_bool_gt": bool(same)}
 
 
 def anchors_sweep(iters, cpu):
