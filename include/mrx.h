@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define MRX_ABI_VERSION 11
+#define MRX_ABI_VERSION 12
 
 #define MRX_OK              0
 #define MRX_E_INVALID      -1   /* bad argument (null pointer, size out of range) */
@@ -374,6 +374,63 @@ int mrx_mask_matches(const float *d_overlaps, const int *d_pred_counts,
                      const int *d_gt_counts, const int *d_gt_class_ids, const double *thresholds,
                      int T, double score_threshold, int *d_order, int *d_pred_match,
                      int *d_gt_match, int B, int R1, int R2, void *stream);
+
+/* ---------------------------------------------------------------- COCO mask evaluation */
+/* EXTENSION: the per-image half of pycocotools' COCOeval for iouType "segm" (computeIoU with
+ * maskApi.c's rleIou, and the matching loop of evaluateImg) on the packed slots (see "Output
+ * slots"); the host accumulates the per-detection flags (cocoeval.cu).  Categories are dense
+ * indices >= 0; -1 is a category that is not evaluated.
+ *
+ * mrx_coco_ranks: per image b, its N_b = d_counts[b] predictions (d_class_ids [B,R] int32,
+ *   d_scores [B,R] of score_dtype), d_class_map [C] int32 (class id -> dense category or -1; a
+ *   class id outside [0, C) is -1).  Writes, for k < N_b,
+ *     d_cat  [B,R] int32: the dense category;
+ *     d_rank [B,R] int32: the rank within (image, category) in np.argsort(-score,
+ *                         kind="mergesort") order: descending, equal scores by smaller index,
+ *                         NaN after every number;
+ *     d_keep [B,R] uint8: d_cat >= 0 and d_rank < max_det (maxDets[-1]);
+ *     d_walk [B,R] int32: rank -> prediction in that order across categories.
+ * mrx_coco_ious: two slot sets of one batch sharing d_geom, with areas and extents from
+ *   mrx_mask_extents; d_pred_cat / d_pred_keep from mrx_coco_ranks, d_gt_cat [B,R2] int32 and
+ *   d_gt_crowd [B,R2] uint8 (iscrowd).  d_iou [B,R1,R2] float64: element (b, i, j) for a kept
+ *   i < N1_b and j < N2_b of the same category is (double)inter / (double)u rounded once, 0 when
+ *   inter = 0, u = area(i) for a crowd j and area(i) + area(j) - inter otherwise; other elements
+ *   are not written.  d_packed1 and d_packed2 must be 4-byte aligned.
+ * mrx_coco_match: d_iou as above, the ranks' d_pred_cat, d_pred_keep and d_walk, d_pred_area
+ *   [B,R1] int64 (mask pixels), d_gt_counts [B], d_gt_cat, d_gt_crowd, d_gt_area [B,R2] float64
+ *   (the annotation's area).  thresholds[T] (HOST, compared as IoU >= t: the caller caps them at
+ *   1 - 1e-10 as evaluateImg does) and area_rng[A][2] (HOST, lo and hi, both inclusive).  For
+ *   area range a and threshold t, ground-truth j is ignored when crowd or its area is outside
+ *   [lo, hi]; predictions go in walk order, each kept one takes, among the instances of its
+ *   category that are unmatched or crowd with IoU >= t, the non-ignored one with the largest IoU,
+ *   else the ignored one with the largest IoU, ties the larger index.  Writes, for kept i,
+ *     d_dt_match  [A,T,B,R1] int32: the matched ground-truth index or -1;
+ *     d_dt_ignore [A,T,B,R1] uint8: the matched instance's ignore flag, or for an unmatched
+ *                                   prediction whether its area is outside [lo, hi].
+ *   Other elements are not written.
+ * Checks: mrx_coco_ious: those of "Output slots" for each slot set, then null pointers and the
+ * alignment; the others: null pointers, B outside [0, MRX_MAX_BATCH], R (R1, R2) outside
+ * [1, 65534], for mrx_coco_ranks C or max_det below 1 or a bad score_dtype, for mrx_coco_match T
+ * outside [1, MRX_MAX_IOU_THRESHOLDS] or A outside [1, MRX_MAX_AREA_RANGES]: MRX_E_INVALID.
+ * B = 0 returns MRX_OK without launching anything. */
+#define MRX_MAX_AREA_RANGES 16
+int mrx_coco_ranks(const int *d_class_ids, const void *d_scores, int score_dtype,
+                   const int *d_counts, const int *d_class_map, int C, int max_det, int *d_cat,
+                   int *d_rank, unsigned char *d_keep, int *d_walk, int B, int R, void *stream);
+int mrx_coco_ious(const unsigned char *d_packed1, const long long *d_packed_off1,
+                  const int *d_counts1, const long long *d_areas1, const int *d_extents1,
+                  const int *d_pred_cat, const unsigned char *d_pred_keep, int R1,
+                  const unsigned char *d_packed2, const long long *d_packed_off2,
+                  const int *d_counts2, const long long *d_areas2, const int *d_extents2,
+                  const int *d_gt_cat, const unsigned char *d_gt_crowd, int R2, const int *d_geom,
+                  double *d_iou, int B, void *stream);
+int mrx_coco_match(const double *d_iou, const int *d_pred_counts, const int *d_pred_cat,
+                   const unsigned char *d_pred_keep, const int *d_walk,
+                   const long long *d_pred_area, const int *d_gt_counts, const int *d_gt_cat,
+                   const unsigned char *d_gt_crowd, const double *d_gt_area,
+                   const double *thresholds, int T, const double *area_rng, int A,
+                   int *d_dt_match, unsigned char *d_dt_ignore, int B, int R1, int R2,
+                   void *stream);
 
 /* ---------------------------------------------------------------- COCO RLE to packed planes */
 /* EXTENSION: the inverse of mrx_rle_strings / mrx_rle_write, for ground truth held as COCO RLE

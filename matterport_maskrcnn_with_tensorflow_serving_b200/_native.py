@@ -26,11 +26,12 @@ MRX_GEOM_INTS = 8
 MRX_MAX_BATCH = 4096
 MRX_MAX_MASK_DIM = 64
 MRX_MAX_LANE_MASK_W = 30    # tile width of the lane kernels: mw + 2 lanes per warp
-ABI_VERSION = 11
+ABI_VERSION = 12
 MRX_SCHED_WORDS = 4
 MRX_PEER_HANDLE_BYTES = 64
 MRX_MAX_CONTOUR_SEGMENTS = 1 << 30
 MRX_MAX_IOU_THRESHOLDS = 64
+MRX_MAX_AREA_RANGES = 16
 MRX_RLE_ST_CHAR = 1
 MRX_RLE_ST_TRUNC = 2
 MRX_RLE_ST_RANGE = 4
@@ -81,6 +82,11 @@ SIGNATURES = {
                                _i, _vp]),
     "mrx_mask_matches": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _dp, _i, C.c_double, _vp, _vp,
                               _vp, _i, _i, _i, _vp]),
+    "mrx_coco_ranks": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp]),
+    "mrx_coco_ious": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                           _i, _vp, _vp, _i, _vp]),
+    "mrx_coco_match": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _dp, _i, _dp, _i, _vp,
+                            _vp, _i, _i, _i, _vp]),
     "mrx_rle_parse": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "mrx_rle_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "mrx_device_alloc": (_i, [C.c_ulonglong, C.POINTER(C.c_void_p), _ip]),

@@ -10,8 +10,9 @@ NumPy value semantics, computed by the sm_90a kernels in libmrx.so.
 Plus batched entry points the reference lacks (it is hard-wired to one image per call,
 serve.py:48): `unmold_detections_batch`, `unmold_detections_packed_batch`,
 `unmold_detections_rle_batch`, `unmold_detections_contours_batch`, `unmold_overlay_batch`,
-`unmold_coco_results_batch` (upstream's `build_coco_results` of the unmolded detections) and
-`unmold_compute_ap_batch` (upstream's `compute_ap` of them against ground truth).
+`unmold_coco_results_batch` (upstream's `build_coco_results` of the unmolded detections),
+`unmold_compute_ap_batch` (upstream's `compute_ap` of them against ground truth) and
+`unmold_coco_eval_batch` (pycocotools' COCOeval "segm" of them, streamed batch by batch).
 
 Numerical contract (checked by tests/ against the float64 oracle): N, boxes, class ids and
 scores are bit-exact.  The mask resize runs in float32 on exact integer source coordinates;
@@ -452,6 +453,17 @@ def unmold_compute_ap_batch(items, gts, iou_thresholds=(0.5,), score_threshold=0
         if b in gt_rois:
             out[-1]["gt_rois"] = gt_rois[b]
     return out
+
+
+def unmold_coco_eval_batch(items, image_ids, gt_anns, evaluator, category_ids=None):
+    """`unmold_detections` scored as pycocotools' COCOeval scores segm results, without the
+    masks leaving the device: adds the batch to `evaluator` (an `evaluate.COCOevalSegm`), whose
+    `accumulate()` and `summarize()` give COCO mask AP once every batch is in.  items as for
+    `unmold_detections_batch`; image_ids, one per item; gt_anns[b], image b's COCO annotation
+    dicts with RLE segmentations; category_ids as for `unmold_coco_results_batch`.  Equivalent to
+    `evaluator.add_results(unmold_coco_results_batch(items, image_ids, category_ids), gt_anns,
+    image_ids)`, but the predicted masks go straight to packed planes and are never encoded."""
+    evaluator.add_batch(items, image_ids, gt_anns, category_ids)
 
 
 def unmold_detections_contours_batch(items):

@@ -1,0 +1,299 @@
+// cocoeval.cu -- the per-image half of pycocotools' COCOeval for iouType "segm" on the packed
+// planes: computeIoU (maskApi.c rleIou) and the matching loop of evaluateImg.  The host keeps
+// what accumulate needs: per detection its category, rank, score, area and match / ignore bits.
+//
+//   coco_rank_kernel   CTA per image: each prediction's dense category (through a class map),
+//                      its rank within (image, category) in np.argsort(-score, kind="mergesort")
+//                      order (descending, ties smaller index first, NaN last), whether that rank
+//                      is below maxDets[-1], and the image's walk order (the same order across
+//                      categories), by counting
+//   coco_iou_kernel    CTA per (image, prediction), warp per ground-truth instance, as
+//                      mask_overlaps_kernel: only pairs of one category whose prediction is kept;
+//                      a pair whose extents do not meet gets 0 without a read
+//   coco_match_kernel  warp per (image, threshold, area range): predictions in walk order, each
+//                      takes the argmax of (not ignored, IoU, position) over its candidates
+//
+// IoU arithmetic is rleIou's: (double)i / (double)u of exact counts, 0 when i = 0, u = the
+// detection's area for a crowd instance and a_dt + a_gt - i otherwise.
+#include "planes.cuh"
+
+namespace mrx {
+
+namespace cocoeval {
+
+using overlaps::Planes;
+using overlaps::and_count;
+using overlaps::plane_of;
+
+constexpr int kWarps = 8;
+
+// ---------------------------------------------------------------- ranks
+struct RankParams {
+  const int *class_ids;       // [B, R]
+  const void *scores;         // [B, R] f32 / f64
+  const int *counts;          // [B]
+  const int *class_map;       // [C]
+  int *cat;                   // [B, R]
+  int *rank;                  // [B, R]
+  unsigned char *keep;        // [B, R]
+  int *walk;                  // [B, R]
+  int R, C, score_f64, max_det;
+};
+
+__device__ __forceinline__ double score_at(const void *scores, int f64, size_t i) {
+  return f64 ? static_cast<const double *>(scores)[i]
+             : static_cast<double>(static_cast<const float *>(scores)[i]);
+}
+
+// k comes before i in np.argsort(-score, kind="mergesort"): numbers before NaN, higher scores
+// first, equal scores (and NaN among NaN) by index
+__device__ __forceinline__ bool before(double sk, int k, double si, int i) {
+  const bool nk = isnan(sk), ni = isnan(si);
+  if (nk != ni) return ni;
+  if (!nk && sk != si) return sk > si;
+  return k < i;
+}
+
+__global__ void __launch_bounds__(256) coco_rank_kernel(const RankParams p) {
+  const int b = blockIdx.x;
+  const int N = p.counts[b];
+  const size_t base = static_cast<size_t>(b) * p.R;
+  for (int i = threadIdx.x; i < N; i += blockDim.x) {
+    const int c = p.class_ids[base + i];
+    const int k = c >= 0 && c < p.C ? p.class_map[c] : -1;
+    p.cat[base + i] = k < 0 ? -1 : k;
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < N; i += blockDim.x) {
+    const double si = score_at(p.scores, p.score_f64, base + i);
+    const int ci = p.cat[base + i];
+    int rank = 0, walk = 0;
+    for (int k = 0; k < N; ++k) {
+      const bool bf = before(score_at(p.scores, p.score_f64, base + k), k, si, i);
+      walk += bf;
+      rank += bf && p.cat[base + k] == ci;
+    }
+    p.rank[base + i] = rank;
+    p.keep[base + i] = ci >= 0 && rank < p.max_det;
+    p.walk[base + walk] = i;
+  }
+}
+
+// ---------------------------------------------------------------- IoUs
+__global__ void __launch_bounds__(kWarps * 32)
+coco_iou_kernel(const Planes p1, const Planes p2, const int *__restrict__ geom,
+                const int *__restrict__ pred_cat, const unsigned char *__restrict__ pred_keep,
+                const int *__restrict__ gt_cat, const unsigned char *__restrict__ gt_crowd,
+                double *__restrict__ out) {
+  const int i = blockIdx.x, b = blockIdx.y;
+  const int N = p1.counts[b], M = p2.counts[b];
+  if (i >= N) return;
+  const size_t i1 = static_cast<size_t>(b) * p1.R + i;
+  if (!pred_keep[i1]) return;
+  const int ci = pred_cat[i1];
+  const int H = geom[b * MRX_GEOM_INTS + 0], W = geom[b * MRX_GEOM_INTS + 1];
+  const int wb = (W + 7) >> 3;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long a1 = p1.areas[i1];
+  const int4 e1 = p1.extents[i1];
+  const unsigned char *plane1 = plane_of(p1.packed, b, i, H, wb);
+  double *row = out + i1 * p2.R;
+  for (int j = warp; j < M; j += kWarps) {
+    const size_t i2 = static_cast<size_t>(b) * p2.R + j;
+    if (gt_cat[i2] != ci) continue;
+    const long long a2 = p2.areas[i2];
+    const int4 e2 = p2.extents[i2];
+    const int y1 = max(e1.x, e2.x), x1 = max(e1.y, e2.y), y2 = min(e1.z, e2.z), x2 = min(e1.w, e2.w);
+    long long inter = 0;
+    if (a1 && a2 && y2 > y1 && x2 > x1)
+      inter = and_count(plane1, plane_of(p2.packed, b, j, H, wb), wb, y1, x1, y2, x2, lane);
+    if (lane == 0) {
+      const long long u = gt_crowd[i2] ? a1 : a1 + a2 - inter;
+      row[j] = inter ? __ddiv_rn(static_cast<double>(inter), static_cast<double>(u)) : 0.0;
+    }
+  }
+}
+
+// ---------------------------------------------------------------- matches
+struct MatchParams {
+  const double *iou;          // [B, R1, R2]
+  const int *pred_counts;     // [B]
+  const int *pred_cat;        // [B, R1]
+  const unsigned char *pred_keep;
+  const int *walk;            // [B, R1]
+  const long long *pred_area; // [B, R1]
+  const int *gt_counts;       // [B]
+  const int *gt_cat;          // [B, R2]
+  const unsigned char *gt_crowd;
+  const double *gt_area;      // [B, R2]
+  int *dt_match;              // [A, T, B, R1]
+  unsigned char *dt_ignore;   // [A, T, B, R1]
+  int B, R1, R2, T;
+  double thresholds[MRX_MAX_IOU_THRESHOLDS];
+  double area_rng[2 * MRX_MAX_AREA_RANGES];
+};
+
+// evaluateImg's loop in closed form: the candidates of a prediction are the instances of its
+// category that are unmatched (or crowd) with IoU >= the threshold; it takes the non-ignored one
+// with the largest IoU, else the ignored one with the largest IoU, ties going to the later one of
+// the ground truth stable-sorted with the non-ignored first -- within each of the two groups that
+// order is the index order, so the key is (not ignored, IoU bits, then j).  Lane j % 32 scans
+// instance j; the matched set is a bitmask in shared memory, written by the one winning lane.
+__global__ void __launch_bounds__(32) coco_match_kernel(const MatchParams p) {
+  __shared__ unsigned s_matched[(65534 + 31) / 32];
+  const int b = blockIdx.x, t = blockIdx.y, a = blockIdx.z, lane = threadIdx.x;
+  const int N = p.pred_counts[b], M = p.gt_counts[b];
+  const double thr = p.thresholds[t], lo = p.area_rng[2 * a], hi = p.area_rng[2 * a + 1];
+  const size_t pb = static_cast<size_t>(b) * p.R1, gb = static_cast<size_t>(b) * p.R2;
+  const size_t ob = (static_cast<size_t>(a) * p.T + t) * p.B * p.R1 + pb;
+  for (int w = lane; w < (M + 31) / 32; w += 32) s_matched[w] = 0u;
+  __syncwarp();
+  for (int r = 0; r < N; ++r) {
+    const int i = p.walk[pb + r];
+    if (!p.pred_keep[pb + i]) continue;
+    const int ci = p.pred_cat[pb + i];
+    const double *row = p.iou + (pb + i) * p.R2;
+    unsigned long long best = 0ull;
+    int bj = -1;
+    for (int j = lane; j < M; j += 32) {
+      if (p.gt_cat[gb + j] != ci) continue;
+      const bool crowd = p.gt_crowd[gb + j];
+      if (!crowd && (s_matched[j >> 5] >> (j & 31) & 1u)) continue;
+      const double v = row[j];
+      if (!(v >= thr)) continue;
+      const double ga = p.gt_area[gb + j];
+      const bool ig = crowd || ga < lo || ga > hi;
+      const unsigned long long key =
+          (ig ? 0ull : 1ull << 62) | static_cast<unsigned long long>(__double_as_longlong(v));
+      if (key >= best || bj < 0) {
+        best = key;
+        bj = j;
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long ok = __shfl_xor_sync(0xffffffffu, best, o);
+      const int oj = __shfl_xor_sync(0xffffffffu, bj, o);
+      if (oj >= 0 && (bj < 0 || ok > best || (ok == best && oj > bj))) {
+        best = ok;
+        bj = oj;
+      }
+    }
+    if (bj >= 0 && lane == (bj & 31)) s_matched[bj >> 5] |= 1u << (bj & 31);
+    if (lane == 0) {
+      bool ig;
+      if (bj >= 0) {
+        ig = !(best >> 62);
+      } else {
+        const double da = static_cast<double>(p.pred_area[pb + i]);
+        ig = da < lo || da > hi;
+      }
+      p.dt_match[ob + i] = bj;
+      p.dt_ignore[ob + i] = ig;
+    }
+    __syncwarp();
+  }
+}
+
+}  // namespace cocoeval
+
+}  // namespace mrx
+
+using namespace mrx;
+
+extern "C" int mrx_coco_ranks(const int *d_class_ids, const void *d_scores, int score_dtype,
+                              const int *d_counts, const int *d_class_map, int C, int max_det,
+                              int *d_cat, int *d_rank, unsigned char *d_keep, int *d_walk, int B,
+                              int R, void *stream) {
+  const char *fn = "mrx_coco_ranks";
+  MRX_CHECK_ARG(d_class_ids && d_scores && d_counts && d_class_map && d_cat && d_rank && d_keep &&
+                    d_walk,
+                "%s: null pointer", fn);
+  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH, "%s: bad B %d (need 0<=B<=%d)", fn, B, MRX_MAX_BATCH);
+  MRX_CHECK_ARG(R >= 1 && R <= 65534, "%s: bad R %d (need 1<=R<=65534)", fn, R);
+  MRX_CHECK_ARG(C >= 1, "%s: bad C %d (need C>=1)", fn, C);
+  MRX_CHECK_ARG(max_det >= 1, "%s: bad max_det %d (need max_det>=1)", fn, max_det);
+  MRX_CHECK_ARG(score_dtype == MRX_F32 || score_dtype == MRX_F64, "%s: bad score dtype %d", fn,
+                score_dtype);
+  if (B == 0) return MRX_OK;
+  const cocoeval::RankParams p{d_class_ids, d_scores, d_counts, d_class_map, d_cat, d_rank,
+                               d_keep,      d_walk,   R,        C,           score_dtype == MRX_F64,
+                               max_det};
+  cocoeval::coco_rank_kernel<<<B, 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  MRX_LAUNCH_CHECK("coco_rank_kernel");
+  return MRX_OK;
+}
+
+extern "C" int mrx_coco_ious(const unsigned char *d_packed1, const long long *d_packed_off1,
+                             const int *d_counts1, const long long *d_areas1,
+                             const int *d_extents1, const int *d_pred_cat,
+                             const unsigned char *d_pred_keep, int R1,
+                             const unsigned char *d_packed2, const long long *d_packed_off2,
+                             const int *d_counts2, const long long *d_areas2,
+                             const int *d_extents2, const int *d_gt_cat,
+                             const unsigned char *d_gt_crowd, int R2, const int *d_geom,
+                             double *d_iou, int B, void *stream) {
+  const char *fn = "mrx_coco_ious";
+  if (int rc = check_slots(fn, d_packed1, d_packed_off1, d_counts1, d_geom, B, R1)) return rc;
+  if (int rc = check_slots(fn, d_packed2, d_packed_off2, d_counts2, d_geom, B, R2)) return rc;
+  MRX_CHECK_ARG(d_areas1 && d_extents1 && d_areas2 && d_extents2, "%s: null areas or extents", fn);
+  MRX_CHECK_ARG(d_pred_cat && d_pred_keep && d_gt_cat && d_gt_crowd && d_iou, "%s: null pointer",
+                fn);
+  MRX_CHECK_ARG(((reinterpret_cast<uintptr_t>(d_packed1) | reinterpret_cast<uintptr_t>(d_packed2)) &
+                 3u) == 0u,
+                "%s: packed bases must be 4-byte aligned", fn);
+  if (B == 0) return MRX_OK;
+  const overlaps::Planes p1{{d_packed1, d_packed_off1}, d_counts1, d_areas1,
+                            reinterpret_cast<const int4 *>(d_extents1), R1};
+  const overlaps::Planes p2{{d_packed2, d_packed_off2}, d_counts2, d_areas2,
+                            reinterpret_cast<const int4 *>(d_extents2), R2};
+  cocoeval::coco_iou_kernel<<<dim3(R1, B), cocoeval::kWarps * 32, 0,
+                              static_cast<cudaStream_t>(stream)>>>(
+      p1, p2, d_geom, d_pred_cat, d_pred_keep, d_gt_cat, d_gt_crowd, d_iou);
+  MRX_LAUNCH_CHECK("coco_iou_kernel");
+  return MRX_OK;
+}
+
+extern "C" int mrx_coco_match(const double *d_iou, const int *d_pred_counts, const int *d_pred_cat,
+                              const unsigned char *d_pred_keep, const int *d_walk,
+                              const long long *d_pred_area, const int *d_gt_counts,
+                              const int *d_gt_cat, const unsigned char *d_gt_crowd,
+                              const double *d_gt_area, const double *thresholds, int T,
+                              const double *area_rng, int A, int *d_dt_match,
+                              unsigned char *d_dt_ignore, int B, int R1, int R2, void *stream) {
+  const char *fn = "mrx_coco_match";
+  MRX_CHECK_ARG(d_iou && d_pred_counts && d_pred_cat && d_pred_keep && d_walk && d_pred_area &&
+                    d_gt_counts && d_gt_cat && d_gt_crowd && d_gt_area && thresholds && area_rng &&
+                    d_dt_match && d_dt_ignore,
+                "%s: null pointer", fn);
+  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH, "%s: bad B %d (need 0<=B<=%d)", fn, B, MRX_MAX_BATCH);
+  MRX_CHECK_ARG(R1 >= 1 && R1 <= 65534 && R2 >= 1 && R2 <= 65534,
+                "%s: bad R1 %d / R2 %d (need 1<=R<=65534)", fn, R1, R2);
+  MRX_CHECK_ARG(T >= 1 && T <= MRX_MAX_IOU_THRESHOLDS, "%s: bad T %d (need 1<=T<=%d)", fn, T,
+                MRX_MAX_IOU_THRESHOLDS);
+  MRX_CHECK_ARG(A >= 1 && A <= MRX_MAX_AREA_RANGES, "%s: bad A %d (need 1<=A<=%d)", fn, A,
+                MRX_MAX_AREA_RANGES);
+  if (B == 0) return MRX_OK;
+  cocoeval::MatchParams p{};
+  p.iou = d_iou;
+  p.pred_counts = d_pred_counts;
+  p.pred_cat = d_pred_cat;
+  p.pred_keep = d_pred_keep;
+  p.walk = d_walk;
+  p.pred_area = d_pred_area;
+  p.gt_counts = d_gt_counts;
+  p.gt_cat = d_gt_cat;
+  p.gt_crowd = d_gt_crowd;
+  p.gt_area = d_gt_area;
+  p.dt_match = d_dt_match;
+  p.dt_ignore = d_dt_ignore;
+  p.B = B;
+  p.R1 = R1;
+  p.R2 = R2;
+  p.T = T;
+  for (int t = 0; t < T; ++t) p.thresholds[t] = thresholds[t];
+  for (int a = 0; a < 2 * A; ++a) p.area_rng[a] = area_rng[a];
+  cocoeval::coco_match_kernel<<<dim3(B, T, A), 32, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  MRX_LAUNCH_CHECK("coco_match_kernel");
+  return MRX_OK;
+}

@@ -471,6 +471,30 @@ class UnmoldEngine:
         return mask_matches(self.lib, last[1], self.d_counts, self.d_class_ids, self.d_scores,
                             _dtype_code(self.det_dtype), gt, thresholds, score_threshold, stream)
 
+    def enqueue_coco_eval(self, gt, gt_crowd, gt_area, class_map, params, stream=None):
+        """EXTENSION: `coco_evaluate_batch` of the planned batch's kept instances against `gt` (a
+        `MaskBatch` from `ground_truth` / `ground_truth_rle` whose class ids are dense category
+        indices), on the packed planes (after `enqueue_expand_packed` or `pack_masks`); each
+        prediction is read only inside its box.  class_map [C] maps the engine's class ids to
+        dense categories (-1: not evaluated).  Synchronises once; returns its dict."""
+        if self.layout is None or self.d_packed is None:
+            raise RuntimeError("enqueue_coco_eval needs the packed planes: call "
+                               "enqueue_expand_packed or pack_masks first")
+        n = self._n_images
+        if gt.n != n or not np.array_equal(gt.geom, self.layout.geom):
+            raise ValueError("the ground truth was staged for another plan")
+        torch = _torch()
+        bufs = self._eval_bufs
+        d_areas = _buffer(bufs, "areas", n * self.R, torch.int64, self.device)
+        d_ext = _buffer(bufs, "extents", n * self.R * 4, torch.int32, self.device)
+        N.check(self.lib.mrx_mask_extents(
+            _ptr(self.d_packed), _ptr(self.d_packed_off), _ptr(self.d_counts), _ptr(self.d_geom),
+            _ptr(self.d_boxes), _ptr(d_areas), _ptr(d_ext), n, self.R, N.stream_ptr(stream)),
+            "mrx_mask_extents")
+        pred = Planes(self.d_packed, self.d_packed_off, self.d_counts, d_areas, d_ext, self.R)
+        return coco_evaluate_batch(self.lib, pred, self.d_class_ids[:n], self.d_scores[:n], gt,
+                                   gt_crowd, gt_area, class_map, params, stream)
+
     def pack_masks(self, stream=None):
         """EXTENSION: bit-pack the byte canvases already written for the planned batch
         (mrx_pack_masks; same output layout as `enqueue_expand_packed`).  Returns
@@ -707,7 +731,8 @@ _RLE_STATUS = [
 def _torch_of(np_dtype):
     torch = _torch()
     return {np.dtype(np.int64): torch.int64, np.dtype(np.int32): torch.int32,
-            np.dtype(np.uint32): torch.int32, np.dtype(np.uint8): torch.uint8}[np.dtype(np_dtype)]
+            np.dtype(np.uint32): torch.int32, np.dtype(np.uint8): torch.uint8,
+            np.dtype(np.float64): torch.float64}[np.dtype(np_dtype)]
 
 
 def _class_id_table(class_ids, n, R):
@@ -855,6 +880,110 @@ def mask_matches(lib, d_overlaps, d_pred_counts, d_pred_class_ids, d_scores, sco
             C.c_double(comparison_threshold(score_threshold)), _ptr(d_order), _ptr(d_pm[t0]),
             _ptr(d_gm[t0]), n, R1, R2, N.stream_ptr(stream)), "mrx_mask_matches")
     return d_order, d_pm, d_gm
+
+
+def coco_device_params(params):
+    """(thresholds, area_rng, max_det) of a COCOeval-style params object (`iouThrs`, `areaRng`,
+    `maxDets`) as the COCO kernels take them: the thresholds capped at 1 - 1e-10 as evaluateImg
+    caps them, the area ranges flattened to [A * 2] float64, maxDets[-1].  Raises ValueError
+    outside the kernels' limits."""
+    thr = [min(float(t), 1 - 1e-10) for t in np.ravel(params.iouThrs)]
+    rng = np.asarray(params.areaRng, dtype=np.float64).reshape(-1, 2)
+    max_det = int(params.maxDets[-1])
+    if not 1 <= len(thr) <= N.MRX_MAX_IOU_THRESHOLDS:
+        raise ValueError(f"{len(thr)} IoU thresholds (need 1 to {N.MRX_MAX_IOU_THRESHOLDS})")
+    if not 1 <= rng.shape[0] <= N.MRX_MAX_AREA_RANGES:
+        raise ValueError(f"{rng.shape[0]} area ranges (need 1 to {N.MRX_MAX_AREA_RANGES})")
+    if max_det < 1:
+        raise ValueError(f"maxDets[-1] = {max_det} (need >= 1)")
+    return thr, rng.reshape(-1).tolist(), max_det
+
+
+def _upload_parts(parts, device):
+    """One host-to-device copy of NumPy arrays, each at a multiple of 16 bytes; returns typed
+    device views of the same shapes."""
+    torch = _torch()
+    sizes = [p.nbytes for p in parts]
+    starts = np.concatenate([[0], np.cumsum([(s + 15) // 16 * 16 for s in sizes])]).astype(np.int64)
+    blob = np.zeros(max(int(starts[-1]), 16), np.uint8)
+    for p, a, s in zip(parts, starts, sizes):
+        blob[a:a + s] = np.ascontiguousarray(p).view(np.uint8).reshape(-1)
+    d_blob = torch.from_numpy(blob).to(device)
+    return [d_blob[a:a + s].view(_torch_of(p.dtype)).view(p.shape)
+            for p, a, s in zip(parts, starts, sizes)]
+
+
+def coco_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt_area, class_map,
+                        params, stream=None):
+    """The per-image half of COCOeval (iouType "segm") for one batch: mrx_coco_ranks,
+    mrx_coco_ious and mrx_coco_match, then one download and one synchronisation.
+
+    pred: `Planes` of the predictions (areas and extents from mrx_mask_extents) of gt's images,
+    pred_class_ids [n, pred.R] int32 and pred_scores [n, pred.R] float32 / float64 device tensors;
+    gt: a `MaskBatch` whose class ids are dense category indices; gt_crowd [n, gt.R] (iscrowd)
+    and gt_area [n, gt.R] (the annotations' areas, float64) host arrays; class_map [C] int32 host
+    array, prediction class id -> dense category or -1 (not evaluated); params: `iouThrs`,
+    `areaRng`, `maxDets` (`coco_device_params`).
+
+    Returns a dict of host arrays: `counts` [n]; per prediction [n, pred.R] `cat`, `rank` (in
+    its (image, category), in score order), `keep` (cat >= 0 and rank < maxDets[-1], and within
+    the count), `area` (int64 pixels), `score` (float64); `match` [A, T, n, pred.R] int32 (the
+    ground-truth index or -1) and `ignore` [A, T, n, pred.R] bool, defined where `keep` is; and
+    `d_iou`, the float64 device tensor [n, pred.R, gt.R] of mrx_coco_ious."""
+    torch = _torch()
+    thr, rng, max_det = coco_device_params(params)
+    n, R1, R2 = gt.n, int(pred.R), int(gt.R)
+    T, A = len(thr), len(rng) // 2
+    dev = gt.d_geom.device
+    class_map = np.asarray(class_map, dtype=np.int32).reshape(-1)
+    if class_map.size == 0:
+        class_map = np.full(1, -1, np.int32)
+    score_code = {torch.float32: N.MRX_F32, torch.float64: N.MRX_F64}[pred_scores.dtype]
+    st = N.stream_ptr(stream)
+    # everything that comes back lives in one device blob, each part at a multiple of 16 bytes
+    shapes = [("counts", (n,), np.int32), ("cat", (n, R1), np.int32), ("rank", (n, R1), np.int32),
+              ("keep", (n, R1), np.uint8), ("area", (n, R1), np.int64),
+              ("score", (n, R1), np.float64), ("match", (A, T, n, R1), np.int32),
+              ("ignore", (A, T, n, R1), np.uint8)]
+    starts, o = [], 0
+    for _, shape, dt in shapes:
+        starts.append(o)
+        o += (int(np.prod(shape)) * np.dtype(dt).itemsize + 15) // 16 * 16
+    with _stream_ctx(stream):
+        d_crowd, d_area, d_map = _upload_parts(
+            [np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
+             np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map], dev)
+        d_out = torch.empty((max(o, 16),), dtype=torch.uint8, device=dev)
+        v = {name: d_out[a:a + int(np.prod(shape)) * np.dtype(dt).itemsize]
+             .view(_torch_of(dt)).view(shape)
+             for (name, shape, dt), a in zip(shapes, starts)}
+        d_walk = torch.empty((n, R1), dtype=torch.int32, device=dev)
+        d_iou = torch.empty((n, R1, R2), dtype=torch.float64, device=dev)
+        v["counts"].copy_(pred.d_counts[:n])
+        v["area"].copy_(pred.d_areas.view(-1)[:n * R1].view(n, R1))
+        v["score"].copy_(pred_scores[:n])
+        N.check(lib.mrx_coco_ranks(
+            _ptr(pred_class_ids), _ptr(pred_scores), score_code, _ptr(pred.d_counts), _ptr(d_map),
+            int(class_map.size), max_det, _ptr(v["cat"]), _ptr(v["rank"]), _ptr(v["keep"]),
+            _ptr(d_walk), n, R1, st), "mrx_coco_ranks")
+        N.check(lib.mrx_coco_ious(
+            _ptr(pred.d_packed), _ptr(pred.d_packed_off), _ptr(pred.d_counts), _ptr(pred.d_areas),
+            _ptr(pred.d_extents), _ptr(v["cat"]), _ptr(v["keep"]), R1,
+            _ptr(gt.planes.d_packed), _ptr(gt.planes.d_packed_off), _ptr(gt.planes.d_counts),
+            _ptr(gt.planes.d_areas), _ptr(gt.planes.d_extents), _ptr(gt.d_class_ids),
+            _ptr(d_crowd), R2, _ptr(gt.d_geom), _ptr(d_iou), n, st), "mrx_coco_ious")
+        N.check(lib.mrx_coco_match(
+            _ptr(d_iou), _ptr(pred.d_counts), _ptr(v["cat"]), _ptr(v["keep"]), _ptr(d_walk),
+            _ptr(v["area"]), _ptr(gt.d_counts), _ptr(gt.d_class_ids), _ptr(d_crowd), _ptr(d_area),
+            N.double_array(thr), T, N.double_array(rng), A, _ptr(v["match"]), _ptr(v["ignore"]),
+            n, R1, R2, st), "mrx_coco_match")
+        host = d_out.cpu().numpy()         # the one synchronisation
+    out = {name: host[a:a + int(np.prod(shape)) * np.dtype(dt).itemsize].view(dt).reshape(shape)
+           for (name, shape, dt), a in zip(shapes, starts)}
+    out["keep"] = (out["keep"] != 0) & (np.arange(R1)[None, :] < out["counts"][:, None])
+    out["ignore"] = out["ignore"] != 0
+    out["d_iou"] = d_iou
+    return out
 
 
 def trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom, d_regions, layout,

@@ -10,6 +10,11 @@ quicksort, so the order of equal scores and equal IoUs is implementation-defined
 is what a stable sort reversed gives: descending, NaN first, ties larger index first.  Overlaps
 equal NumPy's bit for bit while H*W <= 2^24; above that NumPy's float32 sums stop counting and
 the device rounds the exact counts once each.
+
+`COCOevalSegm` is pycocotools' COCOeval for iouType "segm" (COCO mask AP) as a streaming
+evaluator: the IoUs and matching of `evaluate()` run on the device as each batch is added
+(`mrx_coco_ranks`, `mrx_coco_ious`, `mrx_coco_match`, DESIGN.md section 3.15); `accumulate()` and
+`summarize()` run on the host and equal pycocotools' exactly.
 """
 from __future__ import annotations
 
@@ -132,3 +137,372 @@ def compute_ap_range(gt_box, gt_class_id, gt_mask, pred_box, pred_class_id, pred
     if verbose:
         print("AP @{:.2f}-{:.2f}:\t {:.3f}".format(iou_thresholds[0], iou_thresholds[-1], AP))
     return AP
+
+
+# ----------------------------------------------------------------------------- COCO mask AP
+class Params:
+    """COCOeval's parameters for iouType "segm", with pycocotools' attribute names and defaults.
+    `imgIds` is the sorted ids of the images added so far (it may be set to a subset before
+    `accumulate`); `catIds` is the sorted category ids of the ground truth added so far unless
+    given.  Only `useCats = 1` is supported."""
+
+    def __init__(self, cat_ids=None, iou_thrs=None, rec_thrs=None, max_dets=(1, 10, 100),
+                 area_rng=None, area_rng_lbl=None):
+        self.imgIds = []
+        self.catIds = [] if cat_ids is None else sorted(set(int(c) for c in cat_ids))
+        self.iouThrs = (np.linspace(.5, 0.95, int(np.round((0.95 - .5) / .05)) + 1, endpoint=True)
+                        if iou_thrs is None else np.asarray(iou_thrs, dtype=np.float64))
+        self.recThrs = (np.linspace(.0, 1.00, int(np.round((1.00 - .0) / .01)) + 1, endpoint=True)
+                        if rec_thrs is None else np.asarray(rec_thrs, dtype=np.float64))
+        self.maxDets = sorted(int(m) for m in max_dets)
+        self.areaRng = ([[0 ** 2, 1e5 ** 2], [0 ** 2, 32 ** 2], [32 ** 2, 96 ** 2],
+                         [96 ** 2, 1e5 ** 2]] if area_rng is None else
+                        [[float(lo), float(hi)] for lo, hi in area_rng])
+        self.areaRngLbl = (["all", "small", "medium", "large"] if area_rng_lbl is None
+                           else list(area_rng_lbl))
+        if len(self.areaRngLbl) != len(self.areaRng):
+            raise ValueError(f"{len(self.areaRngLbl)} area labels for {len(self.areaRng)} ranges")
+        self.useCats = 1
+        self.iouType = "segm"
+
+
+class COCOevalSegm:
+    """pycocotools' `COCOeval(cocoGt, cocoDt, "segm")` as a streaming evaluator: batches are added
+    one at a time (`add_batch` with model outputs, `add_results` with COCO segm results), the
+    per-image work of `evaluate()` -- mask IoUs and matching for every (image, category, area
+    range, threshold) -- runs on the device as each batch arrives, and only compact
+    per-detection records stay on the host.  `accumulate()` and `summarize()` then give
+    pycocotools' `eval` arrays (`precision` and `scores` [T, R, K, A, M], `recall` [T, K, A, M],
+    float64, -1 where undefined) and its twelve `stats`, exactly.
+
+    Ground-truth annotations are COCO dicts: `category_id`, `segmentation` an RLE dict ({'size':
+    [H, W], 'counts': compressed `str` / `bytes` or an uncompressed count list}), `iscrowd`
+    (default 0; a crowd region's IoU is intersection / detection area, it absorbs any number of
+    detections and never counts as a miss), and `area` (the annotation's area, which decides its
+    area range; a detection's area is its mask's pixel count).
+
+    Stated differences from pycocotools: matches are recorded by position, where pycocotools
+    stores annotation ids and tests them for truth (so an annotation with id 0 counts as
+    unmatched there); a ground-truth dict without `area` gets its mask's pixel count, where
+    pycocotools raises KeyError; polygon segmentations raise ValueError (rasterise them to RLE
+    first).  `iouThrs`, `areaRng` and `maxDets[-1]` are used on the device as each batch is
+    added, so they must not change after the first batch."""
+
+    def __init__(self, cat_ids=None, iou_thrs=None, rec_thrs=None, max_dets=(1, 10, 100),
+                 area_rng=None, area_rng_lbl=None):
+        from .engine import coco_device_params
+
+        self.params = Params(cat_ids, iou_thrs, rec_thrs, max_dets, area_rng, area_rng_lbl)
+        self._device_params = coco_device_params(self.params)
+        self._auto_cats = cat_ids is None
+        self._frozen = None
+        self._cat_index = {}          # category id -> dense index used on the device
+        self._gt_cats = set()
+        self._img_index = {}          # image id -> position in add order
+        self._dets = []               # per batch: (img, cat, rank, score, matched, ignored)
+        self._gts = []                # per batch: (img, cat, not ignored [n, A])
+        self.eval = {}
+        self.stats = None
+
+    # ------------------------------------------------------------------ adding batches
+    def _dense(self, cat_id):
+        return self._cat_index.setdefault(int(cat_id), len(self._cat_index))
+
+    def _freeze(self):
+        p = self.params
+        key = (tuple(np.ravel(p.iouThrs).tolist()), tuple(np.ravel(p.areaRng).tolist()),
+               int(p.maxDets[-1]))
+        if self._frozen is None:
+            self._frozen = key
+        elif key != self._frozen:
+            raise ValueError("iouThrs, areaRng and maxDets[-1] changed after the first batch")
+        from .engine import coco_device_params
+        self._device_params = coco_device_params(p)
+
+    def _new_images(self, image_ids, n_items, gt_anns, what):
+        if len(image_ids) != n_items:
+            raise ValueError(f"{n_items} {what} but {len(image_ids)} image ids")
+        if len(gt_anns) != len(image_ids):
+            raise ValueError(f"{len(gt_anns)} ground-truth annotation lists for {len(image_ids)} "
+                             "images")
+        seen = set()
+        for i in image_ids:
+            if i in self._img_index or i in seen:
+                raise ValueError(f"image {i!r} was already added")
+            seen.add(i)
+
+    def _gt_tables(self, image_ids, gt_anns, shapes):
+        """Per image: dense category ids, crowd flags, areas (NaN where absent) and RLE dicts,
+        each annotation checked."""
+        cats, crowd, area, rles = [], [], [], []
+        for image_id, anns, hw in zip(image_ids, gt_anns, shapes):
+            c, cr, ar, rl = [], [], [], []
+            for k, ann in enumerate(anns):
+                where = f"image {image_id!r}, annotation {k}" + (
+                    f" (id {ann['id']!r})" if isinstance(ann, dict) and "id" in ann else "")
+                seg = ann.get("segmentation") if isinstance(ann, dict) else None
+                if isinstance(seg, list):
+                    raise ValueError(f"{where}: polygon segmentations are not supported; give "
+                                     "the mask as RLE")
+                if not isinstance(seg, dict) or "counts" not in seg or "size" not in seg:
+                    raise ValueError(f"{where}: segmentation must be an RLE dict with 'size' and "
+                                     "'counts'")
+                size = [int(v) for v in np.ravel(seg["size"])]
+                if hw is not None and size != list(hw):
+                    raise ValueError(f"{where}: RLE size {size} is not the image's {list(hw)}")
+                cat = int(ann["category_id"])
+                self._gt_cats.add(cat)
+                c.append(self._dense(cat))
+                cr.append(1 if ann.get("iscrowd", 0) else 0)
+                ar.append(float(ann["area"]) if "area" in ann else np.nan)
+                rl.append(seg)
+            cats.append(np.asarray(c, np.int32))
+            crowd.append(np.asarray(cr, np.uint8))
+            area.append(np.asarray(ar, np.float64))
+            rles.append(rl)
+        return cats, crowd, area, rles
+
+    def _padded(self, rows, R, dtype):
+        out = np.zeros((len(rows), R), dtype)
+        for b, r in enumerate(rows):
+            out[b, :len(r)] = r
+        return out
+
+    def _record(self, image_ids, res, gt_cats, gt_crowd, gt_area):
+        """Append the per-detection records of one batch (`coco_evaluate_batch`'s dict) and the
+        ground truth's non-ignored flags per area range."""
+        first = len(self._img_index)
+        for b, i in enumerate(image_ids):
+            self._img_index[i] = first + b
+        b, i = np.nonzero(res["keep"])
+        self._dets.append((first + b, res["cat"][b, i], res["rank"][b, i], res["score"][b, i],
+                           res["match"][:, :, b, i].transpose(2, 0, 1) > -1,
+                           res["ignore"][:, :, b, i].transpose(2, 0, 1)))
+        rng = np.asarray(self.params.areaRng, np.float64).reshape(-1, 2)
+        img = np.concatenate([np.full(len(c), first + b, np.int64) for b, c in enumerate(gt_cats)]
+                             + [np.zeros(0, np.int64)])
+        crowd = np.concatenate(gt_crowd + [np.zeros(0, np.uint8)]).astype(bool)
+        area = np.concatenate(gt_area + [np.zeros(0)])
+        nonig = ~crowd[:, None] & (area[:, None] >= rng[:, 0]) & (area[:, None] <= rng[:, 1])
+        self._gts.append((img, np.concatenate(gt_cats + [np.zeros(0, np.int32)]), nonig))
+        p = self.params
+        p.imgIds = sorted(self._img_index)
+        if self._auto_cats:
+            p.catIds = sorted(self._gt_cats)
+
+    def _areas(self, gt, area):
+        """Annotation areas, the mask's pixel count where the annotation has none."""
+        if not any(np.isnan(a).any() for a in area):
+            return area
+        mask_area = gt.planes.d_areas.cpu().numpy()
+        return [np.where(np.isnan(a), mask_area[b, :len(a)], a) for b, a in enumerate(area)]
+
+    def add_batch(self, items, image_ids, gt_anns, category_ids=None):
+        """Evaluate model outputs against COCO ground truth: items as for
+        `api_utils.unmold_detections_batch`, one image id and one list of annotation dicts per
+        item.  The kept instances are expanded straight to packed planes on the device
+        (`enqueue_packed`; no mask or RLE is made), the annotations are decoded there
+        (`MaskBatch.from_rle`), and `category_ids` maps class ids to category ids as in
+        `unmold_coco_results_batch` (None keeps the class id)."""
+        from . import api_utils
+
+        self._new_images(image_ids, len(items), gt_anns, "items")
+        self._freeze()
+        if len(items) == 0:
+            return
+        shapes = [(int(it[2][0]), int(it[2][1])) for it in items]
+        cats, crowd, area, rles = self._gt_tables(image_ids, gt_anns, shapes)
+        with api_utils._Staged(items, canvas=False) as st:
+            eng = st.eng
+            eng.enqueue_packed(st.d_det, st.d_msk)
+            st.meta()                      # raises for bad class ids or boxes
+            gt = eng.ground_truth_rle(cats, rles)
+            area = self._areas(gt, area)
+            class_map = np.full(eng.C, -1, np.int32)
+            for c in range(eng.C):
+                try:
+                    class_map[c] = self._dense(c if category_ids is None else category_ids[c])
+                except (IndexError, KeyError):
+                    pass
+            res = eng.enqueue_coco_eval(gt, self._padded(crowd, gt.R, np.uint8),
+                                        self._padded(area, gt.R, np.float64), class_map,
+                                        self.params)
+        self._record(image_ids, res, cats, crowd, area)
+
+    def add_results(self, results, gt_anns, image_ids):
+        """Evaluate COCO segm results -- dicts {'image_id', 'category_id', 'score',
+        'segmentation': RLE dict} as `loadRes` takes them and `unmold_coco_results_batch`
+        returns them -- against gt_anns[b], the annotation dicts of image_ids[b].  Every result's
+        image must be one of image_ids.  Both sides are decoded on the device; an image's shape
+        is its RLEs' size."""
+        import torch
+
+        from .engine import MaskBatch, Planes, coco_evaluate_batch
+
+        self._new_images(image_ids, len(gt_anns), gt_anns, "annotation lists")
+        self._freeze()
+        if len(image_ids) == 0:
+            return
+        pos = {i: b for b, i in enumerate(image_ids)}
+        dets = [[] for _ in image_ids]
+        for k, r in enumerate(results):
+            if r.get("image_id") not in pos:
+                raise ValueError(f"result {k}: image {r.get('image_id')!r} is not one of the "
+                                 "batch's image ids")
+            seg = r.get("segmentation")
+            if not isinstance(seg, dict) or "counts" not in seg or "size" not in seg:
+                raise ValueError(f"result {k}: segmentation must be an RLE dict with 'size' and "
+                                 "'counts'")
+            dets[pos[r["image_id"]]].append(r)
+        shapes = []
+        for image_id, d, anns in zip(image_ids, dets, gt_anns):
+            sizes = {tuple(int(v) for v in np.ravel(x["segmentation"]["size"])) for x in d}
+            sizes |= {tuple(int(v) for v in np.ravel(a["segmentation"]["size"])) for a in anns
+                      if isinstance(a, dict) and isinstance(a.get("segmentation"), dict)
+                      and "size" in a["segmentation"]}
+            if len(sizes) > 1:
+                raise ValueError(f"image {image_id!r}: RLE sizes {sorted(sizes)} differ")
+            shapes.append(sizes.pop() if sizes else (1, 1))
+        cats, crowd, area, rles = self._gt_tables(image_ids, gt_anns, shapes)
+        N.require_cuda()
+        lib = N.load()
+        dev = torch.device("cuda", torch.cuda.current_device())
+        geoms = [[H, W, H, W, 0, 0, H, W] for H, W in shapes]
+        pred_cls = [np.asarray([self._dense(x["category_id"]) for x in d], np.int32) for d in dets]
+        pred = MaskBatch.from_rle(lib, dev, geoms, pred_cls, [[x["segmentation"] for x in d]
+                                                              for d in dets])
+        gt = MaskBatch.from_rle(lib, dev, geoms, cats, rles)
+        area = self._areas(gt, area)
+        scores = self._padded([[float(x["score"]) for x in d] for d in dets], pred.R, np.float64)
+        d_scores = torch.from_numpy(scores).to(dev)
+        res = coco_evaluate_batch(lib, Planes(*pred.planes), pred.d_class_ids, d_scores, gt,
+                                  self._padded(crowd, gt.R, np.uint8),
+                                  self._padded(area, gt.R, np.float64),
+                                  np.arange(max(len(self._cat_index), 1), dtype=np.int32),
+                                  self.params)
+        self._record(image_ids, res, cats, crowd, area)
+
+    # ------------------------------------------------------------------ pycocotools' API
+    def evaluate(self):
+        """pycocotools runs the per-image evaluation here; this evaluator has already run it on
+        the device as each batch was added, so there is nothing left to do."""
+
+    def accumulate(self):
+        """pycocotools' accumulate over the images of `params.imgIds` (in sorted id order) and
+        the categories of `params.catIds`, vectorised: per category one lexsort of its
+        detections by (-score, image, rank), the maxDets cuts as masks, cumulative sums of the
+        match flags, a running maximum for the precision envelope and searchsorted at
+        `recThrs`.  Bit-equal to pycocotools' loop."""
+        self._freeze()
+        p = self.params
+        img_ids = list(np.unique(p.imgIds)) if len(p.imgIds) else []
+        cat_ids = list(np.unique(p.catIds)) if len(p.catIds) else []
+        T, R, K = len(p.iouThrs), len(p.recThrs), len(cat_ids)
+        A, M = len(p.areaRng), len(p.maxDets)
+        precision = -np.ones((T, R, K, A, M))
+        recall = -np.ones((T, K, A, M))
+        scores = -np.ones((T, R, K, A, M))
+        n_img = len(self._img_index)
+        img_rank = np.full(n_img + 1, -1, np.int64)       # add position -> imgIds position
+        for r, i in enumerate(img_ids):
+            if i in self._img_index:
+                img_rank[self._img_index[i]] = r
+        cat_k = np.full(len(self._cat_index) + 1, -1, np.int64)   # dense -> catIds position
+        for k, c in enumerate(cat_ids):
+            if int(c) in self._cat_index:
+                cat_k[self._cat_index[int(c)]] = k
+
+        def cat(parts, i, empty):
+            return np.concatenate([x[i] for x in parts] + [empty])
+
+        d_img = img_rank[cat(self._dets, 0, np.zeros(0, np.int64))]
+        d_k = cat_k[cat(self._dets, 1, np.zeros(0, np.int32))]
+        d_rank = cat(self._dets, 2, np.zeros(0, np.int32))
+        d_score = cat(self._dets, 3, np.zeros(0))
+        d_tp = cat(self._dets, 4, np.zeros((0, A, T), bool))
+        d_ig = cat(self._dets, 5, np.zeros((0, A, T), bool))
+        g_img = img_rank[cat(self._gts, 0, np.zeros(0, np.int64))]
+        g_k = cat_k[cat(self._gts, 1, np.zeros(0, np.int32))]
+        g_nonig = cat(self._gts, 2, np.zeros((0, A), bool))
+        npig = np.zeros((K + 1, A), np.int64)
+        ok = (g_img >= 0) & (g_k >= 0)
+        np.add.at(npig, g_k[ok], g_nonig[ok])
+        ok = (d_img >= 0) & (d_k >= 0)
+        d_img, d_k, d_rank, d_score, d_tp, d_ig = (x[ok] for x in (d_img, d_k, d_rank, d_score,
+                                                                   d_tp, d_ig))
+        by_k = np.argsort(d_k, kind="stable")
+        bounds = np.searchsorted(d_k[by_k], np.arange(K + 1))
+        eps = np.spacing(1)
+        for k in range(K):
+            if not (npig[k] > 0).any():
+                continue
+            sel = by_k[bounds[k]:bounds[k + 1]]
+            order = sel[np.lexsort((d_rank[sel], d_img[sel], -d_score[sel]))]
+            rank, score = d_rank[order], d_score[order]
+            matched = d_tp[order].transpose(1, 2, 0)        # [A, T, n]
+            ignored = d_ig[order].transpose(1, 2, 0)
+            for m, max_det in enumerate(p.maxDets):
+                cut = rank < max_det
+                s = score[cut]
+                nd = s.size
+                dtm, dtig = matched[:, :, cut], ignored[:, :, cut]
+                tp_sum = np.cumsum(dtm & ~dtig, axis=2).astype(dtype=float)
+                fp_sum = np.cumsum(~dtm & ~dtig, axis=2).astype(dtype=float)
+                for a in range(A):
+                    if npig[k, a] == 0:
+                        continue
+                    tp, fp = tp_sum[a], fp_sum[a]
+                    rc = tp / npig[k, a]
+                    pr = tp / (fp + tp + eps)
+                    recall[:, k, a, m] = rc[:, -1] if nd else 0
+                    pr = np.maximum.accumulate(pr[:, ::-1], axis=1)[:, ::-1]
+                    for t in range(T):
+                        inds = np.searchsorted(rc[t], p.recThrs, side="left")
+                        q = np.zeros(R)
+                        ss = np.zeros(R)
+                        hit = inds < nd
+                        q[hit] = pr[t, inds[hit]]
+                        ss[hit] = s[inds[hit]]
+                        precision[t, :, k, a, m] = q
+                        scores[t, :, k, a, m] = ss
+        self.eval = {"params": p, "counts": [T, R, K, A, M], "precision": precision,
+                     "recall": recall, "scores": scores}
+
+    def summarize(self):
+        """pycocotools' twelve `stats` (each the mean of the entries > -1, or -1 if none), printed
+        in its format."""
+        if not self.eval:
+            raise Exception("Please run accumulate() first")
+        p = self.params
+
+        def _summarize(ap=1, iouThr=None, areaRng="all", maxDets=100):
+            iStr = " {:<18} {} @[ IoU={:<9} | area={:>6s} | maxDets={:>3d} ] = {:0.3f}"
+            titleStr = "Average Precision" if ap == 1 else "Average Recall"
+            typeStr = "(AP)" if ap == 1 else "(AR)"
+            iouStr = "{:0.2f}:{:0.2f}".format(p.iouThrs[0], p.iouThrs[-1]) \
+                if iouThr is None else "{:0.2f}".format(iouThr)
+            aind = [i for i, aRng in enumerate(p.areaRngLbl) if aRng == areaRng]
+            mind = [i for i, mDet in enumerate(p.maxDets) if mDet == maxDets]
+            s = self.eval["precision"] if ap == 1 else self.eval["recall"]
+            if iouThr is not None:
+                s = s[np.where(iouThr == p.iouThrs)[0]]
+            s = s[:, :, :, aind, mind] if ap == 1 else s[:, :, aind, mind]
+            mean_s = -1 if len(s[s > -1]) == 0 else np.mean(s[s > -1])
+            print(iStr.format(titleStr, typeStr, iouStr, areaRng, maxDets, mean_s))
+            return mean_s
+
+        md = p.maxDets
+        stats = np.zeros((12,))
+        stats[0] = _summarize(1)
+        stats[1] = _summarize(1, iouThr=.5, maxDets=md[2])
+        stats[2] = _summarize(1, iouThr=.75, maxDets=md[2])
+        stats[3] = _summarize(1, areaRng="small", maxDets=md[2])
+        stats[4] = _summarize(1, areaRng="medium", maxDets=md[2])
+        stats[5] = _summarize(1, areaRng="large", maxDets=md[2])
+        stats[6] = _summarize(0, maxDets=md[0])
+        stats[7] = _summarize(0, maxDets=md[1])
+        stats[8] = _summarize(0, maxDets=md[2])
+        stats[9] = _summarize(0, areaRng="small", maxDets=md[2])
+        stats[10] = _summarize(0, areaRng="medium", maxDets=md[2])
+        stats[11] = _summarize(0, areaRng="large", maxDets=md[2])
+        self.stats = stats

@@ -134,6 +134,22 @@ def jitter_ground_truth(im, rng, max_shift=8, class_flip_frac=0.1):
     return SynthImage(det, im.mrcnn_mask, im.original_image_shape, im.image_shape, im.window, n)
 
 
+def jitter_coco_ground_truth(im, rng, crowd_frac=0.1, **kw):
+    """`jitter_ground_truth` plus the COCO annotation fields that are not the mask: about
+    `crowd_frac` of the instances marked iscrowd, and annotation areas (which COCOeval's area
+    ranges use instead of the mask's pixel count) drawn around and on the 32^2 and 96^2
+    boundaries and across all three ranges.  Returns (SynthImage, iscrowd int [n], area
+    float64 [n])."""
+    jit = jitter_ground_truth(im, rng, **kw)
+    n = im.n_valid
+    iscrowd = (rng.random(n) < crowd_frac).astype(np.int64)
+    edges = np.array([32.0 ** 2 - 1, 32.0 ** 2, 32.0 ** 2 + 0.5, 96.0 ** 2 - 0.5, 96.0 ** 2,
+                      96.0 ** 2 + 1])
+    spread = np.exp(rng.uniform(np.log(10.0), np.log(1e5), size=n)).round(1)
+    area = np.where(rng.random(n) < 0.3, edges[rng.integers(0, edges.size, size=n)], spread)
+    return jit, iscrowd, area
+
+
 def synth_rgb_image(rng, h, w):
     """uint8 RGB image with smooth structure + noise (for the mold step)."""
     yy, xx = np.mgrid[0:h, 0:w]

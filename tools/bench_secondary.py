@@ -4,6 +4,7 @@ numbers go into README.md.  One JSON line per workload on stdout; the COCO compr
 each unmold workload also names the GPU and its power limit.
 
   python tools/bench_secondary.py [--iters 20] [--cpu]     (--cpu also times the oracle)
+  python tools/bench_secondary.py --only-eval | --only-cocoeval
 """
 import argparse
 import ctypes as C
@@ -230,6 +231,125 @@ def eval_case(iters, cpu):
     torch.cuda.empty_cache()
 
 
+def cocoeval_case(iters, n_batches=4):
+    """COCO mask AP over a stream of configs[1]-shaped batches: 32 x 1024x1024, 100 predictions
+    against the 100 instances of the same image jittered, about 10 % of them crowd regions
+    (synth.jitter_coco_ground_truth), default COCOeval params.  The three kernels alone on one
+    batch, add_batch end to end per batch (input upload, unmold, packed expand, ground-truth
+    decode, the kernels and the download), accumulate() over the whole stream, and the restated
+    pycocotools evaluate (computeIoU + evaluateImg, tests/cocoeval_oracle.py) per image on the
+    host."""
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, evaluate
+    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import coco_device_params
+
+    batch, base_n = 32, 4
+    base = synth.make_batch(11, base_n, (1024, 1024), 100)
+    rng = np.random.default_rng(12)
+    jit = [synth.jitter_coco_ground_truth(im, rng, crowd_frac=0.1, max_shift=12) for im in base]
+    jit_items = [(j.detections, j.mrcnn_mask, j.original_image_shape, j.image_shape, j.window)
+                 for j, _, _ in jit]
+    gt_rle = api_utils.unmold_detections_rle_batch(jit_items, compressed=True)
+    base_anns = [[{"category_id": int(c), "iscrowd": int(cr), "area": float(a), "segmentation": r}
+                  for c, cr, a, r in zip(g[1], crowd, area, g[3])]
+                 for g, (_, crowd, area) in zip(gt_rle, jit)]
+    items = [(im.detections, im.mrcnn_mask, im.original_image_shape, im.image_shape, im.window)
+             for im in (base[i % base_n] for i in range(batch))]
+    anns = [base_anns[i % base_n] for i in range(batch)]
+    ev = evaluate.COCOevalSegm()
+    per_batch = []
+    for k in range(n_batches):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        ev.add_batch(items, list(range(k * batch, (k + 1) * batch)), anns)
+        per_batch.append((time.perf_counter() - t0) * 1e3)
+    t0 = time.perf_counter()
+    ev.accumulate()
+    acc_ms = (time.perf_counter() - t0) * 1e3
+    with open(os.devnull, "w") as null:
+        stdout, sys.stdout = sys.stdout, null
+        try:
+            ev.summarize()
+        finally:
+            sys.stdout = stdout
+    n_dets = int(sum(d[0].size for d in ev._dets))
+
+    # the kernels alone on one planned batch
+    eng = UnmoldEngine(batch, 100, (28, 28), 81)
+    eng.plan([make_geom(*it[2:]) for it in items], canvas=False)
+    d_det = torch.from_numpy(np.stack([it[0] for it in items])).cuda()
+    d_msk = torch.from_numpy(np.stack([it[1] for it in items])).cuda()
+    eng.enqueue_packed(d_det, d_msk)
+    gt = eng.ground_truth_rle([np.array([a["category_id"] for a in x], np.int32) for x in anns],
+                              [[a["segmentation"] for a in x] for x in anns])
+    crowd = np.zeros((batch, gt.R), np.uint8)
+    area = np.zeros((batch, gt.R))
+    for b, x in enumerate(anns):
+        crowd[b, :len(x)] = [a["iscrowd"] for a in x]
+        area[b, :len(x)] = [a["area"] for a in x]
+    res = eng.enqueue_coco_eval(gt, crowd, area, np.arange(81, dtype=np.int32), ev.params)
+    thr, rngs, max_det = coco_device_params(ev.params)
+    n, R1, R2, T, A = batch, eng.R, gt.R, len(thr), len(rngs) // 2
+    dev = eng.device
+    P = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+    d_map = torch.arange(81, dtype=torch.int32, device=dev)
+    d_cat = torch.empty((n, R1), dtype=torch.int32, device=dev)
+    d_rank, d_walk = torch.empty_like(d_cat), torch.empty_like(d_cat)
+    d_keep = torch.empty((n, R1), dtype=torch.uint8, device=dev)
+    d_crowd = torch.from_numpy(crowd).to(dev)
+    d_area = torch.from_numpy(area).to(dev)
+    d_pa = eng._eval_bufs["areas"]
+    d_match = torch.empty((A, T, n, R1), dtype=torch.int32, device=dev)
+    d_ign = torch.empty((A, T, n, R1), dtype=torch.uint8, device=dev)
+    d_iou = res["d_iou"]
+    st = N.stream_ptr(None)
+    ranks = lambda: N.check(eng.lib.mrx_coco_ranks(  # noqa: E731
+        P(eng.d_class_ids), P(eng.d_scores), N.MRX_F32, P(eng.d_counts), P(d_map), 81, max_det,
+        P(d_cat), P(d_rank), P(d_keep), P(d_walk), n, R1, st), "mrx_coco_ranks")
+    ious = lambda: N.check(eng.lib.mrx_coco_ious(  # noqa: E731
+        P(eng.d_packed), P(eng.d_packed_off), P(eng.d_counts), P(d_pa),
+        P(eng._eval_bufs["extents"]), P(d_cat), P(d_keep), R1, P(gt.planes.d_packed),
+        P(gt.planes.d_packed_off), P(gt.d_counts), P(gt.planes.d_areas), P(gt.planes.d_extents),
+        P(gt.d_class_ids), P(d_crowd), R2, P(gt.d_geom), P(d_iou), n, st), "mrx_coco_ious")
+    match = lambda: N.check(eng.lib.mrx_coco_match(  # noqa: E731
+        P(d_iou), P(eng.d_counts), P(d_cat), P(d_keep), P(d_walk), P(d_pa), P(gt.d_counts),
+        P(gt.d_class_ids), P(d_crowd), P(d_area), N.double_array(thr), T, N.double_array(rngs), A,
+        P(d_match), P(d_ign), n, R1, R2, st), "mrx_coco_match")
+    ranks()
+    rank_ms, _ = time_ms(ranks, iters)
+    iou_ms, _ = time_ms(ious, iters)
+    match_ms, _ = time_ms(match, iters)
+
+    # the restated pycocotools evaluate on the host, one image
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import cocoeval_oracle as co
+    _, cls, scores, masks = api_utils.unmold_detections_batch(items[:1])[0]
+    gts = [{"image_id": 0, "category_id": a["category_id"], "mask": gm, "iscrowd": a["iscrowd"],
+            "area": a["area"]}
+           for a, gm in zip(anns[0], np.moveaxis(api_utils.unmold_detections_batch(
+               jit_items[:1])[0][3], 2, 0))]
+    dts = [{"image_id": 0, "category_id": int(c), "mask": masks[:, :, i], "score": float(s)}
+           for i, (c, s) in enumerate(zip(cls, scores))]
+    oracle = co.COCOevalOracle(gts, dts)
+    t0 = time.perf_counter()
+    oracle.evaluate()
+    host_ms = (time.perf_counter() - t0) * 1e3
+    print(json.dumps({
+        "workload": f"COCOeval segm: {n_batches} batches of configs[1] 32 x 1024x1024, "
+                    "100 predictions vs 100 jittered gt (~10 % crowd), default params",
+        "detections_recorded": n_dets, "gt_crowd": int(sum(int(c.sum()) for _, c, _ in jit)) * (batch // base_n),
+        "stats_0_AP": round(float(ev.stats[0]), 4),
+        "ranks_kernel_ms": round(rank_ms, 4), "ious_kernel_ms": round(iou_ms, 4),
+        "match_kernel_ms_40_area_thresholds": round(match_ms, 4),
+        "add_batch_ms_per_batch": [round(t, 1) for t in per_batch],
+        "accumulate_ms_whole_stream": round(acc_ms, 1),
+        "host_oracle_evaluate_ms_per_image": round(host_ms, 1),
+        "note": "add_batch: H2D of the configs[1] inputs (28x28x81 float32 tiles), unmold, packed "
+                "expand, gt decode from compressed strings, the three kernels, one download",
+        **card()}), flush=True)
+    del eng, d_det, d_msk, gt, res, d_iou
+    torch.cuda.empty_cache()
+
+
 def rle_gt_record(eng, gts, base_rle, base_n, items, thr10, iters):
     """The ground truth of eval_case as COCO compressed strings: mrx_rle_parse, mrx_rle_decode
     and the whole-image mrx_mask_extents alone on the uploaded strings, and
@@ -355,8 +475,12 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--cpu", action="store_true")
     ap.add_argument("--only-eval", action="store_true", help="only the mask IoU / AP record")
+    ap.add_argument("--only-cocoeval", action="store_true", help="only the COCO mask AP record")
     args = ap.parse_args()
     torch.cuda.set_device(0)
+    if args.only_cocoeval:
+        cocoeval_case(args.iters)
+        return
     eval_case(args.iters, args.cpu)
     if args.only_eval:
         return
