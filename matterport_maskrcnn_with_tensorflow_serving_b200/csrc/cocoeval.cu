@@ -7,9 +7,10 @@
 //                      order (descending, ties smaller index first, NaN last), whether that rank
 //                      is below maxDets[-1], and the image's walk order (the same order across
 //                      categories), by counting
-//   coco_iou_kernel    CTA per (image, prediction), warp per ground-truth instance, as
-//                      mask_overlaps_kernel: only pairs of one category whose prediction is kept;
-//                      a pair whose extents do not meet gets 0 without a read
+//   coco_iou_kernel    CTA per (image, prediction), warp per ground-truth instance: the pair walk
+//                      of mask_overlaps_kernel (walk_pairs, planes.cuh) over the pairs of one
+//                      category whose prediction is kept; a pair whose extents do not meet gets 0
+//                      without a read
 //   coco_match_kernel  warp per (image, threshold, area range): predictions in walk order, each
 //                      takes the argmax of (not ignored, IoU, position) over its candidates
 //
@@ -22,8 +23,8 @@ namespace mrx {
 namespace cocoeval {
 
 using overlaps::Planes;
-using overlaps::and_count;
-using overlaps::plane_of;
+using overlaps::score_at;
+using overlaps::walk_pairs;
 
 constexpr int kWarps = 8;
 
@@ -39,11 +40,6 @@ struct RankParams {
   int *walk;                  // [B, R]
   int R, C, score_f64, max_det;
 };
-
-__device__ __forceinline__ double score_at(const void *scores, int f64, size_t i) {
-  return f64 ? static_cast<const double *>(scores)[i]
-             : static_cast<double>(static_cast<const float *>(scores)[i]);
-}
 
 // k comes before i in np.argsort(-score, kind="mergesort"): numbers before NaN, higher scores
 // first, equal scores (and NaN among NaN) by index
@@ -86,32 +82,18 @@ coco_iou_kernel(const Planes p1, const Planes p2, const int *__restrict__ geom,
                 const int *__restrict__ gt_cat, const unsigned char *__restrict__ gt_crowd,
                 double *__restrict__ out) {
   const int i = blockIdx.x, b = blockIdx.y;
-  const int N = p1.counts[b], M = p2.counts[b];
-  if (i >= N) return;
+  if (i >= p1.counts[b]) return;
   const size_t i1 = static_cast<size_t>(b) * p1.R + i;
   if (!pred_keep[i1]) return;
   const int ci = pred_cat[i1];
-  const int H = geom[b * MRX_GEOM_INTS + 0], W = geom[b * MRX_GEOM_INTS + 1];
-  const int wb = (W + 7) >> 3;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const long long a1 = p1.areas[i1];
-  const int4 e1 = p1.extents[i1];
-  const unsigned char *plane1 = plane_of(p1.packed, b, i, H, wb);
+  const size_t gb = static_cast<size_t>(b) * p2.R;
   double *row = out + i1 * p2.R;
-  for (int j = warp; j < M; j += kWarps) {
-    const size_t i2 = static_cast<size_t>(b) * p2.R + j;
-    if (gt_cat[i2] != ci) continue;
-    const long long a2 = p2.areas[i2];
-    const int4 e2 = p2.extents[i2];
-    const int y1 = max(e1.x, e2.x), x1 = max(e1.y, e2.y), y2 = min(e1.z, e2.z), x2 = min(e1.w, e2.w);
-    long long inter = 0;
-    if (a1 && a2 && y2 > y1 && x2 > x1)
-      inter = and_count(plane1, plane_of(p2.packed, b, j, H, wb), wb, y1, x1, y2, x2, lane);
-    if (lane == 0) {
-      const long long u = gt_crowd[i2] ? a1 : a1 + a2 - inter;
-      row[j] = inter ? __ddiv_rn(static_cast<double>(inter), static_cast<double>(u)) : 0.0;
-    }
-  }
+  walk_pairs<kWarps>(
+      p1, p2, geom, b, i, [&](int j) { return gt_cat[gb + j] == ci; },
+      [&](int j, long long inter, long long a1, long long a2) {
+        const long long u = gt_crowd[gb + j] ? a1 : a1 + a2 - inter;
+        row[j] = inter ? __ddiv_rn(static_cast<double>(inter), static_cast<double>(u)) : 0.0;
+      });
 }
 
 // ---------------------------------------------------------------- matches
@@ -233,20 +215,13 @@ extern "C" int mrx_coco_ious(const unsigned char *d_packed1, const long long *d_
                              const int *d_extents2, const int *d_gt_cat,
                              const unsigned char *d_gt_crowd, int R2, const int *d_geom,
                              double *d_iou, int B, void *stream) {
-  const char *fn = "mrx_coco_ious";
-  if (int rc = check_slots(fn, d_packed1, d_packed_off1, d_counts1, d_geom, B, R1)) return rc;
-  if (int rc = check_slots(fn, d_packed2, d_packed_off2, d_counts2, d_geom, B, R2)) return rc;
-  MRX_CHECK_ARG(d_areas1 && d_extents1 && d_areas2 && d_extents2, "%s: null areas or extents", fn);
-  MRX_CHECK_ARG(d_pred_cat && d_pred_keep && d_gt_cat && d_gt_crowd && d_iou, "%s: null pointer",
-                fn);
-  MRX_CHECK_ARG(((reinterpret_cast<uintptr_t>(d_packed1) | reinterpret_cast<uintptr_t>(d_packed2)) &
-                 3u) == 0u,
-                "%s: packed bases must be 4-byte aligned", fn);
+  overlaps::Planes p1, p2;
+  if (int rc = overlaps::check_plane_pair(
+          "mrx_coco_ious", d_packed1, d_packed_off1, d_counts1, d_areas1, d_extents1, R1,
+          d_packed2, d_packed_off2, d_counts2, d_areas2, d_extents2, R2, d_geom, B,
+          d_pred_cat && d_pred_keep && d_gt_cat && d_gt_crowd && d_iou, p1, p2))
+    return rc;
   if (B == 0) return MRX_OK;
-  const overlaps::Planes p1{{d_packed1, d_packed_off1}, d_counts1, d_areas1,
-                            reinterpret_cast<const int4 *>(d_extents1), R1};
-  const overlaps::Planes p2{{d_packed2, d_packed_off2}, d_counts2, d_areas2,
-                            reinterpret_cast<const int4 *>(d_extents2), R2};
   cocoeval::coco_iou_kernel<<<dim3(R1, B), cocoeval::kWarps * 32, 0,
                               static_cast<cudaStream_t>(stream)>>>(
       p1, p2, d_geom, d_pred_cat, d_pred_keep, d_gt_cat, d_gt_crowd, d_iou);

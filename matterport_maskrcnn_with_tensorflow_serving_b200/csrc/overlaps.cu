@@ -5,10 +5,9 @@
 //
 //   mask_extents_kernel  CTA per plane: popcount area and tight extent inside a region, warps on
 //                        rows, lanes on bytes
-//   mask_overlaps_kernel CTA per (image, prediction), warp per ground-truth instance: a pair whose
-//                        extents do not meet (or with an empty mask) gets its IoU without a read;
-//                        the others AND and popcount the intersection rectangle, four bytes of a
-//                        row per lane, each realigned from aligned words with a funnel shift
+//   mask_overlaps_kernel CTA per (image, prediction), warp per ground-truth instance: every pair
+//                        through walk_pairs (planes.cuh), so a pair whose extents do not meet (or
+//                        with an empty mask) gets its IoU without a read
 //   mask_rank_kernel     CTA per image: rank of every prediction by score (descending, NaN first,
 //                        ties larger index first), by counting
 //   mask_match_kernel    warp per (image, threshold): predictions in rank order, each takes the
@@ -93,30 +92,15 @@ __global__ void __launch_bounds__(kWarps * 32)
 mask_overlaps_kernel(const Planes p1, const Planes p2, const int *__restrict__ geom,
                      float *__restrict__ out) {
   const int i = blockIdx.x, b = blockIdx.y;
-  const int N = p1.counts[b], M = p2.counts[b];
-  if (i >= N) return;
-  const int H = geom[b * MRX_GEOM_INTS + 0], W = geom[b * MRX_GEOM_INTS + 1];
-  const int wb = (W + 7) >> 3;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const size_t i1 = static_cast<size_t>(b) * p1.R + i;
-  const long long a1 = p1.areas[i1];
-  const int4 e1 = p1.extents[i1];
-  const unsigned char *plane1 = plane_of(p1.packed, b, i, H, wb);
-  float *row = out + i1 * p2.R;
-  for (int j = warp; j < M; j += kWarps) {
-    const size_t i2 = static_cast<size_t>(b) * p2.R + j;
-    const long long a2 = p2.areas[i2];
-    const int4 e2 = p2.extents[i2];
-    const int y1 = max(e1.x, e2.x), x1 = max(e1.y, e2.y), y2 = min(e1.z, e2.z), x2 = min(e1.w, e2.w);
-    long long inter = 0;
-    if (a1 && a2 && y2 > y1 && x2 > x1)
-      inter = and_count(plane1, plane_of(p2.packed, b, j, H, wb), wb, y1, x1, y2, x2, lane);
-    if (lane == 0) {
-      const float fi = __ll2float_rn(inter);
-      const float u = __fsub_rn(__fadd_rn(__ll2float_rn(a1), __ll2float_rn(a2)), fi);
-      row[j] = __fdiv_rn(fi, u);   // 0 / 0 = NaN: both masks empty
-    }
-  }
+  if (i >= p1.counts[b]) return;
+  float *row = out + (static_cast<size_t>(b) * p1.R + i) * p2.R;
+  walk_pairs<kWarps>(
+      p1, p2, geom, b, i, [](int) { return true; },
+      [&](int j, long long inter, long long a1, long long a2) {
+        const float fi = __ll2float_rn(inter);
+        const float u = __fsub_rn(__fadd_rn(__ll2float_rn(a1), __ll2float_rn(a2)), fi);
+        row[j] = __fdiv_rn(fi, u);   // 0 / 0 = NaN: both masks empty
+      });
 }
 
 // ---------------------------------------------------------------- ranks and matches
@@ -135,11 +119,6 @@ struct MatchParams {
   double thresholds[MRX_MAX_IOU_THRESHOLDS];
 };
 
-__device__ __forceinline__ double score_at(const MatchParams &p, size_t i) {
-  return p.score_f64 ? static_cast<const double *>(p.scores)[i]
-                     : static_cast<double>(static_cast<const float *>(p.scores)[i]);
-}
-
 // rank of prediction i = the predictions before it: higher score, NaN above every number, equal
 // scores by larger index (np.argsort(kind="stable")[::-1])
 __global__ void __launch_bounds__(256) mask_rank_kernel(const MatchParams p) {
@@ -147,11 +126,11 @@ __global__ void __launch_bounds__(256) mask_rank_kernel(const MatchParams p) {
   const int N = p.pred_counts[b];
   const size_t base = static_cast<size_t>(b) * p.R1;
   for (int i = threadIdx.x; i < N; i += blockDim.x) {
-    const double si = score_at(p, base + i);
+    const double si = score_at(p.scores, p.score_f64, base + i);
     const bool ni = isnan(si);
     int rank = 0;
     for (int k = 0; k < N; ++k) {
-      const double sk = score_at(p, base + k);
+      const double sk = score_at(p.scores, p.score_f64, base + k);
       const bool nk = isnan(sk);
       const bool tie = (nk && ni) || sk == si;
       rank += (nk && !ni) || (!nk && !ni && sk > si) || (tie && k > i);
@@ -228,19 +207,13 @@ extern "C" int mrx_mask_overlaps(const unsigned char *d_packed1, const long long
                                  const int *d_counts2, const long long *d_areas2,
                                  const int *d_extents2, int R2, const int *d_geom,
                                  float *d_overlaps, int B, void *stream) {
-  const char *fn = "mrx_mask_overlaps";
-  if (int rc = check_slots(fn, d_packed1, d_packed_off1, d_counts1, d_geom, B, R1)) return rc;
-  if (int rc = check_slots(fn, d_packed2, d_packed_off2, d_counts2, d_geom, B, R2)) return rc;
-  MRX_CHECK_ARG(d_areas1 && d_extents1 && d_areas2 && d_extents2, "%s: null areas or extents", fn);
-  MRX_CHECK_ARG(d_overlaps, "%s: null pointer", fn);
-  MRX_CHECK_ARG(((reinterpret_cast<uintptr_t>(d_packed1) | reinterpret_cast<uintptr_t>(d_packed2)) &
-                 3u) == 0u,
-                "%s: packed bases must be 4-byte aligned", fn);
+  overlaps::Planes p1, p2;
+  if (int rc = overlaps::check_plane_pair("mrx_mask_overlaps", d_packed1, d_packed_off1, d_counts1,
+                                          d_areas1, d_extents1, R1, d_packed2, d_packed_off2,
+                                          d_counts2, d_areas2, d_extents2, R2, d_geom, B,
+                                          d_overlaps != nullptr, p1, p2))
+    return rc;
   if (B == 0) return MRX_OK;
-  const overlaps::Planes p1{{d_packed1, d_packed_off1}, d_counts1, d_areas1,
-                            reinterpret_cast<const int4 *>(d_extents1), R1};
-  const overlaps::Planes p2{{d_packed2, d_packed_off2}, d_counts2, d_areas2,
-                            reinterpret_cast<const int4 *>(d_extents2), R2};
   overlaps::mask_overlaps_kernel<<<dim3(R1, B), overlaps::kWarps * 32, 0,
                                    static_cast<cudaStream_t>(stream)>>>(p1, p2, d_geom, d_overlaps);
   MRX_LAUNCH_CHECK("mask_overlaps_kernel");

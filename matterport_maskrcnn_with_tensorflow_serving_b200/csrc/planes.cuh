@@ -1,6 +1,7 @@
-// planes.cuh -- reading two bit-packed plane sets of one batch together: the side description
-// (Planes) and the AND-popcount of an intersection rectangle, shared by mask_overlaps_kernel
-// (overlaps.cu) and coco_iou_kernel (cocoeval.cu).
+// planes.cuh -- reading two bit-packed plane sets of one batch together, shared by the mask scorers
+// mask_overlaps_kernel (overlaps.cu) and coco_iou_kernel (cocoeval.cu): the side description
+// (Planes) and its argument check, the culled walk over the pairs of one prediction with the
+// AND-popcount of their intersection rectangle, and the scores of the rank kernels.
 //
 // Planes are uint8 [N, H, ceil(W/8)], most significant bit first, as mrx_pack_masks /
 // mrx_mask_expand_packed write them.  Pixel x of a row is bit 7 - (x & 7) of byte x >> 3 in every
@@ -21,6 +22,27 @@ struct Planes {
   const int4 *extents;                 // [B, R] (y1, x1, y2, x2), exclusive ends
   int R;
 };
+
+// The checks of mrx_mask_overlaps and mrx_coco_ious on their two plane sets, in the order mrx.h
+// states: "Output slots" for each set, null areas or extents, `outputs` (false when one of the
+// caller's own pointers is null), then 4-byte-aligned bases; every message starts with fn.  On
+// MRX_OK, p1 and p2 describe the two sets.
+inline int check_plane_pair(const char *fn, const unsigned char *packed1, const long long *off1,
+                            const int *counts1, const long long *areas1, const int *extents1,
+                            int R1, const unsigned char *packed2, const long long *off2,
+                            const int *counts2, const long long *areas2, const int *extents2,
+                            int R2, const int *geom, int B, bool outputs, Planes &p1, Planes &p2) {
+  if (int rc = check_slots(fn, packed1, off1, counts1, geom, B, R1)) return rc;
+  if (int rc = check_slots(fn, packed2, off2, counts2, geom, B, R2)) return rc;
+  MRX_CHECK_ARG(areas1 && extents1 && areas2 && extents2, "%s: null areas or extents", fn);
+  MRX_CHECK_ARG(outputs, "%s: null pointer", fn);
+  MRX_CHECK_ARG(((reinterpret_cast<uintptr_t>(packed1) | reinterpret_cast<uintptr_t>(packed2)) &
+                 3u) == 0u,
+                "%s: packed bases must be 4-byte aligned", fn);
+  p1 = {{packed1, off1}, counts1, areas1, reinterpret_cast<const int4 *>(extents1), R1};
+  p2 = {{packed2, off2}, counts2, areas2, reinterpret_cast<const int4 *>(extents2), R2};
+  return MRX_OK;
+}
 
 __device__ __forceinline__ const unsigned char *plane_of(const Slots<const unsigned char> &s,
                                                          int b, int k, int H, int wb) {
@@ -61,6 +83,42 @@ __device__ __forceinline__ long long and_count(const unsigned char *p1, const un
     n += __popc(m);
   }
   return warp_sum(n);
+}
+
+// Plane i of p1 against every plane j < M_b of p2 with keep(j), in image b: one CTA of kWarps
+// warps, a warp per j.  A pair whose extents do not meet (or with an empty mask) gets inter = 0
+// without a read; the others AND and popcount the intersection rectangle, four bytes of a row per
+// lane, each realigned from aligned words with a funnel shift.  Lane 0 then calls
+// emit(j, inter, a1, a2) with the exact counts.
+template <int kWarps, class Keep, class Emit>
+__device__ __forceinline__ void walk_pairs(const Planes &p1, const Planes &p2,
+                                           const int *__restrict__ geom, int b, int i, Keep keep,
+                                           Emit emit) {
+  const int M = p2.counts[b];
+  const int H = geom[b * MRX_GEOM_INTS + 0], W = geom[b * MRX_GEOM_INTS + 1];
+  const int wb = (W + 7) >> 3;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const size_t i1 = static_cast<size_t>(b) * p1.R + i;
+  const long long a1 = p1.areas[i1];
+  const int4 e1 = p1.extents[i1];
+  const unsigned char *plane1 = plane_of(p1.packed, b, i, H, wb);
+  for (int j = warp; j < M; j += kWarps) {
+    if (!keep(j)) continue;
+    const size_t i2 = static_cast<size_t>(b) * p2.R + j;
+    const long long a2 = p2.areas[i2];
+    const int4 e2 = p2.extents[i2];
+    const int y1 = max(e1.x, e2.x), x1 = max(e1.y, e2.y), y2 = min(e1.z, e2.z), x2 = min(e1.w, e2.w);
+    long long inter = 0;
+    if (a1 && a2 && y2 > y1 && x2 > x1)
+      inter = and_count(plane1, plane_of(p2.packed, b, j, H, wb), wb, y1, x1, y2, x2, lane);
+    if (lane == 0) emit(j, inter, a1, a2);
+  }
+}
+
+// score i of a rank kernel's [B, R] scores, float32 or (f64) float64
+__device__ __forceinline__ double score_at(const void *scores, int f64, size_t i) {
+  return f64 ? static_cast<const double *>(scores)[i]
+             : static_cast<double>(static_cast<const float *>(scores)[i]);
 }
 
 }  // namespace overlaps

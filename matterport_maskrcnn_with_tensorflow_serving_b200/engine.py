@@ -38,9 +38,11 @@ def _dtype_code(np_dtype):
 
 
 def _torch_dtype(np_dtype):
+    """The torch dtype of a device tensor holding np_dtype's values (uint32 as int32 bits)."""
     torch = _torch()
-    return {np.dtype(np.float32): torch.float32, np.dtype(np.float64): torch.float64}[
-        np.dtype(np_dtype)]
+    return {np.dtype(np.float32): torch.float32, np.dtype(np.float64): torch.float64,
+            np.dtype(np.int64): torch.int64, np.dtype(np.int32): torch.int32,
+            np.dtype(np.uint32): torch.int32, np.dtype(np.uint8): torch.uint8}[np.dtype(np_dtype)]
 
 
 def _ptr(t):
@@ -60,6 +62,33 @@ def _slot_offsets(sizes, align):
     off = np.zeros(len(sizes) + 1, dtype=np.int64)
     np.cumsum((sizes + align - 1) // align * align, out=off[1:])
     return off
+
+
+def _part_offsets(specs):
+    """int64 [k+1]: where each of k arrays, given as (shape, dtype), starts in one buffer that
+    holds them one after another, each from a multiple of 16 bytes (so a kernel may read any of
+    them as int4); [k] the buffer's size."""
+    return _slot_offsets(np.array([int(np.prod(s)) * np.dtype(d).itemsize for s, d in specs],
+                                  dtype=np.int64), 16)
+
+
+def _part_views(buf, specs):
+    """Typed views of the arrays of `specs` in `buf`, a uint8 NumPy array or device tensor laid
+    out by `_part_offsets`."""
+    host = isinstance(buf, np.ndarray)
+    return [buf[a:a + int(np.prod(s)) * np.dtype(d).itemsize]
+            .view(np.dtype(d) if host else _torch_dtype(d)).reshape(s)
+            for (s, d), a in zip(specs, _part_offsets(specs))]
+
+
+def _upload_parts(parts, device):
+    """One host-to-device copy of NumPy arrays in a buffer laid out by `_part_offsets`; returns
+    typed device views of the same shapes."""
+    specs = [(p.shape, p.dtype) for p in parts]
+    blob = np.zeros(max(int(_part_offsets(specs)[-1]), 16), np.uint8)
+    for v, p in zip(_part_views(blob, specs), parts):
+        v[...] = p
+    return _part_views(_torch().from_numpy(blob).to(device), specs)
 
 
 class BatchLayout:
@@ -170,7 +199,7 @@ class UnmoldEngine:
         self._packed_off_layout = None  # the layout whose packed offsets d_packed_off holds
         self.layout = None              # BatchLayout of the planned batch
         self._contour_bufs = {}     # work and output buffers of trace_contours, grown as needed
-        self._eval_bufs = {}        # prediction areas and extents of enqueue_overlaps
+        self._eval_bufs = {}        # prediction areas and extents of _prediction_planes
         self._overlaps = None       # (ground truth, overlaps) of the last enqueue_overlaps
         self.lock = threading.RLock()
         # pinned staging for fetch_meta (one D2H batch + one synchronisation per call)
@@ -441,22 +470,9 @@ class UnmoldEngine:
         `enqueue_expand_packed` or `pack_masks`); each prediction is read only inside its box.
         Returns the float32 device tensor [n, R, gt.R]: element (b, i, j) for i < N_b, j < M_b is
         the IoU of kept instance i and ground-truth instance j."""
-        if self.layout is None or self.d_packed is None:
-            raise RuntimeError("enqueue_overlaps needs the packed planes: call "
-                               "enqueue_expand_packed or pack_masks first")
-        n = self._n_images
-        if gt.n != n or not np.array_equal(gt.geom, self.layout.geom):
-            raise ValueError("the ground truth was staged for another plan")
-        torch = _torch()
-        bufs = self._eval_bufs
-        d_areas = _buffer(bufs, "areas", n * self.R, torch.int64, self.device)
-        d_ext = _buffer(bufs, "extents", n * self.R * 4, torch.int32, self.device)
-        N.check(self.lib.mrx_mask_extents(
-            _ptr(self.d_packed), _ptr(self.d_packed_off), _ptr(self.d_counts), _ptr(self.d_geom),
-            _ptr(self.d_boxes), _ptr(d_areas), _ptr(d_ext), n, self.R, N.stream_ptr(stream)),
-            "mrx_mask_extents")
-        pred = Planes(self.d_packed, self.d_packed_off, self.d_counts, d_areas, d_ext, self.R)
-        self._overlaps = (gt, mask_overlaps(self.lib, pred, gt.planes, self.d_geom, n, stream))
+        pred = self._prediction_planes(gt, "enqueue_overlaps", stream)
+        self._overlaps = (gt, mask_overlaps(self.lib, pred, gt.planes, self.d_geom,
+                                            self._n_images, stream))
         return self._overlaps[1]
 
     def enqueue_matches(self, gt, thresholds, score_threshold=0.0, stream=None):
@@ -477,9 +493,17 @@ class UnmoldEngine:
         indices), on the packed planes (after `enqueue_expand_packed` or `pack_masks`); each
         prediction is read only inside its box.  class_map [C] maps the engine's class ids to
         dense categories (-1: not evaluated).  Synchronises once; returns its dict."""
+        pred = self._prediction_planes(gt, "enqueue_coco_eval", stream)
+        n = self._n_images
+        return coco_evaluate_batch(self.lib, pred, self.d_class_ids[:n], self.d_scores[:n], gt,
+                                   gt_crowd, gt_area, class_map, params, stream)
+
+    def _prediction_planes(self, gt, fn, stream):
+        """`Planes` of the planned batch's kept instances to score against `gt` (a `MaskBatch` of
+        the same plan), each counted only inside its box (mrx_mask_extents into `_eval_bufs`)."""
         if self.layout is None or self.d_packed is None:
-            raise RuntimeError("enqueue_coco_eval needs the packed planes: call "
-                               "enqueue_expand_packed or pack_masks first")
+            raise RuntimeError(f"{fn} needs the packed planes: call enqueue_expand_packed or "
+                               "pack_masks first")
         n = self._n_images
         if gt.n != n or not np.array_equal(gt.geom, self.layout.geom):
             raise ValueError("the ground truth was staged for another plan")
@@ -491,9 +515,7 @@ class UnmoldEngine:
             _ptr(self.d_packed), _ptr(self.d_packed_off), _ptr(self.d_counts), _ptr(self.d_geom),
             _ptr(self.d_boxes), _ptr(d_areas), _ptr(d_ext), n, self.R, N.stream_ptr(stream)),
             "mrx_mask_extents")
-        pred = Planes(self.d_packed, self.d_packed_off, self.d_counts, d_areas, d_ext, self.R)
-        return coco_evaluate_batch(self.lib, pred, self.d_class_ids[:n], self.d_scores[:n], gt,
-                                   gt_crowd, gt_area, class_map, params, stream)
+        return Planes(self.d_packed, self.d_packed_off, self.d_counts, d_areas, d_ext, self.R)
 
     def pack_masks(self, stream=None):
         """EXTENSION: bit-pack the byte canvases already written for the planned batch
@@ -591,7 +613,7 @@ class MaskBatch:
     def __init__(self, lib, device, geoms, class_ids, masks, stream=None):
         torch = _torch()
         g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
-        n = self.n = g.shape[0]
+        n = g.shape[0]
         if len(masks) != n or len(class_ids) != n:
             raise ValueError(f"{len(masks)} masks and {len(class_ids)} class-id arrays for "
                              f"{n} images")
@@ -606,21 +628,10 @@ class MaskBatch:
             m = m if m.dtype == np.bool_ else m > .5
             staged.append(np.ascontiguousarray(m).view(np.uint8))
             counts[b] = m.shape[2]
-        self.R = R = max(int(counts.max(initial=0)), 1)
-        layout = BatchLayout(g, R, limits=False)
-        self.geom, self.counts = layout.geom, counts
-        cls = _class_id_table(class_ids, n, R)
-        st = N.stream_ptr(stream)
-        with _stream_ctx(stream):
-            self.d_geom = torch.from_numpy(layout.geom).to(device)
-            self.d_counts = torch.from_numpy(counts).to(device)
-            self.d_class_ids = torch.from_numpy(cls).to(device)
-            d_off = torch.from_numpy(layout.packed_off[:-1].copy()).to(device)
-            d_packed = torch.empty((max(int(layout.packed_off[-1]), 1),), dtype=torch.uint8,
-                                   device=device)
+
+        def fill(layout, d_packed, d_off, d_zero):
             canvas = torch.empty((max(max(s.size for s in staged), 1) + 15) // 16 * 16,
                                  dtype=torch.uint8, device=device)
-            d_zero = torch.zeros((1,), dtype=torch.int64, device=device)
             for b, s in enumerate(staged):
                 if s.size == 0:
                     continue
@@ -628,15 +639,12 @@ class MaskBatch:
                 H, W = layout.hw(b)
                 rc = lib.mrx_pack_masks(_ptr(canvas), _ptr(d_zero), _ptr(self.d_counts[b:]),
                                         _ptr(self.d_geom[b:]), _ptr(d_packed), _ptr(d_off[b:]),
-                                        1, R, H, W, st)
+                                        1, layout.R, H, W, N.stream_ptr(stream))
                 if rc == N.MRX_E_UNSUPPORTED:
                     raise ValueError(lib.mrx_last_error().decode())
                 N.check(rc, "mrx_pack_masks")
-            del canvas
-            d_regions = torch.from_numpy(_whole_image_regions(layout.geom, R)).to(device)
-            d_areas, d_ext = _whole_image_extents(lib, d_packed, d_off, self.d_counts, self.d_geom,
-                                                  d_regions, n, R, st)
-        self.planes = Planes(d_packed, d_off, self.d_counts, d_areas, d_ext, R)
+
+        self._stage(lib, device, g, class_ids, counts, [np.zeros(1, np.int64)], fill, stream)
 
     @classmethod
     def from_rle(cls, lib, device, geoms, class_ids, rles, stream=None):
@@ -658,37 +666,15 @@ class MaskBatch:
         torch = _torch()
         self = cls.__new__(cls)
         g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
-        n = self.n = g.shape[0]
         pk = pack_rle(g, class_ids, rles)
-        counts, R = pk["counts"], pk["R"]
-        self.R = R
-        layout = BatchLayout(g, R, limits=False)
-        self.geom, self.counts = layout.geom, counts
-        S = pk["strings"].size
-        # one upload: every table, each at a multiple of 16 bytes (mrx_mask_extents reads the
-        # regions as int4), then the runs and the strings
-        parts = [pk["str_off"], pk["run_off"], layout.packed_off[:-1], pk["run_count"],
-                 np.zeros(n * R, np.int32), counts, _class_id_table(class_ids, n, R).reshape(-1),
-                 layout.geom.reshape(-1), _whole_image_regions(layout.geom, R).reshape(-1),
-                 pk["runs"], pk["strings"]]
-        sizes = [p.nbytes for p in parts]
-        starts = np.concatenate([[0], np.cumsum([(s + 15) // 16 * 16 for s in sizes])])
-        blob = np.zeros(int(starts[-1]), np.uint8)
-        for p, a, s in zip(parts, starts, sizes):
-            blob[a:a + s] = np.ascontiguousarray(p).view(np.uint8).reshape(-1)
-        st = N.stream_ptr(stream)
-        with _stream_ctx(stream):
-            d_blob = torch.from_numpy(blob).to(device)
-            views = [d_blob[a:a + s].view(_torch_of(p.dtype)) for p, a, s in zip(parts, starts, sizes)]
-            (d_str_off, d_run_off, d_off, d_run_count, d_status, self.d_counts, d_cls, d_geom,
-             d_regions, d_uploaded_runs, d_str) = views
-            self.d_class_ids = d_cls.view(n, R)
-            self.d_geom = d_geom.view(n, N.MRX_GEOM_INTS)
+        n, R, S = g.shape[0], pk["R"], pk["strings"].size
+
+        def fill(layout, d_packed, d_off, d_status, d_str_off, d_run_off, d_run_count,
+                 d_uploaded_runs, d_str):
+            st = N.stream_ptr(stream)
             d_runs = torch.empty((max(S + pk["runs"].size, 1),), dtype=torch.int32, device=device)
             d_runs[S:S + pk["runs"].size].copy_(d_uploaded_runs)
             d_ends = torch.empty((d_runs.numel(),), dtype=torch.int64, device=device)
-            d_packed = torch.empty((max(int(layout.packed_off[-1]), 1),), dtype=torch.uint8,
-                                   device=device)
             if S:
                 N.check(lib.mrx_rle_parse(_ptr(d_str), _ptr(d_str_off), _ptr(self.d_counts),
                                           _ptr(d_runs), _ptr(d_run_count), _ptr(d_status), n, R,
@@ -698,16 +684,47 @@ class MaskBatch:
                                        _ptr(self.d_geom), _ptr(d_off), _ptr(d_packed), n, R,
                                        max(layout.max_h, 1), max(layout.max_w, 1), st),
                     "mrx_rle_decode")
-            d_areas, d_ext = _whole_image_extents(lib, d_packed, d_off, self.d_counts, self.d_geom,
-                                                  d_regions.view(n, R, 4), n, R, st)
+
+        d_status, *_ = self._stage(lib, device, g, class_ids, pk["counts"],
+                                   [np.zeros(n * R, np.int32), pk["str_off"], pk["run_off"],
+                                    pk["run_count"], pk["runs"], pk["strings"]], fill, stream)
+        with _stream_ctx(stream):
             status = d_status.cpu().numpy().reshape(n, R)     # the one synchronisation
-            self.extents = d_ext.cpu().numpy()
+            self.extents = self.planes.d_extents.cpu().numpy()
         for b, k in zip(*np.nonzero(status)):
             what = [msg for bit, msg in _RLE_STATUS if status[b, k] & bit]
-            H, W = layout.hw(b)
-            raise ValueError(f"image {b}, instance {k}: " + "; ".join(what).format(hw=H * W))
-        self.planes = Planes(d_packed, d_off, self.d_counts, d_areas, d_ext, R)
+            hw = int(self.geom[b, 0]) * int(self.geom[b, 1])
+            raise ValueError(f"image {b}, instance {k}: " + "; ".join(what).format(hw=hw))
         return self
+
+    def _stage(self, lib, device, geoms, class_ids, counts, extra, fill, stream):
+        """The one staging step of both constructors, once they have checked their input: the
+        layout and the class-id table, one upload of every table (the fill's own arrays `extra`
+        last), the packed slots, fill(layout, d_packed, d_off, *device views of extra) writing
+        the planes, and mrx_mask_extents of every plane over its whole image.  Sets the
+        attributes and `planes`; returns the device views of `extra`."""
+        torch = _torch()
+        n, R = geoms.shape[0], max(int(counts.max(initial=0)), 1)
+        layout = BatchLayout(geoms, R, limits=False)
+        self.n, self.R, self.geom, self.counts = n, R, layout.geom, counts
+        regions = np.zeros((n, R, 4), dtype=np.int32)      # (0, 0, H_b, W_b): the whole image
+        regions[:, :, 2:] = layout.geom[:, None, :2]
+        tables = [layout.packed_off[:-1], counts, _class_id_table(class_ids, n, R), layout.geom,
+                  regions, *extra]
+        with _stream_ctx(stream):
+            d_off, self.d_counts, self.d_class_ids, self.d_geom, d_regions, *d_extra = \
+                _upload_parts(tables, device)
+            d_packed = torch.empty((max(int(layout.packed_off[-1]), 1),), dtype=torch.uint8,
+                                   device=device)
+            fill(layout, d_packed, d_off, *d_extra)
+            d_areas = torch.empty((n, R), dtype=torch.int64, device=device)
+            d_ext = torch.empty((n, R, 4), dtype=torch.int32, device=device)
+            N.check(lib.mrx_mask_extents(_ptr(d_packed), _ptr(d_off), _ptr(self.d_counts),
+                                         _ptr(self.d_geom), _ptr(d_regions), _ptr(d_areas),
+                                         _ptr(d_ext), n, R, N.stream_ptr(stream)),
+                    "mrx_mask_extents")
+        self.planes = Planes(d_packed, d_off, self.d_counts, d_areas, d_ext, R)
+        return d_extra
 
     def set_counts(self, counts, stream=None):
         """Keep only the first counts[b] instances of each image (counts[b] <= M_b), as upstream
@@ -728,13 +745,6 @@ _RLE_STATUS = [
 ]
 
 
-def _torch_of(np_dtype):
-    torch = _torch()
-    return {np.dtype(np.int64): torch.int64, np.dtype(np.int32): torch.int32,
-            np.dtype(np.uint32): torch.int32, np.dtype(np.uint8): torch.uint8,
-            np.dtype(np.float64): torch.float64}[np.dtype(np_dtype)]
-
-
 def _class_id_table(class_ids, n, R):
     """int32 [n, R]: image b's class ids first, zeros after them."""
     cls = np.zeros((n, R), dtype=np.int32)
@@ -744,23 +754,6 @@ def _class_id_table(class_ids, n, R):
             raise ValueError(f"image {b}: class ids must be integers within int32")
         cls[b, :c.size] = c
     return cls
-
-
-def _whole_image_regions(geom, R):
-    """int32 [n, R, 4]: (0, 0, H_b, W_b) for every instance."""
-    regions = np.zeros((geom.shape[0], R, 4), dtype=np.int32)
-    regions[:, :, 2:] = geom[:, None, :2]
-    return regions
-
-
-def _whole_image_extents(lib, d_packed, d_off, d_counts, d_geom, d_regions, n, R, st):
-    torch = _torch()
-    d_areas = torch.empty((n, R), dtype=torch.int64, device=d_packed.device)
-    d_ext = torch.empty((n, R, 4), dtype=torch.int32, device=d_packed.device)
-    N.check(lib.mrx_mask_extents(_ptr(d_packed), _ptr(d_off), _ptr(d_counts), _ptr(d_geom),
-                                 _ptr(d_regions), _ptr(d_areas), _ptr(d_ext), n, R, st),
-            "mrx_mask_extents")
-    return d_areas, d_ext
 
 
 def pack_rle(geoms, class_ids, rles):
@@ -899,20 +892,6 @@ def coco_device_params(params):
     return thr, rng.reshape(-1).tolist(), max_det
 
 
-def _upload_parts(parts, device):
-    """One host-to-device copy of NumPy arrays, each at a multiple of 16 bytes; returns typed
-    device views of the same shapes."""
-    torch = _torch()
-    sizes = [p.nbytes for p in parts]
-    starts = np.concatenate([[0], np.cumsum([(s + 15) // 16 * 16 for s in sizes])]).astype(np.int64)
-    blob = np.zeros(max(int(starts[-1]), 16), np.uint8)
-    for p, a, s in zip(parts, starts, sizes):
-        blob[a:a + s] = np.ascontiguousarray(p).view(np.uint8).reshape(-1)
-    d_blob = torch.from_numpy(blob).to(device)
-    return [d_blob[a:a + s].view(_torch_of(p.dtype)).view(p.shape)
-            for p, a, s in zip(parts, starts, sizes)]
-
-
 def coco_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt_area, class_map,
                         params, stream=None):
     """The per-image half of COCOeval (iouType "segm") for one batch: mrx_coco_ranks,
@@ -940,23 +919,19 @@ def coco_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt
         class_map = np.full(1, -1, np.int32)
     score_code = {torch.float32: N.MRX_F32, torch.float64: N.MRX_F64}[pred_scores.dtype]
     st = N.stream_ptr(stream)
-    # everything that comes back lives in one device blob, each part at a multiple of 16 bytes
-    shapes = [("counts", (n,), np.int32), ("cat", (n, R1), np.int32), ("rank", (n, R1), np.int32),
-              ("keep", (n, R1), np.uint8), ("area", (n, R1), np.int64),
-              ("score", (n, R1), np.float64), ("match", (A, T, n, R1), np.int32),
-              ("ignore", (A, T, n, R1), np.uint8)]
-    starts, o = [], 0
-    for _, shape, dt in shapes:
-        starts.append(o)
-        o += (int(np.prod(shape)) * np.dtype(dt).itemsize + 15) // 16 * 16
+    # everything that comes back lives in one device buffer laid out by _part_offsets
+    parts = {"counts": ((n,), np.int32), "cat": ((n, R1), np.int32), "rank": ((n, R1), np.int32),
+             "keep": ((n, R1), np.uint8), "area": ((n, R1), np.int64),
+             "score": ((n, R1), np.float64), "match": ((A, T, n, R1), np.int32),
+             "ignore": ((A, T, n, R1), np.uint8)}
+    specs = list(parts.values())
     with _stream_ctx(stream):
         d_crowd, d_area, d_map = _upload_parts(
             [np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
              np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map], dev)
-        d_out = torch.empty((max(o, 16),), dtype=torch.uint8, device=dev)
-        v = {name: d_out[a:a + int(np.prod(shape)) * np.dtype(dt).itemsize]
-             .view(_torch_of(dt)).view(shape)
-             for (name, shape, dt), a in zip(shapes, starts)}
+        d_out = torch.empty((max(int(_part_offsets(specs)[-1]), 16),), dtype=torch.uint8,
+                            device=dev)
+        v = dict(zip(parts, _part_views(d_out, specs)))
         d_walk = torch.empty((n, R1), dtype=torch.int32, device=dev)
         d_iou = torch.empty((n, R1, R2), dtype=torch.float64, device=dev)
         v["counts"].copy_(pred.d_counts[:n])
@@ -978,8 +953,7 @@ def coco_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt
             N.double_array(thr), T, N.double_array(rng), A, _ptr(v["match"]), _ptr(v["ignore"]),
             n, R1, R2, st), "mrx_coco_match")
         host = d_out.cpu().numpy()         # the one synchronisation
-    out = {name: host[a:a + int(np.prod(shape)) * np.dtype(dt).itemsize].view(dt).reshape(shape)
-           for (name, shape, dt), a in zip(shapes, starts)}
+    out = dict(zip(parts, _part_views(host, specs)))
     out["keep"] = (out["keep"] != 0) & (np.arange(R1)[None, :] < out["counts"][:, None])
     out["ignore"] = out["ignore"] != 0
     out["d_iou"] = d_iou
@@ -1191,8 +1165,7 @@ class Molder:
         B = len(images)
         dh, dw = int(size_hw[0]), int(size_hw[1])
         sizes = [int(im.shape[0]) * int(im.shape[1]) * 3 for im in images]
-        off = np.zeros(B + 1, dtype=np.int64)
-        np.cumsum((np.asarray(sizes, dtype=np.int64) + 15) // 16 * 16, out=off[1:])
+        off = _slot_offsets(np.asarray(sizes, dtype=np.int64), 16)
         total = int(off[-1])
         if getattr(self, "_h_stage", None) is None or self._h_stage.numel() < total:
             self._h_stage = torch.empty((total,), dtype=torch.uint8).pin_memory()

@@ -21,7 +21,8 @@ from __future__ import annotations
 import numpy as np
 
 from . import _native as N
-from .engine import MaskBatch, mask_matches, mask_overlaps
+from .engine import (MaskBatch, coco_device_params, coco_evaluate_batch, mask_matches,
+                     mask_overlaps)
 
 
 def trim_zeros(x):
@@ -190,8 +191,6 @@ class COCOevalSegm:
 
     def __init__(self, cat_ids=None, iou_thrs=None, rec_thrs=None, max_dets=(1, 10, 100),
                  area_rng=None, area_rng_lbl=None):
-        from .engine import coco_device_params
-
         self.params = Params(cat_ids, iou_thrs, rec_thrs, max_dets, area_rng, area_rng_lbl)
         self._device_params = coco_device_params(self.params)
         self._auto_cats = cat_ids is None
@@ -216,7 +215,6 @@ class COCOevalSegm:
             self._frozen = key
         elif key != self._frozen:
             raise ValueError("iouThrs, areaRng and maxDets[-1] changed after the first batch")
-        from .engine import coco_device_params
         self._device_params = coco_device_params(p)
 
     def _new_images(self, image_ids, n_items, gt_anns, what):
@@ -337,8 +335,6 @@ class COCOevalSegm:
         is its RLEs' size."""
         import torch
 
-        from .engine import MaskBatch, Planes, coco_evaluate_batch
-
         self._new_images(image_ids, len(gt_anns), gt_anns, "annotation lists")
         self._freeze()
         if len(image_ids) == 0:
@@ -375,7 +371,7 @@ class COCOevalSegm:
         area = self._areas(gt, area)
         scores = self._padded([[float(x["score"]) for x in d] for d in dets], pred.R, np.float64)
         d_scores = torch.from_numpy(scores).to(dev)
-        res = coco_evaluate_batch(lib, Planes(*pred.planes), pred.d_class_ids, d_scores, gt,
+        res = coco_evaluate_batch(lib, pred.planes, pred.d_class_ids, d_scores, gt,
                                   self._padded(crowd, gt.R, np.uint8),
                                   self._padded(area, gt.R, np.float64),
                                   np.arange(max(len(self._cat_index), 1), dtype=np.int32),
