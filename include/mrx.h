@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define MRX_ABI_VERSION 12
+#define MRX_ABI_VERSION 13
 
 #define MRX_OK              0
 #define MRX_E_INVALID      -1   /* bad argument (null pointer, size out of range) */
@@ -455,11 +455,15 @@ int mrx_coco_match(const double *d_iou, const int *d_pred_counts, const int *d_p
  * Checks: mrx_rle_parse: null pointers, B outside [0, MRX_MAX_BATCH] or R outside [1, 65534]:
  * MRX_E_INVALID.  mrx_rle_decode: those of "Output slots", then null pointers and the extents.
  * B = 0 returns MRX_OK without launching anything.  Areas and extents: mrx_mask_extents with the
- * whole image as region. */
+ * whole image as region.  The plane of an instance whose status word has any bit is not written;
+ * a batch that mixes RLE with another path (mrx_poly_decode) sets MRX_RLE_ST_SKIP in the status
+ * of that path's instances (empty strings, no runs) before the decode, and ignores their status
+ * afterwards. */
 #define MRX_RLE_ST_CHAR   1   /* a character outside '0' .. '0' + 63 */
 #define MRX_RLE_ST_TRUNC  2   /* the string ends inside a value */
 #define MRX_RLE_ST_RANGE  4   /* a count negative or above 2^32 - 1 (or a value of > 7 groups) */
 #define MRX_RLE_ST_SUM    8   /* the counts do not sum to H*W */
+#define MRX_RLE_ST_SKIP  16   /* set by the caller: another path writes the plane */
 int mrx_rle_parse(const unsigned char *d_str, const long long *d_str_off, const int *d_counts,
                   unsigned int *d_runs, int *d_run_count, int *d_status, int B, int R,
                   void *stream);
@@ -467,6 +471,35 @@ int mrx_rle_decode(const unsigned int *d_runs, const long long *d_run_off, const
                    long long *d_run_end, int *d_status, const int *d_counts, const int *d_geom,
                    const long long *d_packed_off, unsigned char *d_packed, int B, int R,
                    int max_h, int max_w, void *stream);
+
+/* ---------------------------------------------------------------- COCO polygons to packed planes */
+/* EXTENSION: pycocotools' annToRLE of a polygon annotation (frPyObjects: rleFrPoly per part, then
+ * rleMerge with intersect = 0, the union of the parts) decoded, into the packed slots (see
+ * "Output slots"; polygons.cu).  Instance i = b*R + k for k < N_b = d_counts[b].
+ *
+ * d_vert [V, 2] int32: the vertices (x, y) of every part, each coordinate rleFrPoly's
+ *   (int)(5.0 * c + .5) (the caller scales and rounds them, and checks that they and the
+ *   differences of consecutive vertices fit in int); part p's nv_p >= 1 vertices at
+ *   d_part_vert[p] .. d_part_vert[p+1] (d_part_vert [P+1] int64), closed from the last to the
+ *   first.  d_part_inst [P] int32: the instance i of part p.  d_inst_part [B*R+1] int32: instance
+ *   i's parts are d_inst_part[i] .. d_inst_part[i+1], an instance's parts consecutive.
+ * Scratch: d_col_start [C] int64 and d_carry [C] uint8, part p's W_b + 1 entries from
+ *   d_part_col[p] (d_part_col [P] int64); d_tog int32, part p's toggle rows at d_part_tog[p] ..
+ *   d_part_tog[p+1] (d_part_tog [P+1] int64), at least sum over its edges of
+ *   min(W_b, (|dx| + 2) / 5 + 1) + 1 entries (dx: the edge's scaled x difference).
+ * Every byte of the plane k < N_b of an instance with parts, pad bits included, is written, so no
+ * memset is needed; the planes of instances without parts are not touched.  Positions are int64
+ * (pycocotools' int positions overflow once H*W >= 2^31).  max_h, max_w: the extents of "Output
+ * slots", at least 1.
+ * Checks: those of "Output slots", then null pointers, P below 0 and the extents: MRX_E_INVALID.
+ * B = 0 or P = 0 returns MRX_OK without launching anything.  Areas and extents: mrx_mask_extents
+ * with the whole image as region. */
+int mrx_poly_decode(const int *d_vert, const long long *d_part_vert, const int *d_part_inst,
+                    const long long *d_part_col, const long long *d_part_tog, int P,
+                    const int *d_inst_part, int *d_tog, long long *d_col_start,
+                    unsigned char *d_carry, const int *d_counts, const int *d_geom,
+                    const long long *d_packed_off, unsigned char *d_packed, int B, int R,
+                    int max_h, int max_w, void *stream);
 
 /* ---------------------------------------------------------------- multi-GPU gather (8e) */
 /* Peer-memory plumbing for the final gather of the canvases to rank 0 (one process per GPU).

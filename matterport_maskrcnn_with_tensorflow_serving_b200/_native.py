@@ -26,7 +26,7 @@ MRX_GEOM_INTS = 8
 MRX_MAX_BATCH = 4096
 MRX_MAX_MASK_DIM = 64
 MRX_MAX_LANE_MASK_W = 30    # tile width of the lane kernels: mw + 2 lanes per warp
-ABI_VERSION = 12
+ABI_VERSION = 13
 MRX_SCHED_WORDS = 4
 MRX_PEER_HANDLE_BYTES = 64
 MRX_MAX_CONTOUR_SEGMENTS = 1 << 30
@@ -36,6 +36,7 @@ MRX_RLE_ST_CHAR = 1
 MRX_RLE_ST_TRUNC = 2
 MRX_RLE_ST_RANGE = 4
 MRX_RLE_ST_SUM = 8
+MRX_RLE_ST_SKIP = 16
 
 
 def contour_scratch_bytes(total_segments):
@@ -89,6 +90,8 @@ SIGNATURES = {
                             _vp, _i, _i, _i, _vp]),
     "mrx_rle_parse": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "mrx_rle_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "mrx_poly_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                             _i, _i, _i, _i, _vp]),
     "mrx_device_alloc": (_i, [C.c_ulonglong, C.POINTER(C.c_void_p), _ip]),
     "mrx_device_free": (_i, [_vp, C.c_ulonglong]),
     "mrx_peer_alloc": (_i, [C.c_ulonglong, C.POINTER(C.c_void_p)]),

@@ -394,7 +394,10 @@ def unmold_compute_ap_batch(items, gts, iou_thresholds=(0.5,), score_threshold=0
     `annToRLE` returns) or uncompressed count lists -- for every image of the batch.  They are
     decoded on the device (`MaskBatch.from_rle`, which raises ValueError for malformed ones), so
     only the strings and runs are uploaded; the results are the same as for the decoded bool
-    masks.  gt_boxes may be None: the boxes are then upstream's `extract_bboxes` of the decoded
+    masks.  gt_rles may also hold COCO polygon or box lists, next to RLE dicts or alone, as a
+    COCO instances file gives every non-crowd annotation: they are rasterised on the device as
+    pycocotools' annToRLE does (`MaskBatch.from_coco`), with the same results as their RLE.
+    gt_boxes may be None: the boxes are then upstream's `extract_bboxes` of the decoded
     masks (y1, x1, y2, x2, exclusive ends, zeros for an empty mask), read from the device with
     one synchronisation, `trim_zeros`-ed and applied as above; that image's dict also has them
     as `gt_rois` (int32 [M, 4])."""
@@ -405,11 +408,13 @@ def unmold_compute_ap_batch(items, gts, iou_thresholds=(0.5,), score_threshold=0
     if len(items) == 0:
         return []
     thresholds = list(iou_thresholds)
-    rle = [isinstance(g[2], (list, tuple)) and all(isinstance(r, dict) for r in g[2]) for g in gts]
+    rle = [isinstance(g[2], (list, tuple)) and all(isinstance(r, (dict, list)) for r in g[2])
+           for g in gts]
     if any(rle) and not all(rle):
         raise ValueError("ground truth must be bool mask arrays for every image or RLE lists for "
                          "every image")
     rle = all(rle)
+    polygons = rle and any(isinstance(r, list) for g in gts for r in g[2])
     gt_cls, gt_masks = [], []
     for boxes, cls, masks in gts:
         if rle and boxes is None:
@@ -424,7 +429,7 @@ def unmold_compute_ap_batch(items, gts, iou_thresholds=(0.5,), score_threshold=0
         eng = st.eng
         eng.enqueue_packed(st.d_det, st.d_msk)
         if rle:
-            gt = eng.ground_truth_rle(gt_cls, gt_masks)
+            gt = (eng.ground_truth_coco if polygons else eng.ground_truth_rle)(gt_cls, gt_masks)
             keep = gt.counts.copy()
             for b, g in enumerate(gts):
                 if g[0] is None:

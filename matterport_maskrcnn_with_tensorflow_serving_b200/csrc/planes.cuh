@@ -13,6 +13,37 @@
 
 namespace mrx {
 
+// The store of a CTA of kWarps warps that writes one band of 32 rows x 32 * kWarps columns of a
+// packed plane (rle_planes_kernel, poly_planes_kernel): lane l of warp w holds in `word` the
+// column word of column x0 + 32w + (l ^ 7), bit r for row y0 + r.  A 5-step __shfl_xor_sync
+// transpose turns the 32 column words into 32 row words (assigning the columns as lane ^ 7 puts
+// every row word in np.packbits byte order); the band goes through shared memory and leaves as
+// rows of 32 contiguous bytes, byte columns cb0 .. cb0 + 31.  Every byte of the band inside the
+// plane (rows < H, byte columns < wb) is written.  Called by every thread of the CTA.
+template <int kWarps>
+__device__ __forceinline__ void store_band(uint32_t word, uint32_t (&s_band)[32][kWarps],
+                                           unsigned char *plane, int y0, int cb0, int H, int wb) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  // 32 x 32 bit transpose: lane l's bit r is (row r, column l ^ 7); afterwards lane r's bit l is
+#pragma unroll
+  for (int sh = 16; sh > 0; sh >>= 1) {
+    const uint32_t lo_mask = sh == 16 ? 0x0000FFFFu : sh == 8 ? 0x00FF00FFu : sh == 4 ? 0x0F0F0F0Fu
+                             : sh == 2 ? 0x33333333u : 0x55555555u;
+    const uint32_t v = __shfl_xor_sync(0xffffffffu, word, sh);
+    word = (lane & sh) ? (word & ~lo_mask) | ((v >> sh) & lo_mask)
+                       : (word & lo_mask) | ((v << sh) & ~lo_mask);
+  }
+  s_band[lane][warp] = word;   // little endian: byte q holds columns 8q .. 8q + 7, MSB first
+  __syncthreads();
+  const unsigned char *band = reinterpret_cast<const unsigned char *>(s_band);
+  const int cb = cb0 + lane;
+#pragma unroll
+  for (int pass = 0; pass < 32 / kWarps; ++pass) {
+    const int r = pass * kWarps + warp, y = y0 + r;
+    if (y < H && cb < wb) plane[static_cast<long long>(y) * wb + cb] = band[r * 32 + lane];
+  }
+}
+
 namespace overlaps {
 
 struct Planes {

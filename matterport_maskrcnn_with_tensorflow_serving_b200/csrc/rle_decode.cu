@@ -9,16 +9,14 @@
 //                      pass 2^31 when H*W does) and the check that they sum to H*W
 //   rle_planes_kernel  CTA per band of 32 rows x 256 columns of one plane, warp per 32 x 32 block,
 //                      lane per column: the lane finds the run covering its first pixel by binary
-//                      search over the run ends and ORs the ones-runs into a 32-bit column word; a
-//                      5-step __shfl_xor_sync transpose turns 32 column words into 32 row words
-//                      (columns assigned as lane ^ 7, so that every row word is already in
-//                      np.packbits byte order); the band goes through shared memory and leaves as
-//                      rows of 32 contiguous bytes
+//                      search over the run ends and ORs the ones-runs into a 32-bit column word;
+//                      store_band (planes.cuh) transposes the 32 column words of each warp and
+//                      stores the band as rows of 32 contiguous bytes
 //
 // Runs are column-major (Fortran order, pixel (y, x) at x*H + y), starting with zeros.
 #include <climits>
 
-#include "common.cuh"
+#include "planes.cuh"
 
 namespace mrx {
 
@@ -187,25 +185,9 @@ rle_planes_kernel(Slots<unsigned char> packed, const long long *__restrict__ run
       }
     }
   }
-  // 32 x 32 bit transpose: lane l's bit r is (row r, column l ^ 7); afterwards lane r's bit l is
-#pragma unroll
-  for (int sh = 16; sh > 0; sh >>= 1) {
-    const uint32_t lo_mask = sh == 16 ? 0x0000FFFFu : sh == 8 ? 0x00FF00FFu : sh == 4 ? 0x0F0F0F0Fu
-                             : sh == 2 ? 0x33333333u : 0x55555555u;
-    const uint32_t v = __shfl_xor_sync(0xffffffffu, word, sh);
-    word = (lane & sh) ? (word & ~lo_mask) | ((v >> sh) & lo_mask)
-                       : (word & lo_mask) | ((v << sh) & ~lo_mask);
-  }
-  s_band[lane][warp] = word;   // little endian: byte q holds columns 8q .. 8q + 7, MSB first
-  __syncthreads();
-  unsigned char *plane = packed.base + packed.off[b] + static_cast<long long>(k) * H * wb;
-  const unsigned char *band = reinterpret_cast<const unsigned char *>(s_band);
-  const int cb = cb0 + lane;
-#pragma unroll
-  for (int pass = 0; pass < 32 / kWarps; ++pass) {
-    const int r = pass * kWarps + warp, y = y0 + r;
-    if (y < H && cb < wb) plane[static_cast<long long>(y) * wb + cb] = band[r * 32 + lane];
-  }
+  store_band<kWarps>(word, s_band,
+                     packed.base + packed.off[b] + static_cast<long long>(k) * H * wb, y0, cb0, H,
+                     wb);
 }
 
 }  // namespace rle_decode

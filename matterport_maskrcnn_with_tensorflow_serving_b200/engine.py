@@ -5,8 +5,8 @@ every computation on the path is a libmrx kernel launched through ctypes.
 
   UnmoldEngine     batched `unmold_detections` (serve.py:147-154): prologue -> class-tile
                    gather -> fused mask expand, all stream-ordered, no host sync
-  MaskBatch        caller-held masks (ground truth) as packed planes, from bool arrays or COCO
-                   RLE, scored against an engine's masks by `mask_overlaps` / `mask_matches`
+  MaskBatch        caller-held masks (ground truth) as packed planes, from bool arrays, COCO
+                   RLE or COCO polygons, scored against an engine's masks by `mask_overlaps` / `mask_matches`
   AnchorGenerator  `get_anchors` (serve.py:105)
   Molder           the body of `preprocess_input` (serve.py:83-107): cv2.resize + resize_image
                    + mold_image
@@ -464,6 +464,15 @@ class UnmoldEngine:
             raise RuntimeError("plan() first")
         return MaskBatch.from_rle(self.lib, self.device, self.layout.geom, class_ids, rles, stream)
 
+    def ground_truth_coco(self, class_ids, segms, stream=None):
+        """`ground_truth` from COCO `segmentation` values: class_ids[b] [M_b] and segms[b], a
+        list of M_b polygon lists, box lists or RLE dicts (see `MaskBatch.from_coco`, which also
+        states what raises), rasterised and decoded on the device."""
+        if self.layout is None:
+            raise RuntimeError("plan() first")
+        return MaskBatch.from_coco(self.lib, self.device, self.layout.geom, class_ids, segms,
+                                   stream)
+
     def enqueue_overlaps(self, gt, stream=None):
         """EXTENSION: upstream `compute_overlaps_masks(pred_masks, gt_masks)` of every planned image
         against `gt` (a `MaskBatch` from `ground_truth`), on the packed planes (after
@@ -663,34 +672,91 @@ class MaskBatch:
         found on the device: a character outside '0'..'o', a string that ends inside a value, a
         count that is negative or does not fit in uint32, or counts that do not sum to H*W.
         pycocotools decodes such input without a check; this raises instead."""
+        g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
+        return cls._decoded(lib, device, g, class_ids, pack_rle(g, class_ids, rles), None, stream)
+
+    @classmethod
+    def from_coco(cls, lib, device, geoms, class_ids, segms, stream=None):
+        """The same batch from COCO `segmentation` values as a COCO instances file holds them:
+        segms[b] is a list of M_b of them, each a polygon list [[x0, y0, x1, y1, ...], ...], a
+        box list [[x, y, w, h], ...] or an RLE dict (as for `from_rle`); kinds may mix, as crowd
+        RLE sits next to polygons.  Each plane is pycocotools' `decode(annToRLE(ann))` for an
+        annotation of the image's size: a polygon or box list is `frPyObjects` (polygons when the
+        first part has more than 4 numbers, boxes when it has 4) merged as a union, rasterised on
+        the device (mrx_poly_decode) from the scaled vertices `pack_polygons` makes; RLE dicts
+        are decoded as `from_rle` decodes them.  Everything is uploaded once; one synchronisation
+        reads the status words and the extents.
+
+        Raises ValueError naming the image and the instance, before anything is uploaded, for an
+        empty list, a first part of fewer than 4 numbers, a box list with a part that is not 4
+        numbers, a later polygon part of fewer than 2 numbers, a coordinate that is not a finite
+        number, a scaled coordinate (int)(5 * c + .5) or a difference of two consecutive ones
+        outside the int range (pycocotools' behaviour is undefined for all of these but the
+        first three), a value that is neither a list nor a dict, and for RLE dicts what
+        `from_rle` raises.  Positions are exact for any H*W, where pycocotools' int positions
+        overflow once H*W >= 2^31; everything else is bit-exact."""
+        g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
+        pp = pack_polygons(g, class_ids, segms)
+        rles = [[seg if isinstance(seg, dict) else {"size": [int(g[b, 0]), int(g[b, 1])],
+                                                    "counts": b""} for seg in inst]
+                for b, inst in enumerate(segms)]
+        pk = pack_rle(g, class_ids, rles)   # a polygon instance: an empty string, not parsed
+        return cls._decoded(lib, device, g, class_ids, pk, pp, stream)
+
+    @classmethod
+    def _decoded(cls, lib, device, g, class_ids, pk, pp, stream):
+        """`from_rle` (pp None) and `from_coco`: the RLE tables of `pack_rle` and the polygon
+        tables of `pack_polygons` in one upload; the RLE kernels write the planes of the RLE
+        instances (all of them for `from_rle`), mrx_poly_decode those of the polygon ones."""
         torch = _torch()
         self = cls.__new__(cls)
-        g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
-        pk = pack_rle(g, class_ids, rles)
         n, R, S = g.shape[0], pk["R"], pk["strings"].size
+        status = np.zeros(n * R, np.int32)
+        rle_extra = [status, pk["str_off"], pk["run_off"], pk["run_count"], pk["runs"],
+                     pk["strings"]]
+        poly = pp is not None and pp["P"] > 0
+        run_rle = pp is None or bool(pp["rle"].any())
+        if pp is not None:
+            status[pp["poly"]] = N.MRX_RLE_ST_SKIP   # another path's plane: the decode skips it
+        poly_extra = ([pp["vert"], pp["part_vert"], pp["part_inst"], pp["inst_part"],
+                       pp["part_col"], pp["part_tog"]] if poly else [])
 
         def fill(layout, d_packed, d_off, d_status, d_str_off, d_run_off, d_run_count,
-                 d_uploaded_runs, d_str):
+                 d_uploaded_runs, d_str, *d_poly):
             st = N.stream_ptr(stream)
-            d_runs = torch.empty((max(S + pk["runs"].size, 1),), dtype=torch.int32, device=device)
-            d_runs[S:S + pk["runs"].size].copy_(d_uploaded_runs)
-            d_ends = torch.empty((d_runs.numel(),), dtype=torch.int64, device=device)
-            if S:
-                N.check(lib.mrx_rle_parse(_ptr(d_str), _ptr(d_str_off), _ptr(self.d_counts),
-                                          _ptr(d_runs), _ptr(d_run_count), _ptr(d_status), n, R,
-                                          st), "mrx_rle_parse")
-            N.check(lib.mrx_rle_decode(_ptr(d_runs), _ptr(d_run_off), _ptr(d_run_count),
-                                       _ptr(d_ends), _ptr(d_status), _ptr(self.d_counts),
-                                       _ptr(self.d_geom), _ptr(d_off), _ptr(d_packed), n, R,
-                                       max(layout.max_h, 1), max(layout.max_w, 1), st),
-                    "mrx_rle_decode")
+            max_h, max_w = max(layout.max_h, 1), max(layout.max_w, 1)
+            if run_rle:
+                d_runs = torch.empty((max(S + pk["runs"].size, 1),), dtype=torch.int32,
+                                     device=device)
+                d_runs[S:S + pk["runs"].size].copy_(d_uploaded_runs)
+                d_ends = torch.empty((d_runs.numel(),), dtype=torch.int64, device=device)
+                if S:
+                    N.check(lib.mrx_rle_parse(_ptr(d_str), _ptr(d_str_off), _ptr(self.d_counts),
+                                              _ptr(d_runs), _ptr(d_run_count), _ptr(d_status), n,
+                                              R, st), "mrx_rle_parse")
+                N.check(lib.mrx_rle_decode(_ptr(d_runs), _ptr(d_run_off), _ptr(d_run_count),
+                                           _ptr(d_ends), _ptr(d_status), _ptr(self.d_counts),
+                                           _ptr(self.d_geom), _ptr(d_off), _ptr(d_packed), n, R,
+                                           max_h, max_w, st), "mrx_rle_decode")
+            if poly:
+                d_vert, d_part_vert, d_part_inst, d_inst_part, d_part_col, d_part_tog = d_poly
+                n_col, n_tog = int(pp["part_col"][-1]), int(pp["part_tog"][-1])
+                d_tog = torch.empty((max(n_tog, 1),), dtype=torch.int32, device=device)
+                d_col_start = torch.empty((max(n_col, 1),), dtype=torch.int64, device=device)
+                d_carry = torch.empty((max(n_col, 1),), dtype=torch.uint8, device=device)
+                N.check(lib.mrx_poly_decode(
+                    _ptr(d_vert), _ptr(d_part_vert), _ptr(d_part_inst), _ptr(d_part_col),
+                    _ptr(d_part_tog), pp["P"], _ptr(d_inst_part), _ptr(d_tog), _ptr(d_col_start),
+                    _ptr(d_carry), _ptr(self.d_counts), _ptr(self.d_geom), _ptr(d_off),
+                    _ptr(d_packed), n, R, max_h, max_w, st), "mrx_poly_decode")
 
         d_status, *_ = self._stage(lib, device, g, class_ids, pk["counts"],
-                                   [np.zeros(n * R, np.int32), pk["str_off"], pk["run_off"],
-                                    pk["run_count"], pk["runs"], pk["strings"]], fill, stream)
+                                   rle_extra + poly_extra, fill, stream)
         with _stream_ctx(stream):
             status = d_status.cpu().numpy().reshape(n, R)     # the one synchronisation
             self.extents = self.planes.d_extents.cpu().numpy()
+        if pp is not None:
+            status = np.where(pp["poly"].reshape(n, R), 0, status)
         for b, k in zip(*np.nonzero(status)):
             what = [msg for bit, msg in _RLE_STATUS if status[b, k] & bit]
             hw = int(self.geom[b, 0]) * int(self.geom[b, 1])
@@ -825,6 +891,131 @@ def pack_rle(geoms, class_ids, rles):
             "str_off": str_off,
             "runs": np.concatenate(runs) if runs else np.zeros(0, np.uint32),
             "run_off": run_off, "run_count": np.where(is_list, run_len, 0).astype(np.int32)}
+
+
+_INT_MIN, _INT_MAX = -(1 << 31), (1 << 31) - 1
+
+
+def _polygon_parts(segm, where):
+    """The parts of one polygon or box-list annotation as float64 [2V] coordinate arrays, each
+    closed polygon as rleFrPoly receives it (`frPyObjects`' list dispatch on the first part's
+    length; a box [x, y, w, h] becomes rleFrBbox's (x, y) (x, y+h) (x+w, y+h) (x+w, y))."""
+    if len(segm) == 0:
+        raise ValueError(f"{where}: an empty polygon list")
+    parts = []
+    for j, part in enumerate(segm):
+        try:
+            a = np.asarray(part, dtype=np.float64)
+        except (TypeError, ValueError):
+            raise ValueError(f"{where}: part {j} is not a list of numbers") from None
+        if a.ndim != 1:
+            raise ValueError(f"{where}: part {j} is not a flat list of numbers")
+        parts.append(a)
+    n0 = parts[0].size
+    if n0 < 4:
+        raise ValueError(f"{where}: the first part has {n0} numbers; a polygon needs more than "
+                         "4 and a box exactly 4")
+    if n0 == 4:
+        if any(a.size != 4 for a in parts):
+            raise ValueError(f"{where}: a box list (first part of 4 numbers) has a part that is "
+                             "not 4 numbers")
+        out = []
+        for x, y, w, h in parts:
+            xe, ye = x + w, y + h
+            out.append(np.array([x, y, x, ye, xe, ye, xe, y]))
+        return out
+    for j, a in enumerate(parts):
+        if a.size < 2:
+            raise ValueError(f"{where}: part {j} has {a.size} numbers; a polygon part needs at "
+                             "least one vertex")
+    return [a[:a.size // 2 * 2] for a in parts]
+
+
+def pack_polygons(geoms, class_ids, segms):
+    """The host side of `MaskBatch.from_coco`'s polygons, NumPy only: checks every polygon or box
+    list of segms (segms[b] a list of M_b COCO segmentations; RLE dicts are left to `pack_rle`)
+    and lays the batch out for mrx_poly_decode.  Instance i = b*R + k (R = max(1, max M_b)).
+    Each vertex coordinate c becomes rleFrPoly's (int)(5.0 * c + .5): NumPy's multiply, add and
+    trunc round separately, as the C does.  Returns a dict:
+      counts     int32 [n]       M_b
+      R          int
+      P          int             parts of every polygon instance, instance by instance
+      poly       bool [n*R]      instance i is a polygon or box list
+      rle        bool [n*R]      instance i is an RLE dict
+      vert       int32 [V, 2]    the scaled vertices (x, y), part after part
+      part_vert  int64 [P+1]     part p's vertices are vert[part_vert[p]:part_vert[p+1]]
+      part_inst  int32 [P]       part p's instance i
+      inst_part  int32 [n*R+1]   instance i's parts are inst_part[i]:inst_part[i+1]
+      part_col   int64 [P+1]     part p's W_b + 1 column entries start at part_col[p]
+      part_tog   int64 [P+1]     part p's toggle rows: part_tog[p]:part_tog[p+1], a bound of
+                                 min(W_b, (|dx| + 2) // 5 + 1) + 1 per edge"""
+    g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
+    n = g.shape[0]
+    if len(segms) != n or len(class_ids) != n:
+        raise ValueError(f"{len(segms)} segmentation lists and {len(class_ids)} class-id arrays "
+                         f"for {n} images")
+    counts = np.zeros(n, dtype=np.int32)
+    for b, (cls, inst) in enumerate(zip(class_ids, segms)):
+        if np.shape(cls) != (len(inst),):
+            raise ValueError(f"image {b}: {np.shape(cls)} class ids for {len(inst)} "
+                             "segmentations")
+        counts[b] = len(inst)
+    R = max(int(counts.max(initial=0)), 1)
+    poly, rle = np.zeros(n * R, bool), np.zeros(n * R, bool)
+    coords, part_inst = [], []
+    inst_parts = np.zeros(n * R, np.int64)
+    for b, inst in enumerate(segms):
+        for k, segm in enumerate(inst):
+            i, where = b * R + k, f"image {b}, instance {k}"
+            if isinstance(segm, dict):
+                rle[i] = True
+                continue
+            if not isinstance(segm, (list, tuple)):
+                raise ValueError(f"{where}: a segmentation is a polygon list, a box list or an "
+                                 f"RLE dict, got {type(segm).__name__}")
+            poly[i] = True
+            parts = _polygon_parts(segm, where)
+            coords += parts
+            part_inst += [i] * len(parts)
+            inst_parts[i] = len(parts)
+    # the numbers of every part at once: (int)(5.0 * c + .5), then the closed edges
+    P = len(coords)
+    part_inst = np.asarray(part_inst, np.int32)
+    nv = np.array([a.size // 2 for a in coords], np.int64)
+    part_vert = np.zeros(P + 1, np.int64)
+    np.cumsum(nv, out=part_vert[1:])
+    xy = np.concatenate(coords) if P else np.zeros(0)
+    vpart = np.repeat(np.arange(P), nv)          # the part of each vertex
+
+    def fail(bad_vertex, what):
+        i = int(part_inst[vpart[int(np.flatnonzero(bad_vertex)[0])]])
+        raise ValueError(f"image {i // R}, instance {i % R}: {what}")
+
+    fin = np.isfinite(xy).reshape(-1, 2).all(1)
+    if not fin.all():
+        fail(~fin, "a coordinate is NaN or infinite")
+    sc = np.trunc(np.add(np.multiply(5.0, xy), 0.5)).reshape(-1, 2)
+    inr = ((sc >= _INT_MIN) & (sc <= _INT_MAX)).all(1)
+    if not inr.all():
+        fail(~inr, "a coordinate scaled by 5 does not fit in int")
+    v = sc.astype(np.int64)
+    nxt = np.arange(1, v.shape[0] + 1)
+    nxt[part_vert[1:] - 1] = part_vert[:-1]      # the last vertex closes on the first
+    d = np.abs(v[nxt] - v)
+    ok = d.max(1, initial=0) <= _INT_MAX
+    if not ok.all():
+        fail(~ok, "two consecutive vertices scaled by 5 differ by more than int holds")
+    W = g[part_inst // R, 1].astype(np.int64) if P else np.zeros(0, np.int64)
+    edge_tog = np.minimum(W[vpart], (d[:, 0] + 2) // 5 + 1) + 1
+    inst_part = np.zeros(n * R + 1, np.int64)
+    np.cumsum(inst_parts, out=inst_part[1:])
+    part_col, tog_off = np.zeros(P + 1, np.int64), np.zeros(P + 1, np.int64)
+    np.cumsum(W + 1, out=part_col[1:])
+    np.cumsum(np.add.reduceat(edge_tog, part_vert[:-1]) if P else edge_tog, out=tog_off[1:])
+    verts = v.astype(np.int32)
+    return {"counts": counts, "R": R, "P": P, "poly": poly, "rle": rle,
+            "vert": verts, "part_vert": part_vert, "part_inst": part_inst,
+            "inst_part": inst_part.astype(np.int32), "part_col": part_col, "part_tog": tog_off}
 
 
 def mask_overlaps(lib, p1, p2, d_geom, n, stream=None):

@@ -15,6 +15,9 @@ the device rounds the exact counts once each.
 evaluator: the IoUs and matching of `evaluate()` run on the device as each batch is added
 (`mrx_coco_ranks`, `mrx_coco_ious`, `mrx_coco_match`, DESIGN.md section 3.15); `accumulate()` and
 `summarize()` run on the host and equal pycocotools' exactly.
+
+`ann_to_mask` is Matterport's `CocoDataset.annToMask`, rasterised on the device (DESIGN.md
+section 3.16).
 """
 from __future__ import annotations
 
@@ -177,7 +180,10 @@ class COCOevalSegm:
     float64, -1 where undefined) and its twelve `stats`, exactly.
 
     Ground-truth annotations are COCO dicts: `category_id`, `segmentation` an RLE dict ({'size':
-    [H, W], 'counts': compressed `str` / `bytes` or an uncompressed count list}), `iscrowd`
+    [H, W], 'counts': compressed `str` / `bytes` or an uncompressed count list}) or, with
+    `polygons=True`, a polygon or box list as a COCO instances file holds every non-crowd
+    annotation (rasterised on the device as pycocotools' annToRLE does, `MaskBatch.from_coco`),
+    `iscrowd`
     (default 0; a crowd region's IoU is intersection / detection area, it absorbs any number of
     detections and never counts as a miss), and `area` (the annotation's area, which decides its
     area range; a detection's area is its mask's pixel count).
@@ -185,13 +191,15 @@ class COCOevalSegm:
     Stated differences from pycocotools: matches are recorded by position, where pycocotools
     stores annotation ids and tests them for truth (so an annotation with id 0 counts as
     unmatched there); a ground-truth dict without `area` gets its mask's pixel count, where
-    pycocotools raises KeyError; polygon segmentations raise ValueError (rasterise them to RLE
-    first).  `iouThrs`, `areaRng` and `maxDets[-1]` are used on the device as each batch is
+    pycocotools raises KeyError; with the default `polygons=False`, polygon segmentations
+    raise ValueError (rasterise them to RLE first).  Detections are RLE only, with or without
+    `polygons`.  `iouThrs`, `areaRng` and `maxDets[-1]` are used on the device as each batch is
     added, so they must not change after the first batch."""
 
     def __init__(self, cat_ids=None, iou_thrs=None, rec_thrs=None, max_dets=(1, 10, 100),
-                 area_rng=None, area_rng_lbl=None):
+                 area_rng=None, area_rng_lbl=None, polygons=False):
         self.params = Params(cat_ids, iou_thrs, rec_thrs, max_dets, area_rng, area_rng_lbl)
+        self._polygons = bool(polygons)
         self._device_params = coco_device_params(self.params)
         self._auto_cats = cat_ids is None
         self._frozen = None
@@ -230,8 +238,9 @@ class COCOevalSegm:
             seen.add(i)
 
     def _gt_tables(self, image_ids, gt_anns, shapes):
-        """Per image: dense category ids, crowd flags, areas (NaN where absent) and RLE dicts,
-        each annotation checked."""
+        """Per image: dense category ids, crowd flags, areas (NaN where absent) and segmentations
+        (RLE dicts, and polygon or box lists when the evaluator takes them), each annotation
+        checked."""
         cats, crowd, area, rles = [], [], [], []
         for image_id, anns, hw in zip(image_ids, gt_anns, shapes):
             c, cr, ar, rl = [], [], [], []
@@ -239,15 +248,19 @@ class COCOevalSegm:
                 where = f"image {image_id!r}, annotation {k}" + (
                     f" (id {ann['id']!r})" if isinstance(ann, dict) and "id" in ann else "")
                 seg = ann.get("segmentation") if isinstance(ann, dict) else None
-                if isinstance(seg, list):
+                if isinstance(seg, list) and not self._polygons:
                     raise ValueError(f"{where}: polygon segmentations are not supported; give "
                                      "the mask as RLE")
-                if not isinstance(seg, dict) or "counts" not in seg or "size" not in seg:
+                if isinstance(seg, list):
+                    pass                   # checked by pack_polygons, naming the instance
+                elif not isinstance(seg, dict) or "counts" not in seg or "size" not in seg:
                     raise ValueError(f"{where}: segmentation must be an RLE dict with 'size' and "
                                      "'counts'")
-                size = [int(v) for v in np.ravel(seg["size"])]
-                if hw is not None and size != list(hw):
-                    raise ValueError(f"{where}: RLE size {size} is not the image's {list(hw)}")
+                if isinstance(seg, dict):
+                    size = [int(v) for v in np.ravel(seg["size"])]
+                    if hw is not None and size != list(hw):
+                        raise ValueError(f"{where}: RLE size {size} is not the image's "
+                                         f"{list(hw)}")
                 cat = int(ann["category_id"])
                 self._gt_cats.add(cat)
                 c.append(self._dense(cat))
@@ -301,7 +314,8 @@ class COCOevalSegm:
         item.  The kept instances are expanded straight to packed planes on the device
         (`enqueue_packed`; no mask or RLE is made), the annotations are decoded there
         (`MaskBatch.from_rle`), and `category_ids` maps class ids to category ids as in
-        `unmold_coco_results_batch` (None keeps the class id)."""
+        `unmold_coco_results_batch` (None keeps the class id).  With `polygons=True` the
+        annotations may be polygon or box lists, rasterised there (`MaskBatch.from_coco`)."""
         from . import api_utils
 
         self._new_images(image_ids, len(items), gt_anns, "items")
@@ -314,7 +328,7 @@ class COCOevalSegm:
             eng = st.eng
             eng.enqueue_packed(st.d_det, st.d_msk)
             st.meta()                      # raises for bad class ids or boxes
-            gt = eng.ground_truth_rle(cats, rles)
+            gt = (eng.ground_truth_coco if self._polygons else eng.ground_truth_rle)(cats, rles)
             area = self._areas(gt, area)
             class_map = np.full(eng.C, -1, np.int32)
             for c in range(eng.C):
@@ -327,15 +341,19 @@ class COCOevalSegm:
                                         self.params)
         self._record(image_ids, res, cats, crowd, area)
 
-    def add_results(self, results, gt_anns, image_ids):
+    def add_results(self, results, gt_anns, image_ids, image_shapes=None):
         """Evaluate COCO segm results -- dicts {'image_id', 'category_id', 'score',
         'segmentation': RLE dict} as `loadRes` takes them and `unmold_coco_results_batch`
         returns them -- against gt_anns[b], the annotation dicts of image_ids[b].  Every result's
         image must be one of image_ids.  Both sides are decoded on the device; an image's shape
-        is its RLEs' size."""
+        is its RLEs' size, or image_shapes[b] = (height, width) when given (the RLEs must agree
+        with it).  An image whose ground truth has polygons (`polygons=True`) and no RLE at all
+        has no size to take, so it needs image_shapes; without it this raises ValueError."""
         import torch
 
         self._new_images(image_ids, len(gt_anns), gt_anns, "annotation lists")
+        if image_shapes is not None and len(image_shapes) != len(image_ids):
+            raise ValueError(f"{len(image_shapes)} image shapes for {len(image_ids)} images")
         self._freeze()
         if len(image_ids) == 0:
             return
@@ -356,8 +374,14 @@ class COCOevalSegm:
             sizes |= {tuple(int(v) for v in np.ravel(a["segmentation"]["size"])) for a in anns
                       if isinstance(a, dict) and isinstance(a.get("segmentation"), dict)
                       and "size" in a["segmentation"]}
+            if image_shapes is not None:
+                sizes.add(tuple(int(v) for v in image_shapes[len(shapes)]))
             if len(sizes) > 1:
                 raise ValueError(f"image {image_id!r}: RLE sizes {sorted(sizes)} differ")
+            if not sizes and self._polygons and any(isinstance(a, dict) and isinstance(a.get("segmentation"), list)
+                                 for a in anns):
+                raise ValueError(f"image {image_id!r}: its ground truth is polygons only, so its "
+                                 "shape is unknown; give it in image_shapes")
             shapes.append(sizes.pop() if sizes else (1, 1))
         cats, crowd, area, rles = self._gt_tables(image_ids, gt_anns, shapes)
         N.require_cuda()
@@ -367,7 +391,8 @@ class COCOevalSegm:
         pred_cls = [np.asarray([self._dense(x["category_id"]) for x in d], np.int32) for d in dets]
         pred = MaskBatch.from_rle(lib, dev, geoms, pred_cls, [[x["segmentation"] for x in d]
                                                               for d in dets])
-        gt = MaskBatch.from_rle(lib, dev, geoms, cats, rles)
+        gt = (MaskBatch.from_coco if self._polygons else MaskBatch.from_rle)(lib, dev, geoms, cats,
+                                                                            rles)
         area = self._areas(gt, area)
         scores = self._padded([[float(x["score"]) for x in d] for d in dets], pred.R, np.float64)
         d_scores = torch.from_numpy(scores).to(dev)
@@ -502,3 +527,21 @@ class COCOevalSegm:
         stats[10] = _summarize(0, areaRng="medium", maxDets=md[2])
         stats[11] = _summarize(0, areaRng="large", maxDets=md[2])
         self.stats = stats
+
+
+def ann_to_mask(ann, height, width):
+    """[UPSTREAM CocoDataset.annToMask] the uint8 [height, width] mask of a COCO annotation dict,
+    `decode(annToRLE(ann, height, width))`: its `segmentation` a polygon list, a box list or an
+    RLE dict, rasterised or decoded on the device (`MaskBatch.from_coco`, which states what
+    raises and the stated differences from pycocotools)."""
+    import torch
+
+    N.require_cuda()
+    seg = ann["segmentation"] if isinstance(ann, dict) else ann
+    H, W = int(height), int(width)
+    gt = MaskBatch.from_coco(N.load(), torch.device("cuda", torch.cuda.current_device()),
+                             [[H, W, H, W, 0, 0, H, W]], [[0]], [[seg]])
+    wb = (W + 7) // 8
+    o = int(gt.planes.d_packed_off[0].item())
+    packed = gt.planes.d_packed[o:o + H * wb].cpu().numpy().reshape(H, wb)
+    return np.unpackbits(packed, axis=1)[:, :W].copy()

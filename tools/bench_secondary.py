@@ -4,7 +4,7 @@ numbers go into README.md.  One JSON line per workload on stdout; the COCO compr
 each unmold workload also names the GPU and its power limit.
 
   python tools/bench_secondary.py [--iters 20] [--cpu]     (--cpu also times the oracle)
-  python tools/bench_secondary.py --only-eval | --only-cocoeval
+  python tools/bench_secondary.py --only-eval | --only-cocoeval | --only-polygons
 """
 import argparse
 import ctypes as C
@@ -424,6 +424,131 @@ def rle_gt_record(eng, gts, base_rle, base_n, items, thr10, iters):
             "rle_gt_results_equal_bool_gt": bool(same)}
 
 
+def _coco_like_polygons(rng, H, W, n):
+    """n COCO-style polygon annotations: 1-3 parts of 10-60 vertices, star-shaped around a
+    random centre (some reaching past the image)."""
+    out = []
+    for _ in range(n):
+        parts = []
+        for _ in range(int(rng.integers(1, 4))):
+            v = int(rng.integers(10, 61))
+            t = np.sort(rng.uniform(0, 2 * np.pi, v))
+            r = rng.uniform(5, 0.3 * min(H, W)) * rng.uniform(0.6, 1.0, v)
+            cx, cy = rng.uniform(0, W), rng.uniform(0, H)
+            parts.append(np.round(np.stack([cx + r * np.cos(t), cy + r * np.sin(t)], 1), 2)
+                         .ravel().tolist())
+        out.append(parts)
+    return out
+
+
+def _contour_polygons(contours):
+    """A display_instances contour list as a COCO polygon list: parts of >= 3 vertices (an
+    instance with none gets one degenerate part, an empty mask)."""
+    parts = [c.ravel().tolist() for c in contours if len(c) >= 3]
+    return parts or [[0.0, 0.0, 0.0, 0.0, 0.0, 0.0]]
+
+
+def polygons_case(iters):
+    """COCO polygon ground truth rasterised on the device (mrx_poly_decode).  COCO-like: 32 x
+    640x480 images of 5-20 annotations (1-3 parts of 10-60 vertices).  configs[1]: the jittered
+    ground truth of eval_case as the contour polygons of unmold_detections_contours_batch.  The
+    kernels alone, MaskBatch.from_coco end to end, unmold_compute_ap_batch with the polygons
+    against the same batch with RLE strings, and the polygon oracle's host time per image."""
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils
+    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import MaskBatch, pack_polygons
+
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import polygon_oracle
+
+    lib, dev = N.load(), torch.device("cuda", 0)
+    rng = np.random.default_rng(12)
+    rec = {"workload": "COCO polygon ground truth -> packed planes (pycocotools annToRLE + decode)"}
+
+    def kernels_ms(geoms, cls, segms):
+        pp = pack_polygons(geoms, cls, segms)
+        gt = MaskBatch.from_coco(lib, dev, geoms, cls, segms)
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)   # noqa: E731
+        t = [up(pp[k]) for k in ("vert", "part_vert", "part_inst", "part_col", "part_tog",
+                                 "inst_part")]
+        d_tog = torch.empty((int(pp["part_tog"][-1]),), dtype=torch.int32, device=dev)
+        d_cs = torch.empty((int(pp["part_col"][-1]),), dtype=torch.int64, device=dev)
+        d_cy = torch.empty((int(pp["part_col"][-1]),), dtype=torch.uint8, device=dev)
+        p = lambda x: C.c_void_p(x.data_ptr())   # noqa: E731
+        g = np.asarray(geoms)
+        pl = gt.planes
+
+        def run():
+            N.check(lib.mrx_poly_decode(p(t[0]), p(t[1]), p(t[2]), p(t[3]), p(t[4]), pp["P"],
+                                        p(t[5]), p(d_tog), p(d_cs), p(d_cy), p(pl.d_counts),
+                                        p(gt.d_geom), p(pl.d_packed_off), p(pl.d_packed), len(g),
+                                        gt.R, int(g[:, 0].max()), int(g[:, 1].max()),
+                                        N.stream_ptr(None)), "mrx_poly_decode")
+        ms, _ = time_ms(run, iters)
+
+        def e2e():
+            MaskBatch.from_coco(lib, dev, geoms, cls, segms)
+        e2e()
+        t0 = time.perf_counter()
+        reps = max(3, iters // 4)
+        for _ in range(reps):
+            e2e()
+        return pp, ms, (time.perf_counter() - t0) / reps * 1e3
+
+    # 1. COCO-like
+    H, W = 480, 640
+    segms = [_coco_like_polygons(rng, H, W, int(rng.integers(5, 21))) for _ in range(32)]
+    cls = [np.ones(len(s), np.int32) for s in segms]
+    geoms = [[H, W, H, W, 0, 0, H, W]] * 32
+    pp, k_ms, e_ms = kernels_ms(geoms, cls, segms)
+    t0 = time.perf_counter()
+    for s in segms[0]:
+        polygon_oracle.ann_to_rle(s, H, W)
+    rec.update({"coco_like_images": 32, "coco_like_instances": int(pp["counts"].sum()),
+                "coco_like_parts": pp["P"], "coco_like_vertices": int(pp["vert"].shape[0]),
+                "coco_like_poly_decode_kernels_ms": round(k_ms, 4),
+                "coco_like_from_coco_ms": round(e_ms, 2),
+                "oracle_host_ms_per_image": round((time.perf_counter() - t0) * 1e3, 1)})
+
+    # 2. configs[1] ground truth as contour polygons
+    batch, base_n = 32, 4
+    base = synth.make_batch(7, base_n, (1024, 1024), 100)
+    jrng = np.random.default_rng(8)
+    jittered = [(j.detections, j.mrcnn_mask, j.original_image_shape, j.image_shape, j.window)
+                for j in (synth.jitter_ground_truth(im, jrng, 12, 0.1) for im in base)]
+    cont = api_utils.unmold_detections_contours_batch(jittered)
+    polys = [[_contour_polygons(c) for c in r[3]] for r in cont]
+    items = [(im.detections, im.mrcnn_mask, im.original_image_shape, im.image_shape, im.window)
+             for im in (base[i % base_n] for i in range(batch))]
+    gcls = [cont[i % base_n][1] for i in range(batch)]
+    gp = [(None, gcls[i], polys[i % base_n]) for i in range(batch)]
+    # the RLE of the same polygons, so that both routes score identical masks
+    rle_of = [[{"size": [1024, 1024], "counts": polygon_oracle.ann_to_rle(s, 1024, 1024)}
+               for s in polys[b]] for b in range(base_n)]
+    gr = [(None, gcls[i], rle_of[i % base_n]) for i in range(batch)]
+    geoms = [[1024, 1024, 1024, 1024, 0, 0, 1024, 1024]] * batch
+    pp, k_ms, e_ms = kernels_ms(geoms, gcls, [polys[i % base_n] for i in range(batch)])
+    e2e = {}
+    for name, g in (("polygon_gt", gp), ("rle_gt", gr)):
+        api_utils.unmold_compute_ap_batch(items, g, (0.5,))
+        reps = max(2, iters // 8)
+        t0 = time.perf_counter()
+        for _ in range(reps):
+            res = api_utils.unmold_compute_ap_batch(items, g, (0.5,))
+        e2e[name] = ((time.perf_counter() - t0) / reps * 1e3, res)
+    same = all(np.array_equal(a["gt_match"], b["gt_match"]) and
+               np.array_equal(a["pred_match"], b["pred_match"])
+               for a, b in zip(e2e["polygon_gt"][1], e2e["rle_gt"][1]))
+    rec.update({"configs1_instances": int(pp["counts"].sum()), "configs1_parts": pp["P"],
+                "configs1_vertices": int(pp["vert"].shape[0]),
+                "configs1_poly_decode_kernels_ms": round(k_ms, 4),
+                "configs1_from_coco_ms": round(e_ms, 2),
+                "unmold_compute_ap_batch_ms_1_threshold_polygon_gt": round(e2e["polygon_gt"][0], 1),
+                "unmold_compute_ap_batch_ms_1_threshold_rle_list_gt": round(e2e["rle_gt"][0], 1),
+                "polygon_gt_results_equal_rle_gt": bool(same), **card()})
+    print(json.dumps(rec), flush=True)
+    torch.cuda.empty_cache()
+
+
 def anchors_sweep(iters, cpu):
     import oracle
     gen = AnchorGenerator(MaskRCNNServingConfig)
@@ -476,10 +601,15 @@ def main():
     ap.add_argument("--cpu", action="store_true")
     ap.add_argument("--only-eval", action="store_true", help="only the mask IoU / AP record")
     ap.add_argument("--only-cocoeval", action="store_true", help="only the COCO mask AP record")
+    ap.add_argument("--only-polygons", action="store_true", help="only the polygon ground truth "
+                    "record")
     args = ap.parse_args()
     torch.cuda.set_device(0)
     if args.only_cocoeval:
         cocoeval_case(args.iters)
+        return
+    if args.only_polygons:
+        polygons_case(args.iters)
         return
     eval_case(args.iters, args.cpu)
     if args.only_eval:
