@@ -21,6 +21,8 @@
  *   mrx_mask_extents / _overlaps / _matches (extension: mrcnn.utils.compute_overlaps_masks and
  *                             compute_matches, scoring the masks against ground truth)
  *   mrx_rle_parse / _decode (extension: ground truth given as COCO RLE, decoded to packed planes)
+ *   mrx_coco_ranks / _ious / _box_ious / _match[_f64area] (extension: pycocotools' COCOeval for
+ *                             "segm" and "bbox", the per-image half)
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
  *   mrx_device_alloc/_free (the canvas allocation: compressible device memory where offered)
  *
@@ -43,7 +45,7 @@
 extern "C" {
 #endif
 
-#define MRX_ABI_VERSION 13
+#define MRX_ABI_VERSION 14
 
 #define MRX_OK              0
 #define MRX_E_INVALID      -1   /* bad argument (null pointer, size out of range) */
@@ -375,11 +377,12 @@ int mrx_mask_matches(const float *d_overlaps, const int *d_pred_counts,
                      int T, double score_threshold, int *d_order, int *d_pred_match,
                      int *d_gt_match, int B, int R1, int R2, void *stream);
 
-/* ---------------------------------------------------------------- COCO mask evaluation */
+/* ---------------------------------------------------------------- COCO mask and box evaluation */
 /* EXTENSION: the per-image half of pycocotools' COCOeval for iouType "segm" (computeIoU with
- * maskApi.c's rleIou, and the matching loop of evaluateImg) on the packed slots (see "Output
- * slots"); the host accumulates the per-detection flags (cocoeval.cu).  Categories are dense
- * indices >= 0; -1 is a category that is not evaluated.
+ * maskApi.c's rleIou on the packed slots, see "Output slots") and "bbox" (computeIoU with
+ * maskApi.c's bbIou), and the matching loop of evaluateImg for both; the host accumulates the
+ * per-detection flags (cocoeval.cu).  Categories are dense indices >= 0; -1 is a category that
+ * is not evaluated.
  *
  * mrx_coco_ranks: per image b, its N_b = d_counts[b] predictions (d_class_ids [B,R] int32,
  *   d_scores [B,R] of score_dtype), d_class_map [C] int32 (class id -> dense category or -1; a
@@ -396,8 +399,20 @@ int mrx_mask_matches(const float *d_overlaps, const int *d_pred_counts,
  *   i < N1_b and j < N2_b of the same category is (double)inter / (double)u rounded once, 0 when
  *   inter = 0, u = area(i) for a crowd j and area(i) + area(j) - inter otherwise; other elements
  *   are not written.  d_packed1 and d_packed2 must be 4-byte aligned.
+ * mrx_coco_box_ious: the same d_iou for boxes.  d_pred_boxes [B,R1,4] is, by box_form,
+ *   MRX_BOX_YXYX_I32: int32 (y1, x1, y2, x2), e.g. the d_boxes of mrx_unmold_prepare, taken as
+ *     [x1, y1, x2 - x1, y2 - y1] (build_coco_results' `bbox`, exact in double), or
+ *   MRX_BOX_XYWH_F64: float64 [x, y, w, h], a result's `bbox`;
+ *   d_pred_counts [B], d_pred_cat / d_pred_keep from mrx_coco_ranks; d_gt_boxes [B,R2,4] float64
+ *   [x, y, w, h], d_gt_counts [B], d_gt_cat [B,R2] int32, d_gt_crowd [B,R2] uint8.  Element
+ *   (b, i, j) for a kept i < N1_b and j < N2_b of the same category is bbIou's, every operation
+ *   rounded on its own (no FMA): w = fmin(D[2]+D[0], G[2]+G[0]) - fmax(D[0], G[0]), 0 when
+ *   w <= 0, h the same in y, i = w*h, u = D[2]*D[3] for a crowd j and (D[2]*D[3] + G[2]*G[3]) - i
+ *   otherwise, i / u.  Also writes d_pred_area [B,R1] float64 = D[2]*D[3] for kept i (loadRes'
+ *   `area` of a bbox result).  Other elements are not written.
  * mrx_coco_match: d_iou as above, the ranks' d_pred_cat, d_pred_keep and d_walk, d_pred_area
- *   [B,R1] int64 (mask pixels), d_gt_counts [B], d_gt_cat, d_gt_crowd, d_gt_area [B,R2] float64
+ *   [B,R1] int64 (mask pixels; mrx_coco_match_f64area: float64, the box areas of
+ *   mrx_coco_box_ious), d_gt_counts [B], d_gt_cat, d_gt_crowd, d_gt_area [B,R2] float64
  *   (the annotation's area).  thresholds[T] (HOST, compared as IoU >= t: the caller caps them at
  *   1 - 1e-10 as evaluateImg does) and area_rng[A][2] (HOST, lo and hi, both inclusive).  For
  *   area range a and threshold t, ground-truth j is ignored when crowd or its area is outside
@@ -410,10 +425,13 @@ int mrx_mask_matches(const float *d_overlaps, const int *d_pred_counts,
  *   Other elements are not written.
  * Checks: mrx_coco_ious: those of "Output slots" for each slot set, then null pointers and the
  * alignment; the others: null pointers, B outside [0, MRX_MAX_BATCH], R (R1, R2) outside
- * [1, 65534], for mrx_coco_ranks C or max_det below 1 or a bad score_dtype, for mrx_coco_match T
- * outside [1, MRX_MAX_IOU_THRESHOLDS] or A outside [1, MRX_MAX_AREA_RANGES]: MRX_E_INVALID.
+ * [1, 65534], for mrx_coco_ranks C or max_det below 1 or a bad score_dtype, for
+ * mrx_coco_box_ious a bad box_form, for mrx_coco_match[_f64area] T outside
+ * [1, MRX_MAX_IOU_THRESHOLDS] or A outside [1, MRX_MAX_AREA_RANGES]: MRX_E_INVALID.
  * B = 0 returns MRX_OK without launching anything. */
 #define MRX_MAX_AREA_RANGES 16
+#define MRX_BOX_YXYX_I32 0
+#define MRX_BOX_XYWH_F64 1
 int mrx_coco_ranks(const int *d_class_ids, const void *d_scores, int score_dtype,
                    const int *d_counts, const int *d_class_map, int C, int max_det, int *d_cat,
                    int *d_rank, unsigned char *d_keep, int *d_walk, int B, int R, void *stream);
@@ -431,6 +449,18 @@ int mrx_coco_match(const double *d_iou, const int *d_pred_counts, const int *d_p
                    const double *thresholds, int T, const double *area_rng, int A,
                    int *d_dt_match, unsigned char *d_dt_ignore, int B, int R1, int R2,
                    void *stream);
+int mrx_coco_match_f64area(const double *d_iou, const int *d_pred_counts, const int *d_pred_cat,
+                           const unsigned char *d_pred_keep, const int *d_walk,
+                           const double *d_pred_area, const int *d_gt_counts, const int *d_gt_cat,
+                           const unsigned char *d_gt_crowd, const double *d_gt_area,
+                           const double *thresholds, int T, const double *area_rng, int A,
+                           int *d_dt_match, unsigned char *d_dt_ignore, int B, int R1, int R2,
+                           void *stream);
+int mrx_coco_box_ious(const void *d_pred_boxes, int box_form, const int *d_pred_counts,
+                      const int *d_pred_cat, const unsigned char *d_pred_keep, int R1,
+                      const double *d_gt_boxes, const int *d_gt_counts, const int *d_gt_cat,
+                      const unsigned char *d_gt_crowd, int R2, double *d_pred_area, double *d_iou,
+                      int B, void *stream);
 
 /* ---------------------------------------------------------------- COCO RLE to packed planes */
 /* EXTENSION: the inverse of mrx_rle_strings / mrx_rle_write, for ground truth held as COCO RLE

@@ -26,12 +26,14 @@ MRX_GEOM_INTS = 8
 MRX_MAX_BATCH = 4096
 MRX_MAX_MASK_DIM = 64
 MRX_MAX_LANE_MASK_W = 30    # tile width of the lane kernels: mw + 2 lanes per warp
-ABI_VERSION = 13
+ABI_VERSION = 14
 MRX_SCHED_WORDS = 4
 MRX_PEER_HANDLE_BYTES = 64
 MRX_MAX_CONTOUR_SEGMENTS = 1 << 30
 MRX_MAX_IOU_THRESHOLDS = 64
 MRX_MAX_AREA_RANGES = 16
+MRX_BOX_YXYX_I32 = 0
+MRX_BOX_XYWH_F64 = 1
 MRX_RLE_ST_CHAR = 1
 MRX_RLE_ST_TRUNC = 2
 MRX_RLE_ST_RANGE = 4
@@ -88,6 +90,10 @@ SIGNATURES = {
                            _i, _vp, _vp, _i, _vp]),
     "mrx_coco_match": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _dp, _i, _dp, _i, _vp,
                             _vp, _i, _i, _i, _vp]),
+    "mrx_coco_match_f64area": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _dp, _i, _dp,
+                                    _i, _vp, _vp, _i, _i, _i, _vp]),
+    "mrx_coco_box_ious": (_i, [_vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i,
+                               _vp]),
     "mrx_rle_parse": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "mrx_rle_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "mrx_poly_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,

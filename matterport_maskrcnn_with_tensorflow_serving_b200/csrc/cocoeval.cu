@@ -1,6 +1,7 @@
-// cocoeval.cu -- the per-image half of pycocotools' COCOeval for iouType "segm" on the packed
-// planes: computeIoU (maskApi.c rleIou) and the matching loop of evaluateImg.  The host keeps
-// what accumulate needs: per detection its category, rank, score, area and match / ignore bits.
+// cocoeval.cu -- the per-image half of pycocotools' COCOeval: computeIoU for iouType "segm" on the
+// packed planes (maskApi.c rleIou) and for "bbox" on [x, y, w, h] boxes (bbIou), and the matching
+// loop of evaluateImg, which does not care where its IoUs come from.  The host keeps what
+// accumulate needs: per detection its category, rank, score, area and match / ignore bits.
 //
 //   coco_rank_kernel   CTA per image: each prediction's dense category (through a class map),
 //                      its rank within (image, category) in np.argsort(-score, kind="mergesort")
@@ -11,11 +12,16 @@
 //                      of mask_overlaps_kernel (walk_pairs, planes.cuh) over the pairs of one
 //                      category whose prediction is kept; a pair whose extents do not meet gets 0
 //                      without a read
+//   coco_box_iou_kernel CTA per (image, prediction), thread per ground-truth instance: bbIou of
+//                      the pairs of one category whose prediction is kept, and the prediction's
+//                      area w*h (loadRes' area of a bbox result)
 //   coco_match_kernel  warp per (image, threshold, area range): predictions in walk order, each
-//                      takes the argmax of (not ignored, IoU, position) over its candidates
+//                      takes the argmax of (not ignored, IoU, position) over its candidates; one
+//                      template over the detection area's type (mask pixels, or box w*h)
 //
-// IoU arithmetic is rleIou's: (double)i / (double)u of exact counts, 0 when i = 0, u = the
-// detection's area for a crowd instance and a_dt + a_gt - i otherwise.
+// Mask IoU arithmetic is rleIou's: (double)i / (double)u of exact counts, 0 when i = 0, u = the
+// detection's area for a crowd instance and a_dt + a_gt - i otherwise.  Box IoU arithmetic is
+// bbIou's, operation for operation and unfused (see coco_box_iou_kernel).
 #include "planes.cuh"
 
 namespace mrx {
@@ -96,14 +102,76 @@ coco_iou_kernel(const Planes p1, const Planes p2, const int *__restrict__ geom,
       });
 }
 
+constexpr int kBoxThreads = 128;
+
+struct BoxIouParams {
+  const void *pred_boxes;     // [B, R1, 4] int32 (y1, x1, y2, x2) or float64 (x, y, w, h)
+  const int *pred_counts;     // [B]
+  const int *pred_cat;        // [B, R1]
+  const unsigned char *pred_keep;
+  const double *gt_boxes;     // [B, R2, 4] (x, y, w, h)
+  const int *gt_counts;       // [B]
+  const int *gt_cat;          // [B, R2]
+  const unsigned char *gt_crowd;
+  double *pred_area;          // [B, R1]
+  double *iou;                // [B, R1, R2]
+  int R1, R2, pred_xywh;
+};
+
+// maskApi.c bbIou for one prediction against every instance of its category.  pycocotools' x86-64
+// build rounds every operation; nvcc would contract w*h into da + ga - w*h (an FMA), so each one is
+// an explicit _rn intrinsic.  An engine box becomes [x1, y1, x2 - x1, y2 - y1] exactly (int32
+// differences are exact in double), the `bbox` of build_coco_results.
+__global__ void __launch_bounds__(kBoxThreads) coco_box_iou_kernel(const BoxIouParams p) {
+  const int i = blockIdx.x, b = blockIdx.y;
+  if (i >= p.pred_counts[b]) return;
+  const size_t i1 = static_cast<size_t>(b) * p.R1 + i;
+  if (!p.pred_keep[i1]) return;
+  double d[4];
+  if (p.pred_xywh) {
+    const double *q = static_cast<const double *>(p.pred_boxes) + 4 * i1;
+    for (int k = 0; k < 4; ++k) d[k] = q[k];
+  } else {
+    const int *q = static_cast<const int *>(p.pred_boxes) + 4 * i1;
+    d[0] = q[1];
+    d[1] = q[0];
+    d[2] = __dsub_rn(q[3], q[1]);
+    d[3] = __dsub_rn(q[2], q[0]);
+  }
+  const double da = __dmul_rn(d[2], d[3]);
+  if (threadIdx.x == 0) p.pred_area[i1] = da;
+  const int ci = p.pred_cat[i1];
+  const int M = p.gt_counts[b];
+  const size_t gb = static_cast<size_t>(b) * p.R2;
+  double *row = p.iou + i1 * p.R2;
+  for (int j = threadIdx.x; j < M; j += blockDim.x) {
+    if (p.gt_cat[gb + j] != ci) continue;
+    const double *g = p.gt_boxes + 4 * (gb + j);
+    double o = 0.0;
+    const double w = __dsub_rn(fmin(__dadd_rn(d[2], d[0]), __dadd_rn(g[2], g[0])), fmax(d[0], g[0]));
+    if (!(w <= 0)) {
+      const double h =
+          __dsub_rn(fmin(__dadd_rn(d[3], d[1]), __dadd_rn(g[3], g[1])), fmax(d[1], g[1]));
+      if (!(h <= 0)) {
+        const double inter = __dmul_rn(w, h);
+        const double u =
+            p.gt_crowd[gb + j] ? da : __dsub_rn(__dadd_rn(da, __dmul_rn(g[2], g[3])), inter);
+        o = __ddiv_rn(inter, u);
+      }
+    }
+    row[j] = o;
+  }
+}
+
 // ---------------------------------------------------------------- matches
+template <typename Area>
 struct MatchParams {
   const double *iou;          // [B, R1, R2]
   const int *pred_counts;     // [B]
   const int *pred_cat;        // [B, R1]
   const unsigned char *pred_keep;
   const int *walk;            // [B, R1]
-  const long long *pred_area; // [B, R1]
+  const Area *pred_area;      // [B, R1]: mask pixels (int64) or box w*h (float64)
   const int *gt_counts;       // [B]
   const int *gt_cat;          // [B, R2]
   const unsigned char *gt_crowd;
@@ -121,7 +189,8 @@ struct MatchParams {
 // the ground truth stable-sorted with the non-ignored first -- within each of the two groups that
 // order is the index order, so the key is (not ignored, IoU bits, then j).  Lane j % 32 scans
 // instance j; the matched set is a bitmask in shared memory, written by the one winning lane.
-__global__ void __launch_bounds__(32) coco_match_kernel(const MatchParams p) {
+template <typename Area>
+__global__ void __launch_bounds__(32) coco_match_kernel(const MatchParams<Area> p) {
   __shared__ unsigned s_matched[(65534 + 31) / 32];
   const int b = blockIdx.x, t = blockIdx.y, a = blockIdx.z, lane = threadIdx.x;
   const int N = p.pred_counts[b], M = p.gt_counts[b];
@@ -229,14 +298,15 @@ extern "C" int mrx_coco_ious(const unsigned char *d_packed1, const long long *d_
   return MRX_OK;
 }
 
-extern "C" int mrx_coco_match(const double *d_iou, const int *d_pred_counts, const int *d_pred_cat,
-                              const unsigned char *d_pred_keep, const int *d_walk,
-                              const long long *d_pred_area, const int *d_gt_counts,
-                              const int *d_gt_cat, const unsigned char *d_gt_crowd,
-                              const double *d_gt_area, const double *thresholds, int T,
-                              const double *area_rng, int A, int *d_dt_match,
-                              unsigned char *d_dt_ignore, int B, int R1, int R2, void *stream) {
-  const char *fn = "mrx_coco_match";
+namespace {
+
+template <typename Area>
+int coco_match(const char *fn, const double *d_iou, const int *d_pred_counts, const int *d_pred_cat,
+               const unsigned char *d_pred_keep, const int *d_walk, const Area *d_pred_area,
+               const int *d_gt_counts, const int *d_gt_cat, const unsigned char *d_gt_crowd,
+               const double *d_gt_area, const double *thresholds, int T, const double *area_rng,
+               int A, int *d_dt_match, unsigned char *d_dt_ignore, int B, int R1, int R2,
+               void *stream) {
   MRX_CHECK_ARG(d_iou && d_pred_counts && d_pred_cat && d_pred_keep && d_walk && d_pred_area &&
                     d_gt_counts && d_gt_cat && d_gt_crowd && d_gt_area && thresholds && area_rng &&
                     d_dt_match && d_dt_ignore,
@@ -249,7 +319,7 @@ extern "C" int mrx_coco_match(const double *d_iou, const int *d_pred_counts, con
   MRX_CHECK_ARG(A >= 1 && A <= MRX_MAX_AREA_RANGES, "%s: bad A %d (need 1<=A<=%d)", fn, A,
                 MRX_MAX_AREA_RANGES);
   if (B == 0) return MRX_OK;
-  cocoeval::MatchParams p{};
+  cocoeval::MatchParams<Area> p{};
   p.iou = d_iou;
   p.pred_counts = d_pred_counts;
   p.pred_cat = d_pred_cat;
@@ -268,7 +338,60 @@ extern "C" int mrx_coco_match(const double *d_iou, const int *d_pred_counts, con
   p.T = T;
   for (int t = 0; t < T; ++t) p.thresholds[t] = thresholds[t];
   for (int a = 0; a < 2 * A; ++a) p.area_rng[a] = area_rng[a];
-  cocoeval::coco_match_kernel<<<dim3(B, T, A), 32, 0, static_cast<cudaStream_t>(stream)>>>(p);
+  cocoeval::coco_match_kernel<Area>
+      <<<dim3(B, T, A), 32, 0, static_cast<cudaStream_t>(stream)>>>(p);
   MRX_LAUNCH_CHECK("coco_match_kernel");
+  return MRX_OK;
+}
+
+}  // namespace
+
+extern "C" int mrx_coco_match(const double *d_iou, const int *d_pred_counts, const int *d_pred_cat,
+                              const unsigned char *d_pred_keep, const int *d_walk,
+                              const long long *d_pred_area, const int *d_gt_counts,
+                              const int *d_gt_cat, const unsigned char *d_gt_crowd,
+                              const double *d_gt_area, const double *thresholds, int T,
+                              const double *area_rng, int A, int *d_dt_match,
+                              unsigned char *d_dt_ignore, int B, int R1, int R2, void *stream) {
+  return coco_match("mrx_coco_match", d_iou, d_pred_counts, d_pred_cat, d_pred_keep, d_walk,
+                    d_pred_area, d_gt_counts, d_gt_cat, d_gt_crowd, d_gt_area, thresholds, T,
+                    area_rng, A, d_dt_match, d_dt_ignore, B, R1, R2, stream);
+}
+
+extern "C" int mrx_coco_match_f64area(const double *d_iou, const int *d_pred_counts,
+                                      const int *d_pred_cat, const unsigned char *d_pred_keep,
+                                      const int *d_walk, const double *d_pred_area,
+                                      const int *d_gt_counts, const int *d_gt_cat,
+                                      const unsigned char *d_gt_crowd, const double *d_gt_area,
+                                      const double *thresholds, int T, const double *area_rng,
+                                      int A, int *d_dt_match, unsigned char *d_dt_ignore, int B,
+                                      int R1, int R2, void *stream) {
+  return coco_match("mrx_coco_match_f64area", d_iou, d_pred_counts, d_pred_cat, d_pred_keep,
+                    d_walk, d_pred_area, d_gt_counts, d_gt_cat, d_gt_crowd, d_gt_area, thresholds,
+                    T, area_rng, A, d_dt_match, d_dt_ignore, B, R1, R2, stream);
+}
+
+extern "C" int mrx_coco_box_ious(const void *d_pred_boxes, int box_form, const int *d_pred_counts,
+                                 const int *d_pred_cat, const unsigned char *d_pred_keep, int R1,
+                                 const double *d_gt_boxes, const int *d_gt_counts,
+                                 const int *d_gt_cat, const unsigned char *d_gt_crowd, int R2,
+                                 double *d_pred_area, double *d_iou, int B, void *stream) {
+  const char *fn = "mrx_coco_box_ious";
+  MRX_CHECK_ARG(d_pred_boxes && d_pred_counts && d_pred_cat && d_pred_keep && d_gt_boxes &&
+                    d_gt_counts && d_gt_cat && d_gt_crowd && d_pred_area && d_iou,
+                "%s: null pointer", fn);
+  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH, "%s: bad B %d (need 0<=B<=%d)", fn, B, MRX_MAX_BATCH);
+  MRX_CHECK_ARG(R1 >= 1 && R1 <= 65534 && R2 >= 1 && R2 <= 65534,
+                "%s: bad R1 %d / R2 %d (need 1<=R<=65534)", fn, R1, R2);
+  MRX_CHECK_ARG(box_form == MRX_BOX_YXYX_I32 || box_form == MRX_BOX_XYWH_F64,
+                "%s: bad box form %d", fn, box_form);
+  if (B == 0) return MRX_OK;
+  const cocoeval::BoxIouParams p{d_pred_boxes, d_pred_counts, d_pred_cat,  d_pred_keep,
+                                 d_gt_boxes,   d_gt_counts,   d_gt_cat,    d_gt_crowd,
+                                 d_pred_area,  d_iou,         R1,          R2,
+                                 box_form == MRX_BOX_XYWH_F64};
+  cocoeval::coco_box_iou_kernel<<<dim3(R1, B), cocoeval::kBoxThreads, 0,
+                                  static_cast<cudaStream_t>(stream)>>>(p);
+  MRX_LAUNCH_CHECK("coco_box_iou_kernel");
   return MRX_OK;
 }

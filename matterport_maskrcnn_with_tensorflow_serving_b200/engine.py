@@ -507,6 +507,21 @@ class UnmoldEngine:
         return coco_evaluate_batch(self.lib, pred, self.d_class_ids[:n], self.d_scores[:n], gt,
                                    gt_crowd, gt_area, class_map, params, stream)
 
+    def enqueue_coco_box_eval(self, gt_counts, gt_cat, gt_boxes, gt_crowd, gt_area, class_map,
+                              params, stream=None):
+        """EXTENSION: `coco_box_evaluate_batch` (COCOeval "bbox") of the planned batch's kept
+        boxes, after `enqueue(..., expand=False)`: no mask is expanded or read.  The ground truth
+        is host arrays padded to R2 instances per image (gt_counts [n], gt_cat [n, R2] dense
+        categories, gt_boxes [n, R2, 4] float64 [x, y, w, h], gt_crowd, gt_area [n, R2]);
+        class_map [C] maps the engine's class ids to dense categories (-1: not evaluated).
+        Synchronises once; returns its dict."""
+        n = self._n_images
+        if n == 0:
+            raise RuntimeError("call plan() and enqueue() first")
+        return coco_box_evaluate_batch(self.lib, self.d_boxes[:n], self.d_counts[:n],
+                                       self.d_class_ids[:n], self.d_scores[:n], gt_counts, gt_cat,
+                                       gt_boxes, gt_crowd, gt_area, class_map, params, stream)
+
     def _prediction_planes(self, gt, fn, stream):
         """`Planes` of the planned batch's kept instances to score against `gt` (a `MaskBatch` of
         the same plan), each counted only inside its box (mrx_mask_extents into `_eval_bufs`)."""
@@ -1100,50 +1115,122 @@ def coco_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt
     the count), `area` (int64 pixels), `score` (float64); `match` [A, T, n, pred.R] int32 (the
     ground-truth index or -1) and `ignore` [A, T, n, pred.R] bool, defined where `keep` is; and
     `d_iou`, the float64 device tensor [n, pred.R, gt.R] of mrx_coco_ious."""
+    n, R1, R2 = gt.n, int(pred.R), int(gt.R)
+    class_map = _coco_class_map(class_map)
+    with _stream_ctx(stream):
+        d_crowd, d_area, d_map = _upload_parts(
+            [np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
+             np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map],
+            gt.d_geom.device)
+
+        def ious(v, d_iou, st):
+            v["area"].copy_(pred.d_areas.view(-1)[:n * R1].view(n, R1))
+            N.check(lib.mrx_coco_ious(
+                _ptr(pred.d_packed), _ptr(pred.d_packed_off), _ptr(pred.d_counts),
+                _ptr(pred.d_areas), _ptr(pred.d_extents), _ptr(v["cat"]), _ptr(v["keep"]), R1,
+                _ptr(gt.planes.d_packed), _ptr(gt.planes.d_packed_off), _ptr(gt.planes.d_counts),
+                _ptr(gt.planes.d_areas), _ptr(gt.planes.d_extents), _ptr(gt.d_class_ids),
+                _ptr(d_crowd), R2, _ptr(gt.d_geom), _ptr(d_iou), n, st), "mrx_coco_ious")
+
+        return _coco_evaluate(lib, n, R1, R2, pred.d_counts, pred_class_ids, pred_scores,
+                              gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map, params,
+                              np.int64, ious, stream)
+
+
+def coco_box_evaluate_batch(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts,
+                            gt_cat, gt_boxes, gt_crowd, gt_area, class_map, params, stream=None):
+    """The per-image half of COCOeval (iouType "bbox") for one batch of n images: mrx_coco_ranks,
+    mrx_coco_box_ious and mrx_coco_match_f64area, then one download and one synchronisation.  No
+    mask is read.
+
+    pred_boxes [n, R1, 4]: int32 (y1, x1, y2, x2), the kept boxes of mrx_unmold_prepare (their
+    `bbox` is [x1, y1, x2 - x1, y2 - y1]), or float64 [x, y, w, h], results' `bbox`;
+    pred_counts [n] int32, pred_class_ids [n, R1] int32 and pred_scores [n, R1] float32 /
+    float64.  Each of those is a device tensor or a host array; the host arrays go up in one copy
+    with the ground truth.  gt_counts [n], gt_cat [n, R2] (dense category indices), gt_boxes
+    [n, R2, 4] float64 [x, y, w, h], gt_crowd [n, R2] and gt_area [n, R2] host arrays; class_map
+    and params as for `coco_evaluate_batch`.
+
+    Returns `coco_evaluate_batch`'s dict, with `area` float64 (each kept prediction's w*h, as
+    loadRes stores it for a bbox result) and `d_iou` from mrx_coco_box_ious."""
+    torch = _torch()
+    gt_cat = np.ascontiguousarray(gt_cat, dtype=np.int32)
+    n, R2 = gt_cat.shape
+    R1 = int(pred_boxes.shape[1])
+    class_map = _coco_class_map(class_map)
+    if not isinstance(pred_boxes, np.ndarray):
+        dev = pred_boxes.device
+    else:
+        dev = next((x.device for x in (pred_counts, pred_class_ids, pred_scores)
+                    if not isinstance(x, np.ndarray)),
+                   torch.device("cuda", torch.cuda.current_device()))
+    parts = [np.ascontiguousarray(gt_counts, dtype=np.int32).reshape(n), gt_cat,
+             np.ascontiguousarray(gt_boxes, dtype=np.float64).reshape(n, R2, 4),
+             np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
+             np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map]
+    pred = [pred_boxes, pred_counts, pred_class_ids, pred_scores]
+    on_host = [k for k, x in enumerate(pred) if isinstance(x, np.ndarray)]
+    with _stream_ctx(stream):
+        up = _upload_parts(parts + [np.ascontiguousarray(pred[k]) for k in on_host], dev)
+        d_counts, d_cat, d_boxes, d_crowd, d_area, d_map = up[:6]
+        for k, t in zip(on_host, up[6:]):
+            pred[k] = t
+        pred_boxes, pred_counts, pred_class_ids, pred_scores = pred
+        form = {torch.int32: N.MRX_BOX_YXYX_I32, torch.float64: N.MRX_BOX_XYWH_F64}[
+            pred_boxes.dtype]
+
+        def ious(v, d_iou, st):
+            N.check(lib.mrx_coco_box_ious(
+                _ptr(pred_boxes), form, _ptr(pred_counts), _ptr(v["cat"]), _ptr(v["keep"]), R1,
+                _ptr(d_boxes), _ptr(d_counts), _ptr(d_cat), _ptr(d_crowd), R2, _ptr(v["area"]),
+                _ptr(d_iou), n, st), "mrx_coco_box_ious")
+
+        return _coco_evaluate(lib, n, R1, R2, pred_counts, pred_class_ids, pred_scores, d_counts,
+                              d_cat, d_crowd, d_area, d_map, params, np.float64, ious, stream)
+
+
+def _coco_class_map(class_map):
+    class_map = np.asarray(class_map, dtype=np.int32).reshape(-1)
+    return class_map if class_map.size else np.full(1, -1, np.int32)
+
+
+def _coco_evaluate(lib, n, R1, R2, d_pred_counts, pred_class_ids, pred_scores, d_gt_counts,
+                   d_gt_cat, d_crowd, d_area, d_map, params, area_dtype, ious, stream):
+    """What both IoU types share, on the current stream: mrx_coco_ranks, `ious(v, d_iou, st)`
+    (fills d_iou [n, R1, R2] and the predictions' `area` in the output views v), the match kernel
+    for area_dtype (int64 mask pixels or float64 box areas), then the one download of the output
+    buffer and its one synchronisation.  Returns `coco_evaluate_batch`'s dict."""
     torch = _torch()
     thr, rng, max_det = coco_device_params(params)
-    n, R1, R2 = gt.n, int(pred.R), int(gt.R)
     T, A = len(thr), len(rng) // 2
-    dev = gt.d_geom.device
-    class_map = np.asarray(class_map, dtype=np.int32).reshape(-1)
-    if class_map.size == 0:
-        class_map = np.full(1, -1, np.int32)
+    dev = d_map.device
     score_code = {torch.float32: N.MRX_F32, torch.float64: N.MRX_F64}[pred_scores.dtype]
     st = N.stream_ptr(stream)
     # everything that comes back lives in one device buffer laid out by _part_offsets
     parts = {"counts": ((n,), np.int32), "cat": ((n, R1), np.int32), "rank": ((n, R1), np.int32),
-             "keep": ((n, R1), np.uint8), "area": ((n, R1), np.int64),
+             "keep": ((n, R1), np.uint8), "area": ((n, R1), area_dtype),
              "score": ((n, R1), np.float64), "match": ((A, T, n, R1), np.int32),
              "ignore": ((A, T, n, R1), np.uint8)}
     specs = list(parts.values())
-    with _stream_ctx(stream):
-        d_crowd, d_area, d_map = _upload_parts(
-            [np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
-             np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map], dev)
-        d_out = torch.empty((max(int(_part_offsets(specs)[-1]), 16),), dtype=torch.uint8,
-                            device=dev)
-        v = dict(zip(parts, _part_views(d_out, specs)))
-        d_walk = torch.empty((n, R1), dtype=torch.int32, device=dev)
-        d_iou = torch.empty((n, R1, R2), dtype=torch.float64, device=dev)
-        v["counts"].copy_(pred.d_counts[:n])
-        v["area"].copy_(pred.d_areas.view(-1)[:n * R1].view(n, R1))
-        v["score"].copy_(pred_scores[:n])
-        N.check(lib.mrx_coco_ranks(
-            _ptr(pred_class_ids), _ptr(pred_scores), score_code, _ptr(pred.d_counts), _ptr(d_map),
-            int(class_map.size), max_det, _ptr(v["cat"]), _ptr(v["rank"]), _ptr(v["keep"]),
-            _ptr(d_walk), n, R1, st), "mrx_coco_ranks")
-        N.check(lib.mrx_coco_ious(
-            _ptr(pred.d_packed), _ptr(pred.d_packed_off), _ptr(pred.d_counts), _ptr(pred.d_areas),
-            _ptr(pred.d_extents), _ptr(v["cat"]), _ptr(v["keep"]), R1,
-            _ptr(gt.planes.d_packed), _ptr(gt.planes.d_packed_off), _ptr(gt.planes.d_counts),
-            _ptr(gt.planes.d_areas), _ptr(gt.planes.d_extents), _ptr(gt.d_class_ids),
-            _ptr(d_crowd), R2, _ptr(gt.d_geom), _ptr(d_iou), n, st), "mrx_coco_ious")
-        N.check(lib.mrx_coco_match(
-            _ptr(d_iou), _ptr(pred.d_counts), _ptr(v["cat"]), _ptr(v["keep"]), _ptr(d_walk),
-            _ptr(v["area"]), _ptr(gt.d_counts), _ptr(gt.d_class_ids), _ptr(d_crowd), _ptr(d_area),
-            N.double_array(thr), T, N.double_array(rng), A, _ptr(v["match"]), _ptr(v["ignore"]),
-            n, R1, R2, st), "mrx_coco_match")
-        host = d_out.cpu().numpy()         # the one synchronisation
+    d_out = torch.empty((max(int(_part_offsets(specs)[-1]), 16),), dtype=torch.uint8, device=dev)
+    v = dict(zip(parts, _part_views(d_out, specs)))
+    d_walk = torch.empty((n, R1), dtype=torch.int32, device=dev)
+    d_iou = torch.empty((n, R1, R2), dtype=torch.float64, device=dev)
+    v["counts"].copy_(d_pred_counts[:n])
+    v["score"].copy_(pred_scores[:n])
+    N.check(lib.mrx_coco_ranks(
+        _ptr(pred_class_ids), _ptr(pred_scores), score_code, _ptr(d_pred_counts), _ptr(d_map),
+        int(d_map.numel()), max_det, _ptr(v["cat"]), _ptr(v["rank"]), _ptr(v["keep"]),
+        _ptr(d_walk), n, R1, st), "mrx_coco_ranks")
+    ious(v, d_iou, st)
+    match = {np.dtype(np.int64): "mrx_coco_match",
+             np.dtype(np.float64): "mrx_coco_match_f64area"}[np.dtype(area_dtype)]
+    N.check(getattr(lib, match)(
+        _ptr(d_iou), _ptr(d_pred_counts), _ptr(v["cat"]), _ptr(v["keep"]), _ptr(d_walk),
+        _ptr(v["area"]), _ptr(d_gt_counts), _ptr(d_gt_cat), _ptr(d_crowd), _ptr(d_area),
+        N.double_array(thr), T, N.double_array(rng), A, _ptr(v["match"]), _ptr(v["ignore"]),
+        n, R1, R2, st), match)
+    host = d_out.cpu().numpy()         # the one synchronisation
     out = dict(zip(parts, _part_views(host, specs)))
     out["keep"] = (out["keep"] != 0) & (np.arange(R1)[None, :] < out["counts"][:, None])
     out["ignore"] = out["ignore"] != 0

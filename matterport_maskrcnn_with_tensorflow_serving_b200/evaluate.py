@@ -14,7 +14,9 @@ the device rounds the exact counts once each.
 `COCOevalSegm` is pycocotools' COCOeval for iouType "segm" (COCO mask AP) as a streaming
 evaluator: the IoUs and matching of `evaluate()` run on the device as each batch is added
 (`mrx_coco_ranks`, `mrx_coco_ious`, `mrx_coco_match`, DESIGN.md section 3.15); `accumulate()` and
-`summarize()` run on the host and equal pycocotools' exactly.
+`summarize()` run on the host and equal pycocotools' exactly.  `COCOevalBbox` is the same for
+iouType "bbox" (COCO box AP): box IoUs and matching on the device (`mrx_coco_box_ious`,
+`mrx_coco_match_f64area`, DESIGN.md section 3.17), no mask involved.
 
 `ann_to_mask` is Matterport's `CocoDataset.annToMask`, rasterised on the device (DESIGN.md
 section 3.16).
@@ -24,8 +26,8 @@ from __future__ import annotations
 import numpy as np
 
 from . import _native as N
-from .engine import (MaskBatch, coco_device_params, coco_evaluate_batch, mask_matches,
-                     mask_overlaps)
+from .engine import (MaskBatch, coco_box_evaluate_batch, coco_device_params,
+                     coco_evaluate_batch, mask_matches, mask_overlaps)
 
 
 def trim_zeros(x):
@@ -145,13 +147,14 @@ def compute_ap_range(gt_box, gt_class_id, gt_mask, pred_box, pred_class_id, pred
 
 # ----------------------------------------------------------------------------- COCO mask AP
 class Params:
-    """COCOeval's parameters for iouType "segm", with pycocotools' attribute names and defaults.
+    """COCOeval's parameters for iouType "segm" or "bbox", with pycocotools' attribute names and
+    defaults.
     `imgIds` is the sorted ids of the images added so far (it may be set to a subset before
     `accumulate`); `catIds` is the sorted category ids of the ground truth added so far unless
     given.  Only `useCats = 1` is supported."""
 
     def __init__(self, cat_ids=None, iou_thrs=None, rec_thrs=None, max_dets=(1, 10, 100),
-                 area_rng=None, area_rng_lbl=None):
+                 area_rng=None, area_rng_lbl=None, iou_type="segm"):
         self.imgIds = []
         self.catIds = [] if cat_ids is None else sorted(set(int(c) for c in cat_ids))
         self.iouThrs = (np.linspace(.5, 0.95, int(np.round((0.95 - .5) / .05)) + 1, endpoint=True)
@@ -167,39 +170,20 @@ class Params:
         if len(self.areaRngLbl) != len(self.areaRng):
             raise ValueError(f"{len(self.areaRngLbl)} area labels for {len(self.areaRng)} ranges")
         self.useCats = 1
-        self.iouType = "segm"
+        self.iouType = iou_type
 
 
-class COCOevalSegm:
-    """pycocotools' `COCOeval(cocoGt, cocoDt, "segm")` as a streaming evaluator: batches are added
-    one at a time (`add_batch` with model outputs, `add_results` with COCO segm results), the
-    per-image work of `evaluate()` -- mask IoUs and matching for every (image, category, area
-    range, threshold) -- runs on the device as each batch arrives, and only compact
-    per-detection records stay on the host.  `accumulate()` and `summarize()` then give
-    pycocotools' `eval` arrays (`precision` and `scores` [T, R, K, A, M], `recall` [T, K, A, M],
-    float64, -1 where undefined) and its twelve `stats`, exactly.
+class _COCOevalBase:
+    """What `COCOevalSegm` and `COCOevalBbox` share: the parameters, the category and image maps,
+    the per-detection records each batch appends (`_record`), and pycocotools' `evaluate`,
+    `accumulate` and `summarize` over them, which do not depend on the IoU type."""
 
-    Ground-truth annotations are COCO dicts: `category_id`, `segmentation` an RLE dict ({'size':
-    [H, W], 'counts': compressed `str` / `bytes` or an uncompressed count list}) or, with
-    `polygons=True`, a polygon or box list as a COCO instances file holds every non-crowd
-    annotation (rasterised on the device as pycocotools' annToRLE does, `MaskBatch.from_coco`),
-    `iscrowd`
-    (default 0; a crowd region's IoU is intersection / detection area, it absorbs any number of
-    detections and never counts as a miss), and `area` (the annotation's area, which decides its
-    area range; a detection's area is its mask's pixel count).
-
-    Stated differences from pycocotools: matches are recorded by position, where pycocotools
-    stores annotation ids and tests them for truth (so an annotation with id 0 counts as
-    unmatched there); a ground-truth dict without `area` gets its mask's pixel count, where
-    pycocotools raises KeyError; with the default `polygons=False`, polygon segmentations
-    raise ValueError (rasterise them to RLE first).  Detections are RLE only, with or without
-    `polygons`.  `iouThrs`, `areaRng` and `maxDets[-1]` are used on the device as each batch is
-    added, so they must not change after the first batch."""
+    _iou_type = None
 
     def __init__(self, cat_ids=None, iou_thrs=None, rec_thrs=None, max_dets=(1, 10, 100),
-                 area_rng=None, area_rng_lbl=None, polygons=False):
-        self.params = Params(cat_ids, iou_thrs, rec_thrs, max_dets, area_rng, area_rng_lbl)
-        self._polygons = bool(polygons)
+                 area_rng=None, area_rng_lbl=None):
+        self.params = Params(cat_ids, iou_thrs, rec_thrs, max_dets, area_rng, area_rng_lbl,
+                             self._iou_type)
         self._device_params = coco_device_params(self.params)
         self._auto_cats = cat_ids is None
         self._frozen = None
@@ -237,46 +221,41 @@ class COCOevalSegm:
                 raise ValueError(f"image {i!r} was already added")
             seen.add(i)
 
-    def _gt_tables(self, image_ids, gt_anns, shapes):
-        """Per image: dense category ids, crowd flags, areas (NaN where absent) and segmentations
-        (RLE dicts, and polygon or box lists when the evaluator takes them), each annotation
-        checked."""
-        cats, crowd, area, rles = [], [], [], []
-        for image_id, anns, hw in zip(image_ids, gt_anns, shapes):
-            c, cr, ar, rl = [], [], [], []
-            for k, ann in enumerate(anns):
-                where = f"image {image_id!r}, annotation {k}" + (
-                    f" (id {ann['id']!r})" if isinstance(ann, dict) and "id" in ann else "")
-                seg = ann.get("segmentation") if isinstance(ann, dict) else None
-                if isinstance(seg, list) and not self._polygons:
-                    raise ValueError(f"{where}: polygon segmentations are not supported; give "
-                                     "the mask as RLE")
-                if isinstance(seg, list):
-                    pass                   # checked by pack_polygons, naming the instance
-                elif not isinstance(seg, dict) or "counts" not in seg or "size" not in seg:
-                    raise ValueError(f"{where}: segmentation must be an RLE dict with 'size' and "
-                                     "'counts'")
-                if isinstance(seg, dict):
-                    size = [int(v) for v in np.ravel(seg["size"])]
-                    if hw is not None and size != list(hw):
-                        raise ValueError(f"{where}: RLE size {size} is not the image's "
-                                         f"{list(hw)}")
-                cat = int(ann["category_id"])
-                self._gt_cats.add(cat)
-                c.append(self._dense(cat))
-                cr.append(1 if ann.get("iscrowd", 0) else 0)
-                ar.append(float(ann["area"]) if "area" in ann else np.nan)
-                rl.append(seg)
-            cats.append(np.asarray(c, np.int32))
-            crowd.append(np.asarray(cr, np.uint8))
-            area.append(np.asarray(ar, np.float64))
-            rles.append(rl)
-        return cats, crowd, area, rles
+    # add_batch in two halves, which api_utils.unmold_coco_eval_batch runs around one unmold for
+    # several evaluators: `_batch_tables` (host checks and tables, before anything is uploaded;
+    # None for an empty batch) and `_batch_eval` (on the engine after the unmold: prepare, and
+    # the packed expand when `_needs_masks`), whose result is the rest of `_record`'s arguments
+    _needs_masks = False
 
-    def _padded(self, rows, R, dtype):
-        out = np.zeros((len(rows), R), dtype)
+    def _batch_tables(self, items, image_ids, gt_anns):
+        self._new_images(image_ids, len(items), gt_anns, "items")
+        self._freeze()
+        if len(items) == 0:
+            return None
+        return self._gt_tables(image_ids, gt_anns, [(int(it[2][0]), int(it[2][1]))
+                                                    for it in items])
+
+    def _class_map(self, C, category_ids):
+        """int32 [C]: the engine's class id -> dense category (-1 where category_ids has none)."""
+        class_map = np.full(C, -1, np.int32)
+        for c in range(C):
+            try:
+                class_map[c] = self._dense(c if category_ids is None else category_ids[c])
+            except (IndexError, KeyError):
+                pass
+        return class_map
+
+    @staticmethod
+    def _where(image_id, k, ann):
+        return f"image {image_id!r}, annotation {k}" + (
+            f" (id {ann['id']!r})" if isinstance(ann, dict) and "id" in ann else "")
+
+    @staticmethod
+    def _padded(rows, R, dtype, tail=()):
+        out = np.zeros((len(rows), R) + tuple(tail), dtype)
         for b, r in enumerate(rows):
-            out[b, :len(r)] = r
+            if len(r):
+                out[b, :len(r)] = r
         return out
 
     def _record(self, image_ids, res, gt_cats, gt_crowd, gt_area):
@@ -300,108 +279,6 @@ class COCOevalSegm:
         p.imgIds = sorted(self._img_index)
         if self._auto_cats:
             p.catIds = sorted(self._gt_cats)
-
-    def _areas(self, gt, area):
-        """Annotation areas, the mask's pixel count where the annotation has none."""
-        if not any(np.isnan(a).any() for a in area):
-            return area
-        mask_area = gt.planes.d_areas.cpu().numpy()
-        return [np.where(np.isnan(a), mask_area[b, :len(a)], a) for b, a in enumerate(area)]
-
-    def add_batch(self, items, image_ids, gt_anns, category_ids=None):
-        """Evaluate model outputs against COCO ground truth: items as for
-        `api_utils.unmold_detections_batch`, one image id and one list of annotation dicts per
-        item.  The kept instances are expanded straight to packed planes on the device
-        (`enqueue_packed`; no mask or RLE is made), the annotations are decoded there
-        (`MaskBatch.from_rle`), and `category_ids` maps class ids to category ids as in
-        `unmold_coco_results_batch` (None keeps the class id).  With `polygons=True` the
-        annotations may be polygon or box lists, rasterised there (`MaskBatch.from_coco`)."""
-        from . import api_utils
-
-        self._new_images(image_ids, len(items), gt_anns, "items")
-        self._freeze()
-        if len(items) == 0:
-            return
-        shapes = [(int(it[2][0]), int(it[2][1])) for it in items]
-        cats, crowd, area, rles = self._gt_tables(image_ids, gt_anns, shapes)
-        with api_utils._Staged(items, canvas=False) as st:
-            eng = st.eng
-            eng.enqueue_packed(st.d_det, st.d_msk)
-            st.meta()                      # raises for bad class ids or boxes
-            gt = (eng.ground_truth_coco if self._polygons else eng.ground_truth_rle)(cats, rles)
-            area = self._areas(gt, area)
-            class_map = np.full(eng.C, -1, np.int32)
-            for c in range(eng.C):
-                try:
-                    class_map[c] = self._dense(c if category_ids is None else category_ids[c])
-                except (IndexError, KeyError):
-                    pass
-            res = eng.enqueue_coco_eval(gt, self._padded(crowd, gt.R, np.uint8),
-                                        self._padded(area, gt.R, np.float64), class_map,
-                                        self.params)
-        self._record(image_ids, res, cats, crowd, area)
-
-    def add_results(self, results, gt_anns, image_ids, image_shapes=None):
-        """Evaluate COCO segm results -- dicts {'image_id', 'category_id', 'score',
-        'segmentation': RLE dict} as `loadRes` takes them and `unmold_coco_results_batch`
-        returns them -- against gt_anns[b], the annotation dicts of image_ids[b].  Every result's
-        image must be one of image_ids.  Both sides are decoded on the device; an image's shape
-        is its RLEs' size, or image_shapes[b] = (height, width) when given (the RLEs must agree
-        with it).  An image whose ground truth has polygons (`polygons=True`) and no RLE at all
-        has no size to take, so it needs image_shapes; without it this raises ValueError."""
-        import torch
-
-        self._new_images(image_ids, len(gt_anns), gt_anns, "annotation lists")
-        if image_shapes is not None and len(image_shapes) != len(image_ids):
-            raise ValueError(f"{len(image_shapes)} image shapes for {len(image_ids)} images")
-        self._freeze()
-        if len(image_ids) == 0:
-            return
-        pos = {i: b for b, i in enumerate(image_ids)}
-        dets = [[] for _ in image_ids]
-        for k, r in enumerate(results):
-            if r.get("image_id") not in pos:
-                raise ValueError(f"result {k}: image {r.get('image_id')!r} is not one of the "
-                                 "batch's image ids")
-            seg = r.get("segmentation")
-            if not isinstance(seg, dict) or "counts" not in seg or "size" not in seg:
-                raise ValueError(f"result {k}: segmentation must be an RLE dict with 'size' and "
-                                 "'counts'")
-            dets[pos[r["image_id"]]].append(r)
-        shapes = []
-        for image_id, d, anns in zip(image_ids, dets, gt_anns):
-            sizes = {tuple(int(v) for v in np.ravel(x["segmentation"]["size"])) for x in d}
-            sizes |= {tuple(int(v) for v in np.ravel(a["segmentation"]["size"])) for a in anns
-                      if isinstance(a, dict) and isinstance(a.get("segmentation"), dict)
-                      and "size" in a["segmentation"]}
-            if image_shapes is not None:
-                sizes.add(tuple(int(v) for v in image_shapes[len(shapes)]))
-            if len(sizes) > 1:
-                raise ValueError(f"image {image_id!r}: RLE sizes {sorted(sizes)} differ")
-            if not sizes and self._polygons and any(isinstance(a, dict) and isinstance(a.get("segmentation"), list)
-                                 for a in anns):
-                raise ValueError(f"image {image_id!r}: its ground truth is polygons only, so its "
-                                 "shape is unknown; give it in image_shapes")
-            shapes.append(sizes.pop() if sizes else (1, 1))
-        cats, crowd, area, rles = self._gt_tables(image_ids, gt_anns, shapes)
-        N.require_cuda()
-        lib = N.load()
-        dev = torch.device("cuda", torch.cuda.current_device())
-        geoms = [[H, W, H, W, 0, 0, H, W] for H, W in shapes]
-        pred_cls = [np.asarray([self._dense(x["category_id"]) for x in d], np.int32) for d in dets]
-        pred = MaskBatch.from_rle(lib, dev, geoms, pred_cls, [[x["segmentation"] for x in d]
-                                                              for d in dets])
-        gt = (MaskBatch.from_coco if self._polygons else MaskBatch.from_rle)(lib, dev, geoms, cats,
-                                                                            rles)
-        area = self._areas(gt, area)
-        scores = self._padded([[float(x["score"]) for x in d] for d in dets], pred.R, np.float64)
-        d_scores = torch.from_numpy(scores).to(dev)
-        res = coco_evaluate_batch(lib, pred.planes, pred.d_class_ids, d_scores, gt,
-                                  self._padded(crowd, gt.R, np.uint8),
-                                  self._padded(area, gt.R, np.float64),
-                                  np.arange(max(len(self._cat_index), 1), dtype=np.int32),
-                                  self.params)
-        self._record(image_ids, res, cats, crowd, area)
 
     # ------------------------------------------------------------------ pycocotools' API
     def evaluate(self):
@@ -527,6 +404,290 @@ class COCOevalSegm:
         stats[10] = _summarize(0, areaRng="medium", maxDets=md[2])
         stats[11] = _summarize(0, areaRng="large", maxDets=md[2])
         self.stats = stats
+
+
+class COCOevalSegm(_COCOevalBase):
+    """pycocotools' `COCOeval(cocoGt, cocoDt, "segm")` as a streaming evaluator: batches are added
+    one at a time (`add_batch` with model outputs, `add_results` with COCO segm results), the
+    per-image work of `evaluate()` -- mask IoUs and matching for every (image, category, area
+    range, threshold) -- runs on the device as each batch arrives, and only compact
+    per-detection records stay on the host.  `accumulate()` and `summarize()` then give
+    pycocotools' `eval` arrays (`precision` and `scores` [T, R, K, A, M], `recall` [T, K, A, M],
+    float64, -1 where undefined) and its twelve `stats`, exactly.
+
+    Ground-truth annotations are COCO dicts: `category_id`, `segmentation` an RLE dict ({'size':
+    [H, W], 'counts': compressed `str` / `bytes` or an uncompressed count list}) or, with
+    `polygons=True`, a polygon or box list as a COCO instances file holds every non-crowd
+    annotation (rasterised on the device as pycocotools' annToRLE does, `MaskBatch.from_coco`),
+    `iscrowd`
+    (default 0; a crowd region's IoU is intersection / detection area, it absorbs any number of
+    detections and never counts as a miss), and `area` (the annotation's area, which decides its
+    area range; a detection's area is its mask's pixel count).
+
+    Stated differences from pycocotools: matches are recorded by position, where pycocotools
+    stores annotation ids and tests them for truth (so an annotation with id 0 counts as
+    unmatched there); a ground-truth dict without `area` gets its mask's pixel count, where
+    pycocotools raises KeyError; with the default `polygons=False`, polygon segmentations
+    raise ValueError (rasterise them to RLE first).  Detections are RLE only, with or without
+    `polygons`.  `iouThrs`, `areaRng` and `maxDets[-1]` are used on the device as each batch is
+    added, so they must not change after the first batch."""
+
+    _iou_type = "segm"
+
+    def __init__(self, cat_ids=None, iou_thrs=None, rec_thrs=None, max_dets=(1, 10, 100),
+                 area_rng=None, area_rng_lbl=None, polygons=False):
+        super().__init__(cat_ids, iou_thrs, rec_thrs, max_dets, area_rng, area_rng_lbl)
+        self._polygons = bool(polygons)
+
+    def _gt_tables(self, image_ids, gt_anns, shapes):
+        """Per image: dense category ids, crowd flags, areas (NaN where absent) and segmentations
+        (RLE dicts, and polygon or box lists when the evaluator takes them), each annotation
+        checked."""
+        cats, crowd, area, rles = [], [], [], []
+        for image_id, anns, hw in zip(image_ids, gt_anns, shapes):
+            c, cr, ar, rl = [], [], [], []
+            for k, ann in enumerate(anns):
+                where = self._where(image_id, k, ann)
+                seg = ann.get("segmentation") if isinstance(ann, dict) else None
+                if isinstance(seg, list) and not self._polygons:
+                    raise ValueError(f"{where}: polygon segmentations are not supported; give "
+                                     "the mask as RLE")
+                if isinstance(seg, list):
+                    pass                   # checked by pack_polygons, naming the instance
+                elif not isinstance(seg, dict) or "counts" not in seg or "size" not in seg:
+                    raise ValueError(f"{where}: segmentation must be an RLE dict with 'size' and "
+                                     "'counts'")
+                if isinstance(seg, dict):
+                    size = [int(v) for v in np.ravel(seg["size"])]
+                    if hw is not None and size != list(hw):
+                        raise ValueError(f"{where}: RLE size {size} is not the image's "
+                                         f"{list(hw)}")
+                cat = int(ann["category_id"])
+                self._gt_cats.add(cat)
+                c.append(self._dense(cat))
+                cr.append(1 if ann.get("iscrowd", 0) else 0)
+                ar.append(float(ann["area"]) if "area" in ann else np.nan)
+                rl.append(seg)
+            cats.append(np.asarray(c, np.int32))
+            crowd.append(np.asarray(cr, np.uint8))
+            area.append(np.asarray(ar, np.float64))
+            rles.append(rl)
+        return cats, crowd, area, rles
+
+    def _areas(self, gt, area):
+        """Annotation areas, the mask's pixel count where the annotation has none."""
+        if not any(np.isnan(a).any() for a in area):
+            return area
+        mask_area = gt.planes.d_areas.cpu().numpy()
+        return [np.where(np.isnan(a), mask_area[b, :len(a)], a) for b, a in enumerate(area)]
+
+    def add_batch(self, items, image_ids, gt_anns, category_ids=None):
+        """Evaluate model outputs against COCO ground truth: items as for
+        `api_utils.unmold_detections_batch`, one image id and one list of annotation dicts per
+        item.  The kept instances are expanded straight to packed planes on the device
+        (`enqueue_packed`; no mask or RLE is made), the annotations are decoded there
+        (`MaskBatch.from_rle`), and `category_ids` maps class ids to category ids as in
+        `unmold_coco_results_batch` (None keeps the class id).  With `polygons=True` the
+        annotations may be polygon or box lists, rasterised there (`MaskBatch.from_coco`)."""
+        from . import api_utils
+
+        api_utils.unmold_coco_eval_batch(items, image_ids, gt_anns, [self], category_ids)
+
+    _needs_masks = True
+
+    def _batch_eval(self, eng, tables, category_ids):
+        cats, crowd, area, rles = tables
+        gt = (eng.ground_truth_coco if self._polygons else eng.ground_truth_rle)(cats, rles)
+        area = self._areas(gt, area)
+        res = eng.enqueue_coco_eval(gt, self._padded(crowd, gt.R, np.uint8),
+                                    self._padded(area, gt.R, np.float64),
+                                    self._class_map(eng.C, category_ids), self.params)
+        return res, cats, crowd, area
+
+    def add_results(self, results, gt_anns, image_ids, image_shapes=None):
+        """Evaluate COCO segm results -- dicts {'image_id', 'category_id', 'score',
+        'segmentation': RLE dict} as `loadRes` takes them and `unmold_coco_results_batch`
+        returns them -- against gt_anns[b], the annotation dicts of image_ids[b].  Every result's
+        image must be one of image_ids.  Both sides are decoded on the device; an image's shape
+        is its RLEs' size, or image_shapes[b] = (height, width) when given (the RLEs must agree
+        with it).  An image whose ground truth has polygons (`polygons=True`) and no RLE at all
+        has no size to take, so it needs image_shapes; without it this raises ValueError."""
+        import torch
+
+        self._new_images(image_ids, len(gt_anns), gt_anns, "annotation lists")
+        if image_shapes is not None and len(image_shapes) != len(image_ids):
+            raise ValueError(f"{len(image_shapes)} image shapes for {len(image_ids)} images")
+        self._freeze()
+        if len(image_ids) == 0:
+            return
+        pos = {i: b for b, i in enumerate(image_ids)}
+        dets = [[] for _ in image_ids]
+        for k, r in enumerate(results):
+            if r.get("image_id") not in pos:
+                raise ValueError(f"result {k}: image {r.get('image_id')!r} is not one of the "
+                                 "batch's image ids")
+            seg = r.get("segmentation")
+            if not isinstance(seg, dict) or "counts" not in seg or "size" not in seg:
+                raise ValueError(f"result {k}: segmentation must be an RLE dict with 'size' and "
+                                 "'counts'")
+            dets[pos[r["image_id"]]].append(r)
+        shapes = []
+        for image_id, d, anns in zip(image_ids, dets, gt_anns):
+            sizes = {tuple(int(v) for v in np.ravel(x["segmentation"]["size"])) for x in d}
+            sizes |= {tuple(int(v) for v in np.ravel(a["segmentation"]["size"])) for a in anns
+                      if isinstance(a, dict) and isinstance(a.get("segmentation"), dict)
+                      and "size" in a["segmentation"]}
+            if image_shapes is not None:
+                sizes.add(tuple(int(v) for v in image_shapes[len(shapes)]))
+            if len(sizes) > 1:
+                raise ValueError(f"image {image_id!r}: RLE sizes {sorted(sizes)} differ")
+            if not sizes and self._polygons and any(isinstance(a, dict) and isinstance(a.get("segmentation"), list)
+                                 for a in anns):
+                raise ValueError(f"image {image_id!r}: its ground truth is polygons only, so its "
+                                 "shape is unknown; give it in image_shapes")
+            shapes.append(sizes.pop() if sizes else (1, 1))
+        cats, crowd, area, rles = self._gt_tables(image_ids, gt_anns, shapes)
+        N.require_cuda()
+        lib = N.load()
+        dev = torch.device("cuda", torch.cuda.current_device())
+        geoms = [[H, W, H, W, 0, 0, H, W] for H, W in shapes]
+        pred_cls = [np.asarray([self._dense(x["category_id"]) for x in d], np.int32) for d in dets]
+        pred = MaskBatch.from_rle(lib, dev, geoms, pred_cls, [[x["segmentation"] for x in d]
+                                                              for d in dets])
+        gt = (MaskBatch.from_coco if self._polygons else MaskBatch.from_rle)(lib, dev, geoms, cats,
+                                                                            rles)
+        area = self._areas(gt, area)
+        scores = self._padded([[float(x["score"]) for x in d] for d in dets], pred.R, np.float64)
+        d_scores = torch.from_numpy(scores).to(dev)
+        res = coco_evaluate_batch(lib, pred.planes, pred.d_class_ids, d_scores, gt,
+                                  self._padded(crowd, gt.R, np.uint8),
+                                  self._padded(area, gt.R, np.float64),
+                                  np.arange(max(len(self._cat_index), 1), dtype=np.int32),
+                                  self.params)
+        self._record(image_ids, res, cats, crowd, area)
+
+
+
+class COCOevalBbox(_COCOevalBase):
+    """pycocotools' `COCOeval(cocoGt, cocoDt, "bbox")` as a streaming evaluator, with
+    `COCOevalSegm`'s API: `add_batch` with model outputs, `add_results` with COCO bbox results,
+    then `accumulate()` and `summarize()` give pycocotools' `eval` arrays and twelve `stats`
+    exactly.  The per-image work of `evaluate()` -- bbIou, bit for bit, and the matching for every
+    (image, category, area range, threshold) -- runs on the device as each batch arrives; no mask
+    is made or read.
+
+    Ground-truth annotations are COCO dicts with `category_id`, `bbox` ([x, y, w, h]), `area`
+    (which decides the area range) and `iscrowd` (default 0; a crowd box's IoU is intersection /
+    detection area).  `segmentation` is not read.  A detection's area is w*h of its box, as
+    `loadRes` stores it for bbox results.
+
+    Stated differences from pycocotools: matches are recorded by position, as in `COCOevalSegm`;
+    an annotation without `bbox` or `area` raises ValueError where pycocotools raises KeyError; a
+    `bbox` that is not 4 numbers, or whose x, y, w, h, x + w, y + h or w * h is not finite, and a
+    NaN `area`, raise ValueError (pycocotools computes NaN IoUs from such boxes, which its loop
+    takes as matches).  `iouThrs`, `areaRng` and `maxDets[-1]` must not change after the first
+    batch."""
+
+    _iou_type = "bbox"
+
+    @staticmethod
+    def _box(bb, where):
+        """bb as float64 [4], checked: 4 numbers, and x, y, w, h, x+w, y+h, w*h all finite."""
+        try:
+            box = np.asarray(bb, dtype=np.float64)
+        except (TypeError, ValueError):
+            box = None
+        if box is None or box.shape != (4,):
+            raise ValueError(f"{where}: bbox must be 4 numbers [x, y, w, h], got {bb!r}")
+        with np.errstate(over="ignore", invalid="ignore"):
+            derived = np.array([box[0] + box[2], box[1] + box[3], box[2] * box[3]])
+        if not (np.isfinite(box).all() and np.isfinite(derived).all()):
+            raise ValueError(f"{where}: bbox {bb!r} is not finite (its x, y, w, h, x+w, y+h and "
+                             "w*h must be)")
+        return box
+
+    def _gt_tables(self, image_ids, gt_anns, shapes=None):
+        """Per image: dense category ids, crowd flags, areas and boxes [M, 4], each annotation
+        checked (the image shapes are not needed)."""
+        cats, crowd, area, boxes = [], [], [], []
+        for image_id, anns in zip(image_ids, gt_anns):
+            c, cr, ar, bx = [], [], [], []
+            for k, ann in enumerate(anns):
+                where = self._where(image_id, k, ann)
+                for key in ("bbox", "area"):
+                    if not isinstance(ann, dict) or key not in ann:
+                        raise ValueError(f"{where}: no '{key}'")
+                bx.append(self._box(ann["bbox"], where))
+                a = float(ann["area"])
+                if np.isnan(a):
+                    raise ValueError(f"{where}: area is NaN")
+                cat = int(ann["category_id"])
+                self._gt_cats.add(cat)
+                c.append(self._dense(cat))
+                cr.append(1 if ann.get("iscrowd", 0) else 0)
+                ar.append(a)
+            cats.append(np.asarray(c, np.int32))
+            crowd.append(np.asarray(cr, np.uint8))
+            area.append(np.asarray(ar, np.float64))
+            boxes.append(np.asarray(bx, np.float64).reshape(-1, 4))
+        return cats, crowd, area, boxes
+
+    def _gt_arrays(self, tables):
+        """The padded host arrays of coco_box_evaluate_batch's ground truth."""
+        cats, crowd, area, boxes = tables
+        R2 = max(max((len(c) for c in cats), default=0), 1)
+        return (np.asarray([len(c) for c in cats], np.int32), self._padded(cats, R2, np.int32),
+                self._padded(boxes, R2, np.float64, (4,)), self._padded(crowd, R2, np.uint8),
+                self._padded(area, R2, np.float64))
+
+    def add_batch(self, items, image_ids, gt_anns, category_ids=None):
+        """Evaluate model outputs against COCO ground truth: items as for
+        `api_utils.unmold_detections_batch`, one image id and one list of annotation dicts per
+        item, `category_ids` as in `unmold_coco_results_batch` (None keeps the class id).  Only
+        the unmold prepare step runs (`enqueue(..., expand=False)`): the kept boxes are scored
+        where it leaves them, and no mask is expanded."""
+        from . import api_utils
+
+        api_utils.unmold_coco_eval_batch(items, image_ids, gt_anns, [self], category_ids)
+
+    def _batch_eval(self, eng, tables, category_ids):
+        res = eng.enqueue_coco_box_eval(*self._gt_arrays(tables),
+                                        self._class_map(eng.C, category_ids), self.params)
+        cats, crowd, area, _ = tables
+        return res, cats, crowd, area
+
+    def add_results(self, results, gt_anns, image_ids):
+        """Evaluate COCO bbox results -- dicts {'image_id', 'category_id', 'score', 'bbox':
+        [x, y, w, h]} as `loadRes` takes them and `unmold_coco_results_batch` returns them --
+        against gt_anns[b], the annotation dicts of image_ids[b].  Every result's image must be
+        one of image_ids.  No image shape is needed."""
+        self._new_images(image_ids, len(gt_anns), gt_anns, "annotation lists")
+        self._freeze()
+        if len(image_ids) == 0:
+            return
+        pos = {i: b for b, i in enumerate(image_ids)}
+        dets = [[] for _ in image_ids]
+        for k, r in enumerate(results):
+            if r.get("image_id") not in pos:
+                raise ValueError(f"result {k}: image {r.get('image_id')!r} is not one of the "
+                                 "batch's image ids")
+            if "bbox" not in r:
+                raise ValueError(f"result {k}: no 'bbox'")
+            dets[pos[r["image_id"]]].append((self._box(r["bbox"], f"result {k}"), r))
+        tables = self._gt_tables(image_ids, gt_anns)
+        N.require_cuda()
+        R1 = max(max(len(d) for d in dets), 1)
+        pred_boxes = self._padded([[box for box, _ in d] for d in dets], R1, np.float64, (4,))
+        pred_cls = self._padded([[self._dense(r["category_id"]) for _, r in d] for d in dets], R1,
+                                np.int32)
+        scores = self._padded([[float(r["score"]) for _, r in d] for d in dets], R1, np.float64)
+        res = coco_box_evaluate_batch(N.load(), pred_boxes,
+                                      np.asarray([len(d) for d in dets], np.int32), pred_cls,
+                                      scores, *self._gt_arrays(tables),
+                                      np.arange(max(len(self._cat_index), 1), dtype=np.int32),
+                                      self.params)
+        cats, crowd, area, _ = tables
+        self._record(image_ids, res, cats, crowd, area)
 
 
 def ann_to_mask(ann, height, width):

@@ -4,7 +4,7 @@ numbers go into README.md.  One JSON line per workload on stdout; the COCO compr
 each unmold workload also names the GPU and its power limit.
 
   python tools/bench_secondary.py [--iters 20] [--cpu]     (--cpu also times the oracle)
-  python tools/bench_secondary.py --only-eval | --only-cocoeval | --only-polygons
+  python tools/bench_secondary.py --only-eval | --only-cocoeval | --only-bboxeval | --only-polygons
 """
 import argparse
 import ctypes as C
@@ -350,6 +350,134 @@ def cocoeval_case(iters, n_batches=4):
     torch.cuda.empty_cache()
 
 
+def bboxeval_case(iters, n_batches=4):
+    """COCO box AP over the batches of cocoeval_case (configs[1]: 32 x 1024x1024, 100 predictions
+    against 100 jittered instances, ~10 % crowd), the ground-truth boxes the jittered masks'
+    extents with sub-pixel jitter, rounded to 2 decimals.  The three kernels alone on one batch
+    (ranks, box IoUs, match with float64 areas), COCOevalBbox.add_batch end to end per batch
+    (input upload, unmold prepare, the kernels, the download; no mask), segm + bbox from one
+    unmold (unmold_coco_eval_batch with both evaluators) against two separate add_batch calls, and
+    the restated pycocotools bbox evaluate (tests/bbox_cocoeval_oracle.py) per image on the host."""
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, evaluate
+    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import coco_device_params
+
+    batch, base_n = 32, 4
+    base = synth.make_batch(11, base_n, (1024, 1024), 100)
+    rng = np.random.default_rng(12)
+    jit = [synth.jitter_coco_ground_truth(im, rng, crowd_frac=0.1, max_shift=12) for im in base]
+    jit_items = [(j.detections, j.mrcnn_mask, j.original_image_shape, j.image_shape, j.window)
+                 for j, _, _ in jit]
+    gt_rle = api_utils.unmold_detections_rle_batch(jit_items, compressed=True)
+    base_anns = []
+    for g, (_, crowd, area) in zip(gt_rle, jit):
+        y1, x1, y2, x2 = g[0].astype(np.float64).T
+        xywh = np.round(np.stack([x1, y1, x2 - x1, y2 - y1], 1)
+                        + rng.uniform(-0.5, 0.5, (len(x1), 4)), 2)
+        base_anns.append([{"category_id": int(c), "iscrowd": int(cr), "area": float(a),
+                           "bbox": [float(v) for v in bb], "segmentation": r}
+                          for c, cr, a, bb, r in zip(g[1], crowd, area, xywh, g[3])])
+    items = [(im.detections, im.mrcnn_mask, im.original_image_shape, im.image_shape, im.window)
+             for im in (base[i % base_n] for i in range(batch))]
+    anns = [base_anns[i % base_n] for i in range(batch)]
+
+    def stream(make, add):
+        evs, ts = make(), []
+        for k in range(n_batches):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            add(evs, list(range(k * batch, (k + 1) * batch)))
+            ts.append((time.perf_counter() - t0) * 1e3)
+        return evs, ts
+
+    bbox_only = lambda evs, ids: evs[0].add_batch(items, ids, anns)  # noqa: E731
+    (ev,), per_batch = stream(lambda: [evaluate.COCOevalBbox()], bbox_only)
+    _, apart = stream(lambda: [evaluate.COCOevalSegm(), evaluate.COCOevalBbox()],
+                      lambda evs, ids: [e.add_batch(items, ids, anns) for e in evs])
+    both_evs, both = stream(lambda: [evaluate.COCOevalSegm(), evaluate.COCOevalBbox()],
+                            lambda evs, ids: api_utils.unmold_coco_eval_batch(items, ids, anns, evs))
+    with open(os.devnull, "w") as null:
+        stdout, sys.stdout = sys.stdout, null
+        try:
+            for e in [ev] + both_evs:
+                e.accumulate()
+                e.summarize()
+        finally:
+            sys.stdout = stdout
+
+    # the kernels alone on one planned batch, after the prepare step only
+    eng = UnmoldEngine(batch, 100, (28, 28), 81)
+    eng.plan([make_geom(*it[2:]) for it in items], canvas=False)
+    d_det = torch.from_numpy(np.stack([it[0] for it in items])).cuda()
+    d_msk = torch.from_numpy(np.stack([it[1] for it in items])).cuda()
+    eng.enqueue(d_det, d_msk, expand=False)
+    tables = ev._gt_tables(list(range(batch)), anns)
+    g_counts, g_cat, g_boxes, g_crowd, g_area = ev._gt_arrays(tables)
+    res = eng.enqueue_coco_box_eval(g_counts, g_cat, g_boxes, g_crowd, g_area,
+                                    ev._class_map(81, None), ev.params)
+    thr, rngs, max_det = coco_device_params(ev.params)
+    n, R1, R2, T, A = batch, eng.R, g_cat.shape[1], len(thr), len(rngs) // 2
+    dev = eng.device
+    P = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+    d_map = torch.from_numpy(ev._class_map(81, None)).to(dev)
+    d_cat = torch.empty((n, R1), dtype=torch.int32, device=dev)
+    d_rank, d_walk = torch.empty_like(d_cat), torch.empty_like(d_cat)
+    d_keep = torch.empty((n, R1), dtype=torch.uint8, device=dev)
+    d_gcount, d_gcat = torch.from_numpy(g_counts).to(dev), torch.from_numpy(g_cat).to(dev)
+    d_gbox, d_crowd = torch.from_numpy(g_boxes).to(dev), torch.from_numpy(g_crowd).to(dev)
+    d_area = torch.from_numpy(g_area).to(dev)
+    d_pa = torch.empty((n, R1), dtype=torch.float64, device=dev)
+    d_match = torch.empty((A, T, n, R1), dtype=torch.int32, device=dev)
+    d_ign = torch.empty((A, T, n, R1), dtype=torch.uint8, device=dev)
+    d_iou = res["d_iou"]
+    st = N.stream_ptr(None)
+    ranks = lambda: N.check(eng.lib.mrx_coco_ranks(  # noqa: E731
+        P(eng.d_class_ids), P(eng.d_scores), N.MRX_F32, P(eng.d_counts), P(d_map), 81, max_det,
+        P(d_cat), P(d_rank), P(d_keep), P(d_walk), n, R1, st), "mrx_coco_ranks")
+    ious = lambda: N.check(eng.lib.mrx_coco_box_ious(  # noqa: E731
+        P(eng.d_boxes), N.MRX_BOX_YXYX_I32, P(eng.d_counts), P(d_cat), P(d_keep), R1, P(d_gbox),
+        P(d_gcount), P(d_gcat), P(d_crowd), R2, P(d_pa), P(d_iou), n, st), "mrx_coco_box_ious")
+    match = lambda: N.check(eng.lib.mrx_coco_match_f64area(  # noqa: E731
+        P(d_iou), P(eng.d_counts), P(d_cat), P(d_keep), P(d_walk), P(d_pa), P(d_gcount),
+        P(d_gcat), P(d_crowd), P(d_area), N.double_array(thr), T, N.double_array(rngs), A,
+        P(d_match), P(d_ign), n, R1, R2, st), "mrx_coco_match_f64area")
+    ranks()
+    rank_ms, _ = time_ms(ranks, iters)
+    iou_ms, _ = time_ms(ious, iters)
+    match_ms, _ = time_ms(match, iters)
+    counts = eng.d_counts[:n].cpu().numpy()
+    pairs = int(sum(int(counts[b]) * int(g_counts[b]) for b in range(n)))
+
+    # the restated pycocotools bbox evaluate on the host, one image
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import bbox_cocoeval_oracle as bo
+    boxes, cls, scores, _ = api_utils.unmold_detections_packed_batch(items[:1])[0]
+    gts = [{"image_id": 0, "category_id": a["category_id"], "bbox": a["bbox"],
+            "iscrowd": a["iscrowd"], "area": a["area"]} for a in anns[0]]
+    dts = [{"image_id": 0, "category_id": int(c), "score": float(s),
+            "bbox": [int(b[1]), int(b[0]), int(b[3] - b[1]), int(b[2] - b[0])]}
+           for b, c, s in zip(boxes, cls, scores)]
+    oracle = bo.COCOevalBboxOracle(gts, dts)
+    t0 = time.perf_counter()
+    oracle.evaluate()
+    host_ms = (time.perf_counter() - t0) * 1e3
+    print(json.dumps({
+        "workload": f"COCOeval bbox: {n_batches} batches of configs[1] 32 x 1024x1024, "
+                    "100 predictions vs 100 jittered gt boxes (~10 % crowd), default params",
+        "pairs_per_batch": pairs, "bbox_stats_0_AP": round(float(ev.stats[0]), 4),
+        "segm_stats_0_AP": round(float(both_evs[0].stats[0]), 4),
+        "ranks_kernel_ms": round(rank_ms, 4), "box_ious_kernel_ms": round(iou_ms, 4),
+        "match_kernel_ms_40_area_thresholds": round(match_ms, 4),
+        "bbox_add_batch_ms_per_batch": [round(t, 1) for t in per_batch],
+        "segm_plus_bbox_one_unmold_ms_per_batch": [round(t, 1) for t in both],
+        "segm_plus_bbox_two_add_batch_ms_per_batch": [round(t, 1) for t in apart],
+        "host_oracle_bbox_evaluate_ms_per_image": round(host_ms, 1),
+        "note": "add_batch: H2D of the configs[1] inputs (28x28x81 float32 tiles), unmold prepare, "
+                "the three kernels, one download; segm also expands packed planes and decodes "
+                "the gt strings", **card()}), flush=True)
+    del eng, d_det, d_msk, res, d_iou
+    torch.cuda.empty_cache()
+
+
 def rle_gt_record(eng, gts, base_rle, base_n, items, thr10, iters):
     """The ground truth of eval_case as COCO compressed strings: mrx_rle_parse, mrx_rle_decode
     and the whole-image mrx_mask_extents alone on the uploaded strings, and
@@ -601,12 +729,16 @@ def main():
     ap.add_argument("--cpu", action="store_true")
     ap.add_argument("--only-eval", action="store_true", help="only the mask IoU / AP record")
     ap.add_argument("--only-cocoeval", action="store_true", help="only the COCO mask AP record")
+    ap.add_argument("--only-bboxeval", action="store_true", help="only the COCO box AP record")
     ap.add_argument("--only-polygons", action="store_true", help="only the polygon ground truth "
                     "record")
     args = ap.parse_args()
     torch.cuda.set_device(0)
     if args.only_cocoeval:
         cocoeval_case(args.iters)
+        return
+    if args.only_bboxeval:
+        bboxeval_case(args.iters)
         return
     if args.only_polygons:
         polygons_case(args.iters)
