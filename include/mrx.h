@@ -23,6 +23,7 @@
  *   mrx_rle_parse / _decode (extension: ground truth given as COCO RLE, decoded to packed planes)
  *   mrx_coco_ranks / _ious / _box_ious / _match[_f64area] (extension: pycocotools' COCOeval for
  *                             "segm" and "bbox", the per-image half)
+ *   mrx_mask_boundary / mrx_coco_boundary_ious (extension: the same for "boundary", Boundary AP)
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
  *   mrx_device_alloc/_free (the canvas allocation: compressible device memory where offered)
  *
@@ -45,7 +46,7 @@
 extern "C" {
 #endif
 
-#define MRX_ABI_VERSION 14
+#define MRX_ABI_VERSION 15
 
 #define MRX_OK              0
 #define MRX_E_INVALID      -1   /* bad argument (null pointer, size out of range) */
@@ -138,7 +139,8 @@ int mrx_unmold_prepare(const void *d_detections, int det_dtype, const void *d_mr
 /* Output slots: where the masks of a planned batch live (engine.BatchLayout states the same on
  * the host), for every entry point that writes or reads them (mrx_mask_expand,
  * mrx_mask_expand_values, mrx_mask_expand_packed, mrx_pack_masks, mrx_composite_masks,
- * mrx_contours_count, mrx_contours_write, mrx_mask_extents, mrx_mask_overlaps, mrx_rle_decode).
+ * mrx_contours_count, mrx_contours_write, mrx_mask_extents, mrx_mask_overlaps, mrx_rle_decode,
+ * mrx_mask_boundary, mrx_coco_boundary_ious).
  * N_b = d_counts[b], H_b, W_b = d_geom[b][0], [1].
  *   Canvas slots: image b's bool masks [H_b, W_b, N_b] (N innermost, 1 byte per element, values
  *     0/1) at d_canvas + d_canvas_off[b] (int64, each a multiple of 16).  Slot b holds at least
@@ -461,6 +463,52 @@ int mrx_coco_box_ious(const void *d_pred_boxes, int box_form, const int *d_pred_
                       const double *d_gt_boxes, const int *d_gt_counts, const int *d_gt_cat,
                       const unsigned char *d_gt_crowd, int R2, double *d_pred_area, double *d_iou,
                       int B, void *stream);
+
+/* ---------------------------------------------------------------- Boundary IoU evaluation */
+/* EXTENSION: COCOeval for iouType "boundary" (Cheng et al., "Boundary IoU", CVPR 2021; the
+ * boundary_iou_api restatement of pycocotools), whose computeIoU takes the smaller of the mask IoU
+ * and the IoU of the masks' boundaries; ranks and matches are mrx_coco_ranks and mrx_coco_match.
+ *
+ * mrx_mask_boundary: for every plane k < N_b of the packed slots (see "Output slots"), its
+ *   boundary plane into d_boundary at the same slot offsets (d_packed_off): mask AND NOT the mask
+ *   eroded by a (2d+1) x (2d+1) square, d = d_dilation[b] (int32 [B], the caller's
+ *   max(1, round(ratio * sqrt(H_b^2 + W_b^2))); a d below 1 is taken as 1), counting every pixel
+ *   outside d_regions[b][k] (int32 [B,R,4] y1, x1, y2, x2, required, clamped to the image) as 0:
+ *   boundary_iou_api's mask_to_boundary (cv2.erode of the mask padded with one zero pixel, d
+ *   iterations of a 3 x 3 kernel) when the plane is zero outside its region, e.g. an expanded
+ *   plane and its d_boxes of mrx_unmold_prepare, or any plane and (0, 0, H_b, W_b).  A d at or
+ *   above the region's height or width erodes everything: the boundary is the mask.  Written:
+ *   every byte of the plane that holds a pixel of the region, its bits outside the region 0;
+ *   other bytes are not written, and readers that stay inside the region (mrx_mask_extents with
+ *   the same regions, the pair walk of mrx_coco_boundary_ious) never see them.  The boundary of a
+ *   mask has the mask's tight extents.  d_boundary must not overlap d_packed.  max_w: the extent
+ *   of "Output slots", at least 1; rows wider than the device's shared memory holds return
+ *   MRX_E_UNSUPPORTED (on an H100, max_w above 116 224).  Areas: mrx_mask_extents over
+ *   d_boundary with the same regions.
+ * mrx_coco_boundary_ious: mrx_coco_ious's arguments plus each side's boundary planes (d_boundary1,
+ *   d_boundary2, in the slots of d_packed1, d_packed2; 4-byte aligned) and their areas
+ *   (d_boundary_areas1, d_boundary_areas2 [B,R] int64); the extents are the masks'.  Element
+ *   (b, i, j) for a kept i < N1_b and j < N2_b of the same category is fmin(mask IoU, boundary
+ *   IoU), each as mrx_coco_ious computes it (exact counts, one rounding, 0 when the intersection
+ *   is 0, the crowd union = the detection's area: its boundary area for the boundary IoU).  Other
+ *   elements are not written.
+ * Checks: those of "Output slots" (for mrx_coco_boundary_ious, for each slot set), then
+ * mrx_mask_boundary: a null d_regions, a null d_dilation or d_boundary, max_w below 1;
+ * mrx_coco_boundary_ious: null areas or extents, null pointers, the alignment of the packed and
+ * then of the boundary bases: MRX_E_INVALID.  B = 0 returns MRX_OK without launching anything. */
+int mrx_mask_boundary(const unsigned char *d_packed, const long long *d_packed_off,
+                      const int *d_counts, const int *d_geom, const int *d_regions,
+                      const int *d_dilation, unsigned char *d_boundary, int B, int R, int max_w,
+                      void *stream);
+int mrx_coco_boundary_ious(const unsigned char *d_packed1, const long long *d_packed_off1,
+                           const int *d_counts1, const long long *d_areas1, const int *d_extents1,
+                           const unsigned char *d_boundary1, const long long *d_boundary_areas1,
+                           const int *d_pred_cat, const unsigned char *d_pred_keep, int R1,
+                           const unsigned char *d_packed2, const long long *d_packed_off2,
+                           const int *d_counts2, const long long *d_areas2, const int *d_extents2,
+                           const unsigned char *d_boundary2, const long long *d_boundary_areas2,
+                           const int *d_gt_cat, const unsigned char *d_gt_crowd, int R2,
+                           const int *d_geom, double *d_iou, int B, void *stream);
 
 /* ---------------------------------------------------------------- COCO RLE to packed planes */
 /* EXTENSION: the inverse of mrx_rle_strings / mrx_rle_write, for ground truth held as COCO RLE

@@ -26,7 +26,7 @@ MRX_GEOM_INTS = 8
 MRX_MAX_BATCH = 4096
 MRX_MAX_MASK_DIM = 64
 MRX_MAX_LANE_MASK_W = 30    # tile width of the lane kernels: mw + 2 lanes per warp
-ABI_VERSION = 14
+ABI_VERSION = 15
 MRX_SCHED_WORDS = 4
 MRX_PEER_HANDLE_BYTES = 64
 MRX_MAX_CONTOUR_SEGMENTS = 1 << 30
@@ -94,7 +94,10 @@ SIGNATURES = {
                                     _i, _vp, _vp, _i, _i, _i, _vp]),
     "mrx_coco_box_ious": (_i, [_vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i,
                                _vp]),
-    "mrx_rle_parse": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
+    "mrx_mask_boundary": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    "mrx_coco_boundary_ious": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp,
+                                    _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _vp]),
+    "mrx_rle_parse": (_i,[_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
     "mrx_rle_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
     "mrx_poly_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                              _i, _i, _i, _i, _vp]),

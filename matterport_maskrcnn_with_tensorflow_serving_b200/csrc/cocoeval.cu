@@ -1,6 +1,7 @@
 // cocoeval.cu -- the per-image half of pycocotools' COCOeval: computeIoU for iouType "segm" on the
-// packed planes (maskApi.c rleIou) and for "bbox" on [x, y, w, h] boxes (bbIou), and the matching
-// loop of evaluateImg, which does not care where its IoUs come from.  The host keeps what
+// packed planes (maskApi.c rleIou), for "boundary" (boundary_iou_api) on the packed planes and
+// their boundary planes (boundary.cu), and for "bbox" on [x, y, w, h] boxes (bbIou), and the
+// matching loop of evaluateImg, which does not care where its IoUs come from.  The host keeps what
 // accumulate needs: per detection its category, rank, score, area and match / ignore bits.
 //
 //   coco_rank_kernel   CTA per image: each prediction's dense category (through a class map),
@@ -12,6 +13,8 @@
 //                      of mask_overlaps_kernel (walk_pairs, planes.cuh) over the pairs of one
 //                      category whose prediction is kept; a pair whose extents do not meet gets 0
 //                      without a read
+//   coco_boundary_iou_kernel the same grid and walk counting each pair's masks and boundaries
+//                      together (walk_boundary_pairs), writing the smaller of the two IoUs
 //   coco_box_iou_kernel CTA per (image, prediction), thread per ground-truth instance: bbIou of
 //                      the pairs of one category whose prediction is kept, and the prediction's
 //                      area w*h (loadRes' area of a bbox result)
@@ -30,6 +33,7 @@ namespace cocoeval {
 
 using overlaps::Planes;
 using overlaps::score_at;
+using overlaps::walk_boundary_pairs;
 using overlaps::walk_pairs;
 
 constexpr int kWarps = 8;
@@ -82,6 +86,13 @@ __global__ void __launch_bounds__(256) coco_rank_kernel(const RankParams p) {
 }
 
 // ---------------------------------------------------------------- IoUs
+// rleIou of one pair from exact counts: 0 when inter = 0, else inter / u rounded once, u the
+// detection's area a1 for a crowd instance and a1 + a2 - inter otherwise
+__device__ __forceinline__ double rle_iou(long long inter, long long a1, long long a2, bool crowd) {
+  const long long u = crowd ? a1 : a1 + a2 - inter;
+  return inter ? __ddiv_rn(static_cast<double>(inter), static_cast<double>(u)) : 0.0;
+}
+
 __global__ void __launch_bounds__(kWarps * 32)
 coco_iou_kernel(const Planes p1, const Planes p2, const int *__restrict__ geom,
                 const int *__restrict__ pred_cat, const unsigned char *__restrict__ pred_keep,
@@ -97,8 +108,31 @@ coco_iou_kernel(const Planes p1, const Planes p2, const int *__restrict__ geom,
   walk_pairs<kWarps>(
       p1, p2, geom, b, i, [&](int j) { return gt_cat[gb + j] == ci; },
       [&](int j, long long inter, long long a1, long long a2) {
-        const long long u = gt_crowd[gb + j] ? a1 : a1 + a2 - inter;
-        row[j] = inter ? __ddiv_rn(static_cast<double>(inter), static_cast<double>(u)) : 0.0;
+        row[j] = rle_iou(inter, a1, a2, gt_crowd[gb + j]);
+      });
+}
+
+// computeIoU for "boundary": np.minimum of rleIou on the masks and rleIou on the boundaries, both
+// with the crowd rule, from one walk over both pairs (q1, q2: the boundary planes of p1, p2)
+__global__ void __launch_bounds__(kWarps * 32)
+coco_boundary_iou_kernel(const Planes p1, const Planes p2, const Planes q1, const Planes q2,
+                         const int *__restrict__ geom, const int *__restrict__ pred_cat,
+                         const unsigned char *__restrict__ pred_keep,
+                         const int *__restrict__ gt_cat, const unsigned char *__restrict__ gt_crowd,
+                         double *__restrict__ out) {
+  const int i = blockIdx.x, b = blockIdx.y;
+  if (i >= p1.counts[b]) return;
+  const size_t i1 = static_cast<size_t>(b) * p1.R + i;
+  if (!pred_keep[i1]) return;
+  const int ci = pred_cat[i1];
+  const size_t gb = static_cast<size_t>(b) * p2.R;
+  double *row = out + i1 * p2.R;
+  walk_boundary_pairs<kWarps>(
+      p1, p2, q1, q2, geom, b, i, [&](int j) { return gt_cat[gb + j] == ci; },
+      [&](int j, long long inter, long long a1, long long a2, long long binter, long long ba1,
+          long long ba2) {
+        const bool crowd = gt_crowd[gb + j];
+        row[j] = fmin(rle_iou(inter, a1, a2, crowd), rle_iou(binter, ba1, ba2, crowd));
       });
 }
 
@@ -295,6 +329,39 @@ extern "C" int mrx_coco_ious(const unsigned char *d_packed1, const long long *d_
                               static_cast<cudaStream_t>(stream)>>>(
       p1, p2, d_geom, d_pred_cat, d_pred_keep, d_gt_cat, d_gt_crowd, d_iou);
   MRX_LAUNCH_CHECK("coco_iou_kernel");
+  return MRX_OK;
+}
+
+extern "C" int mrx_coco_boundary_ious(
+    const unsigned char *d_packed1, const long long *d_packed_off1, const int *d_counts1,
+    const long long *d_areas1, const int *d_extents1, const unsigned char *d_boundary1,
+    const long long *d_boundary_areas1, const int *d_pred_cat, const unsigned char *d_pred_keep,
+    int R1, const unsigned char *d_packed2, const long long *d_packed_off2, const int *d_counts2,
+    const long long *d_areas2, const int *d_extents2, const unsigned char *d_boundary2,
+    const long long *d_boundary_areas2, const int *d_gt_cat, const unsigned char *d_gt_crowd,
+    int R2, const int *d_geom, double *d_iou, int B, void *stream) {
+  const char *fn = "mrx_coco_boundary_ious";
+  overlaps::Planes p1, p2;
+  if (int rc = overlaps::check_plane_pair(
+          fn, d_packed1, d_packed_off1, d_counts1, d_areas1, d_extents1, R1, d_packed2,
+          d_packed_off2, d_counts2, d_areas2, d_extents2, R2, d_geom, B,
+          d_boundary1 && d_boundary_areas1 && d_boundary2 && d_boundary_areas2 && d_pred_cat &&
+              d_pred_keep && d_gt_cat && d_gt_crowd && d_iou,
+          p1, p2))
+    return rc;
+  MRX_CHECK_ARG(((reinterpret_cast<uintptr_t>(d_boundary1) |
+                  reinterpret_cast<uintptr_t>(d_boundary2)) & 3u) == 0u,
+                "%s: boundary bases must be 4-byte aligned", fn);
+  if (B == 0) return MRX_OK;
+  overlaps::Planes q1 = p1, q2 = p2;
+  q1.packed.base = d_boundary1;
+  q1.areas = d_boundary_areas1;
+  q2.packed.base = d_boundary2;
+  q2.areas = d_boundary_areas2;
+  cocoeval::coco_boundary_iou_kernel<<<dim3(R1, B), cocoeval::kWarps * 32, 0,
+                                       static_cast<cudaStream_t>(stream)>>>(
+      p1, p2, q1, q2, d_geom, d_pred_cat, d_pred_keep, d_gt_cat, d_gt_crowd, d_iou);
+  MRX_LAUNCH_CHECK("coco_boundary_iou_kernel");
   return MRX_OK;
 }
 

@@ -1,7 +1,8 @@
 // planes.cuh -- reading two bit-packed plane sets of one batch together, shared by the mask scorers
-// mask_overlaps_kernel (overlaps.cu) and coco_iou_kernel (cocoeval.cu): the side description
-// (Planes) and its argument check, the culled walk over the pairs of one prediction with the
-// AND-popcount of their intersection rectangle, and the scores of the rank kernels.
+// mask_overlaps_kernel (overlaps.cu), coco_iou_kernel and coco_boundary_iou_kernel (cocoeval.cu):
+// the side description (Planes) and its argument check, the culled walk over the pairs of one
+// prediction with the AND-popcount of their intersection rectangle (and its variant that counts
+// the boundary planes of the pair too), and the scores of the rank kernels.
 //
 // Planes are uint8 [N, H, ceil(W/8)], most significant bit first, as mrx_pack_masks /
 // mrx_mask_expand_packed write them.  Pixel x of a row is bit 7 - (x & 7) of byte x >> 3 in every
@@ -143,6 +144,39 @@ __device__ __forceinline__ void walk_pairs(const Planes &p1, const Planes &p2,
     if (a1 && a2 && y2 > y1 && x2 > x1)
       inter = and_count(plane1, plane_of(p2.packed, b, j, H, wb), wb, y1, x1, y2, x2, lane);
     if (lane == 0) emit(j, inter, a1, a2);
+  }
+}
+
+// walk_pairs over the masks p1, p2 and their boundary planes q1, q2 at once (coco_boundary_iou_kernel):
+// q1, q2 hold the boundaries in the slots of p1, p2 (same offsets, counts and R) with their own
+// areas.  A boundary has its mask's tight extents, so the masks' cull and intersection rectangle
+// serve both counts.  Lane 0 calls emit(j, inter, a1, a2, binter, ba1, ba2).
+template <int kWarps, class Keep, class Emit>
+__device__ __forceinline__ void walk_boundary_pairs(const Planes &p1, const Planes &p2,
+                                                    const Planes &q1, const Planes &q2,
+                                                    const int *__restrict__ geom, int b, int i,
+                                                    Keep keep, Emit emit) {
+  const int M = p2.counts[b];
+  const int H = geom[b * MRX_GEOM_INTS + 0], W = geom[b * MRX_GEOM_INTS + 1];
+  const int wb = (W + 7) >> 3;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const size_t i1 = static_cast<size_t>(b) * p1.R + i;
+  const long long a1 = p1.areas[i1], ba1 = q1.areas[i1];
+  const int4 e1 = p1.extents[i1];
+  const unsigned char *plane1 = plane_of(p1.packed, b, i, H, wb);
+  const unsigned char *bplane1 = plane_of(q1.packed, b, i, H, wb);
+  for (int j = warp; j < M; j += kWarps) {
+    if (!keep(j)) continue;
+    const size_t i2 = static_cast<size_t>(b) * p2.R + j;
+    const long long a2 = p2.areas[i2], ba2 = q2.areas[i2];
+    const int4 e2 = p2.extents[i2];
+    const int y1 = max(e1.x, e2.x), x1 = max(e1.y, e2.y), y2 = min(e1.z, e2.z), x2 = min(e1.w, e2.w);
+    long long inter = 0, binter = 0;
+    if (a1 && a2 && y2 > y1 && x2 > x1) {
+      inter = and_count(plane1, plane_of(p2.packed, b, j, H, wb), wb, y1, x1, y2, x2, lane);
+      binter = and_count(bplane1, plane_of(q2.packed, b, j, H, wb), wb, y1, x1, y2, x2, lane);
+    }
+    if (lane == 0) emit(j, inter, a1, a2, binter, ba1, ba2);
   }
 }
 

@@ -14,6 +14,7 @@ every computation on the path is a libmrx kernel launched through ctypes.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import threading
 import weakref
 from typing import NamedTuple
@@ -522,6 +523,37 @@ class UnmoldEngine:
                                        self.d_class_ids[:n], self.d_scores[:n], gt_counts, gt_cat,
                                        gt_boxes, gt_crowd, gt_area, class_map, params, stream)
 
+    def enqueue_coco_boundary_eval(self, gt, gt_crowd, gt_area, class_map, params,
+                                   dilation_ratio=0.02, stream=None):
+        """EXTENSION: `coco_boundary_evaluate_batch` (COCOeval "boundary", Boundary AP) of the
+        planned batch's kept instances against `gt`, as `enqueue_coco_eval` takes them; each
+        prediction's boundary is eroded inside its box, outside which its plane is zero.  The
+        boundary planes and their areas live in `_eval_bufs`.  Synchronises once; returns its
+        dict."""
+        pred = self._prediction_planes(gt, "enqueue_coco_boundary_eval", stream)
+        n = self._n_images
+        return coco_boundary_evaluate_batch(self.lib, pred, self.d_boxes, self.d_class_ids[:n],
+                                            self.d_scores[:n], gt, gt_crowd, gt_area, class_map,
+                                            params, dilation_ratio, stream, self._eval_bufs)
+
+    def boundary_planes(self, dilation_ratio=0.02, stream=None):
+        """EXTENSION: `Planes` of the boundaries of the planned batch's kept masks (after
+        `enqueue_expand_packed` or `pack_masks`), as boundary_iou_api's mask_to_boundary computes
+        them for `dilation_ratio`: mrx_mask_boundary inside each kept box, then mrx_mask_extents
+        for the areas (the extents are the masks').  Only the bytes of a plane that hold a pixel
+        of its box are written (outside the box the boundary is zero).  The buffers live in
+        `_eval_bufs`."""
+        if self.layout is None or self.d_packed is None:
+            raise RuntimeError("boundary_planes needs the packed planes: call "
+                               "enqueue_expand_packed or pack_masks first")
+        d = boundary_dilation(self.layout.geom, dilation_ratio)
+        with _stream_ctx(stream):
+            d_dil = _torch().from_numpy(d).to(self.device)
+            pred = Planes(self.d_packed, self.d_packed_off, self.d_counts, None, None, self.R)
+            return mask_boundary_planes(self.lib, pred, self.d_geom, self.d_boxes, d_dil,
+                                        self._n_images, self.layout.max_w, self._eval_bufs,
+                                        stream)
+
     def _prediction_planes(self, gt, fn, stream):
         """`Planes` of the planned batch's kept instances to score against `gt` (a `MaskBatch` of
         the same plan), each counted only inside its box (mrx_mask_extents into `_eval_bufs`)."""
@@ -805,7 +837,19 @@ class MaskBatch:
                                          _ptr(d_ext), n, R, N.stream_ptr(stream)),
                     "mrx_mask_extents")
         self.planes = Planes(d_packed, d_off, self.d_counts, d_areas, d_ext, R)
+        self.d_regions = d_regions
         return d_extra
+
+    def boundary_planes(self, dilation_ratio=0.02, stream=None):
+        """EXTENSION: `Planes` of the boundaries of this batch's masks, as boundary_iou_api's
+        mask_to_boundary computes them for `dilation_ratio` (`boundary_dilation`), each over its
+        whole image (mrx_mask_boundary, then mrx_mask_extents for the areas; the extents are the
+        masks')."""
+        d = boundary_dilation(self.geom, dilation_ratio)
+        with _stream_ctx(stream):
+            d_dil = _torch().from_numpy(d).to(self.d_geom.device)
+            return mask_boundary_planes(N.load(), self.planes, self.d_geom, self.d_regions, d_dil,
+                                        self.n, int(self.geom[:, 1].max(initial=1)), {}, stream)
 
     def set_counts(self, counts, stream=None):
         """Keep only the first counts[b] instances of each image (counts[b] <= M_b), as upstream
@@ -1187,6 +1231,90 @@ def coco_box_evaluate_batch(lib, pred_boxes, pred_counts, pred_class_ids, pred_s
 
         return _coco_evaluate(lib, n, R1, R2, pred_counts, pred_class_ids, pred_scores, d_counts,
                               d_cat, d_crowd, d_area, d_map, params, np.float64, ious, stream)
+
+
+def check_dilation_ratio(dilation_ratio):
+    """dilation_ratio as a float: a finite real number > 0, else ValueError."""
+    ok = isinstance(dilation_ratio, (int, float, np.integer, np.floating)) and \
+        not isinstance(dilation_ratio, (bool, np.bool_))
+    r = float(dilation_ratio) if ok else math.nan
+    if not (math.isfinite(r) and r > 0):
+        raise ValueError(f"dilation_ratio must be a finite number > 0, got {dilation_ratio!r}")
+    return r
+
+
+def boundary_dilation(geoms, dilation_ratio):
+    """int32 [n]: boundary_iou_api's dilation of each image of `geoms` ([n, 8], see make_geom),
+    max(1, int(round(dilation_ratio * sqrt(H**2 + W**2)))) with Python's round (half to even).
+    Values above 2^30 are stored as 2^30: any d at or above an image side erodes everything."""
+    r = check_dilation_ratio(dilation_ratio)
+    g = np.asarray(geoms, dtype=np.int64).reshape(-1, N.MRX_GEOM_INTS)
+    return np.array([min(max(1, int(round(r * math.sqrt(int(H) ** 2 + int(W) ** 2)))), 1 << 30)
+                     for H, W in g[:, :2]], dtype=np.int32).reshape(-1)
+
+
+def mask_boundary_planes(lib, planes, d_geom, d_regions, d_dilation, n, max_w, bufs, stream=None,
+                         name="boundary"):
+    """`Planes` of the boundaries of `planes` (n images, d_geom [n, 8]): mrx_mask_boundary with
+    regions d_regions [n, planes.R, 4] and dilations d_dilation [n] int32 into a buffer of the
+    same slot layout, then mrx_mask_extents over it with the same regions for the areas.  The
+    boundary planes, areas and (the masks') extents are kept in `bufs` under `name`."""
+    torch = _torch()
+    R, dev = int(planes.R), d_geom.device
+    d_bnd = _buffer(bufs, name + "_packed", planes.d_packed.numel(), torch.uint8, dev)
+    d_areas = _buffer(bufs, name + "_areas", n * R, torch.int64, dev)
+    d_ext = _buffer(bufs, name + "_extents", n * R * 4, torch.int32, dev)
+    st = N.stream_ptr(stream)
+    N.check(lib.mrx_mask_boundary(
+        _ptr(planes.d_packed), _ptr(planes.d_packed_off), _ptr(planes.d_counts), _ptr(d_geom),
+        _ptr(d_regions), _ptr(d_dilation), _ptr(d_bnd), n, R, max(int(max_w), 1), st),
+        "mrx_mask_boundary")
+    N.check(lib.mrx_mask_extents(
+        _ptr(d_bnd), _ptr(planes.d_packed_off), _ptr(planes.d_counts), _ptr(d_geom),
+        _ptr(d_regions), _ptr(d_areas), _ptr(d_ext), n, R, st), "mrx_mask_extents")
+    return Planes(d_bnd, planes.d_packed_off, planes.d_counts, d_areas[:n * R].view(n, R),
+                  d_ext[:n * R * 4].view(n, R, 4), R)
+
+
+def coco_boundary_evaluate_batch(lib, pred, pred_regions, pred_class_ids, pred_scores, gt,
+                                 gt_crowd, gt_area, class_map, params, dilation_ratio=0.02,
+                                 stream=None, bufs=None):
+    """The per-image half of COCOeval for iouType "boundary" (boundary_iou_api) for one batch:
+    mrx_coco_ranks, the boundaries of both sides (`mask_boundary_planes`: the predictions inside
+    pred_regions [n, pred.R, 4] int32, e.g. their boxes, the ground truth over its whole images),
+    mrx_coco_boundary_ious and mrx_coco_match, then one download and one synchronisation.  The
+    per-image dilations (`boundary_dilation`) go up in the one copy of the ground-truth tables.
+    Arguments and result as for `coco_evaluate_batch` (`area` is the mask's pixel count); `bufs`
+    keeps the boundary buffers between calls."""
+    n, R1, R2 = gt.n, int(pred.R), int(gt.R)
+    class_map = _coco_class_map(class_map)
+    dil = boundary_dilation(gt.geom, dilation_ratio)
+    max_w = int(gt.geom[:, 1].max(initial=1))
+    bufs = {} if bufs is None else bufs
+    with _stream_ctx(stream):
+        d_crowd, d_area, d_map, d_dil = _upload_parts(
+            [np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
+             np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map, dil],
+            gt.d_geom.device)
+
+        def ious(v, d_iou, st):
+            v["area"].copy_(pred.d_areas.view(-1)[:n * R1].view(n, R1))
+            bp = mask_boundary_planes(lib, pred, gt.d_geom, pred_regions, d_dil, n, max_w, bufs,
+                                      stream, "pred_boundary")
+            bg = mask_boundary_planes(lib, gt.planes, gt.d_geom, gt.d_regions, d_dil, n, max_w,
+                                      bufs, stream, "gt_boundary")
+            N.check(lib.mrx_coco_boundary_ious(
+                _ptr(pred.d_packed), _ptr(pred.d_packed_off), _ptr(pred.d_counts),
+                _ptr(pred.d_areas), _ptr(pred.d_extents), _ptr(bp.d_packed), _ptr(bp.d_areas),
+                _ptr(v["cat"]), _ptr(v["keep"]), R1,
+                _ptr(gt.planes.d_packed), _ptr(gt.planes.d_packed_off), _ptr(gt.planes.d_counts),
+                _ptr(gt.planes.d_areas), _ptr(gt.planes.d_extents), _ptr(bg.d_packed),
+                _ptr(bg.d_areas), _ptr(gt.d_class_ids), _ptr(d_crowd), R2, _ptr(gt.d_geom),
+                _ptr(d_iou), n, st), "mrx_coco_boundary_ious")
+
+        return _coco_evaluate(lib, n, R1, R2, pred.d_counts, pred_class_ids, pred_scores,
+                              gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map, params,
+                              np.int64, ious, stream)
 
 
 def _coco_class_map(class_map):

@@ -16,7 +16,10 @@ evaluator: the IoUs and matching of `evaluate()` run on the device as each batch
 (`mrx_coco_ranks`, `mrx_coco_ious`, `mrx_coco_match`, DESIGN.md section 3.15); `accumulate()` and
 `summarize()` run on the host and equal pycocotools' exactly.  `COCOevalBbox` is the same for
 iouType "bbox" (COCO box AP): box IoUs and matching on the device (`mrx_coco_box_ious`,
-`mrx_coco_match_f64area`, DESIGN.md section 3.17), no mask involved.
+`mrx_coco_match_f64area`, DESIGN.md section 3.17), no mask involved.  `COCOevalBoundary` is
+boundary_iou_api's COCOeval for iouType "boundary" (Boundary AP): `COCOevalSegm` with the IoU
+taken as the smaller of the mask IoU and the boundary IoU, the boundaries made on the device
+(`mrx_mask_boundary`, `mrx_coco_boundary_ious`, DESIGN.md section 3.18).
 
 `ann_to_mask` is Matterport's `CocoDataset.annToMask`, rasterised on the device (DESIGN.md
 section 3.16).
@@ -26,8 +29,9 @@ from __future__ import annotations
 import numpy as np
 
 from . import _native as N
-from .engine import (MaskBatch, coco_box_evaluate_batch, coco_device_params,
-                     coco_evaluate_batch, mask_matches, mask_overlaps)
+from .engine import (MaskBatch, check_dilation_ratio, coco_boundary_evaluate_batch,
+                     coco_box_evaluate_batch, coco_device_params, coco_evaluate_batch,
+                     mask_matches, mask_overlaps)
 
 
 def trim_zeros(x):
@@ -499,10 +503,19 @@ class COCOevalSegm(_COCOevalBase):
         cats, crowd, area, rles = tables
         gt = (eng.ground_truth_coco if self._polygons else eng.ground_truth_rle)(cats, rles)
         area = self._areas(gt, area)
-        res = eng.enqueue_coco_eval(gt, self._padded(crowd, gt.R, np.uint8),
-                                    self._padded(area, gt.R, np.float64),
-                                    self._class_map(eng.C, category_ids), self.params)
+        res = self._engine_ious(eng, gt, self._padded(crowd, gt.R, np.uint8),
+                                self._padded(area, gt.R, np.float64),
+                                self._class_map(eng.C, category_ids))
         return res, cats, crowd, area
+
+    # the IoU step, the one part a mask IoU type replaces: on an engine's kept instances
+    # (`add_batch`), or on decoded results (`add_results`, pred a `MaskBatch`)
+    def _engine_ious(self, eng, gt, crowd, area, class_map):
+        return eng.enqueue_coco_eval(gt, crowd, area, class_map, self.params)
+
+    def _result_ious(self, lib, pred, d_scores, gt, crowd, area, class_map):
+        return coco_evaluate_batch(lib, pred.planes, pred.d_class_ids, d_scores, gt, crowd, area,
+                                   class_map, self.params)
 
     def add_results(self, results, gt_anns, image_ids, image_shapes=None):
         """Evaluate COCO segm results -- dicts {'image_id', 'category_id', 'score',
@@ -559,12 +572,51 @@ class COCOevalSegm(_COCOevalBase):
         area = self._areas(gt, area)
         scores = self._padded([[float(x["score"]) for x in d] for d in dets], pred.R, np.float64)
         d_scores = torch.from_numpy(scores).to(dev)
-        res = coco_evaluate_batch(lib, pred.planes, pred.d_class_ids, d_scores, gt,
-                                  self._padded(crowd, gt.R, np.uint8),
-                                  self._padded(area, gt.R, np.float64),
-                                  np.arange(max(len(self._cat_index), 1), dtype=np.int32),
-                                  self.params)
+        res = self._result_ious(lib, pred, d_scores, gt, self._padded(crowd, gt.R, np.uint8),
+                                self._padded(area, gt.R, np.float64),
+                                np.arange(max(len(self._cat_index), 1), dtype=np.int32))
         self._record(image_ids, res, cats, crowd, area)
+
+
+class COCOevalBoundary(COCOevalSegm):
+    """boundary_iou_api's `COCOeval(cocoGt, cocoDt, "boundary", dilation_ratio)` (Boundary AP,
+    Cheng et al., "Boundary IoU", CVPR 2021) as a streaming evaluator: `COCOevalSegm` with only
+    the IoU step replaced.  A pair's IoU is the smaller of its mask IoU and the IoU of the two
+    masks' boundaries (mask AND NOT mask eroded by a (2d+1) x (2d+1) square, nothing outside the
+    image; d = max(1, round(dilation_ratio * image diagonal)) per image), both with the crowd rule
+    (a crowd's union is the detection's mask or boundary area).  The boundaries are made on the
+    device from the packed planes (`mrx_mask_boundary`, DESIGN.md section 3.18) and both IoUs come
+    from one walk over the pair (`mrx_coco_boundary_ious`); areas, ranges, matching,
+    `accumulate()` and `summarize()` are segm's.
+
+    `dilation_ratio` must be a finite number > 0 (else ValueError) and, like `iouThrs`, must not
+    change after the first batch; it is `params.dilation_ratio`.  The stated differences from
+    pycocotools are `COCOevalSegm`'s."""
+
+    _iou_type = "boundary"
+
+    def __init__(self, cat_ids=None, iou_thrs=None, rec_thrs=None, max_dets=(1, 10, 100),
+                 area_rng=None, area_rng_lbl=None, polygons=False, dilation_ratio=0.02):
+        super().__init__(cat_ids, iou_thrs, rec_thrs, max_dets, area_rng, area_rng_lbl, polygons)
+        self.params.dilation_ratio = check_dilation_ratio(dilation_ratio)
+        self._frozen_ratio = None
+
+    def _freeze(self):
+        super()._freeze()
+        r = check_dilation_ratio(self.params.dilation_ratio)
+        if self._frozen_ratio is None:
+            self._frozen_ratio = r
+        elif r != self._frozen_ratio:
+            raise ValueError("dilation_ratio changed after the first batch")
+
+    def _engine_ious(self, eng, gt, crowd, area, class_map):
+        return eng.enqueue_coco_boundary_eval(gt, crowd, area, class_map, self.params,
+                                              self._frozen_ratio)
+
+    def _result_ious(self, lib, pred, d_scores, gt, crowd, area, class_map):
+        return coco_boundary_evaluate_batch(lib, pred.planes, pred.d_regions, pred.d_class_ids,
+                                            d_scores, gt, crowd, area, class_map, self.params,
+                                            self._frozen_ratio)
 
 
 

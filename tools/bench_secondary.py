@@ -4,7 +4,8 @@ numbers go into README.md.  One JSON line per workload on stdout; the COCO compr
 each unmold workload also names the GPU and its power limit.
 
   python tools/bench_secondary.py [--iters 20] [--cpu]     (--cpu also times the oracle)
-  python tools/bench_secondary.py --only-eval | --only-cocoeval | --only-bboxeval | --only-polygons
+  python tools/bench_secondary.py --only-eval | --only-cocoeval | --only-bboxeval | --only-boundaryeval
+                                  | --only-polygons
 """
 import argparse
 import ctypes as C
@@ -350,16 +351,12 @@ def cocoeval_case(iters, n_batches=4):
     torch.cuda.empty_cache()
 
 
-def bboxeval_case(iters, n_batches=4):
-    """COCO box AP over the batches of cocoeval_case (configs[1]: 32 x 1024x1024, 100 predictions
-    against 100 jittered instances, ~10 % crowd), the ground-truth boxes the jittered masks'
-    extents with sub-pixel jitter, rounded to 2 decimals.  The three kernels alone on one batch
-    (ranks, box IoUs, match with float64 areas), COCOevalBbox.add_batch end to end per batch
-    (input upload, unmold prepare, the kernels, the download; no mask), segm + bbox from one
-    unmold (unmold_coco_eval_batch with both evaluators) against two separate add_batch calls, and
-    the restated pycocotools bbox evaluate (tests/bbox_cocoeval_oracle.py) per image on the host."""
-    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, evaluate
-    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import coco_device_params
+def coco_eval_inputs():
+    """(batch, items, anns): the configs[1] batch of bboxeval_case and boundaryeval_case, 32 x
+    1024x1024, 100 predictions against 100 jittered instances (~10 % crowd), annotated with
+    compressed-RLE segmentations, areas and boxes (the jittered masks' extents with sub-pixel
+    jitter, rounded to 2 decimals)."""
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils
 
     batch, base_n = 32, 4
     base = synth.make_batch(11, base_n, (1024, 1024), 100)
@@ -379,6 +376,21 @@ def bboxeval_case(iters, n_batches=4):
     items = [(im.detections, im.mrcnn_mask, im.original_image_shape, im.image_shape, im.window)
              for im in (base[i % base_n] for i in range(batch))]
     anns = [base_anns[i % base_n] for i in range(batch)]
+    return batch, items, anns
+
+
+def bboxeval_case(iters, n_batches=4):
+    """COCO box AP over the batches of cocoeval_case (configs[1]: 32 x 1024x1024, 100 predictions
+    against 100 jittered instances, ~10 % crowd), the ground-truth boxes the jittered masks'
+    extents with sub-pixel jitter, rounded to 2 decimals.  The three kernels alone on one batch
+    (ranks, box IoUs, match with float64 areas), COCOevalBbox.add_batch end to end per batch
+    (input upload, unmold prepare, the kernels, the download; no mask), segm + bbox from one
+    unmold (unmold_coco_eval_batch with both evaluators) against two separate add_batch calls, and
+    the restated pycocotools bbox evaluate (tests/bbox_cocoeval_oracle.py) per image on the host."""
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, evaluate
+    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import coco_device_params
+
+    batch, items, anns = coco_eval_inputs()
 
     def stream(make, add):
         evs, ts = make(), []
@@ -475,6 +487,134 @@ def bboxeval_case(iters, n_batches=4):
                 "the three kernels, one download; segm also expands packed planes and decodes "
                 "the gt strings", **card()}), flush=True)
     del eng, d_det, d_msk, res, d_iou
+    torch.cuda.empty_cache()
+
+
+def boundaryeval_case(iters, n_batches=4):
+    """Boundary AP (COCOeval "boundary", dilation_ratio 0.02: d = 29 at 1024x1024) over the batches
+    of bboxeval_case.  The kernels alone on one batch: the boundaries of the predictions (inside
+    their boxes) and of the ground truth (whole image), and the boundary IoUs;
+    COCOevalBoundary.add_batch end to end per batch; segm + bbox + boundary from one unmold
+    against three separate add_batch calls; and the restated boundary_iou_api evaluate
+    (tests/boundary_cocoeval_oracle.py, cv2 erosion) per image on the host."""
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, evaluate
+    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import (boundary_dilation,
+                                                                         coco_device_params)
+
+    batch, items, anns = coco_eval_inputs()
+
+    def stream(make, add):
+        evs, ts = make(), []
+        for k in range(n_batches):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            add(evs, list(range(k * batch, (k + 1) * batch)))
+            ts.append((time.perf_counter() - t0) * 1e3)
+        return evs, ts
+
+    three = lambda: [evaluate.COCOevalSegm(), evaluate.COCOevalBbox(),  # noqa: E731
+                     evaluate.COCOevalBoundary()]
+    (ev,), per_batch = stream(lambda: [evaluate.COCOevalBoundary()],
+                              lambda evs, ids: evs[0].add_batch(items, ids, anns))
+    _, apart = stream(three, lambda evs, ids: [e.add_batch(items, ids, anns) for e in evs])
+    together, both = stream(three, lambda evs, ids: api_utils.unmold_coco_eval_batch(items, ids,
+                                                                                      anns, evs))
+    with open(os.devnull, "w") as null:
+        stdout, sys.stdout = sys.stdout, null
+        try:
+            for e in [ev] + together:
+                e.accumulate()
+                e.summarize()
+        finally:
+            sys.stdout = stdout
+
+    # the kernels alone on one planned batch
+    eng = UnmoldEngine(batch, 100, (28, 28), 81)
+    eng.plan([make_geom(*it[2:]) for it in items], canvas=False)
+    d_det = torch.from_numpy(np.stack([it[0] for it in items])).cuda()
+    d_msk = torch.from_numpy(np.stack([it[1] for it in items])).cuda()
+    eng.enqueue_packed(d_det, d_msk)
+    gt = eng.ground_truth_rle([np.array([a["category_id"] for a in x], np.int32) for x in anns],
+                              [[a["segmentation"] for a in x] for x in anns])
+    crowd = np.zeros((batch, gt.R), np.uint8)
+    area = np.zeros((batch, gt.R))
+    for b, x in enumerate(anns):
+        crowd[b, :len(x)] = [a["iscrowd"] for a in x]
+        area[b, :len(x)] = [a["area"] for a in x]
+    res = eng.enqueue_coco_boundary_eval(gt, crowd, area, np.arange(81, dtype=np.int32),
+                                         ev.params)
+    thr, rngs, max_det = coco_device_params(ev.params)
+    n, R1, R2 = batch, eng.R, gt.R
+    dev = eng.device
+    P = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+    bufs = eng._eval_bufs
+    d_dil = torch.from_numpy(boundary_dilation(eng.layout.geom, 0.02)).to(dev)
+    d_map = torch.arange(81, dtype=torch.int32, device=dev)
+    d_cat = torch.empty((n, R1), dtype=torch.int32, device=dev)
+    d_rank, d_walk = torch.empty_like(d_cat), torch.empty_like(d_cat)
+    d_keep = torch.empty((n, R1), dtype=torch.uint8, device=dev)
+    d_crowd = torch.from_numpy(crowd).to(dev)
+    d_iou = res["d_iou"]
+    st = N.stream_ptr(None)
+    max_w = eng.layout.max_w
+    N.check(eng.lib.mrx_coco_ranks(
+        P(eng.d_class_ids), P(eng.d_scores), N.MRX_F32, P(eng.d_counts), P(d_map), 81, max_det,
+        P(d_cat), P(d_rank), P(d_keep), P(d_walk), n, R1, st), "mrx_coco_ranks")
+    pred_bnd = lambda: N.check(eng.lib.mrx_mask_boundary(  # noqa: E731
+        P(eng.d_packed), P(eng.d_packed_off), P(eng.d_counts), P(eng.d_geom), P(eng.d_boxes),
+        P(d_dil), P(bufs["pred_boundary_packed"]), n, R1, max_w, st), "mrx_mask_boundary")
+    gt_bnd = lambda: N.check(eng.lib.mrx_mask_boundary(  # noqa: E731
+        P(gt.planes.d_packed), P(gt.planes.d_packed_off), P(gt.d_counts), P(gt.d_geom),
+        P(gt.d_regions), P(d_dil), P(bufs["gt_boundary_packed"]), n, R2, max_w, st),
+        "mrx_mask_boundary")
+    ious = lambda: N.check(eng.lib.mrx_coco_boundary_ious(  # noqa: E731
+        P(eng.d_packed), P(eng.d_packed_off), P(eng.d_counts), P(bufs["areas"]),
+        P(bufs["extents"]), P(bufs["pred_boundary_packed"]), P(bufs["pred_boundary_areas"]),
+        P(d_cat), P(d_keep), R1, P(gt.planes.d_packed), P(gt.planes.d_packed_off),
+        P(gt.d_counts), P(gt.planes.d_areas), P(gt.planes.d_extents),
+        P(bufs["gt_boundary_packed"]), P(bufs["gt_boundary_areas"]), P(gt.d_class_ids),
+        P(d_crowd), R2, P(gt.d_geom), P(d_iou), n, st), "mrx_coco_boundary_ious")
+    pred_ms, _ = time_ms(pred_bnd, iters)
+    gt_ms, _ = time_ms(gt_bnd, iters)
+    iou_ms, _ = time_ms(ious, iters)
+    gt_bytes = int(sum(int(gt.counts[b]) * int(gt.geom[b, 0]) * ((int(gt.geom[b, 1]) + 7) // 8)
+                       for b in range(n)))
+
+    # the restated boundary_iou_api evaluate on the host, one image
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import boundary_cocoeval_oracle as bo
+    _, cls, scores, masks = api_utils.unmold_detections_batch(items[:1])[0]
+    H, W = int(gt.geom[0, 0]), int(gt.geom[0, 1])
+    wb = (W + 7) // 8
+    host = gt.planes.d_packed[:int(gt.counts[0]) * H * wb].cpu().numpy().reshape(-1, H, wb)
+    gt_masks = np.unpackbits(host, axis=2)[:, :, :W].astype(bool)
+    gts = [{"image_id": 0, "category_id": a["category_id"], "mask": gm, "iscrowd": a["iscrowd"],
+            "area": a["area"]} for a, gm in zip(anns[0], gt_masks)]
+    dts = [{"image_id": 0, "category_id": int(c), "mask": masks[:, :, i], "score": float(s)}
+           for i, (c, s) in enumerate(zip(cls, scores))]
+    oracle = bo.COCOevalBoundaryOracle(gts, dts)
+    t0 = time.perf_counter()
+    oracle.evaluate()
+    host_ms = (time.perf_counter() - t0) * 1e3
+    print(json.dumps({
+        "workload": f"COCOeval boundary: {n_batches} batches of configs[1] 32 x 1024x1024, "
+                    "100 predictions vs 100 jittered gt (~10 % crowd), default params, "
+                    "dilation_ratio 0.02 (d = 29)",
+        "boundary_stats_0_AP": round(float(ev.stats[0]), 4),
+        "segm_stats_0_AP": round(float(together[0].stats[0]), 4),
+        "pred_boundary_kernel_ms": round(pred_ms, 4),
+        "gt_boundary_kernel_ms": round(gt_ms, 4),
+        "gt_planes_MB": round(gt_bytes / 1e6, 1),
+        "gt_boundary_read_plus_write_GBps": round(2 * gt_bytes / gt_ms / 1e6, 1),
+        "boundary_ious_kernel_ms": round(iou_ms, 4),
+        "boundary_add_batch_ms_per_batch": [round(t, 1) for t in per_batch],
+        "segm_bbox_boundary_one_unmold_ms_per_batch": [round(t, 1) for t in both],
+        "segm_bbox_boundary_three_add_batch_ms_per_batch": [round(t, 1) for t in apart],
+        "host_oracle_boundary_evaluate_ms_per_image": round(host_ms, 1),
+        "note": "add_batch: H2D of the configs[1] inputs, unmold, packed expand, gt decode from "
+                "compressed strings, both boundary launches and their extents, ranks, boundary "
+                "IoUs, match, one download", **card()}), flush=True)
+    del eng, d_det, d_msk, gt, res, d_iou
     torch.cuda.empty_cache()
 
 
@@ -730,6 +870,8 @@ def main():
     ap.add_argument("--only-eval", action="store_true", help="only the mask IoU / AP record")
     ap.add_argument("--only-cocoeval", action="store_true", help="only the COCO mask AP record")
     ap.add_argument("--only-bboxeval", action="store_true", help="only the COCO box AP record")
+    ap.add_argument("--only-boundaryeval", action="store_true", help="only the Boundary AP "
+                    "record")
     ap.add_argument("--only-polygons", action="store_true", help="only the polygon ground truth "
                     "record")
     args = ap.parse_args()
@@ -739,6 +881,9 @@ def main():
         return
     if args.only_bboxeval:
         bboxeval_case(args.iters)
+        return
+    if args.only_boundaryeval:
+        boundaryeval_case(args.iters)
         return
     if args.only_polygons:
         polygons_case(args.iters)
