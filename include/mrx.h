@@ -24,6 +24,7 @@
  *   mrx_coco_ranks / _ious / _box_ious / _match[_f64area] (extension: pycocotools' COCOeval for
  *                             "segm" and "bbox", the per-image half)
  *   mrx_mask_boundary / mrx_coco_boundary_ious (extension: the same for "boundary", Boundary AP)
+ *   mrx_lvis_ranks         (extension: lvis-api's LVISEval, the per-image cut and federated filter)
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
  *   mrx_device_alloc/_free (the canvas allocation: compressible device memory where offered)
  *
@@ -46,7 +47,7 @@
 extern "C" {
 #endif
 
-#define MRX_ABI_VERSION 15
+#define MRX_ABI_VERSION 16
 
 #define MRX_OK              0
 #define MRX_E_INVALID      -1   /* bad argument (null pointer, size out of range) */
@@ -437,6 +438,25 @@ int mrx_mask_matches(const float *d_overlaps, const int *d_pred_counts,
 int mrx_coco_ranks(const int *d_class_ids, const void *d_scores, int score_dtype,
                    const int *d_counts, const int *d_class_map, int C, int max_det, int *d_cat,
                    int *d_rank, unsigned char *d_keep, int *d_walk, int B, int R, void *stream);
+
+/* mrx_lvis_ranks: the rank step of lvis-api's LVISEval (LVISResults.limit_dets_per_image and the
+ *   federated filter of LVISEval._prepare); the IoUs and matches that follow are
+ *   mrx_coco_[box_]ious and mrx_coco_match[_f64area] with all-zero crowd flags.  Arguments as for
+ *   mrx_coco_ranks, plus d_status [B,K] uint8: bit MRX_LVIS_POSITIVE when image b has ground truth
+ *   of dense category k, MRX_LVIS_NEGATIVE when k is in its neg_category_ids (and
+ *   MRX_LVIS_NOT_EXHAUSTIVE, for the host, when k is in its not_exhaustive_category_ids; not read
+ *   here).  d_cat, d_rank and d_walk are mrx_coco_ranks's; d_keep [B,R] uint8 is d_cat in
+ *   [0, K), the walk position (the number of the image's predictions before it, whatever their
+ *   category) below max_det, and d_status[b][d_cat] & MRX_LVIS_EVALUATED.  Checks: those of
+ *   mrx_coco_ranks, and K below 1: MRX_E_INVALID. */
+#define MRX_LVIS_POSITIVE 1
+#define MRX_LVIS_NEGATIVE 2
+#define MRX_LVIS_EVALUATED 3
+#define MRX_LVIS_NOT_EXHAUSTIVE 4
+int mrx_lvis_ranks(const int *d_class_ids, const void *d_scores, int score_dtype,
+                   const int *d_counts, const int *d_class_map, int C, const unsigned char *d_status,
+                   int K, int max_det, int *d_cat, int *d_rank, unsigned char *d_keep, int *d_walk,
+                   int B, int R, void *stream);
 int mrx_coco_ious(const unsigned char *d_packed1, const long long *d_packed_off1,
                   const int *d_counts1, const long long *d_areas1, const int *d_extents1,
                   const int *d_pred_cat, const unsigned char *d_pred_keep, int R1,

@@ -26,7 +26,7 @@ MRX_GEOM_INTS = 8
 MRX_MAX_BATCH = 4096
 MRX_MAX_MASK_DIM = 64
 MRX_MAX_LANE_MASK_W = 30    # tile width of the lane kernels: mw + 2 lanes per warp
-ABI_VERSION = 15
+ABI_VERSION = 16
 MRX_SCHED_WORDS = 4
 MRX_PEER_HANDLE_BYTES = 64
 MRX_MAX_CONTOUR_SEGMENTS = 1 << 30
@@ -34,6 +34,10 @@ MRX_MAX_IOU_THRESHOLDS = 64
 MRX_MAX_AREA_RANGES = 16
 MRX_BOX_YXYX_I32 = 0
 MRX_BOX_XYWH_F64 = 1
+MRX_LVIS_POSITIVE = 1
+MRX_LVIS_NEGATIVE = 2
+MRX_LVIS_EVALUATED = 3
+MRX_LVIS_NOT_EXHAUSTIVE = 4
 MRX_RLE_ST_CHAR = 1
 MRX_RLE_ST_TRUNC = 2
 MRX_RLE_ST_RANGE = 4
@@ -86,6 +90,8 @@ SIGNATURES = {
     "mrx_mask_matches": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _dp, _i, C.c_double, _vp, _vp,
                               _vp, _i, _i, _i, _vp]),
     "mrx_coco_ranks": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp]),
+    "mrx_lvis_ranks": (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i,
+                            _vp]),
     "mrx_coco_ious": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                            _i, _vp, _vp, _i, _vp]),
     "mrx_coco_match": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _dp, _i, _dp, _i, _vp,

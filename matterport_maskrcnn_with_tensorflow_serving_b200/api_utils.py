@@ -462,18 +462,21 @@ def unmold_compute_ap_batch(items, gts, iou_thresholds=(0.5,), score_threshold=0
 
 def unmold_coco_eval_batch(items, image_ids, gt_anns, evaluator, category_ids=None):
     """`unmold_detections` scored as pycocotools' COCOeval scores segm, bbox or boundary results,
-    without the masks leaving the device: adds the batch to `evaluator` (an
-    `evaluate.COCOevalSegm`, `evaluate.COCOevalBbox` or `evaluate.COCOevalBoundary`), whose
-    `accumulate()` and `summarize()` give COCO mask, box or Boundary AP once every batch is in.  items as for `unmold_detections_batch`; image_ids, one per item;
-    gt_anns[b], image b's COCO annotation dicts; category_ids as for `unmold_coco_results_batch`.
+    or as lvis-api's LVISEval scores segm or bbox results, without the masks leaving the device:
+    adds the batch to `evaluator` (an `evaluate.COCOevalSegm`, `evaluate.COCOevalBbox`,
+    `evaluate.COCOevalBoundary`, `evaluate.LVISEvalSegm` or `evaluate.LVISEvalBbox`), whose
+    `accumulate()` and `summarize()` give COCO mask, box or Boundary AP, or LVIS mask or box AP,
+    once every batch is in.  items as for `unmold_detections_batch`; image_ids, one per item;
+    gt_anns[b], image b's annotation dicts; category_ids as for `unmold_coco_results_batch`.
     Equivalent to `evaluator.add_results(unmold_coco_results_batch(items, image_ids,
     category_ids), gt_anns, image_ids)`, but the predicted masks go straight to packed planes and
     are never encoded, and bbox evaluation expands no mask at all.
 
     `evaluator` may also be a list of evaluators, e.g. `[COCOevalSegm(), COCOevalBbox(),
-    COCOevalBoundary()]` for mask AP, box AP and Boundary AP from one unmold: the items are staged
-    and the prepare step runs once, the packed expand once when a segm or boundary evaluator is
-    among them, and each evaluator gets the records
+    COCOevalBoundary()]` for mask AP, box AP and Boundary AP from one unmold, or
+    `[COCOevalSegm(), LVISEvalSegm(categories, images)]` for COCO and LVIS mask AP on the same
+    annotations: the items are staged and the prepare step runs once, the packed expand once when
+    a segm, boundary or LVIS segm evaluator is among them, and each evaluator gets the records
     its own `add_batch` would give it.  Every evaluator checks the batch before anything runs."""
     evaluators = list(evaluator) if isinstance(evaluator, (list, tuple)) else [evaluator]
     if len({id(e) for e in evaluators}) != len(evaluators):

@@ -9,6 +9,11 @@
 //                      order (descending, ties smaller index first, NaN last), whether that rank
 //                      is below maxDets[-1], and the image's walk order (the same order across
 //                      categories), by counting
+//   lvis_rank_kernel   the same counting loop (rank_image, one template over the keep rule) for
+//                      lvis-api's LVISEval: cat, rank and walk as above, but kept is whether the
+//                      walk position is below max_dets (LVISResults' per-image cut over every
+//                      result) and the category is positive or negative for the image (the
+//                      federated filter of LVISEval._prepare, a [B, K] status table)
 //   coco_iou_kernel    CTA per (image, prediction), warp per ground-truth instance: the pair walk
 //                      of mask_overlaps_kernel (walk_pairs, planes.cuh) over the pairs of one
 //                      category whose prediction is kept; a pair whose extents do not meet gets 0
@@ -60,7 +65,30 @@ __device__ __forceinline__ bool before(double sk, int k, double si, int i) {
   return k < i;
 }
 
-__global__ void __launch_bounds__(256) coco_rank_kernel(const RankParams p) {
+// COCOeval's maxDets cut: the first maxDets[-1] of each (image, category)
+struct CocoKeep {
+  __device__ __forceinline__ bool operator()(const RankParams &p, int, int ci, int rank,
+                                             int) const {
+    return ci >= 0 && rank < p.max_det;
+  }
+};
+
+// LVISEval's: the first max_dets of the image across every category (walk counts them all,
+// categories that are not evaluated included), then only categories positive or negative for it
+struct LvisKeep {
+  const unsigned char *status;  // [B, K]
+  int K;
+  __device__ __forceinline__ bool operator()(const RankParams &p, int b, int ci, int,
+                                             int walk) const {
+    return ci >= 0 && ci < K && walk < p.max_det &&
+           (status[static_cast<size_t>(b) * K + ci] & MRX_LVIS_EVALUATED);
+  }
+};
+
+// one CTA's image b: every prediction's dense category, then its rank within (image, category)
+// and its walk position by counting the predictions before it
+template <typename Keep>
+__device__ __forceinline__ void rank_image(const RankParams &p, const Keep keep) {
   const int b = blockIdx.x;
   const int N = p.counts[b];
   const size_t base = static_cast<size_t>(b) * p.R;
@@ -80,9 +108,19 @@ __global__ void __launch_bounds__(256) coco_rank_kernel(const RankParams p) {
       rank += bf && p.cat[base + k] == ci;
     }
     p.rank[base + i] = rank;
-    p.keep[base + i] = ci >= 0 && rank < p.max_det;
+    p.keep[base + i] = keep(p, b, ci, rank, walk);
     p.walk[base + walk] = i;
   }
+}
+
+__global__ void __launch_bounds__(256) coco_rank_kernel(const RankParams p) {
+  rank_image(p, CocoKeep{});
+}
+
+__global__ void __launch_bounds__(256) lvis_rank_kernel(const RankParams p,
+                                                        const unsigned char *__restrict__ status,
+                                                        int K) {
+  rank_image(p, LvisKeep{status, K});
 }
 
 // ---------------------------------------------------------------- IoUs
@@ -306,6 +344,31 @@ extern "C" int mrx_coco_ranks(const int *d_class_ids, const void *d_scores, int 
                                max_det};
   cocoeval::coco_rank_kernel<<<B, 256, 0, static_cast<cudaStream_t>(stream)>>>(p);
   MRX_LAUNCH_CHECK("coco_rank_kernel");
+  return MRX_OK;
+}
+
+extern "C" int mrx_lvis_ranks(const int *d_class_ids, const void *d_scores, int score_dtype,
+                              const int *d_counts, const int *d_class_map, int C,
+                              const unsigned char *d_status, int K, int max_det, int *d_cat,
+                              int *d_rank, unsigned char *d_keep, int *d_walk, int B, int R,
+                              void *stream) {
+  const char *fn = "mrx_lvis_ranks";
+  MRX_CHECK_ARG(d_class_ids && d_scores && d_counts && d_class_map && d_status && d_cat && d_rank &&
+                    d_keep && d_walk,
+                "%s: null pointer", fn);
+  MRX_CHECK_ARG(B >= 0 && B <= MRX_MAX_BATCH, "%s: bad B %d (need 0<=B<=%d)", fn, B, MRX_MAX_BATCH);
+  MRX_CHECK_ARG(R >= 1 && R <= 65534, "%s: bad R %d (need 1<=R<=65534)", fn, R);
+  MRX_CHECK_ARG(C >= 1, "%s: bad C %d (need C>=1)", fn, C);
+  MRX_CHECK_ARG(K >= 1, "%s: bad K %d (need K>=1)", fn, K);
+  MRX_CHECK_ARG(max_det >= 1, "%s: bad max_det %d (need max_det>=1)", fn, max_det);
+  MRX_CHECK_ARG(score_dtype == MRX_F32 || score_dtype == MRX_F64, "%s: bad score dtype %d", fn,
+                score_dtype);
+  if (B == 0) return MRX_OK;
+  const cocoeval::RankParams p{d_class_ids, d_scores, d_counts, d_class_map, d_cat, d_rank,
+                               d_keep,      d_walk,   R,        C,           score_dtype == MRX_F64,
+                               max_det};
+  cocoeval::lvis_rank_kernel<<<B, 256, 0, static_cast<cudaStream_t>(stream)>>>(p, d_status, K);
+  MRX_LAUNCH_CHECK("lvis_rank_kernel");
   return MRX_OK;
 }
 

@@ -523,6 +523,27 @@ class UnmoldEngine:
                                        self.d_class_ids[:n], self.d_scores[:n], gt_counts, gt_cat,
                                        gt_boxes, gt_crowd, gt_area, class_map, params, stream)
 
+    def enqueue_lvis_eval(self, gt, gt_area, class_map, status, params, stream=None):
+        """EXTENSION: `lvis_evaluate_batch` (LVISEval "segm") of the planned batch's kept
+        instances against `gt`, as `enqueue_coco_eval` takes them, with the [n, K] status table
+        of the federated filter.  Synchronises once; returns its dict."""
+        pred = self._prediction_planes(gt, "enqueue_lvis_eval", stream)
+        n = self._n_images
+        return lvis_evaluate_batch(self.lib, pred, self.d_class_ids[:n], self.d_scores[:n], gt,
+                                   gt_area, class_map, status, params, stream)
+
+    def enqueue_lvis_box_eval(self, gt_counts, gt_cat, gt_boxes, gt_area, class_map, status,
+                              params, stream=None):
+        """EXTENSION: `lvis_box_evaluate_batch` (LVISEval "bbox") of the planned batch's kept
+        boxes, after `enqueue(..., expand=False)`, as `enqueue_coco_box_eval` takes them (no crowd
+        flags), with the [n, K] status table.  Synchronises once; returns its dict."""
+        n = self._n_images
+        if n == 0:
+            raise RuntimeError("call plan() and enqueue() first")
+        return lvis_box_evaluate_batch(self.lib, self.d_boxes[:n], self.d_counts[:n],
+                                       self.d_class_ids[:n], self.d_scores[:n], gt_counts, gt_cat,
+                                       gt_boxes, gt_area, class_map, status, params, stream)
+
     def enqueue_coco_boundary_eval(self, gt, gt_crowd, gt_area, class_map, params,
                                    dilation_ratio=0.02, stream=None):
         """EXTENSION: `coco_boundary_evaluate_batch` (COCOeval "boundary", Boundary AP) of the
@@ -1130,15 +1151,25 @@ def coco_device_params(params):
     `maxDets`) as the COCO kernels take them: the thresholds capped at 1 - 1e-10 as evaluateImg
     caps them, the area ranges flattened to [A * 2] float64, maxDets[-1].  Raises ValueError
     outside the kernels' limits."""
-    thr = [min(float(t), 1 - 1e-10) for t in np.ravel(params.iouThrs)]
-    rng = np.asarray(params.areaRng, dtype=np.float64).reshape(-1, 2)
-    max_det = int(params.maxDets[-1])
+    return _device_params(params.iouThrs, params.areaRng, params.maxDets[-1], "maxDets[-1]")
+
+
+def lvis_device_params(params):
+    """`coco_device_params` of an LVISEval-style params object (`iou_thrs`, `area_rng`, and
+    `max_dets` one int, the per-image cut)."""
+    return _device_params(params.iou_thrs, params.area_rng, params.max_dets, "max_dets")
+
+
+def _device_params(iou_thrs, area_rng, max_det, max_det_name):
+    thr = [min(float(t), 1 - 1e-10) for t in np.ravel(iou_thrs)]
+    rng = np.asarray(area_rng, dtype=np.float64).reshape(-1, 2)
+    max_det = int(max_det)
     if not 1 <= len(thr) <= N.MRX_MAX_IOU_THRESHOLDS:
         raise ValueError(f"{len(thr)} IoU thresholds (need 1 to {N.MRX_MAX_IOU_THRESHOLDS})")
     if not 1 <= rng.shape[0] <= N.MRX_MAX_AREA_RANGES:
         raise ValueError(f"{rng.shape[0]} area ranges (need 1 to {N.MRX_MAX_AREA_RANGES})")
     if max_det < 1:
-        raise ValueError(f"maxDets[-1] = {max_det} (need >= 1)")
+        raise ValueError(f"{max_det_name} = {max_det} (need >= 1)")
     return thr, rng.reshape(-1).tolist(), max_det
 
 
@@ -1159,13 +1190,35 @@ def coco_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt
     the count), `area` (int64 pixels), `score` (float64); `match` [A, T, n, pred.R] int32 (the
     ground-truth index or -1) and `ignore` [A, T, n, pred.R] bool, defined where `keep` is; and
     `d_iou`, the float64 device tensor [n, pred.R, gt.R] of mrx_coco_ious."""
+    return _segm_evaluate(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt_area, class_map,
+                          coco_device_params(params), None, stream)
+
+
+def lvis_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_area, class_map, status,
+                        params, stream=None):
+    """The per-image half of lvis-api's LVISEval (iouType "segm") for one batch: mrx_lvis_ranks
+    (the per-image cut at `params.max_dets` and the federated filter), then mrx_coco_ious and
+    mrx_coco_match with every ground-truth instance non-crowd, one download and one
+    synchronisation.  status [n, K] uint8 host array: MRX_LVIS_* bits of (image, dense category),
+    uploaded in the one copy of the ground-truth tables; class_map's categories must be < K (one
+    at or above K is not evaluated).  params: `iou_thrs`, `area_rng`, `max_dets`
+    (`lvis_device_params`).  Other arguments and the result as for `coco_evaluate_batch`, whose
+    `keep` is mrx_lvis_ranks' here and whose `ignore` does not yet hold the not-exhaustive rule
+    (the caller's)."""
+    return _segm_evaluate(lib, pred, pred_class_ids, pred_scores, gt,
+                          np.zeros((gt.n, int(gt.R)), np.uint8), gt_area, class_map,
+                          lvis_device_params(params), status, stream)
+
+
+def _segm_evaluate(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt_area, class_map,
+                   dparams, status, stream):
     n, R1, R2 = gt.n, int(pred.R), int(gt.R)
     class_map = _coco_class_map(class_map)
     with _stream_ctx(stream):
-        d_crowd, d_area, d_map = _upload_parts(
+        d_crowd, d_area, d_map, *d_status = _upload_parts(
             [np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
-             np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map],
-            gt.d_geom.device)
+             np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map]
+            + _status_part(status, n), gt.d_geom.device)
 
         def ious(v, d_iou, st):
             v["area"].copy_(pred.d_areas.view(-1)[:n * R1].view(n, R1))
@@ -1177,8 +1230,18 @@ def coco_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt
                 _ptr(d_crowd), R2, _ptr(gt.d_geom), _ptr(d_iou), n, st), "mrx_coco_ious")
 
         return _coco_evaluate(lib, n, R1, R2, pred.d_counts, pred_class_ids, pred_scores,
-                              gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map, params,
-                              np.int64, ious, stream)
+                              gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map, dparams,
+                              np.int64, ious, stream, *d_status)
+
+
+def _status_part(status, n):
+    """[status as a C-contiguous uint8 [n, K] array] for the one upload, or [] without one."""
+    if status is None:
+        return []
+    status = np.ascontiguousarray(status, dtype=np.uint8)
+    if status.ndim != 2 or status.shape[0] != n or status.shape[1] < 1:
+        raise ValueError(f"status must be [{n}, K >= 1], got {status.shape}")
+    return [status]
 
 
 def coco_box_evaluate_batch(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts,
@@ -1197,6 +1260,25 @@ def coco_box_evaluate_batch(lib, pred_boxes, pred_counts, pred_class_ids, pred_s
 
     Returns `coco_evaluate_batch`'s dict, with `area` float64 (each kept prediction's w*h, as
     loadRes stores it for a bbox result) and `d_iou` from mrx_coco_box_ious."""
+    return _box_evaluate(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts,
+                         gt_cat, gt_boxes, gt_crowd, gt_area, class_map, coco_device_params(params),
+                         None, stream)
+
+
+def lvis_box_evaluate_batch(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts,
+                            gt_cat, gt_boxes, gt_area, class_map, status, params, stream=None):
+    """The per-image half of lvis-api's LVISEval (iouType "bbox") for one batch: mrx_lvis_ranks,
+    mrx_coco_box_ious and mrx_coco_match_f64area with every ground-truth box non-crowd, one
+    download and one synchronisation.  Arguments as for `coco_box_evaluate_batch` (without
+    gt_crowd), status and params as for `lvis_evaluate_batch`."""
+    gt_cat = np.ascontiguousarray(gt_cat, dtype=np.int32)
+    return _box_evaluate(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts,
+                         gt_cat, gt_boxes, np.zeros(gt_cat.shape, np.uint8), gt_area, class_map,
+                         lvis_device_params(params), status, stream)
+
+
+def _box_evaluate(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts, gt_cat,
+                  gt_boxes, gt_crowd, gt_area, class_map, dparams, status, stream):
     torch = _torch()
     gt_cat = np.ascontiguousarray(gt_cat, dtype=np.int32)
     n, R2 = gt_cat.shape
@@ -1212,12 +1294,14 @@ def coco_box_evaluate_batch(lib, pred_boxes, pred_counts, pred_class_ids, pred_s
              np.ascontiguousarray(gt_boxes, dtype=np.float64).reshape(n, R2, 4),
              np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
              np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map]
+    parts += _status_part(status, n)
     pred = [pred_boxes, pred_counts, pred_class_ids, pred_scores]
     on_host = [k for k, x in enumerate(pred) if isinstance(x, np.ndarray)]
     with _stream_ctx(stream):
         up = _upload_parts(parts + [np.ascontiguousarray(pred[k]) for k in on_host], dev)
         d_counts, d_cat, d_boxes, d_crowd, d_area, d_map = up[:6]
-        for k, t in zip(on_host, up[6:]):
+        d_status = up[6:len(parts)]
+        for k, t in zip(on_host, up[len(parts):]):
             pred[k] = t
         pred_boxes, pred_counts, pred_class_ids, pred_scores = pred
         form = {torch.int32: N.MRX_BOX_YXYX_I32, torch.float64: N.MRX_BOX_XYWH_F64}[
@@ -1230,7 +1314,8 @@ def coco_box_evaluate_batch(lib, pred_boxes, pred_counts, pred_class_ids, pred_s
                 _ptr(d_iou), n, st), "mrx_coco_box_ious")
 
         return _coco_evaluate(lib, n, R1, R2, pred_counts, pred_class_ids, pred_scores, d_counts,
-                              d_cat, d_crowd, d_area, d_map, params, np.float64, ious, stream)
+                              d_cat, d_crowd, d_area, d_map, dparams, np.float64, ious, stream,
+                              *d_status)
 
 
 def check_dilation_ratio(dilation_ratio):
@@ -1313,8 +1398,8 @@ def coco_boundary_evaluate_batch(lib, pred, pred_regions, pred_class_ids, pred_s
                 _ptr(d_iou), n, st), "mrx_coco_boundary_ious")
 
         return _coco_evaluate(lib, n, R1, R2, pred.d_counts, pred_class_ids, pred_scores,
-                              gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map, params,
-                              np.int64, ious, stream)
+                              gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map,
+                              coco_device_params(params), np.int64, ious, stream)
 
 
 def _coco_class_map(class_map):
@@ -1323,13 +1408,16 @@ def _coco_class_map(class_map):
 
 
 def _coco_evaluate(lib, n, R1, R2, d_pred_counts, pred_class_ids, pred_scores, d_gt_counts,
-                   d_gt_cat, d_crowd, d_area, d_map, params, area_dtype, ious, stream):
-    """What both IoU types share, on the current stream: mrx_coco_ranks, `ious(v, d_iou, st)`
-    (fills d_iou [n, R1, R2] and the predictions' `area` in the output views v), the match kernel
-    for area_dtype (int64 mask pixels or float64 box areas), then the one download of the output
-    buffer and its one synchronisation.  Returns `coco_evaluate_batch`'s dict."""
+                   d_gt_cat, d_crowd, d_area, d_map, dparams, area_dtype, ious, stream,
+                   d_status=None):
+    """What every IoU type shares, on the current stream: the rank step (mrx_coco_ranks, or
+    mrx_lvis_ranks with the [n, K] status table d_status), `ious(v, d_iou, st)` (fills d_iou
+    [n, R1, R2] and the predictions' `area` in the output views v), the match kernel for
+    area_dtype (int64 mask pixels or float64 box areas), then the one download of the output
+    buffer and its one synchronisation.  dparams: (thresholds, area_rng, max_det) of
+    `coco_device_params` / `lvis_device_params`.  Returns `coco_evaluate_batch`'s dict."""
     torch = _torch()
-    thr, rng, max_det = coco_device_params(params)
+    thr, rng, max_det = dparams
     T, A = len(thr), len(rng) // 2
     dev = d_map.device
     score_code = {torch.float32: N.MRX_F32, torch.float64: N.MRX_F64}[pred_scores.dtype]
@@ -1346,10 +1434,16 @@ def _coco_evaluate(lib, n, R1, R2, d_pred_counts, pred_class_ids, pred_scores, d
     d_iou = torch.empty((n, R1, R2), dtype=torch.float64, device=dev)
     v["counts"].copy_(d_pred_counts[:n])
     v["score"].copy_(pred_scores[:n])
-    N.check(lib.mrx_coco_ranks(
-        _ptr(pred_class_ids), _ptr(pred_scores), score_code, _ptr(d_pred_counts), _ptr(d_map),
-        int(d_map.numel()), max_det, _ptr(v["cat"]), _ptr(v["rank"]), _ptr(v["keep"]),
-        _ptr(d_walk), n, R1, st), "mrx_coco_ranks")
+    if d_status is None:
+        N.check(lib.mrx_coco_ranks(
+            _ptr(pred_class_ids), _ptr(pred_scores), score_code, _ptr(d_pred_counts), _ptr(d_map),
+            int(d_map.numel()), max_det, _ptr(v["cat"]), _ptr(v["rank"]), _ptr(v["keep"]),
+            _ptr(d_walk), n, R1, st), "mrx_coco_ranks")
+    else:
+        N.check(lib.mrx_lvis_ranks(
+            _ptr(pred_class_ids), _ptr(pred_scores), score_code, _ptr(d_pred_counts), _ptr(d_map),
+            int(d_map.numel()), _ptr(d_status), int(d_status.shape[1]), max_det, _ptr(v["cat"]),
+            _ptr(v["rank"]), _ptr(v["keep"]), _ptr(d_walk), n, R1, st), "mrx_lvis_ranks")
     ious(v, d_iou, st)
     match = {np.dtype(np.int64): "mrx_coco_match",
              np.dtype(np.float64): "mrx_coco_match_f64area"}[np.dtype(area_dtype)]

@@ -21,16 +21,24 @@ boundary_iou_api's COCOeval for iouType "boundary" (Boundary AP): `COCOevalSegm`
 taken as the smaller of the mask IoU and the boundary IoU, the boundaries made on the device
 (`mrx_mask_boundary`, `mrx_coco_boundary_ious`, DESIGN.md section 3.18).
 
+`LVISEvalSegm` and `LVISEvalBbox` are lvis-api's LVISEval for "segm" and "bbox" (LVIS mask and box
+AP, with APr / APc / APf) as streaming evaluators on the same device steps: `mrx_lvis_ranks` keeps
+the first `max_dets` results of each image and only the categories the image is federated for,
+DESIGN.md section 3.19.
+
 `ann_to_mask` is Matterport's `CocoDataset.annToMask`, rasterised on the device (DESIGN.md
 section 3.16).
 """
 from __future__ import annotations
+
+from collections import OrderedDict
 
 import numpy as np
 
 from . import _native as N
 from .engine import (MaskBatch, check_dilation_ratio, coco_boundary_evaluate_batch,
                      coco_box_evaluate_batch, coco_device_params, coco_evaluate_batch,
+                     lvis_box_evaluate_batch, lvis_device_params, lvis_evaluate_batch,
                      mask_matches, mask_overlaps)
 
 
@@ -177,6 +185,36 @@ class Params:
         self.iouType = iou_type
 
 
+def _curves(score, matched, ignored, npig, rec_thrs):
+    """accumulate's curves of one category from its detections in accumulate's order (score
+    [n], matched and ignored [A, T, n]) and npig [A], its non-ignored ground truth per area range:
+    for every area range a with npig[a] > 0, (a, recall [T] (the last recall, 0 without
+    detections), precision [T, R] and scores [T, R] at rec_thrs).  Cumulative sums of the flags, a
+    running maximum for the precision envelope and searchsorted, bit-equal to pycocotools' and
+    lvis-api's loops."""
+    nd = score.size
+    T, R = matched.shape[1], len(rec_thrs)
+    tp_sum = np.cumsum(matched & ~ignored, axis=2).astype(dtype=float)
+    fp_sum = np.cumsum(~matched & ~ignored, axis=2).astype(dtype=float)
+    eps = np.spacing(1)
+    for a in range(matched.shape[0]):
+        if npig[a] == 0:
+            continue
+        tp, fp = tp_sum[a], fp_sum[a]
+        rc = tp / npig[a]
+        pr = tp / (fp + tp + eps)
+        last = rc[:, -1] if nd else 0
+        pr = np.maximum.accumulate(pr[:, ::-1], axis=1)[:, ::-1]
+        q = np.zeros((T, R))
+        ss = np.zeros((T, R))
+        for t in range(T):
+            inds = np.searchsorted(rc[t], rec_thrs, side="left")
+            hit = inds < nd
+            q[t, hit] = pr[t, inds[hit]]
+            ss[t, hit] = score[inds[hit]]
+        yield a, last, q, ss
+
+
 class _COCOevalBase:
     """What `COCOevalSegm` and `COCOevalBbox` share: the parameters, the category and image maps,
     the per-detection records each batch appends (`_record`), and pycocotools' `evaluate`,
@@ -272,13 +310,19 @@ class _COCOevalBase:
         self._dets.append((first + b, res["cat"][b, i], res["rank"][b, i], res["score"][b, i],
                            res["match"][:, :, b, i].transpose(2, 0, 1) > -1,
                            res["ignore"][:, :, b, i].transpose(2, 0, 1)))
-        rng = np.asarray(self.params.areaRng, np.float64).reshape(-1, 2)
+        rng = np.asarray(self._area_rng(), np.float64).reshape(-1, 2)
         img = np.concatenate([np.full(len(c), first + b, np.int64) for b, c in enumerate(gt_cats)]
                              + [np.zeros(0, np.int64)])
         crowd = np.concatenate(gt_crowd + [np.zeros(0, np.uint8)]).astype(bool)
         area = np.concatenate(gt_area + [np.zeros(0)])
         nonig = ~crowd[:, None] & (area[:, None] >= rng[:, 0]) & (area[:, None] <= rng[:, 1])
         self._gts.append((img, np.concatenate(gt_cats + [np.zeros(0, np.int32)]), nonig))
+        self._sync_params()
+
+    def _area_rng(self):
+        return self.params.areaRng
+
+    def _sync_params(self):
         p = self.params
         p.imgIds = sorted(self._img_index)
         if self._auto_cats:
@@ -304,12 +348,29 @@ class _COCOevalBase:
         precision = -np.ones((T, R, K, A, M))
         recall = -np.ones((T, K, A, M))
         scores = -np.ones((T, R, K, A, M))
-        n_img = len(self._img_index)
-        img_rank = np.full(n_img + 1, -1, np.int64)       # add position -> imgIds position
+        for k, npig, rank, score, matched, ignored in self._by_category(img_ids, cat_ids, A, T):
+            for m, max_det in enumerate(p.maxDets):
+                cut = rank < max_det
+                for a, rc, q, ss in _curves(score[cut], matched[:, :, cut], ignored[:, :, cut],
+                                            npig, p.recThrs):
+                    recall[:, k, a, m] = rc
+                    precision[:, :, k, a, m] = q
+                    scores[:, :, k, a, m] = ss
+        self.eval = {"params": p, "counts": [T, R, K, A, M], "precision": precision,
+                     "recall": recall, "scores": scores}
+
+    def _by_category(self, img_ids, cat_ids, A, T):
+        """The records of the images of img_ids and the categories of cat_ids, per category
+        position k that has non-ignored ground truth in some area range: (k, npig [A], the
+        number of non-ignored instances per range, and its detections' rank, score, matched and
+        ignored [A, T, n] in accumulate's order: one lexsort by (-score, image position in img_ids,
+        rank within (image, category)))."""
+        K = len(cat_ids)
+        img_rank = np.full(len(self._img_index) + 1, -1, np.int64)   # add position -> img_ids
         for r, i in enumerate(img_ids):
             if i in self._img_index:
                 img_rank[self._img_index[i]] = r
-        cat_k = np.full(len(self._cat_index) + 1, -1, np.int64)   # dense -> catIds position
+        cat_k = np.full(len(self._cat_index) + 1, -1, np.int64)   # dense -> cat_ids position
         for k, c in enumerate(cat_ids):
             if int(c) in self._cat_index:
                 cat_k[self._cat_index[int(c)]] = k
@@ -334,41 +395,13 @@ class _COCOevalBase:
                                                                    d_tp, d_ig))
         by_k = np.argsort(d_k, kind="stable")
         bounds = np.searchsorted(d_k[by_k], np.arange(K + 1))
-        eps = np.spacing(1)
         for k in range(K):
             if not (npig[k] > 0).any():
                 continue
             sel = by_k[bounds[k]:bounds[k + 1]]
             order = sel[np.lexsort((d_rank[sel], d_img[sel], -d_score[sel]))]
-            rank, score = d_rank[order], d_score[order]
-            matched = d_tp[order].transpose(1, 2, 0)        # [A, T, n]
-            ignored = d_ig[order].transpose(1, 2, 0)
-            for m, max_det in enumerate(p.maxDets):
-                cut = rank < max_det
-                s = score[cut]
-                nd = s.size
-                dtm, dtig = matched[:, :, cut], ignored[:, :, cut]
-                tp_sum = np.cumsum(dtm & ~dtig, axis=2).astype(dtype=float)
-                fp_sum = np.cumsum(~dtm & ~dtig, axis=2).astype(dtype=float)
-                for a in range(A):
-                    if npig[k, a] == 0:
-                        continue
-                    tp, fp = tp_sum[a], fp_sum[a]
-                    rc = tp / npig[k, a]
-                    pr = tp / (fp + tp + eps)
-                    recall[:, k, a, m] = rc[:, -1] if nd else 0
-                    pr = np.maximum.accumulate(pr[:, ::-1], axis=1)[:, ::-1]
-                    for t in range(T):
-                        inds = np.searchsorted(rc[t], p.recThrs, side="left")
-                        q = np.zeros(R)
-                        ss = np.zeros(R)
-                        hit = inds < nd
-                        q[hit] = pr[t, inds[hit]]
-                        ss[hit] = s[inds[hit]]
-                        precision[t, :, k, a, m] = q
-                        scores[t, :, k, a, m] = ss
-        self.eval = {"params": p, "counts": [T, R, K, A, M], "precision": precision,
-                     "recall": recall, "scores": scores}
+            yield (k, npig[k], d_rank[order], d_score[order], d_tp[order].transpose(1, 2, 0),
+                   d_ig[order].transpose(1, 2, 0))
 
     def summarize(self):
         """pycocotools' twelve `stats` (each the mean of the entries > -1, or -1 if none), printed
@@ -733,13 +766,333 @@ class COCOevalBbox(_COCOevalBase):
         pred_cls = self._padded([[self._dense(r["category_id"]) for _, r in d] for d in dets], R1,
                                 np.int32)
         scores = self._padded([[float(r["score"]) for _, r in d] for d in dets], R1, np.float64)
-        res = coco_box_evaluate_batch(N.load(), pred_boxes,
-                                      np.asarray([len(d) for d in dets], np.int32), pred_cls,
-                                      scores, *self._gt_arrays(tables),
-                                      np.arange(max(len(self._cat_index), 1), dtype=np.int32),
-                                      self.params)
+        res = self._evaluate_boxes(pred_boxes, np.asarray([len(d) for d in dets], np.int32),
+                                   pred_cls, scores, *self._gt_arrays(tables),
+                                   np.arange(max(len(self._cat_index), 1), dtype=np.int32))
         cats, crowd, area, _ = tables
         self._record(image_ids, res, cats, crowd, area)
+
+    def _evaluate_boxes(self, *arrays):
+        """`coco_box_evaluate_batch` of `add_results`' host arrays."""
+        return coco_box_evaluate_batch(N.load(), *arrays, self.params)
+
+
+# ----------------------------------------------------------------------------- LVIS mask and box AP
+class LVISParams:
+    """LVISEval's parameters (lvis-api's `Params`, snake_case names and defaults): `iou_thrs`,
+    `rec_thrs`, `area_rng` and `area_rng_lbl` as pycocotools', `max_dets` one int (300, the
+    per-image cut of LVISResults), `img_count_lbl` ["r", "c", "f"], `use_cats` 1 (the only one
+    supported).  `cat_ids` is the sorted ids of every category of the dataset unless given;
+    `img_ids` is the sorted ids of the images added so far (either may be set to a subset before
+    `accumulate`)."""
+
+    def __init__(self, cat_ids, iou_thrs=None, rec_thrs=None, max_dets=300, area_rng=None,
+                 area_rng_lbl=None, img_count_lbl=None, iou_type="segm"):
+        coco = Params(cat_ids, iou_thrs, rec_thrs, (1,), area_rng, area_rng_lbl, iou_type)
+        self.img_ids = []
+        self.cat_ids = coco.catIds
+        self.iou_thrs = coco.iouThrs
+        self.rec_thrs = coco.recThrs
+        self.max_dets = int(max_dets)
+        self.area_rng = coco.areaRng
+        self.area_rng_lbl = coco.areaRngLbl
+        self.use_cats = 1
+        self.img_count_lbl = ["r", "c", "f"] if img_count_lbl is None else list(img_count_lbl)
+        self.iou_type = iou_type
+
+
+_LVIS_IMAGE_KEYS = ("id", "height", "width", "neg_category_ids", "not_exhaustive_category_ids")
+
+
+class _LVISeval:
+    """What `LVISEvalSegm` and `LVISEvalBbox` add to the COCO evaluator of their IoU type (the
+    class that follows this one in their bases): lvis-api's parameters, the per-batch status table
+    of the federated filter, the not-exhaustive rule on the downloaded flags, and LVISEval's
+    `accumulate`, `summarize` and `print_results` over the same records."""
+
+    def __init__(self, categories, images, cat_ids=None, iou_thrs=None, rec_thrs=None,
+                 max_dets=300, area_rng=None, area_rng_lbl=None, img_count_lbl=None):
+        self._freq = {}
+        for k, c in enumerate(categories):
+            if not isinstance(c, dict) or "id" not in c or "frequency" not in c:
+                raise ValueError(f"category {k}: needs 'id' and 'frequency'")
+            self._freq[int(c["id"])] = c["frequency"]
+        self.params = LVISParams(sorted(self._freq) if cat_ids is None else cat_ids, iou_thrs,
+                                 rec_thrs, max_dets, area_rng, area_rng_lbl, img_count_lbl,
+                                 self._iou_type)
+        for c, f in self._freq.items():
+            if f not in self.params.img_count_lbl:
+                raise ValueError(f"category {c}: frequency {f!r} is not one of "
+                                 f"{self.params.img_count_lbl}")
+        unknown = [c for c in self.params.cat_ids if c not in self._freq]
+        if unknown:
+            raise ValueError(f"cat_ids {unknown[:5]} are not categories of the dataset")
+        if not self.params.cat_ids:
+            raise ValueError("no categories to evaluate")
+        self._device_params = lvis_device_params(self.params)
+        self._images = {}
+        for k, im in enumerate(images):
+            missing = [key for key in _LVIS_IMAGE_KEYS
+                       if not isinstance(im, dict) or key not in im]
+            if missing:
+                name = im.get("id", k) if isinstance(im, dict) else k
+                raise ValueError(f"image {name!r}: no {missing}")
+            self._images[im["id"]] = im
+        # the dense category index is the position in the constructor's cat_ids, fixed for good
+        self._cat_index = {c: k for k, c in enumerate(self.params.cat_ids)}
+        self._auto_cats = False
+        self._frozen = None
+        self._gt_cats = set()
+        self._img_index = {}
+        self._dets = []
+        self._gts = []
+        self._polygons = True
+        self._status = None
+        self.eval = {}
+        self.results = {}
+
+    def _dense(self, cat_id):
+        """The dense index of a category, -1 for one outside the constructor's cat_ids (its
+        ground truth is not read and its detections are not evaluated, as in lvis-api)."""
+        return self._cat_index.get(int(cat_id), -1)
+
+    def _freeze(self):
+        p = self.params
+        key = (tuple(np.ravel(p.iou_thrs).tolist()), tuple(np.ravel(p.area_rng).tolist()),
+               int(p.max_dets))
+        if self._frozen is None:
+            self._device_params = lvis_device_params(p)
+            self._frozen = key
+        elif key != self._frozen:
+            raise ValueError("iou_thrs, area_rng and max_dets changed after the first batch")
+
+    def _new_images(self, image_ids, n_items, gt_anns, what):
+        for i in image_ids:
+            if i not in self._images:
+                raise ValueError(f"image {i!r} is not one of the dataset's images")
+        super()._new_images(image_ids, n_items, gt_anns, what)
+
+    def _gt_tables(self, image_ids, gt_anns, shapes=None):
+        """The COCO evaluator's tables with every instance non-crowd (LVISEval's compute_iou
+        passes iscrowd = 0), after the LVIS checks; leaves the batch's status table in
+        `_status` for the IoU step that follows."""
+        for image_id, anns, hw in zip(image_ids, gt_anns,
+                                      shapes if shapes is not None else [None] * len(image_ids)):
+            im = self._images[image_id]
+            if hw is not None and tuple(hw) != (int(im["height"]), int(im["width"])):
+                raise ValueError(f"image {image_id!r}: shape {tuple(hw)} is not its height and "
+                                 f"width {(im['height'], im['width'])}")
+            for k, ann in enumerate(anns):
+                if isinstance(ann, dict) and ann.get("ignore"):
+                    raise ValueError(f"{self._where(image_id, k, ann)}: 'ignore' annotations are "
+                                     "not supported")
+        cats, crowd, area, segs = super()._gt_tables(image_ids, gt_anns, shapes)
+        crowd = [np.zeros_like(c) for c in crowd]
+        self._status = self.status_table(image_ids, cats)
+        return cats, crowd, area, segs
+
+    def status_table(self, image_ids, gt_cats):
+        """uint8 [n, K]: per image and dense category the MRX_LVIS_* bits, POSITIVE where
+        gt_cats[b] (dense categories of image b's ground truth) has it, NEGATIVE where it is in
+        the image's neg_category_ids, NOT_EXHAUSTIVE where it is in its
+        not_exhaustive_category_ids."""
+        status = np.zeros((len(image_ids), len(self._cat_index)), np.uint8)
+        for b, (image_id, c) in enumerate(zip(image_ids, gt_cats)):
+            im = self._images[image_id]
+            c = np.asarray(c, np.int64)
+            status[b, c[c >= 0]] |= N.MRX_LVIS_POSITIVE
+            for bit, key in ((N.MRX_LVIS_NEGATIVE, "neg_category_ids"),
+                             (N.MRX_LVIS_NOT_EXHAUSTIVE, "not_exhaustive_category_ids")):
+                k = [self._dense(x) for x in im[key]]
+                status[b, [x for x in k if x >= 0]] |= bit
+        return status
+
+    @staticmethod
+    def not_exhaustive(res, status):
+        """evaluate_img's last rule on a batch's downloaded flags: an unmatched detection of a
+        category in its image's not_exhaustive_category_ids is ignored (a matched one still
+        counts).  Updates res["ignore"] [A, T, n, R] in place where res["keep"] holds (the
+        other entries of the downloaded buffer are not written on the device)."""
+        nel = (status & N.MRX_LVIS_NOT_EXHAUSTIVE) != 0
+        keep = res["keep"]
+        cat = np.where(keep, res["cat"], 0)
+        dt_nel = np.take_along_axis(nel, cat, axis=1) & keep
+        res["ignore"] |= (res["match"] == -1) & dt_nel
+
+    def _record(self, image_ids, res, gt_cats, gt_crowd, gt_area):
+        self.not_exhaustive(res, self.status_table(image_ids, gt_cats))
+        super()._record(image_ids, res, gt_cats, gt_crowd, gt_area)
+
+    def _area_rng(self):
+        return self.params.area_rng
+
+    def _sync_params(self):
+        self.params.img_ids = sorted(self._img_index)
+
+    # ------------------------------------------------------------------ lvis-api's API
+    def accumulate(self):
+        """LVISEval's accumulate over the images of `params.img_ids` and the categories of
+        `params.cat_ids`: pycocotools' per-category curves without a maxDets axis, from the
+        same vectorised core as the COCO evaluators.  `eval` holds `params`, `counts` [T, R, K,
+        A], `precision` [T, R, K, A] and `recall` [T, K, A] (float64, -1 where undefined)."""
+        self._freeze()
+        p = self.params
+        img_ids = list(np.unique(p.img_ids)) if len(p.img_ids) else []
+        cat_ids = [int(c) for c in p.cat_ids]
+        unknown = [c for c in cat_ids if c not in self._cat_index]
+        if unknown or len(set(cat_ids)) != len(cat_ids):
+            raise ValueError("params.cat_ids must be distinct ids of the constructor's cat_ids")
+        T, R, K, A = len(p.iou_thrs), len(p.rec_thrs), len(cat_ids), len(p.area_rng)
+        precision = -np.ones((T, R, K, A))
+        recall = -np.ones((T, K, A))
+        for k, npig, _, score, matched, ignored in self._by_category(img_ids, cat_ids, A, T):
+            for a, rc, q, _ in _curves(score, matched, ignored, npig, p.rec_thrs):
+                recall[:, k, a] = rc
+                precision[:, :, k, a] = q
+        self.eval = {"params": p, "counts": [T, R, K, A], "precision": precision,
+                     "recall": recall}
+
+    def _summarize(self, summary_type, iou_thr=None, area_rng="all", freq_group_idx=None):
+        p = self.params
+        aidx = [i for i, lbl in enumerate(p.area_rng_lbl) if lbl == area_rng]
+        s = self.eval["precision"] if summary_type == "ap" else self.eval["recall"]
+        if iou_thr is not None:
+            s = s[np.where(iou_thr == p.iou_thrs)[0]]
+        if summary_type == "ap":
+            if freq_group_idx is not None:
+                group = [k for k, c in enumerate(p.cat_ids)
+                         if self._freq[int(c)] == p.img_count_lbl[freq_group_idx]]
+                s = s[:, :, group, aidx]
+            else:
+                s = s[:, :, :, aidx]
+        else:
+            s = s[:, :, aidx]
+        return -1 if len(s[s > -1]) == 0 else np.mean(s[s > -1])
+
+    def summarize(self):
+        """LVISEval's `results`: AP, AP50, AP75, APs, APm, APl, APr, APc, APf (the mean over the
+        categories of each frequency group), AR@max_dets and ARs / ARm / ARl@max_dets, each the
+        mean of the entries > -1 or -1 when there are none."""
+        if not self.eval:
+            raise RuntimeError("Please run accumulate() first.")
+        md = self.params.max_dets
+        r = self.results = OrderedDict()
+        r["AP"] = self._summarize("ap")
+        r["AP50"] = self._summarize("ap", iou_thr=0.50)
+        r["AP75"] = self._summarize("ap", iou_thr=0.75)
+        r["APs"] = self._summarize("ap", area_rng="small")
+        r["APm"] = self._summarize("ap", area_rng="medium")
+        r["APl"] = self._summarize("ap", area_rng="large")
+        r["APr"] = self._summarize("ap", freq_group_idx=0)
+        r["APc"] = self._summarize("ap", freq_group_idx=1)
+        r["APf"] = self._summarize("ap", freq_group_idx=2)
+        r[f"AR@{md}"] = self._summarize("ar")
+        for rng in ("small", "medium", "large"):
+            r[f"AR{rng[0]}@{md}"] = self._summarize("ar", area_rng=rng)
+
+    def print_results(self):
+        """`results` in lvis-api's line format."""
+        template = (" {:<18} {} @[ IoU={:<9} | area={:>6s} | maxDets={:>3d} catIds={:>3s}] = "
+                    "{:0.3f}")
+        p = self.params
+        for key, value in self.results.items():
+            title, kind = (("Average Precision", "(AP)") if "AP" in key
+                           else ("Average Recall", "(AR)"))
+            if len(key) > 2 and key[2].isdigit():
+                iou = "{:0.2f}".format(float(key[2:]) / 100)
+            else:
+                iou = "{:0.2f}:{:0.2f}".format(p.iou_thrs[0], p.iou_thrs[-1])
+            group = key[2] if len(key) > 2 and key[2] in ["r", "c", "f"] else "all"
+            area = key[2] if len(key) > 2 and key[2] in ["s", "m", "l"] else "all"
+            print(template.format(title, kind, iou, area, p.max_dets, group, value))
+
+    def get_results(self):
+        return self.results
+
+    def run(self):
+        """evaluate(), accumulate() and summarize(), as LVISEval.run."""
+        self.evaluate()
+        self.accumulate()
+        self.summarize()
+
+
+class LVISEvalSegm(_LVISeval, COCOevalSegm):
+    """lvis-api's `LVISEval(lvis_gt, LVISResults(lvis_gt, results), "segm")` (LVIS mask AP) as a
+    streaming evaluator, with `COCOevalSegm`'s batch API: `add_batch` with model outputs,
+    `add_results` with segm results, then `accumulate()` and `summarize()` (or `run()`) give
+    LVISEval's `eval` arrays and `results`.
+
+    `categories` and `images` are the LVIS dataset's category dicts (`id`, `frequency`) and image
+    dicts (`id`, `height`, `width`, `neg_category_ids`, `not_exhaustive_category_ids`).  Per image,
+    on the device (`mrx_lvis_ranks`, DESIGN.md section 3.19): only the first `max_dets` results by
+    score are kept, counted over every category (LVISResults' cut); of those, a result is
+    evaluated only when its category is in `cat_ids` and the image has ground truth of it or lists
+    it as negative.  Then mask IoUs and matching as `COCOevalSegm`'s, with every instance
+    non-crowd, and no per-(image, category) cut.  An unmatched detection of a category in the
+    image's not_exhaustive_category_ids is ignored.  Ground truth is polygon lists, box lists or
+    RLE dicts (`MaskBatch.from_coco`); its `area` decides its range.
+
+    Stated differences from lvis-api: matches are recorded by position, as in `COCOevalSegm`; a
+    detection's area is its mask's pixel count, where LVISResults stores w*h of the result's
+    `bbox` when results carry one; NaN scores sort last, where Python's `sorted` leaves their
+    order undefined; an annotation with a truthy `ignore` raises ValueError (no LVIS file carries
+    the field); `eval` has no `dt_pointers`.  An image id that is not in `images`, an image dict
+    without one of its keys, a category whose `frequency` is not in `img_count_lbl` and
+    `max_dets` below 1 raise ValueError; `iou_thrs`, `area_rng` and `max_dets` must not change
+    after the first batch."""
+
+    _iou_type = "segm"
+
+    def _engine_ious(self, eng, gt, crowd, area, class_map):
+        return eng.enqueue_lvis_eval(gt, area, class_map, self._status, self.params)
+
+    def _result_ious(self, lib, pred, d_scores, gt, crowd, area, class_map):
+        return lvis_evaluate_batch(lib, pred.planes, pred.d_class_ids, d_scores, gt, area,
+                                   class_map, self._status, self.params)
+
+    def add_batch(self, items, image_ids, gt_anns, category_ids=None):
+        """Evaluate model outputs against LVIS ground truth: items as for
+        `api_utils.unmold_detections_batch`, one image id (of `images`) and one list of
+        annotation dicts per item, `category_ids` as in `unmold_coco_results_batch`.  The kept
+        masks go straight to packed planes, the annotations are rasterised on the device."""
+        from . import api_utils
+
+        api_utils.unmold_coco_eval_batch(items, image_ids, gt_anns, [self], category_ids)
+
+    def add_results(self, results, gt_anns, image_ids):
+        """Evaluate LVIS segm results -- dicts {'image_id', 'category_id', 'score',
+        'segmentation': RLE dict} -- against gt_anns[b], the annotation dicts of image_ids[b].
+        Every result's image must be one of image_ids; image shapes come from `images`."""
+        for i in image_ids:
+            if i not in self._images:
+                raise ValueError(f"image {i!r} is not one of the dataset's images")
+        shapes = [(int(self._images[i]["height"]), int(self._images[i]["width"]))
+                  for i in image_ids]
+        super().add_results(results, gt_anns, image_ids, image_shapes=shapes)
+
+
+class LVISEvalBbox(_LVISeval, COCOevalBbox):
+    """lvis-api's `LVISEval(lvis_gt, LVISResults(lvis_gt, results), "bbox")` (LVIS box AP) as a
+    streaming evaluator: `LVISEvalSegm`'s rules and API on `COCOevalBbox`'s box IoUs (bbIou, no
+    mask), every instance non-crowd; a detection's area is w*h of its box.  Annotations need
+    `category_id`, `bbox` and `area`.  The stated differences are `LVISEvalSegm`'s, except the
+    one on areas."""
+
+    _iou_type = "bbox"
+
+    def _batch_eval(self, eng, tables, category_ids):
+        counts, cat, boxes, _, area = self._gt_arrays(tables)
+        res = eng.enqueue_lvis_box_eval(counts, cat, boxes, area,
+                                        self._class_map(eng.C, category_ids), self._status,
+                                        self.params)
+        cats, crowd, area, _ = tables
+        return res, cats, crowd, area
+
+    def _evaluate_boxes(self, pred_boxes, pred_counts, pred_cls, scores, gt_counts, gt_cat,
+                        gt_boxes, gt_crowd, gt_area, class_map):
+        return lvis_box_evaluate_batch(N.load(), pred_boxes, pred_counts, pred_cls, scores,
+                                       gt_counts, gt_cat, gt_boxes, gt_area, class_map,
+                                       self._status, self.params)
 
 
 def ann_to_mask(ann, height, width):

@@ -5,7 +5,7 @@ each unmold workload also names the GPU and its power limit.
 
   python tools/bench_secondary.py [--iters 20] [--cpu]     (--cpu also times the oracle)
   python tools/bench_secondary.py --only-eval | --only-cocoeval | --only-bboxeval | --only-boundaryeval
-                                  | --only-polygons
+                                  | --only-polygons | --only-lvis
 """
 import argparse
 import ctypes as C
@@ -817,6 +817,152 @@ def polygons_case(iters):
     torch.cuda.empty_cache()
 
 
+def _lvis_dataset(rng, n_img, K=1203):
+    """LVIS-like category dicts (v1's split: 337 rare, 461 common, 405 frequent) and image dicts
+    of n_img 1024x1024 images, each with ~20 negative and ~2 not-exhaustive categories."""
+    freq = np.array(["r"] * 337 + ["c"] * 461 + ["f"] * 405)[rng.permutation(K)]
+    cats = [{"id": k + 1, "frequency": str(freq[k])} for k in range(K)]
+    images = [{"id": i, "height": 1024, "width": 1024,
+               "neg_category_ids": [int(c) for c in rng.choice(K, 20, replace=False) + 1],
+               "not_exhaustive_category_ids": [int(c) for c in rng.choice(K, 2, replace=False) + 1]}
+              for i in range(n_img)]
+    return cats, images
+
+
+def lvis_case(iters, n_batches=4, batch=32, R=300):
+    """LVIS mask AP (LVISEvalSegm) on 32 x 1024x1024 images with 300 predictions each and
+    jittered polygon ground truth (a 4-vertex polygon around every third predicted box, 100 per
+    image, 15 % of them with another category), 1 203 categories, and neg / not-exhaustive lists.
+    The three device kernels alone on one planned batch (mrx_lvis_ranks over K = 1 203 with the
+    predictions' categories spread over all 1 203, mrx_coco_ious, mrx_coco_match),
+    LVISEvalSegm.add_batch end to end per batch, and the host accumulate() + summarize() on
+    synthetic records at LVIS-val scale (20 000 images x 300 detections, 1 203 categories)."""
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import evaluate
+    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import lvis_device_params
+
+    rng = np.random.default_rng(11)
+    K = 1203
+    ims = [synth.make_image(rng, (1024, 1024), R, num_classes=81, max_instances=R)
+           for _ in range(batch)]
+    items = [(im.detections.astype(np.float32), im.mrcnn_mask.astype(np.float32),
+              im.original_image_shape, im.image_shape, im.window) for im in ims]
+    cmap81 = [0] + [int(c) for c in rng.choice(K, 80, replace=False) + 1]   # class -> category
+    lvis_cls = rng.integers(1, K + 1, size=(batch, R)).astype(np.int32)      # for the kernels
+    cats, images = _lvis_dataset(rng, n_batches * batch)
+    segs, cls81, cls_all = [], [], []
+    for b, im in enumerate(ims):
+        det = im.detections
+        s, c1, c2 = [], [], []
+        for k in range(0, im.n_valid, 3):
+            y1, x1, y2, x2 = (det[k, :4] * 1024 + rng.integers(-6, 7, 4)).tolist()
+            s.append([[x1, y1, x2, y1 + 3, x2 - 4, y2, x1 + 2, y2 - 2]])
+            flip = rng.random() < 0.15
+            c1.append(int(rng.integers(1, 81)) if flip else int(det[k, 4]))
+            c2.append(int(rng.integers(1, K + 1)) if flip else int(lvis_cls[b, k]))
+        segs.append(s)
+        cls81.append(c1)
+        cls_all.append(c2)
+    anns = [[{"category_id": cmap81[c], "segmentation": sg, "area": 5000.0, "iscrowd": 0}
+             for c, sg in zip(c1, s)] for c1, s in zip(cls81, segs)]
+
+    per_batch, ev = [], evaluate.LVISEvalSegm(cats, images)
+    for k in range(n_batches):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        ev.add_batch(items, list(range(k * batch, (k + 1) * batch)), anns, category_ids=cmap81)
+        per_batch.append((time.perf_counter() - t0) * 1e3)
+    ev.run()
+
+    # the kernels alone on one planned batch, every category of the 1 203 in play
+    eng = UnmoldEngine(batch, R, (28, 28), 81)
+    eng.plan([make_geom(*it[2:]) for it in items], canvas=False)
+    d_det = torch.from_numpy(np.stack([it[0] for it in items])).cuda()
+    d_msk = torch.from_numpy(np.stack([it[1] for it in items])).cuda()
+    eng.enqueue_packed(d_det, d_msk)
+    gt_dense = [np.asarray(c, np.int32) - 1 for c in cls_all]
+    gt = eng.ground_truth_coco(gt_dense, segs)
+    pred = eng._prediction_planes(gt, "lvis_case", None)
+    status = ev.status_table(list(range(batch)), gt_dense)
+    thr, rngs, max_det = lvis_device_params(ev.params)
+    n, R1, R2, T, A = batch, eng.R, gt.R, len(thr), len(rngs) // 2
+    dev = eng.device
+    P = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+    d_cls = torch.from_numpy(lvis_cls).to(dev)
+    d_map = torch.arange(-1, K, dtype=torch.int32, device=dev)      # category id -> dense
+    d_status = torch.from_numpy(status).to(dev)
+    d_cat = torch.empty((n, R1), dtype=torch.int32, device=dev)
+    d_rank, d_walk = torch.empty_like(d_cat), torch.empty_like(d_cat)
+    d_keep = torch.empty((n, R1), dtype=torch.uint8, device=dev)
+    d_crowd = torch.zeros((n, R2), dtype=torch.uint8, device=dev)
+    d_area = torch.full((n, R2), 5000.0, dtype=torch.float64, device=dev)
+    d_match = torch.empty((A, T, n, R1), dtype=torch.int32, device=dev)
+    d_ign = torch.empty((A, T, n, R1), dtype=torch.uint8, device=dev)
+    d_iou = torch.empty((n, R1, R2), dtype=torch.float64, device=dev)
+    st = N.stream_ptr(None)
+    ranks = lambda: N.check(eng.lib.mrx_lvis_ranks(  # noqa: E731
+        P(d_cls), P(eng.d_scores), N.MRX_F32, P(eng.d_counts), P(d_map), K + 1, P(d_status), K,
+        max_det, P(d_cat), P(d_rank), P(d_keep), P(d_walk), n, R1, st), "mrx_lvis_ranks")
+    ious = lambda: N.check(eng.lib.mrx_coco_ious(  # noqa: E731
+        P(pred.d_packed), P(pred.d_packed_off), P(pred.d_counts), P(pred.d_areas),
+        P(pred.d_extents), P(d_cat), P(d_keep), R1, P(gt.planes.d_packed),
+        P(gt.planes.d_packed_off), P(gt.planes.d_counts), P(gt.planes.d_areas),
+        P(gt.planes.d_extents), P(gt.d_class_ids), P(d_crowd), R2, P(gt.d_geom), P(d_iou), n,
+        st), "mrx_coco_ious")
+    match = lambda: N.check(eng.lib.mrx_coco_match(  # noqa: E731
+        P(d_iou), P(eng.d_counts), P(d_cat), P(d_keep), P(d_walk), P(pred.d_areas),
+        P(gt.planes.d_counts), P(gt.d_class_ids), P(d_crowd), P(d_area), N.double_array(thr), T,
+        N.double_array(rngs), A, P(d_match), P(d_ign), n, R1, R2, st), "mrx_coco_match")
+    ranks()
+    rank_ms, _ = time_ms(ranks, iters)
+    iou_ms, _ = time_ms(ious, iters)
+    match_ms, _ = time_ms(match, iters)
+    kept = int(d_keep.sum().item())
+    cat_h, keep_h = d_cat.cpu().numpy(), d_keep.cpu().numpy().astype(bool)
+    pairs = int(sum(np.sum(cat_h[b][keep_h[b]][:, None] == gt_dense[b][None, :])
+                    for b in range(n)))
+    del eng, d_det, d_msk, gt, pred, d_iou
+    torch.cuda.empty_cache()
+
+    # host accumulate + summarize at LVIS-val scale on synthetic records
+    n_img, D, G, T, A = 20000, 300, 12, 10, 4
+    host = evaluate.LVISEvalSegm(cats, _lvis_dataset(rng, n_img)[1])
+    host._img_index = {i: i for i in range(n_img)}
+    d_img = np.repeat(np.arange(n_img, dtype=np.int64), D)
+    d_cat = rng.integers(0, K, size=n_img * D).astype(np.int32)
+    d_score = np.round(rng.random(n_img * D), 3)
+    order = np.lexsort((-d_score, d_cat, d_img))
+    d_rank = np.empty(n_img * D, np.int32)
+    first = np.r_[True, (d_img[order][1:] != d_img[order][:-1])
+                  | (d_cat[order][1:] != d_cat[order][:-1])]
+    run = np.cumsum(first) - 1
+    start = np.flatnonzero(first)
+    d_rank[order] = np.arange(n_img * D) - start[run]
+    d_tp = rng.random((n_img * D, A, T)) < 0.3
+    d_ig = rng.random((n_img * D, A, T)) < 0.1
+    host._dets = [(d_img, d_cat, d_rank, d_score, d_tp, d_ig)]
+    host._gts = [(np.repeat(np.arange(n_img, dtype=np.int64), G),
+                  rng.integers(0, K, size=n_img * G).astype(np.int32),
+                  rng.random((n_img * G, A)) < 0.8)]
+    host._sync_params()
+    t0 = time.perf_counter()
+    host.accumulate()
+    host.summarize()
+    host_s = time.perf_counter() - t0
+    print(json.dumps({
+        "workload": f"LVISEval segm: {n_batches} batches of 32 x 1024x1024, 300 predictions vs "
+                    "100 jittered polygon gt, 1 203 categories, neg / not-exhaustive lists",
+        "kept_predictions_per_batch_kernels": kept, "pairs_per_batch_kernels": pairs,
+        "lvis_ranks_kernel_ms": round(rank_ms, 4), "ious_kernel_ms": round(iou_ms, 4),
+        "match_kernel_ms_40_area_thresholds": round(match_ms, 4),
+        "add_batch_ms_per_batch": [round(t, 1) for t in per_batch],
+        "AP": round(float(ev.results["AP"]), 4),
+        "host_accumulate_summarize_s_20000_images_x_300": round(host_s, 2),
+        "note": "add_batch: the model's 81 mask classes mapped onto 80 of the 1 203 categories "
+                "(a 1 204-class mask head input would be 1.1 GB per image); H2D of the inputs, "
+                "unmold prepare, packed expand, polygon rasterisation, the three kernels, one "
+                "download", **card()}), flush=True)
+
+
 def anchors_sweep(iters, cpu):
     import oracle
     gen = AnchorGenerator(MaskRCNNServingConfig)
@@ -874,6 +1020,7 @@ def main():
                     "record")
     ap.add_argument("--only-polygons", action="store_true", help="only the polygon ground truth "
                     "record")
+    ap.add_argument("--only-lvis", action="store_true", help="only the LVIS mask AP record")
     args = ap.parse_args()
     torch.cuda.set_device(0)
     if args.only_cocoeval:
@@ -887,6 +1034,9 @@ def main():
         return
     if args.only_polygons:
         polygons_case(args.iters)
+        return
+    if args.only_lvis:
+        lvis_case(args.iters)
         return
     eval_case(args.iters, args.cpu)
     if args.only_eval:
