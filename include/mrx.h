@@ -25,6 +25,8 @@
  *                             "segm" and "bbox", the per-image half)
  *   mrx_mask_boundary / mrx_coco_boundary_ious (extension: the same for "boundary", Boundary AP)
  *   mrx_lvis_ranks         (extension: lvis-api's LVISEval, the per-image cut and federated filter)
+ *   mrx_jpeg_coefficients / _pixels <- api_utils.load_img (cv2.imread)   serve.py:85-86
+ *                             (extension: JPEG request bytes decoded on the device, as cv2.imdecode)
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
  *   mrx_device_alloc/_free (the canvas allocation: compressible device memory where offered)
  *
@@ -47,7 +49,7 @@
 extern "C" {
 #endif
 
-#define MRX_ABI_VERSION 16
+#define MRX_ABI_VERSION 17
 
 #define MRX_OK              0
 #define MRX_E_INVALID      -1   /* bad argument (null pointer, size out of range) */
@@ -598,6 +600,44 @@ int mrx_poly_decode(const int *d_vert, const long long *d_part_vert, const int *
                     unsigned char *d_carry, const int *d_counts, const int *d_geom,
                     const long long *d_packed_off, unsigned char *d_packed, int B, int R,
                     int max_h, int max_w, void *stream);
+
+/* ---------------------------------------------------------------- JPEG decode (load_img) */
+/* Baseline JPEG files decoded bit for bit as cv2.imdecode(buf, IMREAD_COLOR) then BGR2RGB
+ * (libjpeg-turbo: JDCT_ISLOW, fancy upsampling, EXIF orientation; csrc/jpeg.cu).  The host
+ * (jpeg.Plan) parses the headers and lays the batch out: the files at d_files + desc[b][0],
+ * desc [B, 80] int64 words per image (geometry and every buffer offset, jpeg.py's D_* indices),
+ * d_tabs [B, 9312] bytes (per component: quant int32[64] in natural order, DC and AC Huffman
+ * lookups), d_unit_img [U] int32 (the image of each of the batch's U restart units).
+ *
+ * mrx_jpeg_coefficients: unstuffs each scan into d_unst, splits it at RSTn into units, decodes the
+ *   Huffman data by self-synchronisation over subsequences of S bits (scratch in d_work) and
+ *   writes the quantised coefficients, int16 [blocks, 64] in natural order and decode (MCU) order,
+ *   DC after the prediction (JCOEF), into d_coef (zeroed here first; coef_blocks of them) at
+ *   desc's block offsets.  d_status [B] int32 (zeroed here first) gets MRX_JPEG_ST_* bits for
+ *   corrupt entropy-coded data; libjpeg-turbo warns and substitutes zeros instead (a stated
+ *   difference).  max_subs: the largest per-image subsequence count desc plans, which is the S
+ *   desc was planned with.
+ * mrx_jpeg_pixels: the islow IDCT of every block into the component planes (d_planes, at their
+ *   full padded block size), then upsampling, colour conversion and orientation into uint8 RGB
+ *   [H', W', 3] at d_out + d_out_off[b] -- the source slots mrx_cv2_resize_u8c3_batch reads.
+ *   Images whose status word has a bit are not written.  max_blocks, max_pixels: the largest
+ *   per-image block and pixel counts.
+ * Checks: null pointers, B outside [0, MRX_MAX_BATCH], S not a multiple of 32 in [32, 65536],
+ * U below B, a max extent below 1: MRX_E_INVALID.  B = 0 returns MRX_OK without launching
+ * anything. */
+#define MRX_JPEG_ST_CODE   1   /* a bad Huffman code */
+#define MRX_JPEG_ST_TRUNC  2   /* the data ends before the last MCU */
+#define MRX_JPEG_ST_RST    4   /* a missing or out-of-order RSTn */
+#define MRX_JPEG_ST_DC     8   /* a DC value outside int32 */
+#define MRX_JPEG_ST_MARKER 16  /* a marker other than EOI ends the scan (a second scan) */
+int mrx_jpeg_coefficients(const unsigned char *d_files, const long long *d_desc,
+                          const unsigned char *d_tabs, const int *d_unit_img, int B, int U, int S,
+                          int max_subs, unsigned char *d_unst, int *d_work, short *d_coef,
+                          long long coef_blocks, int *d_status, void *stream);
+int mrx_jpeg_pixels(const long long *d_desc, const unsigned char *d_tabs, const short *d_coef,
+                    const int *d_status, int B, int max_blocks, long long max_pixels,
+                    unsigned char *d_planes, unsigned char *d_out, const long long *d_out_off,
+                    void *stream);
 
 /* ---------------------------------------------------------------- multi-GPU gather (8e) */
 /* Peer-memory plumbing for the final gather of the canvases to rank 0 (one process per GPU).

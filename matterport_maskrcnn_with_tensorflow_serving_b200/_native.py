@@ -26,7 +26,7 @@ MRX_GEOM_INTS = 8
 MRX_MAX_BATCH = 4096
 MRX_MAX_MASK_DIM = 64
 MRX_MAX_LANE_MASK_W = 30    # tile width of the lane kernels: mw + 2 lanes per warp
-ABI_VERSION = 16
+ABI_VERSION = 17
 MRX_SCHED_WORDS = 4
 MRX_PEER_HANDLE_BYTES = 64
 MRX_MAX_CONTOUR_SEGMENTS = 1 << 30
@@ -43,6 +43,11 @@ MRX_RLE_ST_TRUNC = 2
 MRX_RLE_ST_RANGE = 4
 MRX_RLE_ST_SUM = 8
 MRX_RLE_ST_SKIP = 16
+MRX_JPEG_ST_CODE = 1
+MRX_JPEG_ST_TRUNC = 2
+MRX_JPEG_ST_RST = 4
+MRX_JPEG_ST_DC = 8
+MRX_JPEG_ST_MARKER = 16
 
 
 def contour_scratch_bytes(total_segments):
@@ -124,6 +129,9 @@ SIGNATURES = {
     "mrx_composite_masks": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_double, _vp, _i, _i,
                                  C.c_longlong, _vp]),
     "mrx_pack_masks": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
+    "mrx_jpeg_coefficients": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp,
+                                   C.c_longlong, _vp, _vp]),
+    "mrx_jpeg_pixels": (_i, [_vp, _vp, _vp, _vp, _i, _i, C.c_longlong, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

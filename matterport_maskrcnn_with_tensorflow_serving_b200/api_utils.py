@@ -38,6 +38,7 @@ from .model_configs import mconfig as _default_config
 
 _state = {"config": _default_config, "anchors": None, "engines": OrderedDict()}
 _state_lock = threading.RLock()
+_jpeg_lock = threading.Lock()
 
 # at most this many cached engines (one per device / R / mask shape / dtypes); the least
 # recently used one is released (its canvas and input buffers freed) when a new one is needed
@@ -63,6 +64,7 @@ def release():
             eng._inputs = None
         _state["engines"].clear()
         _state["anchors"] = None
+        _state.pop("molder", None)
         _pool.clear()
 
 
@@ -74,6 +76,21 @@ def load_img(path):
     if img is None:
         raise FileNotFoundError(path)
     return cv2.cvtColor(img, cv2.COLOR_BGR2RGB)
+
+
+def decode_jpeg_batch(blobs):
+    """JPEG files (bytes, bytearray or memoryview) -> one uint8 [H, W, 3] RGB CUDA tensor each,
+    equal bit for bit to `load_img` of the same file (cv2.imdecode, BGR -> RGB), decoded on the
+    device (csrc/jpeg.cu).  A file the decoder does not accept raises ValueError naming its index
+    and the reason before anything is uploaded; corrupt entropy-coded data raises ValueError after
+    the decode (libjpeg-turbo would warn and substitute zeros)."""
+    from .engine import Molder
+
+    with _jpeg_lock:     # the decoder's buffers are reused; other api_utils calls do not wait
+        m = _state.get("molder")
+        if m is None or m.config is not get_config():
+            m = _state["molder"] = Molder(get_config())
+        return m.decode_jpeg_batch(list(blobs))
 
 
 def get_anchors(image_shape):

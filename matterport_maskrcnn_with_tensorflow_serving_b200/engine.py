@@ -1656,32 +1656,148 @@ class Molder:
         return out, u8, window, scale, padding
 
 
+    # ------------------------------------------------------------------ JPEG (csrc/jpeg.cu)
+    def _jpeg_buffer(self, name, n, dtype):
+        """The decoder's reusable device buffers, grown when a batch needs more."""
+        torch = _torch()
+        bufs = self.__dict__.setdefault("_jpeg_bufs", {})
+        t = bufs.get(name)
+        if t is None or t.numel() < n:
+            t = bufs[name] = torch.empty((max(int(n), 1),), dtype=dtype, device=self.device)
+        return t
+
+    def _jpeg_upload(self, plan):
+        """The batch's one upload: desc, unit -> image table, tables and files in one pinned
+        buffer and one H2D copy.  Returns device views (desc, unit_img, tabs, files)."""
+        torch = _torch()
+        parts = [plan.desc.view(np.uint8).reshape(-1), plan.unit_img.view(np.uint8),
+                 plan.tabs.reshape(-1), plan.files]
+        off = _slot_offsets(np.asarray([p.size for p in parts], dtype=np.int64), 16)
+        total = int(off[-1])
+        if getattr(self, "_h_jpeg", None) is None or self._h_jpeg.numel() < total:
+            self._h_jpeg = torch.empty((total,), dtype=torch.uint8).pin_memory()
+        hs = self._h_jpeg.numpy()
+        for p, o in zip(parts, off[:-1]):
+            hs[int(o):int(o) + p.size] = p
+        d = self._jpeg_buffer("upload", total, torch.uint8)
+        d[:total].copy_(self._h_jpeg[:total], non_blocking=True)
+        views = [d[int(o):int(o) + p.size] for p, o in zip(parts, off[:-1])]
+        return views[0].view(torch.int64), views[1].view(torch.int32), views[2], views[3]
+
+    def jpeg_coefficients(self, plan, stream=None):
+        """Enqueue `mrx_jpeg_coefficients` for a `jpeg.Plan`: returns (d_coef int16 [blocks, 64]
+        in decode order, d_status [B] int32, the device upload).  Nothing is synchronised."""
+        torch = _torch()
+        d_desc, d_unit_img, d_tabs, d_files = up = self._jpeg_upload(plan)
+        d_unst = self._jpeg_buffer("unst", plan.unst_bytes, torch.uint8)
+        d_work = self._jpeg_buffer("work", plan.work_words, torch.int32)
+        d_coef = self._jpeg_buffer("coef", plan.coef_blocks * 64, torch.int16)
+        d_status = self._jpeg_buffer("status", plan.B, torch.int32)
+        N.check(self.lib.mrx_jpeg_coefficients(
+            _ptr(d_files), _ptr(d_desc), _ptr(d_tabs), _ptr(d_unit_img), plan.B,
+            max(plan.units, 1), plan.S, plan.max_subs, _ptr(d_unst), _ptr(d_work), _ptr(d_coef),
+            plan.coef_blocks, _ptr(d_status), N.stream_ptr(stream)), "mrx_jpeg_coefficients")
+        return d_coef[:plan.coef_blocks * 64].view(-1, 64), d_status[:plan.B], up
+
+    def jpeg_decode_into(self, plan, d_out, out_off, stream=None):
+        """Enqueue the decode of every file of `plan` into the uint8 slots d_out + out_off[b]
+        (int64 byte offsets; image b is plan.shapes[b]).  Returns d_status [B] (device); call
+        `jpeg_check` on it once the work that reads the slots has been enqueued."""
+        torch = _torch()
+        d_coef, d_status, (d_desc, _, d_tabs, _) = self.jpeg_coefficients(plan, stream)
+        d_planes = self._jpeg_buffer("planes", plan.plane_bytes, torch.uint8)
+        d_off = torch.from_numpy(np.ascontiguousarray(out_off, dtype=np.int64)).to(
+            self.device, non_blocking=True)
+        N.check(self.lib.mrx_jpeg_pixels(
+            _ptr(d_desc), _ptr(d_tabs), _ptr(d_coef), _ptr(d_status), plan.B, plan.max_blocks,
+            plan.max_pixels, _ptr(d_planes), _ptr(d_out), _ptr(d_off), N.stream_ptr(stream)),
+            "mrx_jpeg_pixels")
+        return d_status
+
+    @staticmethod
+    def jpeg_check(d_status, index=None):
+        """Download the status words (the one synchronisation) and raise ValueError naming the
+        first image whose entropy-coded data was corrupt.  index[b]: the caller's index of b."""
+        from . import jpeg
+
+        st = d_status.cpu().numpy()
+        for b in np.flatnonzero(st):
+            i = int(index[b]) if index is not None else int(b)
+            raise jpeg.JpegError(f"image {i}: corrupt JPEG data ({jpeg.status_reasons(st[b])})")
+
+    def decode_jpeg_batch(self, blobs, S=None, stream=None):
+        """uint8 [H, W, 3] RGB CUDA tensors, one per JPEG file: cv2.imdecode + BGR2RGB bit for
+        bit.  The images share one buffer; equal sizes make them one contiguous [B, H, W, 3]."""
+        from . import jpeg
+
+        torch = _torch()
+        plan = jpeg.Plan(blobs, jpeg.DEFAULT_S if S is None else S)
+        if plan.B == 0:
+            return []
+        sizes = np.asarray([h * w * 3 for h, w, _ in plan.shapes], dtype=np.int64)
+        off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        out = torch.empty((int(off[-1]),), dtype=torch.uint8, device=self.device)
+        self.jpeg_check(self.jpeg_decode_into(plan, out, off[:-1], stream))
+        return [out[int(off[b]):int(off[b + 1])].view(plan.shapes[b]) for b in range(plan.B)]
+
     # ------------------------------------------------------------------ batched (one launch each)
-    def cv2_resize_batch_device(self, images, size_hw, stream=None):
-        """`cv2.resize(img, (S, S))` for a list of uint8 HxWx3 NumPy images of ANY sizes in one
-        launch: one pinned staging buffer, one H2D copy.  Returns uint8 [B, dh, dw, 3] on the
-        device."""
+    def stage_images(self, images, align=16, stream=None):
+        """Every image in its slot of one device buffer: uint8 HxWx3 NumPy images through one
+        pinned staging buffer and one H2D copy, JPEG files (bytes) decoded on the device into
+        their slots.  Returns (d_src, off [B+1] int64 slot offsets, shapes, d_status or None,
+        jidx: the indices of the JPEG items).  Call `jpeg_check(d_status, jidx)` once the work
+        that reads the slots has been enqueued."""
+        from . import jpeg
+
         torch = _torch()
         B = len(images)
-        dh, dw = int(size_hw[0]), int(size_hw[1])
-        sizes = [int(im.shape[0]) * int(im.shape[1]) * 3 for im in images]
-        off = _slot_offsets(np.asarray(sizes, dtype=np.int64), 16)
+        is_jpeg = [isinstance(im, (bytes, bytearray, memoryview)) for im in images]
+        jidx = [b for b in range(B) if is_jpeg[b]]
+        plan = jpeg.Plan([images[b] for b in jidx], index=jidx) if jidx else None
+        shapes = [None] * B
+        for k, b in enumerate(jidx):
+            shapes[b] = plan.shapes[k]
+        for b in range(B):
+            if shapes[b] is None:
+                shapes[b] = tuple(int(v) for v in images[b].shape)
+        sizes = [sh[0] * sh[1] * 3 for sh in shapes]
+        off = _slot_offsets(np.asarray(sizes, dtype=np.int64), align)
         total = int(off[-1])
         if getattr(self, "_h_stage", None) is None or self._h_stage.numel() < total:
             self._h_stage = torch.empty((total,), dtype=torch.uint8).pin_memory()
         hs = self._h_stage.numpy()
-        hw = np.empty((B, 2), dtype=np.int32)
         for b, im in enumerate(images):
-            hs[int(off[b]):int(off[b]) + sizes[b]] = np.ascontiguousarray(im).reshape(-1)
-            hw[b] = im.shape[:2]
+            if not is_jpeg[b]:
+                hs[int(off[b]):int(off[b]) + sizes[b]] = np.ascontiguousarray(im).reshape(-1)
         d_src = self._h_stage[:total].to(self.device, non_blocking=True)
+        d_status = self.jpeg_decode_into(plan, d_src, off[jidx], stream) if jidx else None
+        return d_src, off, shapes, d_status, jidx
+
+    # ------------------------------------------------------------------ batched (one launch each)
+    def cv2_resize_batch_device(self, images, size_hw, stream=None, return_sources=False):
+        """`cv2.resize(img, (S, S))` for a list of images of ANY sizes in one launch: uint8 HxWx3
+        NumPy images or JPEG files as bytes, staged by `stage_images` (JPEG files decoded on the
+        device into their slots).  Returns uint8 [B, dh, dw, 3] on the device; with
+        return_sources also each image's pixels for later steps: the array itself, or for a JPEG
+        file its decoded slot (uint8 [H, W, 3] on the device)."""
+        torch = _torch()
+        B = len(images)
+        dh, dw = int(size_hw[0]), int(size_hw[1])
+        d_src, off, shapes, d_status, jidx = self.stage_images(images, 16, stream)
+        hw = np.asarray([sh[:2] for sh in shapes], dtype=np.int32).reshape(B, 2)
         d_off = torch.from_numpy(off[:B].copy()).to(self.device)
         d_hw = torch.from_numpy(hw).to(self.device)
         out = torch.empty((B, dh, dw, 3), dtype=torch.uint8, device=self.device)
         N.check(self.lib.mrx_cv2_resize_u8c3_batch(
             _ptr(d_src), _ptr(d_off), _ptr(d_hw), _ptr(out), B, dh, dw, N.stream_ptr(stream)),
             "mrx_cv2_resize_u8c3_batch")
-        return out
+        if d_status is not None:
+            self.jpeg_check(d_status, jidx)
+        if not return_sources:
+            return out
+        sources = [d_src[int(off[b]):int(off[b]) + int(np.prod(shapes[b]))].view(shapes[b])
+                   if b in jidx else images[b] for b in range(B)]
+        return out, sources
 
     def mold_batch_device(self, d_imgs, out_dtype=np.float32, stream=None):
         """resize_image + mold_image for uint8 [B,h,w,3] device images of one size, one launch.

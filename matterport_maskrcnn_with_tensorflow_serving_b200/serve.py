@@ -21,6 +21,10 @@ image and the picture is written to `media/mask-<uuid>.png`, whose path is retur
 blend runs on the device canvas the unmold kernels just wrote (`mrx_composite_masks`): the
 105 MB of masks per 1024x1024x100 image never travel to the host.  Boxes, captions and
 contour polygons are matplotlib artists in the reference and are not drawn (DESIGN.md 7).
+
+Wherever an image is accepted, a JPEG file's bytes (bytes, bytearray or memoryview) are accepted
+too: they are decoded on the device (`api_utils.decode_jpeg_batch`, bit for bit as `load_img`), so
+the decoded pixels never reach the host.  A `str` path still goes through `load_img`.
 """
 from __future__ import annotations
 
@@ -61,13 +65,30 @@ def _get_molder():
     return _molder
 
 
+def _is_jpeg(img):
+    return isinstance(img, (bytes, bytearray, memoryview))
+
+
 def _check_image(img):
+    """An image argument: a path (loaded by `load_img`), JPEG bytes (kept for the device decoder)
+    or an HxWx3 uint8 array."""
     if isinstance(img, str):
         img = api_utils.load_img(img)
+    if _is_jpeg(img):
+        return img
     img = np.asarray(img)
     if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
         raise TypeError("preprocess_input expects an HxWx3 uint8 image")
     return img
+
+
+def _image_shape(img):
+    """(H, W, 3) of a checked image argument; for JPEG bytes from the header alone."""
+    if _is_jpeg(img):
+        from . import jpeg
+
+        return jpeg.parse(img).shape
+    return tuple(img.shape)
 
 
 def preprocess_input(img, img_size=640, molded_dtype=np.float64):
@@ -80,7 +101,10 @@ def preprocess_input(img, img_size=640, molded_dtype=np.float64):
     img = _check_image(img)
     with _molder_lock:
         molder = _get_molder()
-        d_img = torch.from_numpy(np.ascontiguousarray(img)).to(molder.device)
+        if _is_jpeg(img):
+            d_img, = molder.decode_jpeg_batch([img])
+        else:
+            d_img = torch.from_numpy(np.ascontiguousarray(img)).to(molder.device)
         if img_size is not None:
             d_img = molder.cv2_resize_device(d_img, (img_size, img_size))
         img_shape = tuple(d_img.shape)
@@ -102,28 +126,47 @@ def preprocess_input_batch(imgs, img_size=640, molded_dtype=np.float32):
     (molded_images [B,H,W,3], image_metas [B,M], anchors [A,4] (shared), windows: list of
     4-tuples) -- row b equals `preprocess_input(imgs[b], img_size, molded_dtype)`.
     Default dtype float32: what serve.py:117 puts on the wire."""
+    imgs = [_check_image(im) for im in imgs]
+    return _preprocess_batch(imgs, img_size, molded_dtype)[:4]
+
+
+def _preprocess_batch(imgs, img_size, molded_dtype):
+    """`preprocess_input_batch` of checked images, plus each image's pixels for the overlay: the
+    array itself, or for JPEG bytes its decoded slot of the buffer the resize read (uint8
+    [H, W, 3] on the device, consumed in place)."""
     import torch
 
     mcf = api_utils.get_config()
-    imgs = [_check_image(im) for im in imgs]
     if len(imgs) == 0:
         raise ValueError("empty batch")
     with _molder_lock:
         molder = _get_molder()
         if img_size is not None:
-            d_imgs = molder.cv2_resize_batch_device(imgs, (img_size, img_size))
+            d_imgs, sources = molder.cv2_resize_batch_device(imgs, (img_size, img_size),
+                                                             return_sources=True)
+            d_status = None
         else:
-            if any(im.shape != imgs[0].shape for im in imgs):
+            shapes = [_image_shape(im) for im in imgs]
+            if any(sh != shapes[0] for sh in shapes):
                 raise ValueError("img_size=None needs equally sized images")
-            d_imgs = torch.from_numpy(np.stack(imgs)).to(molder.device)
+            if not any(_is_jpeg(im) for im in imgs):
+                d_imgs = torch.from_numpy(np.stack(imgs)).to(molder.device)
+                sources, d_status = list(imgs), None
+            else:
+                # one contiguous [B, H, W, 3] buffer: arrays staged, JPEG files decoded in place
+                d_src, off, _, d_status, jidx = molder.stage_images(imgs, align=1)
+                d_imgs = d_src[:int(off[-1])].view(len(imgs), *shapes[0])
+                sources = [d_imgs[b] if b in jidx else imgs[b] for b in range(len(imgs))]
         img_shape = tuple(d_imgs.shape[1:])
         d_molded, window, scale, _padding = molder.mold_batch_device(d_imgs, out_dtype=molded_dtype)
+        if d_status is not None:
+            molder.jpeg_check(d_status, jidx)
         molded = d_molded.cpu().numpy()
     meta = compose_image_meta(0, img_shape, molded.shape[1:], window, scale,
                               np.zeros([mcf.NUM_CLASSES], dtype=np.int32))
     metas = np.stack([meta] * len(imgs))
     anchors = api_utils.get_anchors(molded.shape[1:])
-    return molded, metas, anchors, [window] * len(imgs)
+    return molded, metas, anchors, [window] * len(imgs), sources
 
 
 def _is_tensor_proto(x):
@@ -158,16 +201,21 @@ def grpc_inference_batch(imgs):
     """`grpc_inference` for a list of images: batched pre-processing, then one RPC per image
     (the served model's signature is batch 1, serve.py:48).  Returns a list of
     (mrcnn_detection, mrcnn_mask, molded_image_shape, window)."""
+    return _grpc_inference_batch([_check_image(im) for im in imgs])[0]
+
+
+def _grpc_inference_batch(imgs):
+    """`grpc_inference_batch` of checked images, plus each image's pixels (`_preprocess_batch`)."""
     if _predict_fn is None:
         raise RuntimeError("no TensorFlow-Serving client installed: call set_predict_fn()")
-    molded, metas, anchors, windows = preprocess_input_batch(imgs, cf.IMAGE_SIZE, np.float32)
+    molded, metas, anchors, windows, sources = _preprocess_batch(imgs, cf.IMAGE_SIZE, np.float32)
     anchors32 = anchors.astype(np.float32)
     out = []
     for b in range(len(imgs)):
         det, msk = _predict_fn(molded[b], metas[b].astype(np.float32), anchors32)
         det, msk = _decode_outputs(det, msk)
         out.append((det, msk, molded[b].shape, windows[b]))
-    return out
+    return out, sources
 
 
 def do_inference_unmolded(img):
@@ -176,7 +224,7 @@ def do_inference_unmolded(img):
     img = _check_image(img)
     mrcnn_detection, mrcnn_mask, molded_image, window = grpc_inference(img)
     return api_utils.unmold_detections(
-        mrcnn_detection, mrcnn_mask, img.shape, molded_image.shape, window)
+        mrcnn_detection, mrcnn_mask, _image_shape(img), molded_image.shape, window)
 
 
 def _save_overlay(overlay_rgb, media_dir=None):
@@ -203,10 +251,10 @@ def do_inference_batch(imgs, colors=None, media_dir=None):
     imgs = [_check_image(im) for im in imgs]
     if len(imgs) == 0:
         return []
-    res = grpc_inference_batch(imgs)
-    items = [(det, msk, img.shape, mshape, window)
-             for (det, msk, mshape, window), img in zip(res, imgs)]
-    outs = api_utils.unmold_overlay_batch(items, imgs, colors=colors)
+    res, sources = _grpc_inference_batch(imgs)
+    items = [(det, msk, tuple(src.shape), mshape, window)
+             for (det, msk, mshape, window), src in zip(res, sources)]
+    outs = api_utils.unmold_overlay_batch(items, sources, colors=colors)
     paths = []
     for _boxes, _cls, _scores, overlay in outs:
         paths.append(_save_overlay(overlay, media_dir))
@@ -226,7 +274,7 @@ def do_inference_coco_batch(imgs, image_ids, category_ids=None):
         raise ValueError(f"{len(imgs)} images but {len(image_ids)} image ids")
     if len(imgs) == 0:
         return []
-    res = grpc_inference_batch(imgs)
-    items = [(det, msk, img.shape, mshape, window)
-             for (det, msk, mshape, window), img in zip(res, imgs)]
+    res, sources = _grpc_inference_batch(imgs)
+    items = [(det, msk, tuple(src.shape), mshape, window)
+             for (det, msk, mshape, window), src in zip(res, sources)]
     return api_utils.unmold_coco_results_batch(items, image_ids, category_ids)

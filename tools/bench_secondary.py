@@ -5,7 +5,7 @@ each unmold workload also names the GPU and its power limit.
 
   python tools/bench_secondary.py [--iters 20] [--cpu]     (--cpu also times the oracle)
   python tools/bench_secondary.py --only-eval | --only-cocoeval | --only-bboxeval | --only-boundaryeval
-                                  | --only-polygons | --only-lvis
+                                  | --only-polygons | --only-lvis | --only-jpeg
 """
 import argparse
 import ctypes as C
@@ -1009,6 +1009,93 @@ def mold_cases(iters, cpu):
                       "gpu_us_per_image": round(med * 1e3, 2)}), flush=True)
 
 
+def jpeg_case(iters):
+    """JPEG request bytes decoded on the device (csrc/jpeg.cu) against cv2.imdecode on the host,
+    each followed by preprocess_input_batch: 32 x 1024^2 and 16 x 2160x3840, quality 90, 4:2:0,
+    no restart markers (cv2.imencode's defaults)."""
+    import cv2
+    from concurrent.futures import ThreadPoolExecutor
+
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, jpeg, serve
+
+    rng = np.random.default_rng(11)
+    params = [cv2.IMWRITE_JPEG_QUALITY, 90, cv2.IMWRITE_JPEG_SAMPLING_FACTOR,
+              cv2.IMWRITE_JPEG_SAMPLING_FACTOR_420]
+    m = Molder(api_utils.get_config())
+    for name, batch, hw in [("32 x 1024x1024", 32, (1024, 1024)),
+                            ("configs[3] size: 16 x 2160x3840", 16, (2160, 3840))]:
+        base = [synth.synth_rgb_image(rng, *hw) for _ in range(4)]
+        blobs = [cv2.imencode(".jpg", base[b % 4][:, :, ::-1], params)[1].tobytes()
+                 for b in range(batch)]
+        mb = sum(len(b) for b in blobs) / 1e6
+        # S sweep: Molder.decode_jpeg_batch, host parse and status read included
+        sweep = {}
+        for S in (256, 512, 1024, 2048, 4096):
+            sweep[S], _ = time_ms(lambda: m.decode_jpeg_batch(blobs, S=S), iters)
+        # kernel times, one profiled run of its own
+        from torch.profiler import ProfilerActivity, profile
+        m.decode_jpeg_batch(blobs)
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(5):
+                m.decode_jpeg_batch(blobs)
+            torch.cuda.synchronize()
+        kern = {}
+        for ev in prof.key_averages():
+            if "jpeg_" in ev.key:
+                short = ev.key.split("jpeg_")[1].split("_kernel")[0]
+                kern[short] = round(ev.device_time_total / 1e3 / 5, 4)
+        plan = jpeg.Plan(blobs)
+        # sync rounds (largest over an image's CTAs) and the walk's re-decoded subsequences, per
+        # image, from the counters the kernels leave after each image's subsequence arrays
+        m.decode_jpeg_batch(blobs)
+        work = m._jpeg_bufs["work"].cpu().numpy()
+        tail = [int(plan.desc[b, jpeg.D_SUB_OFF] + 4 * plan.desc[b, jpeg.D_SUB_CAP])
+                for b in range(batch)]
+        rounds = [int(work[t + 1]) for t in tail]
+        redone = [int(work[t + 2]) for t in tail]
+        dec_ms, _ = time_ms(lambda: api_utils.decode_jpeg_batch(blobs), iters)
+        pre_ms, _ = time_ms(lambda: serve.preprocess_input_batch(blobs), iters)
+
+        def host(pool):
+            dec = (lambda b: cv2.cvtColor(cv2.imdecode(np.frombuffer(b, np.uint8), cv2.IMREAD_COLOR),
+                                          cv2.COLOR_BGR2RGB))
+            arrs = list(pool.map(dec, blobs)) if pool else [dec(b) for b in blobs]
+            return serve.preprocess_input_batch(arrs)
+
+        def host_clock(fn, n):
+            fn()
+            ts = []
+            for _ in range(n):
+                t0 = time.perf_counter()
+                fn()
+                torch.cuda.synchronize()
+                ts.append((time.perf_counter() - t0) * 1e3)
+            return float(np.median(ts))
+
+        one_ms = host_clock(lambda: host(None), max(3, iters // 4))
+        with ThreadPoolExecutor(os.cpu_count()) as pool:
+            pool_ms = host_clock(lambda: host(pool), max(3, iters // 4))
+        t_dec = time.perf_counter()
+        cv2.imdecode(np.frombuffer(blobs[0], np.uint8), cv2.IMREAD_COLOR)
+        imdecode_ms = (time.perf_counter() - t_dec) * 1e3
+        print(json.dumps({
+            "workload": f"JPEG decode {name} q90 4:2:0, no RST ({mb:.1f} MB of files)",
+            "kernel_ms": kern, "subsequences_per_image_at_default_S": int(plan.max_subs),
+            "default_S": jpeg.DEFAULT_S,
+            "sync_rounds_per_image_min_median_max": [min(rounds), int(np.median(rounds)),
+                                                     max(rounds)],
+            "walk_redecoded_subsequences_per_image_min_median_max": [
+                min(redone), int(np.median(redone)), max(redone)],
+            "molder_decode_ms_by_S": {str(k): round(v, 3) for k, v in sweep.items()},
+            "api_utils_decode_jpeg_batch_ms": round(dec_ms, 3),
+            "preprocess_input_batch_bytes_ms": round(pre_ms, 3),
+            "host_imdecode_one_thread_then_preprocess_ms": round(one_ms, 3),
+            "host_imdecode_pool_then_preprocess_ms": round(pool_ms, 3),
+            "host_threads": os.cpu_count(), "one_imdecode_ms": round(imdecode_ms, 3),
+            **card()}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
@@ -1021,8 +1108,12 @@ def main():
     ap.add_argument("--only-polygons", action="store_true", help="only the polygon ground truth "
                     "record")
     ap.add_argument("--only-lvis", action="store_true", help="only the LVIS mask AP record")
+    ap.add_argument("--only-jpeg", action="store_true", help="only the JPEG decode record")
     args = ap.parse_args()
     torch.cuda.set_device(0)
+    if args.only_jpeg:
+        jpeg_case(args.iters)
+        return
     if args.only_cocoeval:
         cocoeval_case(args.iters)
         return
