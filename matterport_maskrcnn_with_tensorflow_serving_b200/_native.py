@@ -1,5 +1,9 @@
 """ctypes binding of lib/libmrx.so (C ABI: include/mrx.h).
 
+The header is the only declaration of the ABI: every `#define MRX_<NAME> <integer>` is a module
+attribute here, and every `mrx_*` prototype gives the restype and argtypes of its function.  A
+pointer parameter takes a torch tensor whose dtype holds the C element type (see `Pointer`).
+
 There is no CPU fallback: if the library is missing or a call fails, this raises.
 PyTorch is imported first so that libmrx.so resolves libcudart.so.12 to the CUDA
 runtime instance torch already loaded (shared device / stream state).
@@ -10,44 +14,125 @@ import ctypes as C
 import os
 import re
 
+import torch
+
 _PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 # MRX_LIB=<file name under lib/> selects another build of the library (development only:
 # e.g. libmrx_dev.so built with MRX_NVCC_FLAGS=-DMRX_DEV); the default is the shipped one
 LIB_PATH = os.path.join(_PKG_DIR, "lib", os.environ.get("MRX_LIB", "libmrx.so"))
 HEADER_PATH = os.path.join(os.path.dirname(_PKG_DIR), "include", "mrx.h")
 
-MRX_OK = 0
-MRX_E_UNSUPPORTED = -2
-MRX_F32 = 0
-MRX_F64 = 1
-MRX_ST_CLASS_RANGE = 1
-MRX_ST_BOX_RANGE = 2
-MRX_GEOM_INTS = 8
-MRX_MAX_BATCH = 4096
-MRX_MAX_MASK_DIM = 64
-MRX_MAX_LANE_MASK_W = 30    # tile width of the lane kernels: mw + 2 lanes per warp
-ABI_VERSION = 17
-MRX_SCHED_WORDS = 4
-MRX_PEER_HANDLE_BYTES = 64
-MRX_MAX_CONTOUR_SEGMENTS = 1 << 30
-MRX_MAX_IOU_THRESHOLDS = 64
-MRX_MAX_AREA_RANGES = 16
-MRX_BOX_YXYX_I32 = 0
-MRX_BOX_XYWH_F64 = 1
-MRX_LVIS_POSITIVE = 1
-MRX_LVIS_NEGATIVE = 2
-MRX_LVIS_EVALUATED = 3
-MRX_LVIS_NOT_EXHAUSTIVE = 4
-MRX_RLE_ST_CHAR = 1
-MRX_RLE_ST_TRUNC = 2
-MRX_RLE_ST_RANGE = 4
-MRX_RLE_ST_SUM = 8
-MRX_RLE_ST_SKIP = 16
-MRX_JPEG_ST_CODE = 1
-MRX_JPEG_ST_TRUNC = 2
-MRX_JPEG_ST_RST = 4
-MRX_JPEG_ST_DC = 8
-MRX_JPEG_ST_MARKER = 16
+
+class MrxError(RuntimeError):
+    """A libmrx call returned a negative status."""
+
+
+class Pointer(C.c_void_p):
+    """A pointer parameter of the header, one subclass per C element type (`element`).  A torch
+    tensor (device, pinned or CPU memory) passes its data_ptr() when it is contiguous and its
+    dtype holds the element type; anything else goes through as c_void_p takes it (None, an
+    integer address, c_void_p, byref(...), bytes), a ctypes array only when its elements have the
+    element's size.  Wrong arguments raise TypeError, which ctypes reports as
+    ctypes.ArgumentError."""
+    element = "void"
+
+
+# C element type of a pointer parameter -> (bytes, tensor dtypes that hold it; None: any).
+# unsigned int data lives in int32 tensors (torch has few uint32 kernels); void * is the element
+# of a void ** out-parameter, given as byref(c_void_p()).
+_ELEMENTS = {
+    "void": (None, None),
+    "unsigned char": (1, (torch.uint8,)),
+    "short": (2, (torch.int16,)),
+    "int": (4, (torch.int32,)),
+    "unsigned int": (4, (torch.int32, torch.uint32)),
+    "float": (4, (torch.float32,)),
+    "long long": (8, (torch.int64,)),
+    "double": (8, (torch.float64,)),
+    "void *": (8, ()),
+}
+
+
+def _pointer_type(element, size, dtypes):
+    """The `Pointer` subclass of one element type."""
+    dtypes = None if dtypes is None else frozenset(dtypes)
+
+    # runs for every pointer of every launch: its names are locals
+    def from_param(obj, _tensor=torch.Tensor, _void_p=C.c_void_p):
+        if isinstance(obj, _tensor):
+            if (dtypes is None or obj.dtype in dtypes) and obj.is_contiguous():
+                return _void_p(obj.data_ptr())
+            got = str(obj.dtype) if obj.is_contiguous() else "non-contiguous"
+            raise TypeError(f"{element} * parameter: got a {got} tensor")
+        if isinstance(obj, C.Array) and size is not None and C.sizeof(obj._type_) != size:
+            raise TypeError(f"{element} * parameter: got an array of {obj._type_.__name__}")
+        return _void_p.from_param(obj)
+
+    return type(f"Pointer[{element}]", (Pointer,),
+                {"element": element, "from_param": staticmethod(from_param)})
+
+
+_POINTERS = {e: _pointer_type(e, size, dtypes) for e, (size, dtypes) in _ELEMENTS.items()}
+_SCALARS = {"int": C.c_int, "unsigned int": C.c_uint, "long long": C.c_longlong,
+            "unsigned long long": C.c_ulonglong, "double": C.c_double}
+_RESTYPES = {"int": C.c_int, "const char *": C.c_char_p}
+
+
+def _words(decl):
+    """A C declaration with one space between its words and around each '*'."""
+    return " ".join(decl.replace("*", " * ").split())
+
+
+def _parameter(fn, param):
+    """The ctypes argtype of one parameter declaration (in `_words` form) of function `fn`."""
+    m = re.fullmatch(r"(?:const )?([a-z]+(?: [a-z]+)*)((?: \*)*) \w+", param)
+    if m is None:
+        kind = None
+    elif not m.group(2):
+        kind = _SCALARS.get(m.group(1))
+    else:   # the element type: one '*' fewer
+        kind = _POINTERS.get(m.group(1) + " *" * (m.group(2).count("*") - 1))
+    if kind is None:
+        raise ValueError(f"mrx.h: {fn}: no binding for the parameter {param!r}")
+    return kind
+
+
+def parse_header(text):
+    """(constants, signatures) of a header's text: constants {MRX_NAME: int} of every object-like
+    `#define MRX_*` (a decimal integer, possibly negative, or `(a << b)`), signatures
+    {mrx_name: (restype, argtypes)} of every `mrx_*` prototype.  A define or prototype it cannot
+    read, or a type outside its tables, raises ValueError naming it."""
+    text = re.sub(r"/\*.*?\*/|//[^\n]*", " ", text, flags=re.S)
+    constants = {}
+    for name, value in re.findall(r"^[ \t]*#[ \t]*define[ \t]+(MRX_\w+)[ \t]+(\S.*?)[ \t]*$",
+                                  text, flags=re.M):
+        m = re.fullmatch(r"(-?\d+)|\( *(\d+) *<< *(\d+) *\)", value)
+        if m is None:
+            raise ValueError(f"mrx.h: {name}: {value!r} is not an integer constant")
+        constants[name] = int(m.group(1)) if m.group(1) else int(m.group(2)) << int(m.group(3))
+    body = re.sub(r"^[ \t]*#.*$", "", text, flags=re.M)
+    signatures = {}
+    for ret, fn, params in re.findall(r"([^;{}]*?)\b(mrx_\w+)\s*\(([^;{}]*)\)\s*;", body):
+        restype = _RESTYPES.get(_words(ret))
+        if restype is None:
+            raise ValueError(f"mrx.h: {fn}: no binding for the return type {_words(ret)!r}")
+        params = [_words(p) for p in params.split(",")]
+        signatures[fn] = (restype, [] if params == ["void"] else
+                          [_parameter(fn, p) for p in params])
+    unread = sorted(set(re.findall(r"\b(mrx_\w+)\s*\(", body)) - set(signatures))
+    if unread:
+        raise ValueError(f"mrx.h: cannot read the declaration of {', '.join(unread)}")
+    return constants, signatures
+
+
+def _read_header(header_path=HEADER_PATH):
+    with open(header_path) as f:
+        return parse_header(f.read())
+
+
+_CONSTANTS, SIGNATURES = _read_header()   # SIGNATURES: name -> (restype, argtypes)
+globals().update(_CONSTANTS)
+ABI_VERSION = _CONSTANTS["MRX_ABI_VERSION"]
 
 
 def contour_scratch_bytes(total_segments):
@@ -61,88 +146,12 @@ def rle_string_bound(total_changes, n_instances):
     return 7 * (int(total_changes) + int(n_instances))
 
 
-class MrxError(RuntimeError):
-    """A libmrx call returned a negative status."""
-
-
-_vp, _i, _ip = C.c_void_p, C.c_int, C.POINTER(C.c_int)
-_dp = C.POINTER(C.c_double)
-
-# name -> (restype, argtypes); must list every function include/mrx.h declares
-SIGNATURES = {
-    "mrx_abi_version": (_i, []),
-    "mrx_last_error": (C.c_char_p, []),
-    "mrx_device_props": (_i, [_i, _ip, _ip, _ip, _ip]),
-    "mrx_anchor_count": (_i, [_i, _i, _ip, _i, _i, _i, C.POINTER(C.c_longlong)]),
-    "mrx_anchors": (_i, [_vp, _i, _i, _dp, _dp, _ip, _i, _i, _i, _vp]),
-    "mrx_unmold_prepare": (_i, [_vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp, _vp,
-                                _vp, _vp, _vp, _vp, _vp]),
-    "mrx_mask_expand": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp,
-                             _vp]),
-    "mrx_mask_expand_values": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i,
-                                    _vp, _vp]),
-    "mrx_mask_expand_packed": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp,
-                                    _vp]),
-    "mrx_rle_count": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
-    "mrx_rle_write": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
-    "mrx_rle_strings": (_i, [_vp, _vp, _vp, _i, _i, _vp, _vp, _vp]),
-    "mrx_contours_count": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
-    "mrx_contours_write": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_longlong, C.c_longlong,
-                                _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
-    "mrx_mask_extents": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
-    "mrx_mask_overlaps": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp,
-                               _i, _vp]),
-    "mrx_mask_matches": (_i, [_vp, _vp, _vp, _vp, _i, _vp, _vp, _dp, _i, C.c_double, _vp, _vp,
-                              _vp, _i, _i, _i, _vp]),
-    "mrx_coco_ranks": (_i, [_vp, _vp, _i, _vp, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i, _vp]),
-    "mrx_lvis_ranks": (_i, [_vp, _vp, _i, _vp, _vp, _i, _vp, _i, _i, _vp, _vp, _vp, _vp, _i, _i,
-                            _vp]),
-    "mrx_coco_ious": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                           _i, _vp, _vp, _i, _vp]),
-    "mrx_coco_match": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _dp, _i, _dp, _i, _vp,
-                            _vp, _i, _i, _i, _vp]),
-    "mrx_coco_match_f64area": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _dp, _i, _dp,
-                                    _i, _vp, _vp, _i, _i, _i, _vp]),
-    "mrx_coco_box_ious": (_i, [_vp, _i, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i,
-                               _vp]),
-    "mrx_mask_boundary": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
-    "mrx_coco_boundary_ious": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp,
-                                    _vp, _vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _i, _vp]),
-    "mrx_rle_parse": (_i,[_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _vp]),
-    "mrx_rle_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
-    "mrx_poly_decode": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
-                             _i, _i, _i, _i, _vp]),
-    "mrx_device_alloc": (_i, [C.c_ulonglong, C.POINTER(C.c_void_p), _ip]),
-    "mrx_device_free": (_i, [_vp, C.c_ulonglong]),
-    "mrx_peer_alloc": (_i, [C.c_ulonglong, C.POINTER(C.c_void_p)]),
-    "mrx_peer_free": (_i, [_vp]),
-    "mrx_peer_export": (_i, [_vp, C.c_char_p]),
-    "mrx_peer_open": (_i, [C.c_char_p, C.POINTER(C.c_void_p)]),
-    "mrx_peer_close": (_i, [_vp]),
-    "mrx_peer_signal": (_i, [_vp, C.c_uint, _vp]),
-    "mrx_peer_wait": (_i, [_vp, _i, C.c_uint, _vp]),
-    "mrx_cv2_resize_u8c3": (_i, [_vp, _i, _i, _vp, _i, _i, _vp]),
-    "mrx_mold_image": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _dp, _i, _vp, _vp, _vp]),
-    "mrx_cv2_resize_u8c3_batch": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
-    "mrx_mold_image_batch": (_i, [_vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _dp, _i, _vp, _vp,
-                                  _vp]),
-    "mrx_composite_masks": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_double, _vp, _i, _i,
-                                 C.c_longlong, _vp]),
-    "mrx_pack_masks": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp]),
-    "mrx_jpeg_coefficients": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp,
-                                   C.c_longlong, _vp, _vp]),
-    "mrx_jpeg_pixels": (_i, [_vp, _vp, _vp, _vp, _i, _i, C.c_longlong, _vp, _vp, _vp, _vp]),
-}
-
 _lib = None
 
 
 def declared_symbols(header_path=HEADER_PATH):
     """Function names declared in include/mrx.h (used by the symbol-export test)."""
-    with open(header_path) as f:
-        text = f.read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return sorted(set(re.findall(r"\b(mrx_[a-z0-9_]+)\s*\(", text)))
+    return sorted(_read_header(header_path)[1])
 
 
 def load(build_if_missing=True):
@@ -150,7 +159,6 @@ def load(build_if_missing=True):
     global _lib
     if _lib is not None:
         return _lib
-    import torch  # noqa: F401  (loads libcudart.so.12 before libmrx.so asks for it)
 
     default_lib = os.path.basename(LIB_PATH) == "libmrx.so"
     if build_if_missing and default_lib:
@@ -178,7 +186,7 @@ def load(build_if_missing=True):
 
 
 def check(rc, what):
-    if rc != MRX_OK:
+    if rc != _CONSTANTS["MRX_OK"]:
         msg = load().mrx_last_error()
         raise MrxError(f"{what} failed (status {rc}): {msg.decode() if msg else ''}")
 
@@ -195,8 +203,6 @@ def double_array(values):
 
 def stream_ptr(stream):
     """cudaStream_t of a torch.cuda.Stream (or the current stream) as an integer."""
-    import torch
-
     if stream is None:
         stream = torch.cuda.current_stream()
     return C.c_void_p(stream.cuda_stream)
@@ -213,8 +219,6 @@ class DeviceBytes:
 
 
 def require_cuda():
-    import torch
-
     if not torch.cuda.is_available():
         raise MrxError("no CUDA device: this package has no CPU fallback "
                        "(the CPU restatement under oracle/ is test infrastructure only)")

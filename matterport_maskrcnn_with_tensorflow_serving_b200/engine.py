@@ -46,10 +46,6 @@ def _torch_dtype(np_dtype):
             np.dtype(np.uint32): torch.int32, np.dtype(np.uint8): torch.uint8}[np.dtype(np_dtype)]
 
 
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
-
-
 def make_geom(original_image_shape, image_shape, window):
     """Pack one image's geometry the way mrx_unmold_prepare expects (8 x int32)."""
     oh, ow = int(original_image_shape[0]), int(original_image_shape[1])
@@ -270,11 +266,10 @@ class UnmoldEngine:
         # steps 1-6 and the class-tile gather in one launch; tiles are stored by detection row
         # and found through d_src_index by the expand kernels
         N.check(self.lib.mrx_unmold_prepare(
-            _ptr(d_detections), _dtype_code(self.det_dtype), _ptr(d_mrcnn_mask),
-            _dtype_code(self.mask_dtype), n, self.R, self.mh, self.mw, self.C,
-            _ptr(self.d_geom), _ptr(self.d_boxes), _ptr(self.d_class_ids), _ptr(self.d_scores),
-            _ptr(self.d_src_index), _ptr(self.d_counts),
-            _ptr(self.d_status), _ptr(self.d_tiles), _ptr(self.d_sched), st),
+            d_detections, _dtype_code(self.det_dtype), d_mrcnn_mask, _dtype_code(self.mask_dtype),
+            n, self.R, self.mh, self.mw, self.C, self.d_geom, self.d_boxes, self.d_class_ids,
+            self.d_scores, self.d_src_index, self.d_counts, self.d_status, self.d_tiles,
+            self.d_sched, st),
             "mrx_unmold_prepare")
         if expand:
             self.enqueue_expand(stream)
@@ -288,12 +283,11 @@ class UnmoldEngine:
         b0, b1 = (0, self._n_images) if images is None else images
         if b1 <= b0:
             return
-        base = _ptr(self.d_canvas) if canvas_ptr is None else C.c_void_p(int(canvas_ptr))
+        base = self.d_canvas if canvas_ptr is None else int(canvas_ptr)
         N.check(self.lib.mrx_mask_expand(
-            _ptr(self.d_tiles[b0:]), _ptr(self.d_src_index[b0:]), _ptr(self.d_boxes[b0:]),
-            _ptr(self.d_counts[b0:]), _ptr(self.d_geom[b0:]),
-            _ptr(self.d_canvas_off[b0:]), base, b1 - b0, self.R, self.mh, self.mw,
-            self.chunk_bytes, self.ctas_per_sm, _ptr(self.d_sched),
+            self.d_tiles[b0:], self.d_src_index[b0:], self.d_boxes[b0:], self.d_counts[b0:],
+            self.d_geom[b0:], self.d_canvas_off[b0:], base, b1 - b0, self.R, self.mh, self.mw,
+            self.chunk_bytes, self.ctas_per_sm, self.d_sched,
             N.stream_ptr(stream)), "mrx_mask_expand")
 
     def enqueue_expand_values(self, d_values, stream=None):
@@ -303,9 +297,9 @@ class UnmoldEngine:
         if d_values.dtype != _torch().float32 or d_values.numel() < int(self.layout.canvas_off[n]):
             raise ValueError("d_values must be float32 with one element per canvas byte")
         N.check(self.lib.mrx_mask_expand_values(
-            _ptr(self.d_tiles), _ptr(self.d_src_index), _ptr(self.d_boxes), _ptr(self.d_counts),
-            _ptr(self.d_geom), _ptr(self.d_canvas_off), _ptr(self.d_canvas), _ptr(d_values),
-            n, self.R, self.mh, self.mw, _ptr(self.d_sched), N.stream_ptr(stream)),
+            self.d_tiles, self.d_src_index, self.d_boxes, self.d_counts, self.d_geom,
+            self.d_canvas_off, self.d_canvas, d_values, n, self.R, self.mh, self.mw, self.d_sched,
+            N.stream_ptr(stream)),
             "mrx_mask_expand_values")
 
     # ------------------------------------------------------------------ packed output
@@ -336,16 +330,15 @@ class UnmoldEngine:
         b0, b1 = (0, self._n_images) if images is None else images
         if packed_ptr is None:
             off = self._packed_buffer()
-            base = _ptr(self.d_packed)
+            base = self.d_packed
         else:
             off, _ = self.packed_layout()
-            base = C.c_void_p(int(packed_ptr))
+            base = int(packed_ptr)
         if b1 > b0:
             N.check(self.lib.mrx_mask_expand_packed(
-                _ptr(self.d_tiles[b0:]), _ptr(self.d_src_index[b0:]), _ptr(self.d_boxes[b0:]),
-                _ptr(self.d_counts[b0:]),
-                _ptr(self.d_geom[b0:]), _ptr(self.d_packed_off[b0:]), base, b1 - b0, self.R,
-                self.mh, self.mw, self.layout.max_w, _ptr(self.d_sched), N.stream_ptr(stream)),
+                self.d_tiles[b0:], self.d_src_index[b0:], self.d_boxes[b0:], self.d_counts[b0:],
+                self.d_geom[b0:], self.d_packed_off[b0:], base, b1 - b0, self.R, self.mh,
+                self.mw, self.layout.max_w, self.d_sched, N.stream_ptr(stream)),
                 "mrx_mask_expand_packed")
         return self.d_packed, off
 
@@ -396,15 +389,15 @@ class UnmoldEngine:
         d_col = torch.empty((n * self.R * max_w,), dtype=torch.int32, device=dev)
         d_off = torch.empty((n * self.R + 1,), dtype=torch.int64, device=dev)
         st = N.stream_ptr(None)
-        args = (_ptr(self.d_tiles), _ptr(self.d_src_index), _ptr(self.d_boxes), _ptr(self.d_counts),
-                _ptr(self.d_geom), _ptr(d_col), _ptr(d_off))
+        args = (self.d_tiles, self.d_src_index, self.d_boxes, self.d_counts, self.d_geom, d_col,
+                d_off)
         N.check(self.lib.mrx_rle_count(*args, n, self.R, self.mh, self.mw, max_w, st),
                 "mrx_rle_count")
         off = d_off.cpu().numpy()          # the one synchronisation: how many runs there are
         total = int(off[-1])
         d_pos = torch.empty((max(total, 1),), dtype=torch.int32, device=dev)
         d_runs = torch.empty((total + n * self.R,), dtype=torch.int32, device=dev)
-        N.check(self.lib.mrx_rle_write(*args, _ptr(d_pos), _ptr(d_runs), n, self.R, self.mh,
+        N.check(self.lib.mrx_rle_write(*args, d_pos, d_runs, n, self.R, self.mh,
                                        self.mw, max_w, st), "mrx_rle_write")
         return d_runs, d_off, off
 
@@ -421,8 +414,8 @@ class UnmoldEngine:
             d_str = torch.empty((max(N.rle_string_bound(off[-1], ni), 1),), dtype=torch.uint8,
                                 device=self.device)
             d_str_off = torch.empty((ni + 1,), dtype=torch.int64, device=self.device)
-            N.check(self.lib.mrx_rle_strings(_ptr(d_runs), _ptr(d_off), _ptr(self.d_counts),
-                                             self._n_images, self.R, _ptr(d_str_off), _ptr(d_str),
+            N.check(self.lib.mrx_rle_strings(d_runs, d_off, self.d_counts,
+                                             self._n_images, self.R, d_str_off, d_str,
                                              N.stream_ptr(None)), "mrx_rle_strings")
         return d_str, d_str_off
 
@@ -589,8 +582,8 @@ class UnmoldEngine:
         d_areas = _buffer(bufs, "areas", n * self.R, torch.int64, self.device)
         d_ext = _buffer(bufs, "extents", n * self.R * 4, torch.int32, self.device)
         N.check(self.lib.mrx_mask_extents(
-            _ptr(self.d_packed), _ptr(self.d_packed_off), _ptr(self.d_counts), _ptr(self.d_geom),
-            _ptr(self.d_boxes), _ptr(d_areas), _ptr(d_ext), n, self.R, N.stream_ptr(stream)),
+            self.d_packed, self.d_packed_off, self.d_counts, self.d_geom, self.d_boxes, d_areas,
+            d_ext, n, self.R, N.stream_ptr(stream)),
             "mrx_mask_extents")
         return Planes(self.d_packed, self.d_packed_off, self.d_counts, d_areas, d_ext, self.R)
 
@@ -601,8 +594,8 @@ class UnmoldEngine:
         n = self._n_images
         off = self._packed_buffer()
         N.check(self.lib.mrx_pack_masks(
-            _ptr(self.d_canvas), _ptr(self.d_canvas_off), _ptr(self.d_counts), _ptr(self.d_geom),
-            _ptr(self.d_packed), _ptr(self.d_packed_off), n, self.R,
+            self.d_canvas, self.d_canvas_off, self.d_counts, self.d_geom, self.d_packed,
+            self.d_packed_off, n, self.R,
             self.layout.max_h, self.layout.max_w, N.stream_ptr(stream)), "mrx_pack_masks")
         return self.d_packed, off
 
@@ -645,7 +638,7 @@ def _device_bytes(lib, nbytes, device):
     torch = _torch()
     ptr, compressed = C.c_void_p(0), C.c_int(0)
     with torch.cuda.device(device):
-        N.check(lib.mrx_device_alloc(C.c_ulonglong(nbytes), C.byref(ptr), C.byref(compressed)),
+        N.check(lib.mrx_device_alloc(nbytes, C.byref(ptr), C.byref(compressed)),
                 "mrx_device_alloc")
     owner = N.DeviceBytes(ptr.value, nbytes)
     # torch holds `owner` for as long as any view of the tensor lives; at interpreter exit the
@@ -656,7 +649,7 @@ def _device_bytes(lib, nbytes, device):
 
 def _free_device_bytes(lib, ptr, nbytes, device):
     with _torch().cuda.device(device):
-        N.check(lib.mrx_device_free(C.c_void_p(ptr), C.c_ulonglong(nbytes)), "mrx_device_free")
+        N.check(lib.mrx_device_free(ptr, nbytes), "mrx_device_free")
 
 
 def _buffer(bufs, name, numel, dtype, device):
@@ -714,8 +707,8 @@ class MaskBatch:
                     continue
                 canvas[:s.size].copy_(torch.from_numpy(s.reshape(-1)))
                 H, W = layout.hw(b)
-                rc = lib.mrx_pack_masks(_ptr(canvas), _ptr(d_zero), _ptr(self.d_counts[b:]),
-                                        _ptr(self.d_geom[b:]), _ptr(d_packed), _ptr(d_off[b:]),
+                rc = lib.mrx_pack_masks(canvas, d_zero, self.d_counts[b:],
+                                        self.d_geom[b:], d_packed, d_off[b:],
                                         1, layout.R, H, W, N.stream_ptr(stream))
                 if rc == N.MRX_E_UNSUPPORTED:
                     raise ValueError(lib.mrx_last_error().decode())
@@ -799,12 +792,12 @@ class MaskBatch:
                 d_runs[S:S + pk["runs"].size].copy_(d_uploaded_runs)
                 d_ends = torch.empty((d_runs.numel(),), dtype=torch.int64, device=device)
                 if S:
-                    N.check(lib.mrx_rle_parse(_ptr(d_str), _ptr(d_str_off), _ptr(self.d_counts),
-                                              _ptr(d_runs), _ptr(d_run_count), _ptr(d_status), n,
+                    N.check(lib.mrx_rle_parse(d_str, d_str_off, self.d_counts,
+                                              d_runs, d_run_count, d_status, n,
                                               R, st), "mrx_rle_parse")
-                N.check(lib.mrx_rle_decode(_ptr(d_runs), _ptr(d_run_off), _ptr(d_run_count),
-                                           _ptr(d_ends), _ptr(d_status), _ptr(self.d_counts),
-                                           _ptr(self.d_geom), _ptr(d_off), _ptr(d_packed), n, R,
+                N.check(lib.mrx_rle_decode(d_runs, d_run_off, d_run_count,
+                                           d_ends, d_status, self.d_counts,
+                                           self.d_geom, d_off, d_packed, n, R,
                                            max_h, max_w, st), "mrx_rle_decode")
             if poly:
                 d_vert, d_part_vert, d_part_inst, d_inst_part, d_part_col, d_part_tog = d_poly
@@ -813,10 +806,9 @@ class MaskBatch:
                 d_col_start = torch.empty((max(n_col, 1),), dtype=torch.int64, device=device)
                 d_carry = torch.empty((max(n_col, 1),), dtype=torch.uint8, device=device)
                 N.check(lib.mrx_poly_decode(
-                    _ptr(d_vert), _ptr(d_part_vert), _ptr(d_part_inst), _ptr(d_part_col),
-                    _ptr(d_part_tog), pp["P"], _ptr(d_inst_part), _ptr(d_tog), _ptr(d_col_start),
-                    _ptr(d_carry), _ptr(self.d_counts), _ptr(self.d_geom), _ptr(d_off),
-                    _ptr(d_packed), n, R, max_h, max_w, st), "mrx_poly_decode")
+                    d_vert, d_part_vert, d_part_inst, d_part_col, d_part_tog, pp["P"], d_inst_part,
+                    d_tog, d_col_start, d_carry, self.d_counts, self.d_geom, d_off, d_packed, n, R,
+                    max_h, max_w, st), "mrx_poly_decode")
 
         d_status, *_ = self._stage(lib, device, g, class_ids, pk["counts"],
                                    rle_extra + poly_extra, fill, stream)
@@ -853,9 +845,9 @@ class MaskBatch:
             fill(layout, d_packed, d_off, *d_extra)
             d_areas = torch.empty((n, R), dtype=torch.int64, device=device)
             d_ext = torch.empty((n, R, 4), dtype=torch.int32, device=device)
-            N.check(lib.mrx_mask_extents(_ptr(d_packed), _ptr(d_off), _ptr(self.d_counts),
-                                         _ptr(self.d_geom), _ptr(d_regions), _ptr(d_areas),
-                                         _ptr(d_ext), n, R, N.stream_ptr(stream)),
+            N.check(lib.mrx_mask_extents(d_packed, d_off, self.d_counts,
+                                         self.d_geom, d_regions, d_areas,
+                                         d_ext, n, R, N.stream_ptr(stream)),
                     "mrx_mask_extents")
         self.planes = Planes(d_packed, d_off, self.d_counts, d_areas, d_ext, R)
         self.d_regions = d_regions
@@ -1104,9 +1096,8 @@ def mask_overlaps(lib, p1, p2, d_geom, n, stream=None):
     below the image's counts (the rest is not written)."""
     d_out = _torch().empty((n, p1.R, p2.R), dtype=_torch().float32, device=d_geom.device)
     N.check(lib.mrx_mask_overlaps(
-        _ptr(p1.d_packed), _ptr(p1.d_packed_off), _ptr(p1.d_counts), _ptr(p1.d_areas),
-        _ptr(p1.d_extents), p1.R, _ptr(p2.d_packed), _ptr(p2.d_packed_off), _ptr(p2.d_counts),
-        _ptr(p2.d_areas), _ptr(p2.d_extents), p2.R, _ptr(d_geom), _ptr(d_out), n,
+        p1.d_packed, p1.d_packed_off, p1.d_counts, p1.d_areas, p1.d_extents, p1.R, p2.d_packed,
+        p2.d_packed_off, p2.d_counts, p2.d_areas, p2.d_extents, p2.R, d_geom, d_out, n,
         N.stream_ptr(stream)), "mrx_mask_overlaps")
     return d_out
 
@@ -1139,10 +1130,10 @@ def mask_matches(lib, d_overlaps, d_pred_counts, d_pred_class_ids, d_scores, sco
     for t0 in range(0, len(thr), N.MRX_MAX_IOU_THRESHOLDS):
         chunk = thr[t0:t0 + N.MRX_MAX_IOU_THRESHOLDS]
         N.check(lib.mrx_mask_matches(
-            _ptr(d_overlaps), _ptr(d_pred_counts), _ptr(d_pred_class_ids), _ptr(d_scores),
-            score_code, _ptr(gt.d_counts), _ptr(gt.d_class_ids), N.double_array(chunk), len(chunk),
-            C.c_double(comparison_threshold(score_threshold)), _ptr(d_order), _ptr(d_pm[t0]),
-            _ptr(d_gm[t0]), n, R1, R2, N.stream_ptr(stream)), "mrx_mask_matches")
+            d_overlaps, d_pred_counts, d_pred_class_ids, d_scores, score_code, gt.d_counts,
+            gt.d_class_ids, N.double_array(chunk), len(chunk),
+            comparison_threshold(score_threshold), d_order, d_pm[t0], d_gm[t0], n, R1, R2,
+            N.stream_ptr(stream)), "mrx_mask_matches")
     return d_order, d_pm, d_gm
 
 
@@ -1223,11 +1214,10 @@ def _segm_evaluate(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt_area
         def ious(v, d_iou, st):
             v["area"].copy_(pred.d_areas.view(-1)[:n * R1].view(n, R1))
             N.check(lib.mrx_coco_ious(
-                _ptr(pred.d_packed), _ptr(pred.d_packed_off), _ptr(pred.d_counts),
-                _ptr(pred.d_areas), _ptr(pred.d_extents), _ptr(v["cat"]), _ptr(v["keep"]), R1,
-                _ptr(gt.planes.d_packed), _ptr(gt.planes.d_packed_off), _ptr(gt.planes.d_counts),
-                _ptr(gt.planes.d_areas), _ptr(gt.planes.d_extents), _ptr(gt.d_class_ids),
-                _ptr(d_crowd), R2, _ptr(gt.d_geom), _ptr(d_iou), n, st), "mrx_coco_ious")
+                pred.d_packed, pred.d_packed_off, pred.d_counts, pred.d_areas, pred.d_extents,
+                v["cat"], v["keep"], R1, gt.planes.d_packed, gt.planes.d_packed_off,
+                gt.planes.d_counts, gt.planes.d_areas, gt.planes.d_extents, gt.d_class_ids,
+                d_crowd, R2, gt.d_geom, d_iou, n, st), "mrx_coco_ious")
 
         return _coco_evaluate(lib, n, R1, R2, pred.d_counts, pred_class_ids, pred_scores,
                               gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map, dparams,
@@ -1309,9 +1299,8 @@ def _box_evaluate(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_
 
         def ious(v, d_iou, st):
             N.check(lib.mrx_coco_box_ious(
-                _ptr(pred_boxes), form, _ptr(pred_counts), _ptr(v["cat"]), _ptr(v["keep"]), R1,
-                _ptr(d_boxes), _ptr(d_counts), _ptr(d_cat), _ptr(d_crowd), R2, _ptr(v["area"]),
-                _ptr(d_iou), n, st), "mrx_coco_box_ious")
+                pred_boxes, form, pred_counts, v["cat"], v["keep"], R1, d_boxes, d_counts, d_cat,
+                d_crowd, R2, v["area"], d_iou, n, st), "mrx_coco_box_ious")
 
         return _coco_evaluate(lib, n, R1, R2, pred_counts, pred_class_ids, pred_scores, d_counts,
                               d_cat, d_crowd, d_area, d_map, dparams, np.float64, ious, stream,
@@ -1351,12 +1340,12 @@ def mask_boundary_planes(lib, planes, d_geom, d_regions, d_dilation, n, max_w, b
     d_ext = _buffer(bufs, name + "_extents", n * R * 4, torch.int32, dev)
     st = N.stream_ptr(stream)
     N.check(lib.mrx_mask_boundary(
-        _ptr(planes.d_packed), _ptr(planes.d_packed_off), _ptr(planes.d_counts), _ptr(d_geom),
-        _ptr(d_regions), _ptr(d_dilation), _ptr(d_bnd), n, R, max(int(max_w), 1), st),
+        planes.d_packed, planes.d_packed_off, planes.d_counts, d_geom, d_regions, d_dilation,
+        d_bnd, n, R, max(int(max_w), 1), st),
         "mrx_mask_boundary")
     N.check(lib.mrx_mask_extents(
-        _ptr(d_bnd), _ptr(planes.d_packed_off), _ptr(planes.d_counts), _ptr(d_geom),
-        _ptr(d_regions), _ptr(d_areas), _ptr(d_ext), n, R, st), "mrx_mask_extents")
+        d_bnd, planes.d_packed_off, planes.d_counts, d_geom, d_regions, d_areas, d_ext, n, R,
+        st), "mrx_mask_extents")
     return Planes(d_bnd, planes.d_packed_off, planes.d_counts, d_areas[:n * R].view(n, R),
                   d_ext[:n * R * 4].view(n, R, 4), R)
 
@@ -1389,13 +1378,11 @@ def coco_boundary_evaluate_batch(lib, pred, pred_regions, pred_class_ids, pred_s
             bg = mask_boundary_planes(lib, gt.planes, gt.d_geom, gt.d_regions, d_dil, n, max_w,
                                       bufs, stream, "gt_boundary")
             N.check(lib.mrx_coco_boundary_ious(
-                _ptr(pred.d_packed), _ptr(pred.d_packed_off), _ptr(pred.d_counts),
-                _ptr(pred.d_areas), _ptr(pred.d_extents), _ptr(bp.d_packed), _ptr(bp.d_areas),
-                _ptr(v["cat"]), _ptr(v["keep"]), R1,
-                _ptr(gt.planes.d_packed), _ptr(gt.planes.d_packed_off), _ptr(gt.planes.d_counts),
-                _ptr(gt.planes.d_areas), _ptr(gt.planes.d_extents), _ptr(bg.d_packed),
-                _ptr(bg.d_areas), _ptr(gt.d_class_ids), _ptr(d_crowd), R2, _ptr(gt.d_geom),
-                _ptr(d_iou), n, st), "mrx_coco_boundary_ious")
+                pred.d_packed, pred.d_packed_off, pred.d_counts, pred.d_areas, pred.d_extents,
+                bp.d_packed, bp.d_areas, v["cat"], v["keep"], R1, gt.planes.d_packed,
+                gt.planes.d_packed_off, gt.planes.d_counts, gt.planes.d_areas,
+                gt.planes.d_extents, bg.d_packed, bg.d_areas, gt.d_class_ids, d_crowd, R2,
+                gt.d_geom, d_iou, n, st), "mrx_coco_boundary_ious")
 
         return _coco_evaluate(lib, n, R1, R2, pred.d_counts, pred_class_ids, pred_scores,
                               gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map,
@@ -1436,21 +1423,19 @@ def _coco_evaluate(lib, n, R1, R2, d_pred_counts, pred_class_ids, pred_scores, d
     v["score"].copy_(pred_scores[:n])
     if d_status is None:
         N.check(lib.mrx_coco_ranks(
-            _ptr(pred_class_ids), _ptr(pred_scores), score_code, _ptr(d_pred_counts), _ptr(d_map),
-            int(d_map.numel()), max_det, _ptr(v["cat"]), _ptr(v["rank"]), _ptr(v["keep"]),
-            _ptr(d_walk), n, R1, st), "mrx_coco_ranks")
+            pred_class_ids, pred_scores, score_code, d_pred_counts, d_map, int(d_map.numel()),
+            max_det, v["cat"], v["rank"], v["keep"], d_walk, n, R1, st), "mrx_coco_ranks")
     else:
         N.check(lib.mrx_lvis_ranks(
-            _ptr(pred_class_ids), _ptr(pred_scores), score_code, _ptr(d_pred_counts), _ptr(d_map),
-            int(d_map.numel()), _ptr(d_status), int(d_status.shape[1]), max_det, _ptr(v["cat"]),
-            _ptr(v["rank"]), _ptr(v["keep"]), _ptr(d_walk), n, R1, st), "mrx_lvis_ranks")
+            pred_class_ids, pred_scores, score_code, d_pred_counts, d_map, int(d_map.numel()),
+            d_status, int(d_status.shape[1]), max_det, v["cat"], v["rank"], v["keep"], d_walk, n,
+            R1, st), "mrx_lvis_ranks")
     ious(v, d_iou, st)
     match = {np.dtype(np.int64): "mrx_coco_match",
              np.dtype(np.float64): "mrx_coco_match_f64area"}[np.dtype(area_dtype)]
     N.check(getattr(lib, match)(
-        _ptr(d_iou), _ptr(d_pred_counts), _ptr(v["cat"]), _ptr(v["keep"]), _ptr(d_walk),
-        _ptr(v["area"]), _ptr(d_gt_counts), _ptr(d_gt_cat), _ptr(d_crowd), _ptr(d_area),
-        N.double_array(thr), T, N.double_array(rng), A, _ptr(v["match"]), _ptr(v["ignore"]),
+        d_iou, d_pred_counts, v["cat"], v["keep"], d_walk, v["area"], d_gt_counts, d_gt_cat,
+        d_crowd, d_area, N.double_array(thr), T, N.double_array(rng), A, v["match"], v["ignore"],
         n, R1, R2, st), match)
     host = d_out.cpu().numpy()         # the one synchronisation
     out = dict(zip(parts, _part_views(host, specs)))
@@ -1486,8 +1471,7 @@ def _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom
     ni = n * R
     d_rows = _buffer(bufs, "rows", ni * (max_h + 1), torch.int32, device)
     d_inst = _buffer(bufs, "inst", ni + 1, torch.int64, device)
-    args = (_ptr(d_packed), _ptr(d_packed_off), _ptr(d_counts), _ptr(d_geom), _ptr(d_regions),
-            _ptr(d_rows), _ptr(d_inst))
+    args = (d_packed, d_packed_off, d_counts, d_geom, d_regions, d_rows, d_inst)
     N.check(lib.mrx_contours_count(*args, n, R, max_h, st), "mrx_contours_count")
     seg_off = d_inst[:ni + 1].cpu().numpy()     # how many segments: sizes every output
     S = int(seg_off[-1])
@@ -1499,8 +1483,8 @@ def _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom
     d_vert = _buffer(bufs, "vertices", 2 * (S + S // 4), torch.float32, device)
     d_coff = _buffer(bufs, "contour_off", S // 4 + 1, torch.int64, device)
     d_icoff = _buffer(bufs, "inst_contour_off", ni + 1, torch.int64, device)
-    N.check(lib.mrx_contours_write(*args, C.c_longlong(S), C.c_longlong(smax), _ptr(d_scr),
-                                   _ptr(d_vert), _ptr(d_coff), _ptr(d_icoff), n, R, max_h, st),
+    N.check(lib.mrx_contours_write(*args, S, smax, d_scr, d_vert, d_coff, d_icoff, n, R, max_h,
+                                   st),
             "mrx_contours_write")
     icoff = d_icoff[:ni + 1].cpu().numpy()
     n_contours = int(icoff[-1])
@@ -1556,7 +1540,7 @@ class AnchorGenerator:
         if out is None:
             out = torch.empty((A, 4), dtype=torch.float32, device=self.device)
         N.check(self.lib.mrx_anchors(
-            _ptr(out), int(image_shape[0]), int(image_shape[1]),
+            out, int(image_shape[0]), int(image_shape[1]),
             N.double_array(self.scales), N.double_array(self.ratios),
             N.int_array(self.strides), len(self.strides), len(self.ratios),
             self.anchor_stride, N.stream_ptr(stream)), "mrx_anchors")
@@ -1631,7 +1615,7 @@ class Molder:
         sh, sw = int(d_img.shape[0]), int(d_img.shape[1])
         dh, dw = int(size_hw[0]), int(size_hw[1])
         out = torch.empty((dh, dw, 3), dtype=torch.uint8, device=self.device)
-        N.check(self.lib.mrx_cv2_resize_u8c3(_ptr(d_img), sh, sw, _ptr(out), dh, dw,
+        N.check(self.lib.mrx_cv2_resize_u8c3(d_img, sh, sw, out, dh, dw,
                                              N.stream_ptr(stream)), "mrx_cv2_resize_u8c3")
         return out
 
@@ -1649,9 +1633,8 @@ class Molder:
             else None
         mean = [float(v) for v in np.asarray(cfg.MEAN_PIXEL, dtype=np.float64)]
         N.check(self.lib.mrx_mold_image(
-            _ptr(d_img), h, w, nh, nw, top, left, oh, ow, N.double_array(mean),
-            _dtype_code(out_dtype), _ptr(out),
-            _ptr(u8) if u8 is not None else C.c_void_p(0), N.stream_ptr(stream)),
+            d_img, h, w, nh, nw, top, left, oh, ow, N.double_array(mean),
+            _dtype_code(out_dtype), out, u8, N.stream_ptr(stream)),
             "mrx_mold_image")
         return out, u8, window, scale, padding
 
@@ -1694,9 +1677,9 @@ class Molder:
         d_coef = self._jpeg_buffer("coef", plan.coef_blocks * 64, torch.int16)
         d_status = self._jpeg_buffer("status", plan.B, torch.int32)
         N.check(self.lib.mrx_jpeg_coefficients(
-            _ptr(d_files), _ptr(d_desc), _ptr(d_tabs), _ptr(d_unit_img), plan.B,
-            max(plan.units, 1), plan.S, plan.max_subs, _ptr(d_unst), _ptr(d_work), _ptr(d_coef),
-            plan.coef_blocks, _ptr(d_status), N.stream_ptr(stream)), "mrx_jpeg_coefficients")
+            d_files, d_desc, d_tabs, d_unit_img, plan.B,
+            max(plan.units, 1), plan.S, plan.max_subs, d_unst, d_work, d_coef,
+            plan.coef_blocks, d_status, N.stream_ptr(stream)), "mrx_jpeg_coefficients")
         return d_coef[:plan.coef_blocks * 64].view(-1, 64), d_status[:plan.B], up
 
     def jpeg_decode_into(self, plan, d_out, out_off, stream=None):
@@ -1709,8 +1692,8 @@ class Molder:
         d_off = torch.from_numpy(np.ascontiguousarray(out_off, dtype=np.int64)).to(
             self.device, non_blocking=True)
         N.check(self.lib.mrx_jpeg_pixels(
-            _ptr(d_desc), _ptr(d_tabs), _ptr(d_coef), _ptr(d_status), plan.B, plan.max_blocks,
-            plan.max_pixels, _ptr(d_planes), _ptr(d_out), _ptr(d_off), N.stream_ptr(stream)),
+            d_desc, d_tabs, d_coef, d_status, plan.B, plan.max_blocks,
+            plan.max_pixels, d_planes, d_out, d_off, N.stream_ptr(stream)),
             "mrx_jpeg_pixels")
         return d_status
 
@@ -1789,7 +1772,7 @@ class Molder:
         d_hw = torch.from_numpy(hw).to(self.device)
         out = torch.empty((B, dh, dw, 3), dtype=torch.uint8, device=self.device)
         N.check(self.lib.mrx_cv2_resize_u8c3_batch(
-            _ptr(d_src), _ptr(d_off), _ptr(d_hw), _ptr(out), B, dh, dw, N.stream_ptr(stream)),
+            d_src, d_off, d_hw, out, B, dh, dw, N.stream_ptr(stream)),
             "mrx_cv2_resize_u8c3_batch")
         if d_status is not None:
             self.jpeg_check(d_status, jidx)
@@ -1811,8 +1794,8 @@ class Molder:
         out = torch.empty((B, oh, ow, 3), dtype=_torch_dtype(out_dtype), device=self.device)
         mean = [float(v) for v in np.asarray(cfg.MEAN_PIXEL, dtype=np.float64)]
         N.check(self.lib.mrx_mold_image_batch(
-            _ptr(d_imgs), B, h, w, nh, nw, top, left, oh, ow, N.double_array(mean),
-            _dtype_code(out_dtype), _ptr(out), C.c_void_p(0), N.stream_ptr(stream)),
+            d_imgs, B, h, w, nh, nw, top, left, oh, ow, N.double_array(mean),
+            _dtype_code(out_dtype), out, None, N.stream_ptr(stream)),
             "mrx_mold_image_batch")
         return out, window, scale, padding
 

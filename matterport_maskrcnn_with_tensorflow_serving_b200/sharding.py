@@ -235,7 +235,7 @@ class PeerGather:
         handle, err = [None], None
         try:
             if self._owner:
-                N.check(self.lib.mrx_peer_alloc(C.c_ulonglong(self.total), C.byref(self._base)),
+                N.check(self.lib.mrx_peer_alloc(self.total, C.byref(self._base)),
                         "mrx_peer_alloc")
                 buf = C.create_string_buffer(N.MRX_PEER_HANDLE_BYTES)
                 N.check(self.lib.mrx_peer_export(self._base, buf), "mrx_peer_export")
@@ -288,17 +288,16 @@ class PeerGather:
     def signal(self, stream=None):
         """After everything queued on `stream`: tell dst that this rank's bytes have landed."""
         N = self.N
-        N.check(self.lib.mrx_peer_signal(C.c_void_p(self.base + 4 * self.rank),
-                                         C.c_uint(self.epoch), N.stream_ptr(stream)),
-                "mrx_peer_signal")
+        N.check(self.lib.mrx_peer_signal(self.base + 4 * self.rank, self.epoch,
+                                         N.stream_ptr(stream)), "mrx_peer_signal")
 
     def wait(self, stream=None):
         """dst only: `stream` proceeds once every rank has signalled the current epoch."""
         if not self._owner:
             return
         N = self.N
-        N.check(self.lib.mrx_peer_wait(C.c_void_p(self.base), self.world, C.c_uint(self.epoch),
-                                       N.stream_ptr(stream)), "mrx_peer_wait")
+        N.check(self.lib.mrx_peer_wait(self.base, self.world, self.epoch, N.stream_ptr(stream)),
+                "mrx_peer_wait")
 
     def close(self):
         import torch

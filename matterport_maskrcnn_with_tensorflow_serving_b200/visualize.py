@@ -15,7 +15,6 @@ captions and contours are NOT drawn (matplotlib rendering is out of scope, DESIG
 from __future__ import annotations
 
 import colorsys
-import ctypes as C
 import random as _random
 
 import numpy as np
@@ -41,10 +40,6 @@ def blend_table(colors, alpha, R):
         for c in range(3):
             tab[i, c] = alpha * float(col[c]) * 255
     return tab
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
 
 
 def _is_triple(x):
@@ -93,10 +88,8 @@ class CompositeStage:
         eng = self.engine
         B = eng.layout.n
         N.check(self.lib.mrx_composite_masks(
-            _ptr(eng.d_canvas), _ptr(eng.d_canvas_off), _ptr(eng.d_counts),
-            _ptr(eng.d_geom), _ptr(eng.d_boxes), _ptr(self.d_in), _ptr(self.d_off),
-            _ptr(self.d_tab), C.c_double(1 - self.alpha),
-            _ptr(self.d_out), B, eng.R, C.c_longlong(self.max_px),
+            eng.d_canvas, eng.d_canvas_off, eng.d_counts, eng.d_geom, eng.d_boxes, self.d_in,
+            self.d_off, self.d_tab, 1 - self.alpha, self.d_out, B, eng.R, self.max_px,
             N.stream_ptr(stream)), "mrx_composite_masks")
         offs = self.offs
         return [self.d_out[int(offs[b]):int(offs[b + 1])].view(*self.layout.hw(b), 3)
@@ -155,9 +148,8 @@ def apply_masks(image, boxes, masks, colors, alpha=0.5):
     d_out = torch.empty_like(d_img)
     d_tab = torch.from_numpy(blend_table(colors, alpha, n)).to(dev)
     N.check(lib.mrx_composite_masks(
-        _ptr(d_canvas), _ptr(d_off), _ptr(d_counts), _ptr(d_geom), _ptr(d_boxes), _ptr(d_img),
-        _ptr(d_off), _ptr(d_tab), C.c_double(1 - alpha), _ptr(d_out), 1, n,
-        C.c_longlong(H * W), N.stream_ptr(None)), "mrx_composite_masks")
+        d_canvas, d_off, d_counts, d_geom, d_boxes, d_img, d_off, d_tab, 1 - alpha, d_out, 1, n,
+        H * W, N.stream_ptr(None)), "mrx_composite_masks")
     return d_out.cpu().numpy()
 
 
@@ -181,9 +173,8 @@ def mask_contours(boxes, masks):
     layout, dev, d_canvas, d_off, d_counts, d_geom = _stage_masks(
         np.ascontiguousarray(masks).astype(np.bool_, copy=False).view(np.uint8), H, W, n)
     d_packed = torch.empty(int(layout.packed_off[-1]), dtype=torch.uint8, device=dev)
-    N.check(lib.mrx_pack_masks(_ptr(d_canvas), _ptr(d_off), _ptr(d_counts), _ptr(d_geom),
-                               _ptr(d_packed), _ptr(d_off), 1, n, H, W, N.stream_ptr(None)),
-            "mrx_pack_masks")
+    N.check(lib.mrx_pack_masks(d_canvas, d_off, d_counts, d_geom, d_packed, d_off, 1, n, H, W,
+                               N.stream_ptr(None)), "mrx_pack_masks")
     # the whole image, or nothing for an all-zero box (display_instances skips those)
     regions = np.zeros((n, 4), dtype=np.int32)
     regions[boxes.reshape(n, -1).any(axis=1)] = (0, 0, H, W)

@@ -69,10 +69,9 @@ def test_lvis_ranks_equal_the_cut_and_filter(cuda_device, case):
     keep = torch.full((B, R), 9, dtype=torch.uint8, device=dev)
     lib = N.load()
     N.check(lib.mrx_lvis_ranks(
-        d["cls"].data_ptr(), d["scores"].data_ptr(), N.MRX_F64 if sdt == np.float64 else N.MRX_F32,
-        d["counts"].data_ptr(), d["map"].data_ptr(), C, d["status"].data_ptr(), K, max_det,
-        out["cat"].data_ptr(), out["rank"].data_ptr(), keep.data_ptr(), out["walk"].data_ptr(), B,
-        R, N.stream_ptr(None)), "mrx_lvis_ranks")
+        d["cls"], d["scores"], N.MRX_F64 if sdt == np.float64 else N.MRX_F32, d["counts"],
+        d["map"], C, d["status"], K, max_det, out["cat"], out["rank"], keep, out["walk"], B, R,
+        N.stream_ptr(None)), "mrx_lvis_ranks")
     got = {k: v.cpu().numpy() for k, v in out.items()}
     got_keep = keep.cpu().numpy()
     kept_at_cut = 0

@@ -93,10 +93,8 @@ def test_pack_masks_refuses_before_writing(cuda_device):
         d_counts = torch.tensor(counts, dtype=torch.int32, device=dev)
         d_geom = torch.from_numpy(layout.geom).to(dev)
         d_packed = torch.full((int(layout.packed_off[-1]),), 0xAA, dtype=torch.uint8, device=dev)
-        ptr = lambda t: C.c_void_p(t.data_ptr())   # noqa: E731
-        rc = lib.mrx_pack_masks(ptr(d_canvas), ptr(d_canvas_off), ptr(d_counts), ptr(d_geom),
-                                ptr(d_packed), ptr(d_packed_off), 2, R, 16, 16,
-                                N.stream_ptr(None))
+        rc = lib.mrx_pack_masks(d_canvas, d_canvas_off, d_counts, d_geom, d_packed, d_packed_off,
+                                2, R, 16, 16, N.stream_ptr(None))
         assert rc == status, (R, lib.mrx_last_error())
         packed = d_packed.cpu().numpy()
         if status:

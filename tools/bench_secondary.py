@@ -8,7 +8,6 @@ each unmold workload also names the GPU and its power limit.
                                   | --only-polygons | --only-lvis | --only-jpeg
 """
 import argparse
-import ctypes as C
 import json
 import os
 import subprocess
@@ -129,12 +128,11 @@ def rle_strings_record(eng, d_runs, off, masks, iters):
     d_inst_off = torch.from_numpy(off).to(eng.device)
     d_str = torch.empty((N.rle_string_bound(off[-1], ni),), dtype=torch.uint8, device=eng.device)
     d_str_off = torch.empty((ni + 1,), dtype=torch.int64, device=eng.device)
-    args = [C.c_void_p(t.data_ptr()) for t in (d_runs, d_inst_off, eng.d_counts)]
+    args = (d_runs, d_inst_off, eng.d_counts)
 
     def strings():
-        N.check(eng.lib.mrx_rle_strings(*args, eng._n_images, eng.R, C.c_void_p(d_str_off.data_ptr()),
-                                        C.c_void_p(d_str.data_ptr()), N.stream_ptr(None)),
-                "mrx_rle_strings")
+        N.check(eng.lib.mrx_rle_strings(*args, eng._n_images, eng.R, d_str_off, d_str,
+                                        N.stream_ptr(None)), "mrx_rle_strings")
 
     def strings_downloaded():
         s, s_off = eng.enqueue_rle_strings()
@@ -183,9 +181,9 @@ def eval_case(iters, cpu):
     area_buf, ext_buf = eng._eval_bufs["areas"], eng._eval_bufs["extents"]
 
     def extents():
-        N.check(lib.mrx_mask_extents(*(C.c_void_p(t.data_ptr()) for t in (
-            eng.d_packed, eng.d_packed_off, eng.d_counts, eng.d_geom, eng.d_boxes, area_buf,
-            ext_buf)), n, R, N.stream_ptr(None)), "mrx_mask_extents")
+        N.check(lib.mrx_mask_extents(eng.d_packed, eng.d_packed_off, eng.d_counts, eng.d_geom,
+                                     eng.d_boxes, area_buf, ext_buf, n, R, N.stream_ptr(None)),
+                "mrx_mask_extents")
 
     ext_ms, _ = time_ms(extents, iters)
     ov_ms, _ = time_ms(lambda: eng.enqueue_overlaps(gt), iters)
@@ -291,7 +289,6 @@ def cocoeval_case(iters, n_batches=4):
     thr, rngs, max_det = coco_device_params(ev.params)
     n, R1, R2, T, A = batch, eng.R, gt.R, len(thr), len(rngs) // 2
     dev = eng.device
-    P = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
     d_map = torch.arange(81, dtype=torch.int32, device=dev)
     d_cat = torch.empty((n, R1), dtype=torch.int32, device=dev)
     d_rank, d_walk = torch.empty_like(d_cat), torch.empty_like(d_cat)
@@ -304,17 +301,17 @@ def cocoeval_case(iters, n_batches=4):
     d_iou = res["d_iou"]
     st = N.stream_ptr(None)
     ranks = lambda: N.check(eng.lib.mrx_coco_ranks(  # noqa: E731
-        P(eng.d_class_ids), P(eng.d_scores), N.MRX_F32, P(eng.d_counts), P(d_map), 81, max_det,
-        P(d_cat), P(d_rank), P(d_keep), P(d_walk), n, R1, st), "mrx_coco_ranks")
+        eng.d_class_ids, eng.d_scores, N.MRX_F32, eng.d_counts, d_map, 81, max_det,
+        d_cat, d_rank, d_keep, d_walk, n, R1, st), "mrx_coco_ranks")
     ious = lambda: N.check(eng.lib.mrx_coco_ious(  # noqa: E731
-        P(eng.d_packed), P(eng.d_packed_off), P(eng.d_counts), P(d_pa),
-        P(eng._eval_bufs["extents"]), P(d_cat), P(d_keep), R1, P(gt.planes.d_packed),
-        P(gt.planes.d_packed_off), P(gt.d_counts), P(gt.planes.d_areas), P(gt.planes.d_extents),
-        P(gt.d_class_ids), P(d_crowd), R2, P(gt.d_geom), P(d_iou), n, st), "mrx_coco_ious")
+        eng.d_packed, eng.d_packed_off, eng.d_counts, d_pa,
+        eng._eval_bufs["extents"], d_cat, d_keep, R1, gt.planes.d_packed,
+        gt.planes.d_packed_off, gt.d_counts, gt.planes.d_areas, gt.planes.d_extents,
+        gt.d_class_ids, d_crowd, R2, gt.d_geom, d_iou, n, st), "mrx_coco_ious")
     match = lambda: N.check(eng.lib.mrx_coco_match(  # noqa: E731
-        P(d_iou), P(eng.d_counts), P(d_cat), P(d_keep), P(d_walk), P(d_pa), P(gt.d_counts),
-        P(gt.d_class_ids), P(d_crowd), P(d_area), N.double_array(thr), T, N.double_array(rngs), A,
-        P(d_match), P(d_ign), n, R1, R2, st), "mrx_coco_match")
+        d_iou, eng.d_counts, d_cat, d_keep, d_walk, d_pa, gt.d_counts,
+        gt.d_class_ids, d_crowd, d_area, N.double_array(thr), T, N.double_array(rngs), A,
+        d_match, d_ign, n, R1, R2, st), "mrx_coco_match")
     ranks()
     rank_ms, _ = time_ms(ranks, iters)
     iou_ms, _ = time_ms(ious, iters)
@@ -429,7 +426,6 @@ def bboxeval_case(iters, n_batches=4):
     thr, rngs, max_det = coco_device_params(ev.params)
     n, R1, R2, T, A = batch, eng.R, g_cat.shape[1], len(thr), len(rngs) // 2
     dev = eng.device
-    P = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
     d_map = torch.from_numpy(ev._class_map(81, None)).to(dev)
     d_cat = torch.empty((n, R1), dtype=torch.int32, device=dev)
     d_rank, d_walk = torch.empty_like(d_cat), torch.empty_like(d_cat)
@@ -443,15 +439,15 @@ def bboxeval_case(iters, n_batches=4):
     d_iou = res["d_iou"]
     st = N.stream_ptr(None)
     ranks = lambda: N.check(eng.lib.mrx_coco_ranks(  # noqa: E731
-        P(eng.d_class_ids), P(eng.d_scores), N.MRX_F32, P(eng.d_counts), P(d_map), 81, max_det,
-        P(d_cat), P(d_rank), P(d_keep), P(d_walk), n, R1, st), "mrx_coco_ranks")
+        eng.d_class_ids, eng.d_scores, N.MRX_F32, eng.d_counts, d_map, 81, max_det,
+        d_cat, d_rank, d_keep, d_walk, n, R1, st), "mrx_coco_ranks")
     ious = lambda: N.check(eng.lib.mrx_coco_box_ious(  # noqa: E731
-        P(eng.d_boxes), N.MRX_BOX_YXYX_I32, P(eng.d_counts), P(d_cat), P(d_keep), R1, P(d_gbox),
-        P(d_gcount), P(d_gcat), P(d_crowd), R2, P(d_pa), P(d_iou), n, st), "mrx_coco_box_ious")
+        eng.d_boxes, N.MRX_BOX_YXYX_I32, eng.d_counts, d_cat, d_keep, R1, d_gbox,
+        d_gcount, d_gcat, d_crowd, R2, d_pa, d_iou, n, st), "mrx_coco_box_ious")
     match = lambda: N.check(eng.lib.mrx_coco_match_f64area(  # noqa: E731
-        P(d_iou), P(eng.d_counts), P(d_cat), P(d_keep), P(d_walk), P(d_pa), P(d_gcount),
-        P(d_gcat), P(d_crowd), P(d_area), N.double_array(thr), T, N.double_array(rngs), A,
-        P(d_match), P(d_ign), n, R1, R2, st), "mrx_coco_match_f64area")
+        d_iou, eng.d_counts, d_cat, d_keep, d_walk, d_pa, d_gcount,
+        d_gcat, d_crowd, d_area, N.double_array(thr), T, N.double_array(rngs), A,
+        d_match, d_ign, n, R1, R2, st), "mrx_coco_match_f64area")
     ranks()
     rank_ms, _ = time_ms(ranks, iters)
     iou_ms, _ = time_ms(ious, iters)
@@ -546,7 +542,6 @@ def boundaryeval_case(iters, n_batches=4):
     thr, rngs, max_det = coco_device_params(ev.params)
     n, R1, R2 = batch, eng.R, gt.R
     dev = eng.device
-    P = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
     bufs = eng._eval_bufs
     d_dil = torch.from_numpy(boundary_dilation(eng.layout.geom, 0.02)).to(dev)
     d_map = torch.arange(81, dtype=torch.int32, device=dev)
@@ -558,22 +553,22 @@ def boundaryeval_case(iters, n_batches=4):
     st = N.stream_ptr(None)
     max_w = eng.layout.max_w
     N.check(eng.lib.mrx_coco_ranks(
-        P(eng.d_class_ids), P(eng.d_scores), N.MRX_F32, P(eng.d_counts), P(d_map), 81, max_det,
-        P(d_cat), P(d_rank), P(d_keep), P(d_walk), n, R1, st), "mrx_coco_ranks")
+        eng.d_class_ids, eng.d_scores, N.MRX_F32, eng.d_counts, d_map, 81, max_det,
+        d_cat, d_rank, d_keep, d_walk, n, R1, st), "mrx_coco_ranks")
     pred_bnd = lambda: N.check(eng.lib.mrx_mask_boundary(  # noqa: E731
-        P(eng.d_packed), P(eng.d_packed_off), P(eng.d_counts), P(eng.d_geom), P(eng.d_boxes),
-        P(d_dil), P(bufs["pred_boundary_packed"]), n, R1, max_w, st), "mrx_mask_boundary")
+        eng.d_packed, eng.d_packed_off, eng.d_counts, eng.d_geom, eng.d_boxes,
+        d_dil, bufs["pred_boundary_packed"], n, R1, max_w, st), "mrx_mask_boundary")
     gt_bnd = lambda: N.check(eng.lib.mrx_mask_boundary(  # noqa: E731
-        P(gt.planes.d_packed), P(gt.planes.d_packed_off), P(gt.d_counts), P(gt.d_geom),
-        P(gt.d_regions), P(d_dil), P(bufs["gt_boundary_packed"]), n, R2, max_w, st),
+        gt.planes.d_packed, gt.planes.d_packed_off, gt.d_counts, gt.d_geom,
+        gt.d_regions, d_dil, bufs["gt_boundary_packed"], n, R2, max_w, st),
         "mrx_mask_boundary")
     ious = lambda: N.check(eng.lib.mrx_coco_boundary_ious(  # noqa: E731
-        P(eng.d_packed), P(eng.d_packed_off), P(eng.d_counts), P(bufs["areas"]),
-        P(bufs["extents"]), P(bufs["pred_boundary_packed"]), P(bufs["pred_boundary_areas"]),
-        P(d_cat), P(d_keep), R1, P(gt.planes.d_packed), P(gt.planes.d_packed_off),
-        P(gt.d_counts), P(gt.planes.d_areas), P(gt.planes.d_extents),
-        P(bufs["gt_boundary_packed"]), P(bufs["gt_boundary_areas"]), P(gt.d_class_ids),
-        P(d_crowd), R2, P(gt.d_geom), P(d_iou), n, st), "mrx_coco_boundary_ious")
+        eng.d_packed, eng.d_packed_off, eng.d_counts, bufs["areas"],
+        bufs["extents"], bufs["pred_boundary_packed"], bufs["pred_boundary_areas"],
+        d_cat, d_keep, R1, gt.planes.d_packed, gt.planes.d_packed_off,
+        gt.d_counts, gt.planes.d_areas, gt.planes.d_extents,
+        bufs["gt_boundary_packed"], bufs["gt_boundary_areas"], gt.d_class_ids,
+        d_crowd, R2, gt.d_geom, d_iou, n, st), "mrx_coco_boundary_ious")
     pred_ms, _ = time_ms(pred_bnd, iters)
     gt_ms, _ = time_ms(gt_bnd, iters)
     iou_ms, _ = time_ms(ious, iters)
@@ -647,21 +642,20 @@ def rle_gt_record(eng, gts, base_rle, base_n, items, thr10, iters):
     d_regions = up(regions)
     d_areas = torch.empty((n, R), dtype=torch.int64, device=dev)
     d_ext = torch.empty((n, R, 4), dtype=torch.int32, device=dev)
-    p = lambda t: C.c_void_p(t.data_ptr())   # noqa: E731
     st = N.stream_ptr(None)
 
     def parse():
-        N.check(lib.mrx_rle_parse(p(d_str), p(d_str_off), p(d_counts), p(d_runs), p(d_run_count),
-                                  p(d_status), n, R, st), "mrx_rle_parse")
+        N.check(lib.mrx_rle_parse(d_str, d_str_off, d_counts, d_runs, d_run_count,
+                                  d_status, n, R, st), "mrx_rle_parse")
 
     def decode():
-        N.check(lib.mrx_rle_decode(p(d_runs), p(d_run_off), p(d_run_count), p(d_ends), p(d_status),
-                                   p(d_counts), p(d_geom), p(d_off), p(d_packed), n, R,
+        N.check(lib.mrx_rle_decode(d_runs, d_run_off, d_run_count, d_ends, d_status,
+                                   d_counts, d_geom, d_off, d_packed, n, R,
                                    layout.max_h, layout.max_w, st), "mrx_rle_decode")
 
     def extents():
-        N.check(lib.mrx_mask_extents(p(d_packed), p(d_off), p(d_counts), p(d_geom), p(d_regions),
-                                     p(d_areas), p(d_ext), n, R, st), "mrx_mask_extents")
+        N.check(lib.mrx_mask_extents(d_packed, d_off, d_counts, d_geom, d_regions,
+                                     d_areas, d_ext, n, R, st), "mrx_mask_extents")
 
     parse_ms, _ = time_ms(parse, iters)
     decode_ms, _ = time_ms(decode, iters)
@@ -741,14 +735,13 @@ def polygons_case(iters):
         d_tog = torch.empty((int(pp["part_tog"][-1]),), dtype=torch.int32, device=dev)
         d_cs = torch.empty((int(pp["part_col"][-1]),), dtype=torch.int64, device=dev)
         d_cy = torch.empty((int(pp["part_col"][-1]),), dtype=torch.uint8, device=dev)
-        p = lambda x: C.c_void_p(x.data_ptr())   # noqa: E731
         g = np.asarray(geoms)
         pl = gt.planes
 
         def run():
-            N.check(lib.mrx_poly_decode(p(t[0]), p(t[1]), p(t[2]), p(t[3]), p(t[4]), pp["P"],
-                                        p(t[5]), p(d_tog), p(d_cs), p(d_cy), p(pl.d_counts),
-                                        p(gt.d_geom), p(pl.d_packed_off), p(pl.d_packed), len(g),
+            N.check(lib.mrx_poly_decode(t[0], t[1], t[2], t[3], t[4], pp["P"],
+                                        t[5], d_tog, d_cs, d_cy, pl.d_counts,
+                                        gt.d_geom, pl.d_packed_off, pl.d_packed, len(g),
                                         gt.R, int(g[:, 0].max()), int(g[:, 1].max()),
                                         N.stream_ptr(None)), "mrx_poly_decode")
         ms, _ = time_ms(run, iters)
@@ -886,7 +879,6 @@ def lvis_case(iters, n_batches=4, batch=32, R=300):
     thr, rngs, max_det = lvis_device_params(ev.params)
     n, R1, R2, T, A = batch, eng.R, gt.R, len(thr), len(rngs) // 2
     dev = eng.device
-    P = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
     d_cls = torch.from_numpy(lvis_cls).to(dev)
     d_map = torch.arange(-1, K, dtype=torch.int32, device=dev)      # category id -> dense
     d_status = torch.from_numpy(status).to(dev)
@@ -900,18 +892,18 @@ def lvis_case(iters, n_batches=4, batch=32, R=300):
     d_iou = torch.empty((n, R1, R2), dtype=torch.float64, device=dev)
     st = N.stream_ptr(None)
     ranks = lambda: N.check(eng.lib.mrx_lvis_ranks(  # noqa: E731
-        P(d_cls), P(eng.d_scores), N.MRX_F32, P(eng.d_counts), P(d_map), K + 1, P(d_status), K,
-        max_det, P(d_cat), P(d_rank), P(d_keep), P(d_walk), n, R1, st), "mrx_lvis_ranks")
+        d_cls, eng.d_scores, N.MRX_F32, eng.d_counts, d_map, K + 1, d_status, K,
+        max_det, d_cat, d_rank, d_keep, d_walk, n, R1, st), "mrx_lvis_ranks")
     ious = lambda: N.check(eng.lib.mrx_coco_ious(  # noqa: E731
-        P(pred.d_packed), P(pred.d_packed_off), P(pred.d_counts), P(pred.d_areas),
-        P(pred.d_extents), P(d_cat), P(d_keep), R1, P(gt.planes.d_packed),
-        P(gt.planes.d_packed_off), P(gt.planes.d_counts), P(gt.planes.d_areas),
-        P(gt.planes.d_extents), P(gt.d_class_ids), P(d_crowd), R2, P(gt.d_geom), P(d_iou), n,
+        pred.d_packed, pred.d_packed_off, pred.d_counts, pred.d_areas,
+        pred.d_extents, d_cat, d_keep, R1, gt.planes.d_packed,
+        gt.planes.d_packed_off, gt.planes.d_counts, gt.planes.d_areas,
+        gt.planes.d_extents, gt.d_class_ids, d_crowd, R2, gt.d_geom, d_iou, n,
         st), "mrx_coco_ious")
     match = lambda: N.check(eng.lib.mrx_coco_match(  # noqa: E731
-        P(d_iou), P(eng.d_counts), P(d_cat), P(d_keep), P(d_walk), P(pred.d_areas),
-        P(gt.planes.d_counts), P(gt.d_class_ids), P(d_crowd), P(d_area), N.double_array(thr), T,
-        N.double_array(rngs), A, P(d_match), P(d_ign), n, R1, R2, st), "mrx_coco_match")
+        d_iou, eng.d_counts, d_cat, d_keep, d_walk, pred.d_areas,
+        gt.planes.d_counts, gt.d_class_ids, d_crowd, d_area, N.double_array(thr), T,
+        N.double_array(rngs), A, d_match, d_ign, n, R1, R2, st), "mrx_coco_match")
     ranks()
     rank_ms, _ = time_ms(ranks, iters)
     iou_ms, _ = time_ms(ious, iters)
