@@ -508,9 +508,15 @@ def unmold_coco_eval_batch(items, image_ids, gt_anns, evaluator, category_ids=No
         else:
             eng.enqueue(st.d_det, st.d_msk, expand=False)
         st.meta()                          # raises for bad class ids or boxes
-        records = [e._batch_eval(eng, t, category_ids) for e, t in zip(evaluators, tables)]
-    for e, rec in zip(evaluators, records):
-        e._record(image_ids, *rec)
+        records = []
+        for e, t in zip(evaluators, tables):
+            status = e._batch_status(image_ids, t[0])
+            gt, t = e._ground_truth(eng.lib, eng.device, eng.layout.geom, t)
+            res = e._ious(eng.lib, eng.predictions(gt), gt, t, e._class_map(eng.C, category_ids),
+                          status)
+            records.append((res, t, status))
+    for e, (res, t, status) in zip(evaluators, records):
+        e._record(image_ids, res, *t[:3], status)
 
 
 def unmold_detections_contours_batch(items):

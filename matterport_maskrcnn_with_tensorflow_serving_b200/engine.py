@@ -490,65 +490,19 @@ class UnmoldEngine:
         return mask_matches(self.lib, last[1], self.d_counts, self.d_class_ids, self.d_scores,
                             _dtype_code(self.det_dtype), gt, thresholds, score_threshold, stream)
 
-    def enqueue_coco_eval(self, gt, gt_crowd, gt_area, class_map, params, stream=None):
-        """EXTENSION: `coco_evaluate_batch` of the planned batch's kept instances against `gt` (a
-        `MaskBatch` from `ground_truth` / `ground_truth_rle` whose class ids are dense category
-        indices), on the packed planes (after `enqueue_expand_packed` or `pack_masks`); each
-        prediction is read only inside its box.  class_map [C] maps the engine's class ids to
-        dense categories (-1: not evaluated).  Synchronises once; returns its dict."""
-        pred = self._prediction_planes(gt, "enqueue_coco_eval", stream)
-        n = self._n_images
-        return coco_evaluate_batch(self.lib, pred, self.d_class_ids[:n], self.d_scores[:n], gt,
-                                   gt_crowd, gt_area, class_map, params, stream)
-
-    def enqueue_coco_box_eval(self, gt_counts, gt_cat, gt_boxes, gt_crowd, gt_area, class_map,
-                              params, stream=None):
-        """EXTENSION: `coco_box_evaluate_batch` (COCOeval "bbox") of the planned batch's kept
-        boxes, after `enqueue(..., expand=False)`: no mask is expanded or read.  The ground truth
-        is host arrays padded to R2 instances per image (gt_counts [n], gt_cat [n, R2] dense
-        categories, gt_boxes [n, R2, 4] float64 [x, y, w, h], gt_crowd, gt_area [n, R2]);
-        class_map [C] maps the engine's class ids to dense categories (-1: not evaluated).
-        Synchronises once; returns its dict."""
+    def predictions(self, gt=None, stream=None):
+        """EXTENSION: the planned batch's kept predictions as the scorers read them
+        (`coco_evaluate_batch`, `coco_boundary_evaluate_batch`, `coco_box_evaluate_batch`), after
+        `enqueue`: its counts, class ids, scores and boxes.  With `gt` (a `MaskBatch` of the same
+        plan, e.g. from `ground_truth_rle`) also their `Planes` on the packed planes (after
+        `enqueue_expand_packed` or `pack_masks`), each prediction counted only inside its box;
+        without it no mask is read, as box scoring after `enqueue(..., expand=False)` needs."""
+        planes = None if gt is None else self._prediction_planes(gt, "predictions", stream)
         n = self._n_images
         if n == 0:
             raise RuntimeError("call plan() and enqueue() first")
-        return coco_box_evaluate_batch(self.lib, self.d_boxes[:n], self.d_counts[:n],
-                                       self.d_class_ids[:n], self.d_scores[:n], gt_counts, gt_cat,
-                                       gt_boxes, gt_crowd, gt_area, class_map, params, stream)
-
-    def enqueue_lvis_eval(self, gt, gt_area, class_map, status, params, stream=None):
-        """EXTENSION: `lvis_evaluate_batch` (LVISEval "segm") of the planned batch's kept
-        instances against `gt`, as `enqueue_coco_eval` takes them, with the [n, K] status table
-        of the federated filter.  Synchronises once; returns its dict."""
-        pred = self._prediction_planes(gt, "enqueue_lvis_eval", stream)
-        n = self._n_images
-        return lvis_evaluate_batch(self.lib, pred, self.d_class_ids[:n], self.d_scores[:n], gt,
-                                   gt_area, class_map, status, params, stream)
-
-    def enqueue_lvis_box_eval(self, gt_counts, gt_cat, gt_boxes, gt_area, class_map, status,
-                              params, stream=None):
-        """EXTENSION: `lvis_box_evaluate_batch` (LVISEval "bbox") of the planned batch's kept
-        boxes, after `enqueue(..., expand=False)`, as `enqueue_coco_box_eval` takes them (no crowd
-        flags), with the [n, K] status table.  Synchronises once; returns its dict."""
-        n = self._n_images
-        if n == 0:
-            raise RuntimeError("call plan() and enqueue() first")
-        return lvis_box_evaluate_batch(self.lib, self.d_boxes[:n], self.d_counts[:n],
-                                       self.d_class_ids[:n], self.d_scores[:n], gt_counts, gt_cat,
-                                       gt_boxes, gt_area, class_map, status, params, stream)
-
-    def enqueue_coco_boundary_eval(self, gt, gt_crowd, gt_area, class_map, params,
-                                   dilation_ratio=0.02, stream=None):
-        """EXTENSION: `coco_boundary_evaluate_batch` (COCOeval "boundary", Boundary AP) of the
-        planned batch's kept instances against `gt`, as `enqueue_coco_eval` takes them; each
-        prediction's boundary is eroded inside its box, outside which its plane is zero.  The
-        boundary planes and their areas live in `_eval_bufs`.  Synchronises once; returns its
-        dict."""
-        pred = self._prediction_planes(gt, "enqueue_coco_boundary_eval", stream)
-        n = self._n_images
-        return coco_boundary_evaluate_batch(self.lib, pred, self.d_boxes, self.d_class_ids[:n],
-                                            self.d_scores[:n], gt, gt_crowd, gt_area, class_map,
-                                            params, dilation_ratio, stream, self._eval_bufs)
+        return Predictions(self.d_counts[:n], self.d_class_ids[:n], self.d_scores[:n],
+                           self.d_boxes[:n], planes)
 
     def boundary_planes(self, dilation_ratio=0.02, stream=None):
         """EXTENSION: `Planes` of the boundaries of the planned batch's kept masks (after
@@ -670,6 +624,18 @@ class Planes(NamedTuple):
     d_areas: object
     d_extents: object
     R: int
+
+
+class Predictions(NamedTuple):
+    """One batch's predictions as the COCO scorers read them: counts [n], class_ids [n, R] and
+    scores [n, R] (float32 / float64), boxes [n, R, 4] (int32 (y1, x1, y2, x2) boxes, which the
+    boundary scorer also takes as the regions of `planes`, or the float64 [x, y, w, h] of bbox
+    results), and `Planes` of the masks for the mask scorers."""
+    counts: object
+    class_ids: object
+    scores: object
+    boxes: object
+    planes: Planes = None
 
 
 class MaskBatch:
@@ -1165,44 +1131,29 @@ def _device_params(iou_thrs, area_rng, max_det, max_det_name):
 
 
 def coco_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt_area, class_map,
-                        params, stream=None):
+                        params, stream=None, status=None):
     """The per-image half of COCOeval (iouType "segm") for one batch: mrx_coco_ranks,
-    mrx_coco_ious and mrx_coco_match, then one download and one synchronisation.
+    mrx_coco_ious and mrx_coco_match, then one download and one synchronisation.  With `status`
+    it is lvis-api's LVISEval (iouType "segm"): mrx_lvis_ranks (the per-image cut at
+    `params.max_dets` and the federated filter) takes mrx_coco_ranks' place.
 
     pred: `Planes` of the predictions (areas and extents from mrx_mask_extents) of gt's images,
     pred_class_ids [n, pred.R] int32 and pred_scores [n, pred.R] float32 / float64 device tensors;
-    gt: a `MaskBatch` whose class ids are dense category indices; gt_crowd [n, gt.R] (iscrowd)
-    and gt_area [n, gt.R] (the annotations' areas, float64) host arrays; class_map [C] int32 host
-    array, prediction class id -> dense category or -1 (not evaluated); params: `iouThrs`,
-    `areaRng`, `maxDets` (`coco_device_params`).
+    gt: a `MaskBatch` whose class ids are dense category indices; gt_crowd [n, gt.R] (iscrowd;
+    LVISEval passes zeros) and gt_area [n, gt.R] (the annotations' areas, float64) host arrays;
+    class_map [C] int32 host array, prediction class id -> dense category or -1 (not evaluated);
+    params: COCOeval's `iouThrs`, `areaRng`, `maxDets` (`coco_device_params`), or with status
+    LVISEval's `iou_thrs`, `area_rng`, `max_dets` (`lvis_device_params`); status: None, or an
+    [n, K] uint8 host array of MRX_LVIS_* bits per (image, dense category), uploaded in the one
+    copy of the ground-truth tables (class_map's categories must then be < K; one at or above K
+    is not evaluated).
 
     Returns a dict of host arrays: `counts` [n]; per prediction [n, pred.R] `cat`, `rank` (in
     its (image, category), in score order), `keep` (cat >= 0 and rank < maxDets[-1], and within
-    the count), `area` (int64 pixels), `score` (float64); `match` [A, T, n, pred.R] int32 (the
-    ground-truth index or -1) and `ignore` [A, T, n, pred.R] bool, defined where `keep` is; and
-    `d_iou`, the float64 device tensor [n, pred.R, gt.R] of mrx_coco_ious."""
-    return _segm_evaluate(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt_area, class_map,
-                          coco_device_params(params), None, stream)
-
-
-def lvis_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_area, class_map, status,
-                        params, stream=None):
-    """The per-image half of lvis-api's LVISEval (iouType "segm") for one batch: mrx_lvis_ranks
-    (the per-image cut at `params.max_dets` and the federated filter), then mrx_coco_ious and
-    mrx_coco_match with every ground-truth instance non-crowd, one download and one
-    synchronisation.  status [n, K] uint8 host array: MRX_LVIS_* bits of (image, dense category),
-    uploaded in the one copy of the ground-truth tables; class_map's categories must be < K (one
-    at or above K is not evaluated).  params: `iou_thrs`, `area_rng`, `max_dets`
-    (`lvis_device_params`).  Other arguments and the result as for `coco_evaluate_batch`, whose
-    `keep` is mrx_lvis_ranks' here and whose `ignore` does not yet hold the not-exhaustive rule
-    (the caller's)."""
-    return _segm_evaluate(lib, pred, pred_class_ids, pred_scores, gt,
-                          np.zeros((gt.n, int(gt.R)), np.uint8), gt_area, class_map,
-                          lvis_device_params(params), status, stream)
-
-
-def _segm_evaluate(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt_area, class_map,
-                   dparams, status, stream):
+    the count; with status, mrx_lvis_ranks' rule), `area` (int64 pixels), `score` (float64);
+    `match` [A, T, n, pred.R] int32 (the ground-truth index or -1) and `ignore` [A, T, n, pred.R]
+    bool, defined where `keep` is (with status, without LVISEval's not-exhaustive rule, which is
+    the caller's); and `d_iou`, the float64 device tensor [n, pred.R, gt.R] of mrx_coco_ious."""
     n, R1, R2 = gt.n, int(pred.R), int(gt.R)
     class_map = _coco_class_map(class_map)
     with _stream_ctx(stream):
@@ -1220,8 +1171,14 @@ def _segm_evaluate(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt_area
                 d_crowd, R2, gt.d_geom, d_iou, n, st), "mrx_coco_ious")
 
         return _coco_evaluate(lib, n, R1, R2, pred.d_counts, pred_class_ids, pred_scores,
-                              gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map, dparams,
-                              np.int64, ious, stream, *d_status)
+                              gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map,
+                              _scorer_params(params, status), np.int64, ious, stream, *d_status)
+
+
+def _scorer_params(params, status):
+    """The device parameters of COCOeval's params, or of LVISEval's when there is a status
+    table."""
+    return (coco_device_params if status is None else lvis_device_params)(params)
 
 
 def _status_part(status, n):
@@ -1235,57 +1192,35 @@ def _status_part(status, n):
 
 
 def coco_box_evaluate_batch(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts,
-                            gt_cat, gt_boxes, gt_crowd, gt_area, class_map, params, stream=None):
-    """The per-image half of COCOeval (iouType "bbox") for one batch of n images: mrx_coco_ranks,
-    mrx_coco_box_ious and mrx_coco_match_f64area, then one download and one synchronisation.  No
-    mask is read.
+                            gt_cat, gt_boxes, gt_crowd, gt_area, class_map, params, stream=None,
+                            status=None):
+    """The per-image half of COCOeval (iouType "bbox") for one batch of n images: mrx_coco_ranks
+    (mrx_lvis_ranks with `status`: LVISEval "bbox"), mrx_coco_box_ious and
+    mrx_coco_match_f64area, then one download and one synchronisation.  No mask is read.
 
     pred_boxes [n, R1, 4]: int32 (y1, x1, y2, x2), the kept boxes of mrx_unmold_prepare (their
     `bbox` is [x1, y1, x2 - x1, y2 - y1]), or float64 [x, y, w, h], results' `bbox`;
     pred_counts [n] int32, pred_class_ids [n, R1] int32 and pred_scores [n, R1] float32 /
     float64.  Each of those is a device tensor or a host array; the host arrays go up in one copy
     with the ground truth.  gt_counts [n], gt_cat [n, R2] (dense category indices), gt_boxes
-    [n, R2, 4] float64 [x, y, w, h], gt_crowd [n, R2] and gt_area [n, R2] host arrays; class_map
-    and params as for `coco_evaluate_batch`.
+    [n, R2, 4] float64 [x, y, w, h], gt_crowd [n, R2] and gt_area [n, R2] host arrays; class_map,
+    params and status as for `coco_evaluate_batch`.
 
     Returns `coco_evaluate_batch`'s dict, with `area` float64 (each kept prediction's w*h, as
     loadRes stores it for a bbox result) and `d_iou` from mrx_coco_box_ious."""
-    return _box_evaluate(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts,
-                         gt_cat, gt_boxes, gt_crowd, gt_area, class_map, coco_device_params(params),
-                         None, stream)
-
-
-def lvis_box_evaluate_batch(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts,
-                            gt_cat, gt_boxes, gt_area, class_map, status, params, stream=None):
-    """The per-image half of lvis-api's LVISEval (iouType "bbox") for one batch: mrx_lvis_ranks,
-    mrx_coco_box_ious and mrx_coco_match_f64area with every ground-truth box non-crowd, one
-    download and one synchronisation.  Arguments as for `coco_box_evaluate_batch` (without
-    gt_crowd), status and params as for `lvis_evaluate_batch`."""
-    gt_cat = np.ascontiguousarray(gt_cat, dtype=np.int32)
-    return _box_evaluate(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts,
-                         gt_cat, gt_boxes, np.zeros(gt_cat.shape, np.uint8), gt_area, class_map,
-                         lvis_device_params(params), status, stream)
-
-
-def _box_evaluate(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts, gt_cat,
-                  gt_boxes, gt_crowd, gt_area, class_map, dparams, status, stream):
     torch = _torch()
     gt_cat = np.ascontiguousarray(gt_cat, dtype=np.int32)
     n, R2 = gt_cat.shape
     R1 = int(pred_boxes.shape[1])
     class_map = _coco_class_map(class_map)
-    if not isinstance(pred_boxes, np.ndarray):
-        dev = pred_boxes.device
-    else:
-        dev = next((x.device for x in (pred_counts, pred_class_ids, pred_scores)
-                    if not isinstance(x, np.ndarray)),
-                   torch.device("cuda", torch.cuda.current_device()))
+    pred = [pred_boxes, pred_counts, pred_class_ids, pred_scores]
+    dev = next((x.device for x in pred if not isinstance(x, np.ndarray)),
+               torch.device("cuda", torch.cuda.current_device()))
     parts = [np.ascontiguousarray(gt_counts, dtype=np.int32).reshape(n), gt_cat,
              np.ascontiguousarray(gt_boxes, dtype=np.float64).reshape(n, R2, 4),
              np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
              np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map]
     parts += _status_part(status, n)
-    pred = [pred_boxes, pred_counts, pred_class_ids, pred_scores]
     on_host = [k for k, x in enumerate(pred) if isinstance(x, np.ndarray)]
     with _stream_ctx(stream):
         up = _upload_parts(parts + [np.ascontiguousarray(pred[k]) for k in on_host], dev)
@@ -1303,7 +1238,8 @@ def _box_evaluate(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_
                 d_crowd, R2, v["area"], d_iou, n, st), "mrx_coco_box_ious")
 
         return _coco_evaluate(lib, n, R1, R2, pred_counts, pred_class_ids, pred_scores, d_counts,
-                              d_cat, d_crowd, d_area, d_map, dparams, np.float64, ious, stream,
+                              d_cat, d_crowd, d_area, d_map, _scorer_params(params, status),
+                              np.float64, ious, stream,
                               *d_status)
 
 

@@ -36,10 +36,9 @@ from collections import OrderedDict
 import numpy as np
 
 from . import _native as N
-from .engine import (MaskBatch, check_dilation_ratio, coco_boundary_evaluate_batch,
+from .engine import (MaskBatch, Predictions, check_dilation_ratio, coco_boundary_evaluate_batch,
                      coco_box_evaluate_batch, coco_device_params, coco_evaluate_batch,
-                     lvis_box_evaluate_batch, lvis_device_params, lvis_evaluate_batch,
-                     mask_matches, mask_overlaps)
+                     lvis_device_params, mask_matches, mask_overlaps)
 
 
 def trim_zeros(x):
@@ -226,16 +225,21 @@ class _COCOevalBase:
                  area_rng=None, area_rng_lbl=None):
         self.params = Params(cat_ids, iou_thrs, rec_thrs, max_dets, area_rng, area_rng_lbl,
                              self._iou_type)
-        self._device_params = coco_device_params(self.params)
-        self._auto_cats = cat_ids is None
+        coco_device_params(self.params)        # raises outside the kernels' limits
+        self._init_records({}, cat_ids is None)
+        self.stats = None
+
+    def _init_records(self, cat_index, auto_cats):
+        """The state every evaluator starts from, COCO or LVIS: the category and image maps, no
+        records, parameters not yet frozen."""
+        self._cat_index = cat_index   # category id -> dense index used on the device
+        self._auto_cats = auto_cats
         self._frozen = None
-        self._cat_index = {}          # category id -> dense index used on the device
         self._gt_cats = set()
         self._img_index = {}          # image id -> position in add order
         self._dets = []               # per batch: (img, cat, rank, score, matched, ignored)
         self._gts = []                # per batch: (img, cat, not ignored [n, A])
         self.eval = {}
-        self.stats = None
 
     # ------------------------------------------------------------------ adding batches
     def _dense(self, cat_id):
@@ -249,7 +253,7 @@ class _COCOevalBase:
             self._frozen = key
         elif key != self._frozen:
             raise ValueError("iouThrs, areaRng and maxDets[-1] changed after the first batch")
-        self._device_params = coco_device_params(p)
+        coco_device_params(p)
 
     def _new_images(self, image_ids, n_items, gt_anns, what):
         if len(image_ids) != n_items:
@@ -263,10 +267,12 @@ class _COCOevalBase:
                 raise ValueError(f"image {i!r} was already added")
             seen.add(i)
 
-    # add_batch in two halves, which api_utils.unmold_coco_eval_batch runs around one unmold for
-    # several evaluators: `_batch_tables` (host checks and tables, before anything is uploaded;
-    # None for an empty batch) and `_batch_eval` (on the engine after the unmold: prepare, and
-    # the packed expand when `_needs_masks`), whose result is the rest of `_record`'s arguments
+    # A batch takes these steps, run by add_results or, around one unmold for several evaluators,
+    # by api_utils.unmold_coco_eval_batch: `_gt_tables` (host checks and the tables (cats, crowd,
+    # area, segmentations or boxes), before anything is uploaded; `_batch_tables` for model
+    # outputs, None for an empty batch), `_batch_status`, `_ground_truth`, `_ious` (the scorer on
+    # `Predictions`: the engine's, after the packed expand when `_needs_masks`, or decoded
+    # results) and `_record`
     _needs_masks = False
 
     def _batch_tables(self, items, image_ids, gt_anns):
@@ -276,6 +282,27 @@ class _COCOevalBase:
             return None
         return self._gt_tables(image_ids, gt_anns, [(int(it[2][0]), int(it[2][1]))
                                                     for it in items])
+
+    def _batch_status(self, image_ids, gt_cats):
+        """The batch's LVIS status table, which its IoU step and `_record` read; None for COCO."""
+        return None
+
+    def _ground_truth(self, lib, device, geoms, tables):
+        """(None, tables): box ground truth goes up inside the scorer."""
+        return None, tables
+
+    @staticmethod
+    def _by_image(results, image_ids, check):
+        """results as one list per image of image_ids, each result k replaced by check(k, r),
+        which raises for a result it does not take."""
+        pos = {i: b for b, i in enumerate(image_ids)}
+        dets = [[] for _ in image_ids]
+        for k, r in enumerate(results):
+            if r.get("image_id") not in pos:
+                raise ValueError(f"result {k}: image {r.get('image_id')!r} is not one of the "
+                                 "batch's image ids")
+            dets[pos[r["image_id"]]].append(check(k, r))
+        return dets
 
     def _class_map(self, C, category_ids):
         """int32 [C]: the engine's class id -> dense category (-1 where category_ids has none)."""
@@ -300,9 +327,9 @@ class _COCOevalBase:
                 out[b, :len(r)] = r
         return out
 
-    def _record(self, image_ids, res, gt_cats, gt_crowd, gt_area):
+    def _record(self, image_ids, res, gt_cats, gt_crowd, gt_area, status=None):
         """Append the per-detection records of one batch (`coco_evaluate_batch`'s dict) and the
-        ground truth's non-ignored flags per area range."""
+        ground truth's non-ignored flags per area range.  status: `_batch_status`'s table."""
         first = len(self._img_index)
         for b, i in enumerate(image_ids):
             self._img_index[i] = first + b
@@ -511,12 +538,25 @@ class COCOevalSegm(_COCOevalBase):
             rles.append(rl)
         return cats, crowd, area, rles
 
-    def _areas(self, gt, area):
-        """Annotation areas, the mask's pixel count where the annotation has none."""
-        if not any(np.isnan(a).any() for a in area):
-            return area
-        mask_area = gt.planes.d_areas.cpu().numpy()
-        return [np.where(np.isnan(a), mask_area[b, :len(a)], a) for b, a in enumerate(area)]
+    def _ground_truth(self, lib, device, geoms, tables):
+        """The batch's ground truth decoded on the device (a `MaskBatch` of geoms), and tables
+        with each missing area replaced by its mask's pixel count."""
+        cats, crowd, area, segs = tables
+        gt = (MaskBatch.from_coco if self._polygons else MaskBatch.from_rle)(lib, device, geoms,
+                                                                            cats, segs)
+        if any(np.isnan(a).any() for a in area):
+            mask_area = gt.planes.d_areas.cpu().numpy()
+            area = [np.where(np.isnan(a), mask_area[b, :len(a)], a) for b, a in enumerate(area)]
+        return gt, (cats, crowd, area, segs)
+
+    def _ious(self, lib, pred, gt, tables, class_map, status):
+        """The IoU step, the one part a mask IoU type replaces: the scorer's dict of pred (with
+        planes) against gt."""
+        _, crowd, area, _ = tables
+        return coco_evaluate_batch(lib, pred.planes, pred.class_ids, pred.scores, gt,
+                                   self._padded(crowd, gt.R, np.uint8),
+                                   self._padded(area, gt.R, np.float64), class_map, self.params,
+                                   status=status)
 
     def add_batch(self, items, image_ids, gt_anns, category_ids=None):
         """Evaluate model outputs against COCO ground truth: items as for
@@ -531,24 +571,6 @@ class COCOevalSegm(_COCOevalBase):
         api_utils.unmold_coco_eval_batch(items, image_ids, gt_anns, [self], category_ids)
 
     _needs_masks = True
-
-    def _batch_eval(self, eng, tables, category_ids):
-        cats, crowd, area, rles = tables
-        gt = (eng.ground_truth_coco if self._polygons else eng.ground_truth_rle)(cats, rles)
-        area = self._areas(gt, area)
-        res = self._engine_ious(eng, gt, self._padded(crowd, gt.R, np.uint8),
-                                self._padded(area, gt.R, np.float64),
-                                self._class_map(eng.C, category_ids))
-        return res, cats, crowd, area
-
-    # the IoU step, the one part a mask IoU type replaces: on an engine's kept instances
-    # (`add_batch`), or on decoded results (`add_results`, pred a `MaskBatch`)
-    def _engine_ious(self, eng, gt, crowd, area, class_map):
-        return eng.enqueue_coco_eval(gt, crowd, area, class_map, self.params)
-
-    def _result_ious(self, lib, pred, d_scores, gt, crowd, area, class_map):
-        return coco_evaluate_batch(lib, pred.planes, pred.d_class_ids, d_scores, gt, crowd, area,
-                                   class_map, self.params)
 
     def add_results(self, results, gt_anns, image_ids, image_shapes=None):
         """Evaluate COCO segm results -- dicts {'image_id', 'category_id', 'score',
@@ -566,17 +588,15 @@ class COCOevalSegm(_COCOevalBase):
         self._freeze()
         if len(image_ids) == 0:
             return
-        pos = {i: b for b, i in enumerate(image_ids)}
-        dets = [[] for _ in image_ids]
-        for k, r in enumerate(results):
-            if r.get("image_id") not in pos:
-                raise ValueError(f"result {k}: image {r.get('image_id')!r} is not one of the "
-                                 "batch's image ids")
+
+        def check(k, r):
             seg = r.get("segmentation")
             if not isinstance(seg, dict) or "counts" not in seg or "size" not in seg:
                 raise ValueError(f"result {k}: segmentation must be an RLE dict with 'size' and "
                                  "'counts'")
-            dets[pos[r["image_id"]]].append(r)
+            return r
+
+        dets = self._by_image(results, image_ids, check)
         shapes = []
         for image_id, d, anns in zip(image_ids, dets, gt_anns):
             sizes = {tuple(int(v) for v in np.ravel(x["segmentation"]["size"])) for x in d}
@@ -592,7 +612,8 @@ class COCOevalSegm(_COCOevalBase):
                 raise ValueError(f"image {image_id!r}: its ground truth is polygons only, so its "
                                  "shape is unknown; give it in image_shapes")
             shapes.append(sizes.pop() if sizes else (1, 1))
-        cats, crowd, area, rles = self._gt_tables(image_ids, gt_anns, shapes)
+        tables = self._gt_tables(image_ids, gt_anns, shapes)
+        status = self._batch_status(image_ids, tables[0])
         N.require_cuda()
         lib = N.load()
         dev = torch.device("cuda", torch.cuda.current_device())
@@ -600,15 +621,14 @@ class COCOevalSegm(_COCOevalBase):
         pred_cls = [np.asarray([self._dense(x["category_id"]) for x in d], np.int32) for d in dets]
         pred = MaskBatch.from_rle(lib, dev, geoms, pred_cls, [[x["segmentation"] for x in d]
                                                               for d in dets])
-        gt = (MaskBatch.from_coco if self._polygons else MaskBatch.from_rle)(lib, dev, geoms, cats,
-                                                                            rles)
-        area = self._areas(gt, area)
+        gt, tables = self._ground_truth(lib, dev, geoms, tables)
         scores = self._padded([[float(x["score"]) for x in d] for d in dets], pred.R, np.float64)
-        d_scores = torch.from_numpy(scores).to(dev)
-        res = self._result_ious(lib, pred, d_scores, gt, self._padded(crowd, gt.R, np.uint8),
-                                self._padded(area, gt.R, np.float64),
-                                np.arange(max(len(self._cat_index), 1), dtype=np.int32))
-        self._record(image_ids, res, cats, crowd, area)
+        res = self._ious(lib, Predictions(pred.d_counts, pred.d_class_ids,
+                                          torch.from_numpy(scores).to(dev), pred.d_regions,
+                                          pred.planes),
+                         gt, tables, np.arange(max(len(self._cat_index), 1), dtype=np.int32),
+                         status)
+        self._record(image_ids, res, *tables[:3], status)
 
 
 class COCOevalBoundary(COCOevalSegm):
@@ -642,15 +662,12 @@ class COCOevalBoundary(COCOevalSegm):
         elif r != self._frozen_ratio:
             raise ValueError("dilation_ratio changed after the first batch")
 
-    def _engine_ious(self, eng, gt, crowd, area, class_map):
-        return eng.enqueue_coco_boundary_eval(gt, crowd, area, class_map, self.params,
-                                              self._frozen_ratio)
-
-    def _result_ious(self, lib, pred, d_scores, gt, crowd, area, class_map):
-        return coco_boundary_evaluate_batch(lib, pred.planes, pred.d_regions, pred.d_class_ids,
-                                            d_scores, gt, crowd, area, class_map, self.params,
-                                            self._frozen_ratio)
-
+    def _ious(self, lib, pred, gt, tables, class_map, status):
+        _, crowd, area, _ = tables
+        return coco_boundary_evaluate_batch(lib, pred.planes, pred.boxes, pred.class_ids,
+                                            pred.scores, gt, self._padded(crowd, gt.R, np.uint8),
+                                            self._padded(area, gt.R, np.float64), class_map,
+                                            self.params, self._frozen_ratio)
 
 
 class COCOevalBbox(_COCOevalBase):
@@ -725,6 +742,12 @@ class COCOevalBbox(_COCOevalBase):
                 self._padded(boxes, R2, np.float64, (4,)), self._padded(crowd, R2, np.uint8),
                 self._padded(area, R2, np.float64))
 
+    def _ious(self, lib, pred, gt, tables, class_map, status):
+        """The scorer's dict of pred (boxes, no planes) against the tables' boxes (gt is None)."""
+        return coco_box_evaluate_batch(lib, pred.boxes, pred.counts, pred.class_ids, pred.scores,
+                                       *self._gt_arrays(tables), class_map, self.params,
+                                       status=status)
+
     def add_batch(self, items, image_ids, gt_anns, category_ids=None):
         """Evaluate model outputs against COCO ground truth: items as for
         `api_utils.unmold_detections_batch`, one image id and one list of annotation dicts per
@@ -735,12 +758,6 @@ class COCOevalBbox(_COCOevalBase):
 
         api_utils.unmold_coco_eval_batch(items, image_ids, gt_anns, [self], category_ids)
 
-    def _batch_eval(self, eng, tables, category_ids):
-        res = eng.enqueue_coco_box_eval(*self._gt_arrays(tables),
-                                        self._class_map(eng.C, category_ids), self.params)
-        cats, crowd, area, _ = tables
-        return res, cats, crowd, area
-
     def add_results(self, results, gt_anns, image_ids):
         """Evaluate COCO bbox results -- dicts {'image_id', 'category_id', 'score', 'bbox':
         [x, y, w, h]} as `loadRes` takes them and `unmold_coco_results_batch` returns them --
@@ -750,31 +767,26 @@ class COCOevalBbox(_COCOevalBase):
         self._freeze()
         if len(image_ids) == 0:
             return
-        pos = {i: b for b, i in enumerate(image_ids)}
-        dets = [[] for _ in image_ids]
-        for k, r in enumerate(results):
-            if r.get("image_id") not in pos:
-                raise ValueError(f"result {k}: image {r.get('image_id')!r} is not one of the "
-                                 "batch's image ids")
+
+        def check(k, r):
             if "bbox" not in r:
                 raise ValueError(f"result {k}: no 'bbox'")
-            dets[pos[r["image_id"]]].append((self._box(r["bbox"], f"result {k}"), r))
+            return self._box(r["bbox"], f"result {k}"), r
+
+        dets = self._by_image(results, image_ids, check)
         tables = self._gt_tables(image_ids, gt_anns)
+        status = self._batch_status(image_ids, tables[0])
         N.require_cuda()
         R1 = max(max(len(d) for d in dets), 1)
-        pred_boxes = self._padded([[box for box, _ in d] for d in dets], R1, np.float64, (4,))
-        pred_cls = self._padded([[self._dense(r["category_id"]) for _, r in d] for d in dets], R1,
-                                np.int32)
-        scores = self._padded([[float(r["score"]) for _, r in d] for d in dets], R1, np.float64)
-        res = self._evaluate_boxes(pred_boxes, np.asarray([len(d) for d in dets], np.int32),
-                                   pred_cls, scores, *self._gt_arrays(tables),
-                                   np.arange(max(len(self._cat_index), 1), dtype=np.int32))
-        cats, crowd, area, _ = tables
-        self._record(image_ids, res, cats, crowd, area)
-
-    def _evaluate_boxes(self, *arrays):
-        """`coco_box_evaluate_batch` of `add_results`' host arrays."""
-        return coco_box_evaluate_batch(N.load(), *arrays, self.params)
+        pred = Predictions(
+            np.asarray([len(d) for d in dets], np.int32),
+            self._padded([[self._dense(r["category_id"]) for _, r in d] for d in dets], R1,
+                         np.int32),
+            self._padded([[float(r["score"]) for _, r in d] for d in dets], R1, np.float64),
+            self._padded([[box for box, _ in d] for d in dets], R1, np.float64, (4,)))
+        res = self._ious(N.load(), pred, None, tables,
+                         np.arange(max(len(self._cat_index), 1), dtype=np.int32), status)
+        self._record(image_ids, res, *tables[:3], status)
 
 
 # ----------------------------------------------------------------------------- LVIS mask and box AP
@@ -829,7 +841,7 @@ class _LVISeval:
             raise ValueError(f"cat_ids {unknown[:5]} are not categories of the dataset")
         if not self.params.cat_ids:
             raise ValueError("no categories to evaluate")
-        self._device_params = lvis_device_params(self.params)
+        lvis_device_params(self.params)        # raises outside the kernels' limits
         self._images = {}
         for k, im in enumerate(images):
             missing = [key for key in _LVIS_IMAGE_KEYS
@@ -839,16 +851,7 @@ class _LVISeval:
                 raise ValueError(f"image {name!r}: no {missing}")
             self._images[im["id"]] = im
         # the dense category index is the position in the constructor's cat_ids, fixed for good
-        self._cat_index = {c: k for k, c in enumerate(self.params.cat_ids)}
-        self._auto_cats = False
-        self._frozen = None
-        self._gt_cats = set()
-        self._img_index = {}
-        self._dets = []
-        self._gts = []
-        self._polygons = True
-        self._status = None
-        self.eval = {}
+        self._init_records({c: k for k, c in enumerate(self.params.cat_ids)}, False)
         self.results = {}
 
     def _dense(self, cat_id):
@@ -861,7 +864,7 @@ class _LVISeval:
         key = (tuple(np.ravel(p.iou_thrs).tolist()), tuple(np.ravel(p.area_rng).tolist()),
                int(p.max_dets))
         if self._frozen is None:
-            self._device_params = lvis_device_params(p)
+            lvis_device_params(p)
             self._frozen = key
         elif key != self._frozen:
             raise ValueError("iou_thrs, area_rng and max_dets changed after the first batch")
@@ -874,8 +877,7 @@ class _LVISeval:
 
     def _gt_tables(self, image_ids, gt_anns, shapes=None):
         """The COCO evaluator's tables with every instance non-crowd (LVISEval's compute_iou
-        passes iscrowd = 0), after the LVIS checks; leaves the batch's status table in
-        `_status` for the IoU step that follows."""
+        passes iscrowd = 0), after the LVIS checks."""
         for image_id, anns, hw in zip(image_ids, gt_anns,
                                       shapes if shapes is not None else [None] * len(image_ids)):
             im = self._images[image_id]
@@ -887,9 +889,10 @@ class _LVISeval:
                     raise ValueError(f"{self._where(image_id, k, ann)}: 'ignore' annotations are "
                                      "not supported")
         cats, crowd, area, segs = super()._gt_tables(image_ids, gt_anns, shapes)
-        crowd = [np.zeros_like(c) for c in crowd]
-        self._status = self.status_table(image_ids, cats)
-        return cats, crowd, area, segs
+        return cats, [np.zeros_like(c) for c in crowd], area, segs
+
+    def _batch_status(self, image_ids, gt_cats):
+        return self.status_table(image_ids, gt_cats)
 
     def status_table(self, image_ids, gt_cats):
         """uint8 [n, K]: per image and dense category the MRX_LVIS_* bits, POSITIVE where
@@ -919,9 +922,13 @@ class _LVISeval:
         dt_nel = np.take_along_axis(nel, cat, axis=1) & keep
         res["ignore"] |= (res["match"] == -1) & dt_nel
 
-    def _record(self, image_ids, res, gt_cats, gt_crowd, gt_area):
-        self.not_exhaustive(res, self.status_table(image_ids, gt_cats))
-        super()._record(image_ids, res, gt_cats, gt_crowd, gt_area)
+    def _record(self, image_ids, res, gt_cats, gt_crowd, gt_area, status=None):
+        """The not-exhaustive rule, then the COCO evaluator's records; status is the batch's
+        `status_table`, made here from gt_cats when not given."""
+        if status is None:
+            status = self.status_table(image_ids, gt_cats)
+        self.not_exhaustive(res, status)
+        super()._record(image_ids, res, gt_cats, gt_crowd, gt_area, status)
 
     def _area_rng(self):
         return self.params.area_rng
@@ -1042,13 +1049,7 @@ class LVISEvalSegm(_LVISeval, COCOevalSegm):
     after the first batch."""
 
     _iou_type = "segm"
-
-    def _engine_ious(self, eng, gt, crowd, area, class_map):
-        return eng.enqueue_lvis_eval(gt, area, class_map, self._status, self.params)
-
-    def _result_ious(self, lib, pred, d_scores, gt, crowd, area, class_map):
-        return lvis_evaluate_batch(lib, pred.planes, pred.d_class_ids, d_scores, gt, area,
-                                   class_map, self._status, self.params)
+    _polygons = True
 
     def add_batch(self, items, image_ids, gt_anns, category_ids=None):
         """Evaluate model outputs against LVIS ground truth: items as for
@@ -1079,20 +1080,6 @@ class LVISEvalBbox(_LVISeval, COCOevalBbox):
     one on areas."""
 
     _iou_type = "bbox"
-
-    def _batch_eval(self, eng, tables, category_ids):
-        counts, cat, boxes, _, area = self._gt_arrays(tables)
-        res = eng.enqueue_lvis_box_eval(counts, cat, boxes, area,
-                                        self._class_map(eng.C, category_ids), self._status,
-                                        self.params)
-        cats, crowd, area, _ = tables
-        return res, cats, crowd, area
-
-    def _evaluate_boxes(self, pred_boxes, pred_counts, pred_cls, scores, gt_counts, gt_cat,
-                        gt_boxes, gt_crowd, gt_area, class_map):
-        return lvis_box_evaluate_batch(N.load(), pred_boxes, pred_counts, pred_cls, scores,
-                                       gt_counts, gt_cat, gt_boxes, gt_area, class_map,
-                                       self._status, self.params)
 
 
 def ann_to_mask(ann, height, width):

@@ -239,7 +239,8 @@ def cocoeval_case(iters, n_batches=4):
     pycocotools evaluate (computeIoU + evaluateImg, tests/cocoeval_oracle.py) per image on the
     host."""
     from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, evaluate
-    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import coco_device_params
+    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import (coco_device_params,
+                                                                         coco_evaluate_batch)
 
     batch, base_n = 32, 4
     base = synth.make_batch(11, base_n, (1024, 1024), 100)
@@ -285,7 +286,9 @@ def cocoeval_case(iters, n_batches=4):
     for b, x in enumerate(anns):
         crowd[b, :len(x)] = [a["iscrowd"] for a in x]
         area[b, :len(x)] = [a["area"] for a in x]
-    res = eng.enqueue_coco_eval(gt, crowd, area, np.arange(81, dtype=np.int32), ev.params)
+    pred = eng.predictions(gt)
+    res = coco_evaluate_batch(eng.lib, pred.planes, pred.class_ids, pred.scores, gt, crowd, area,
+                              np.arange(81, dtype=np.int32), ev.params)
     thr, rngs, max_det = coco_device_params(ev.params)
     n, R1, R2, T, A = batch, eng.R, gt.R, len(thr), len(rngs) // 2
     dev = eng.device
@@ -385,7 +388,8 @@ def bboxeval_case(iters, n_batches=4):
     unmold (unmold_coco_eval_batch with both evaluators) against two separate add_batch calls, and
     the restated pycocotools bbox evaluate (tests/bbox_cocoeval_oracle.py) per image on the host."""
     from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, evaluate
-    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import coco_device_params
+    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import (coco_box_evaluate_batch,
+                                                                         coco_device_params)
 
     batch, items, anns = coco_eval_inputs()
 
@@ -421,8 +425,10 @@ def bboxeval_case(iters, n_batches=4):
     eng.enqueue(d_det, d_msk, expand=False)
     tables = ev._gt_tables(list(range(batch)), anns)
     g_counts, g_cat, g_boxes, g_crowd, g_area = ev._gt_arrays(tables)
-    res = eng.enqueue_coco_box_eval(g_counts, g_cat, g_boxes, g_crowd, g_area,
-                                    ev._class_map(81, None), ev.params)
+    pred = eng.predictions()
+    res = coco_box_evaluate_batch(eng.lib, pred.boxes, pred.counts, pred.class_ids, pred.scores,
+                                  g_counts, g_cat, g_boxes, g_crowd, g_area,
+                                  ev._class_map(81, None), ev.params)
     thr, rngs, max_det = coco_device_params(ev.params)
     n, R1, R2, T, A = batch, eng.R, g_cat.shape[1], len(thr), len(rngs) // 2
     dev = eng.device
@@ -494,8 +500,8 @@ def boundaryeval_case(iters, n_batches=4):
     against three separate add_batch calls; and the restated boundary_iou_api evaluate
     (tests/boundary_cocoeval_oracle.py, cv2 erosion) per image on the host."""
     from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, evaluate
-    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import (boundary_dilation,
-                                                                         coco_device_params)
+    from matterport_maskrcnn_with_tensorflow_serving_b200.engine import (
+        boundary_dilation, coco_boundary_evaluate_batch, coco_device_params)
 
     batch, items, anns = coco_eval_inputs()
 
@@ -537,12 +543,14 @@ def boundaryeval_case(iters, n_batches=4):
     for b, x in enumerate(anns):
         crowd[b, :len(x)] = [a["iscrowd"] for a in x]
         area[b, :len(x)] = [a["area"] for a in x]
-    res = eng.enqueue_coco_boundary_eval(gt, crowd, area, np.arange(81, dtype=np.int32),
-                                         ev.params)
+    bufs = eng._eval_bufs
+    pred = eng.predictions(gt)
+    res = coco_boundary_evaluate_batch(eng.lib, pred.planes, pred.boxes, pred.class_ids,
+                                       pred.scores, gt, crowd, area, np.arange(81, dtype=np.int32),
+                                       ev.params, bufs=bufs)
     thr, rngs, max_det = coco_device_params(ev.params)
     n, R1, R2 = batch, eng.R, gt.R
     dev = eng.device
-    bufs = eng._eval_bufs
     d_dil = torch.from_numpy(boundary_dilation(eng.layout.geom, 0.02)).to(dev)
     d_map = torch.arange(81, dtype=torch.int32, device=dev)
     d_cat = torch.empty((n, R1), dtype=torch.int32, device=dev)
@@ -874,7 +882,7 @@ def lvis_case(iters, n_batches=4, batch=32, R=300):
     eng.enqueue_packed(d_det, d_msk)
     gt_dense = [np.asarray(c, np.int32) - 1 for c in cls_all]
     gt = eng.ground_truth_coco(gt_dense, segs)
-    pred = eng._prediction_planes(gt, "lvis_case", None)
+    pred = eng.predictions(gt).planes
     status = ev.status_table(list(range(batch)), gt_dense)
     thr, rngs, max_det = lvis_device_params(ev.params)
     n, R1, R2, T, A = batch, eng.R, gt.R, len(thr), len(rngs) // 2
