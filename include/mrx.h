@@ -27,6 +27,7 @@
  *   mrx_lvis_ranks         (extension: lvis-api's LVISEval, the per-image cut and federated filter)
  *   mrx_jpeg_coefficients / _pixels <- api_utils.load_img (cv2.imread)   serve.py:85-86
  *                             (extension: JPEG request bytes decoded on the device, as cv2.imdecode)
+ *   mrx_png_encode         <- cv2.imwrite of the overlay PNG                 serve.py:168
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
  *   mrx_device_alloc/_free (the canvas allocation: compressible device memory where offered)
  *
@@ -638,6 +639,45 @@ int mrx_jpeg_pixels(const long long *d_desc, const unsigned char *d_tabs, const 
                     const int *d_status, int B, int max_blocks, long long max_pixels,
                     unsigned char *d_planes, unsigned char *d_out, const long long *d_out_off,
                     void *stream);
+
+/* ---------------------------------------------------------------- PNG encode (cv2.imwrite) */
+/* uint8 RGB images encoded byte for byte as cv2.imwrite(path, rgb[..., ::-1]) writes them
+ * (libpng: Sub filter, or none when the width is 1; zlib level 1, Z_RLE, memLevel 8; 8192-byte
+ * IDAT chunks; csrc/png.cu, tests/png_oracle.py).  The host (png.Plan) lays the batch out:
+ * d_desc [B, 20] int64 words per image (png.py's D_* indices: the address of the image's
+ * contiguous H x W x 3 bytes, H, W, the filtered stream length n = H * (3W + 1), and the offset of
+ * the image's part of every buffer below).  Buffers, each sized by png.Plan from H and W alone:
+ *   d_stream  uint8 [n] per image (the filtered rows)      d_sym  int16 [n] per image
+ *   d_stretch int32 [2 * cap] per image                    d_tiles int64 [2 * (total_tiles + 1)]
+ *   d_blk_pos int32 [max blocks + 1] per image             d_blk_tab int32 [blocks, 654]
+ *   d_blk_info int64 [blocks, 8] (MRX_PNG_BLK_*)           d_img_info int64 [B, 8] (MRX_PNG_IMG_*)
+ *   d_zbuf    uint32 [zbuf_words] (zeroed here; each image's deflate bits at its offset)
+ *   d_out     uint8: image b's file at its offset, at most png.png_bound(n) bytes
+ *   d_sizes   int64 [B]: the byte count of each file.
+ * max_n, max_blocks, max_chunks: the largest n, block count bound and IDAT count bound of the
+ * batch.  Checks: null pointers, B outside [0, MRX_MAX_BATCH], max_n outside
+ * [4, MRX_PNG_MAX_STREAM], a max extent below 1: MRX_E_INVALID.  B = 0 returns MRX_OK without
+ * launching anything. */
+#define MRX_PNG_MAX_STREAM (1 << 30)   /* filtered bytes per image: positions stay in int32 */
+#define MRX_PNG_BLK_TYPE      0   /* 0 stored, 1 static, 2 dynamic */
+#define MRX_PNG_BLK_LAST      1
+#define MRX_PNG_BLK_HDR_BITS  2   /* the dynamic tree description */
+#define MRX_PNG_BLK_DATA_BITS 3   /* the symbols' codes, extra bits included, end-of-block excluded */
+#define MRX_PNG_BLK_EOB       4   /* end-of-block code | length << 16 */
+#define MRX_PNG_BLK_BIT       5   /* the block's first bit in the deflate stream */
+#define MRX_PNG_BLK_PBASE     6
+#define MRX_PNG_BLK_BITS      7   /* the block's bits, stored padding included */
+#define MRX_PNG_IMG_NSYM      0
+#define MRX_PNG_IMG_NBLK      1
+#define MRX_PNG_IMG_BITS      4   /* deflate stream bits */
+#define MRX_PNG_IMG_ZLEN      5   /* zlib stream bytes */
+#define MRX_PNG_IMG_CHUNKS    6
+#define MRX_PNG_IMG_FILE      7
+int mrx_png_encode(const long long *d_desc, int B, long long max_n, int max_blocks,
+                   long long max_chunks, long long total_tiles, long long zbuf_words,
+                   unsigned char *d_stream, short *d_sym, int *d_stretch, long long *d_tiles,
+                   int *d_blk_pos, int *d_blk_tab, long long *d_blk_info, unsigned int *d_zbuf,
+                   long long *d_img_info, unsigned char *d_out, long long *d_sizes, void *stream);
 
 /* ---------------------------------------------------------------- multi-GPU gather (8e) */
 /* Peer-memory plumbing for the final gather of the canvases to rank 0 (one process per GPU).

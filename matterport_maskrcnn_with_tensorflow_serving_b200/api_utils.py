@@ -12,7 +12,9 @@ serve.py:48): `unmold_detections_batch`, `unmold_detections_packed_batch`,
 `unmold_detections_rle_batch`, `unmold_detections_contours_batch`, `unmold_overlay_batch`,
 `unmold_coco_results_batch` (upstream's `build_coco_results` of the unmolded detections),
 `unmold_compute_ap_batch` (upstream's `compute_ap` of them against ground truth) and
-`unmold_coco_eval_batch` (pycocotools' COCOeval "segm" of them, streamed batch by batch).
+`unmold_coco_eval_batch` (pycocotools' COCOeval "segm" of them, streamed batch by batch), and
+`decode_jpeg_batch` / `encode_png_batch` (request JPEG bytes in, response PNG bytes out, each as
+OpenCV would decode or write them).
 
 Numerical contract (checked by tests/ against the float64 oracle): N, boxes, class ids and
 scores are bit-exact.  The mask resize runs in float32 on exact integer source coordinates;
@@ -91,6 +93,73 @@ def decode_jpeg_batch(blobs):
         if m is None or m.config is not get_config():
             m = _state["molder"] = Molder(get_config())
         return m.decode_jpeg_batch(list(blobs))
+
+
+def encode_png_batch(images):
+    """uint8 RGB [H, W, 3] images (CUDA tensors or arrays; sizes may differ) -> one PNG file's
+    bytes each, equal byte for byte to `cv2.imencode('.png', img[..., ::-1])[1].tobytes()`,
+    encoded on the device (csrc/png.cu).  An image the encoder does not accept raises ValueError
+    naming its index before anything runs.  Only the files travel to the host."""
+    return _png_encode(images)[0]
+
+
+def _png_encode(images, stats=False):
+    """`encode_png_batch`, plus (with stats) the device's per-image and per-block int64 tables
+    (mrx.h MRX_PNG_IMG_* / MRX_PNG_BLK_*) and the plan."""
+    import torch
+
+    from . import png
+
+    images = list(images)
+    if len(images) == 0:
+        return ([], None, None, None) if stats else ([],)
+    N.require_cuda()
+    meta = []
+    for b, img in enumerate(images):
+        if torch.is_tensor(img):
+            meta.append((tuple(img.shape), str(img.dtype).replace("torch.", "")))
+        else:
+            a = np.asarray(img)
+            meta.append((a.shape, a.dtype))
+    plan = png.Plan(meta)
+    dev = next((im.device for im in images if torch.is_tensor(im) and im.is_cuda),
+               torch.device("cuda", torch.cuda.current_device()))
+    srcs = []
+    for img in images:
+        t = img if torch.is_tensor(img) else torch.from_numpy(np.ascontiguousarray(img))
+        srcs.append(t.to(dev, non_blocking=True).contiguous())
+    plan.set_sources([t.data_ptr() for t in srcs])
+    lib = N.load()
+
+    def buf(n, dtype):
+        return torch.empty(int(n), dtype=dtype, device=dev)
+
+    d_desc = torch.from_numpy(plan.desc).to(dev)
+    d_stream, d_sym = buf(plan.stream_bytes, torch.uint8), buf(plan.stream_bytes, torch.int16)
+    d_stretch = buf(plan.stretch_words, torch.int32)
+    d_tiles = buf(2 * (plan.total_tiles + 1), torch.int64)
+    d_blk_pos = buf(plan.blkpos_words, torch.int32)
+    d_blk_tab = buf(plan.blocks * png.BLK_TAB_WORDS, torch.int32)
+    d_blk_info = buf(plan.blocks * png.BLK_INFO_WORDS, torch.int64)
+    d_zbuf = buf(plan.zbuf_words, torch.int32)
+    d_img_info = buf(plan.B * png.IMG_INFO_WORDS, torch.int64)
+    d_out = buf(plan.out_bytes, torch.uint8)
+    d_sizes = buf(plan.B, torch.int64)
+    with torch.cuda.device(dev):
+        N.check(lib.mrx_png_encode(
+            d_desc, plan.B, plan.max_n, plan.max_blocks, plan.max_chunks, plan.total_tiles,
+            plan.zbuf_words, d_stream, d_sym, d_stretch, d_tiles, d_blk_pos, d_blk_tab,
+            d_blk_info, d_zbuf, d_img_info, d_out, d_sizes, N.stream_ptr(None)), "mrx_png_encode")
+        sizes = d_sizes.cpu().numpy()
+        offs = plan.desc[:, png.D_OUT_OFF]
+        files = torch.cat([d_out[int(o):int(o) + int(s)] for o, s in zip(offs, sizes)]).cpu()
+    host = files.numpy().tobytes()
+    ends = np.cumsum(sizes)
+    out = [host[int(e - s):int(e)] for s, e in zip(sizes, ends)]
+    if not stats:
+        return (out,)
+    return out, d_img_info.view(plan.B, -1).cpu().numpy(), \
+        d_blk_info.view(plan.blocks, -1).cpu().numpy(), plan
 
 
 def get_anchors(image_shape):
@@ -557,6 +626,26 @@ def unmold_overlay_batch(items, images, colors=None, alpha=0.5):
         counts, metas = st.meta()
         host = [o.cpu().numpy() for o in overlays]
     return [metas[b] + (host[b],) for b in range(st.n)]
+
+
+def _unmold_overlay_png_batch(items, images, colors=None, alpha=0.5):
+    """`unmold_overlay_batch` that stops at the device overlays and encodes them there: returns
+    (boxes, class_ids, scores, png_bytes) per image, the file being what
+    `cv2.imencode('.png', overlay[..., ::-1])` gives for the overlay `unmold_overlay_batch`
+    returns.  Only the PNG bytes leave the device."""
+    from . import visualize
+
+    if len(items) == 0:
+        return []
+    with _Staged(items) as st:
+        eng = st.eng
+        eng.enqueue(st.d_det, st.d_msk)
+        if colors is None:
+            colors = visualize.random_colors(eng.R)
+        overlays = visualize.composite_batch(eng, images, colors, alpha)
+        counts, metas = st.meta()
+        files = encode_png_batch(overlays)
+    return [metas[b] + (files[b],) for b in range(st.n)]
 
 
 def unmold_detections(detections, mrcnn_mask, original_image_shape, image_shape, window):

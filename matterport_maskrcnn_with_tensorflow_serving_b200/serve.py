@@ -19,7 +19,9 @@ without a Python float per element (`wire.py`); without one `grpc_inference` rai
 `do_inference` ends like the reference (serve.py:156-173): the masks are blended into the
 image and the picture is written to `media/mask-<uuid>.png`, whose path is returned.  The
 blend runs on the device canvas the unmold kernels just wrote (`mrx_composite_masks`): the
-105 MB of masks per 1024x1024x100 image never travel to the host.  Boxes, captions and
+105 MB of masks per 1024x1024x100 image never travel to the host, and neither do the blended
+pixels: the PNG file is encoded on the device, byte for byte what `cv2.imwrite` writes
+(`api_utils.encode_png_batch`), and only its bytes are downloaded.  Boxes, captions and
 contour polygons are matplotlib artists in the reference and are not drawn (DESIGN.md 7).
 
 Wherever an image is accepted, a JPEG file's bytes (bytes, bytearray or memoryview) are accepted
@@ -227,15 +229,17 @@ def do_inference_unmolded(img):
         mrcnn_detection, mrcnn_mask, _image_shape(img), molded_image.shape, window)
 
 
-def _save_overlay(overlay_rgb, media_dir=None):
-    """serve.py:156-158,168: media/mask-<uuid4>.png"""
-    import cv2
-
+def _save_png(png_bytes, media_dir=None):
+    """serve.py:156-158,168: media/mask-<uuid4>.png, the file's bytes encoded on the device (what
+    cv2.imwrite of the overlay writes)."""
     media_dir = media_dir if media_dir is not None else getattr(cf, "MEDIA_DIR", "media")
     os.makedirs(media_dir, exist_ok=True)
     save_path = os.path.join(media_dir, "mask-{}.png".format(str(uuid.uuid4())))
-    if not cv2.imwrite(save_path, overlay_rgb[:, :, ::-1]):     # OpenCV writes BGR
-        raise IOError(f"could not write {save_path}")
+    try:
+        with open(save_path, "wb") as f:
+            f.write(png_bytes)
+    except OSError as e:
+        raise IOError(f"could not write {save_path}") from e
     return save_path
 
 
@@ -254,10 +258,10 @@ def do_inference_batch(imgs, colors=None, media_dir=None):
     res, sources = _grpc_inference_batch(imgs)
     items = [(det, msk, tuple(src.shape), mshape, window)
              for (det, msk, mshape, window), src in zip(res, sources)]
-    outs = api_utils.unmold_overlay_batch(items, sources, colors=colors)
+    outs = api_utils._unmold_overlay_png_batch(items, sources, colors=colors)
     paths = []
-    for _boxes, _cls, _scores, overlay in outs:
-        paths.append(_save_overlay(overlay, media_dir))
+    for _boxes, _cls, _scores, png_bytes in outs:
+        paths.append(_save_png(png_bytes, media_dir))
         print(">>> Save image: {}".format(paths[-1]))
     print(">>> Complete!")
     return paths

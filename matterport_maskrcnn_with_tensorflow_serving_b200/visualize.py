@@ -191,7 +191,8 @@ def display_instances(image, boxes, masks, class_ids=None, class_names=None, sco
     """Argument-compatible with the fork's `visualize.display_instances(..., save_path=)`
     (serve.py:160-169).  Computes the masked image (the pixels matplotlib would `imshow`);
     boxes, captions and contours are not drawn.  Returns the uint8 image; writes it to
-    `save_path` (PNG via OpenCV) when given."""
+    `save_path` when given: a `.png` path gets the bytes cv2.imwrite would write, encoded on the
+    device (`api_utils.encode_png_batch`); any other extension goes through cv2.imwrite."""
     n = int(boxes.shape[0])
     if n:
         assert boxes.shape[0] == masks.shape[-1]
@@ -199,7 +200,14 @@ def display_instances(image, boxes, masks, class_ids=None, class_names=None, sco
     out = apply_masks(image, boxes, masks, colors) if (show_mask and n) else \
         np.ascontiguousarray(image).astype(np.uint8).copy()
     if save_path is not None:
-        import cv2
+        if str(save_path).lower().endswith(".png"):
+            # the bytes cv2.imwrite would write, encoded on the device (api_utils.encode_png_batch)
+            from . import api_utils
 
-        cv2.imwrite(save_path, out[:, :, ::-1])   # OpenCV writes BGR
+            with open(save_path, "wb") as f:
+                f.write(api_utils.encode_png_batch([out])[0])
+        else:
+            import cv2
+
+            cv2.imwrite(save_path, out[:, :, ::-1])   # OpenCV writes BGR
     return out

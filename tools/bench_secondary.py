@@ -5,7 +5,7 @@ each unmold workload also names the GPU and its power limit.
 
   python tools/bench_secondary.py [--iters 20] [--cpu]     (--cpu also times the oracle)
   python tools/bench_secondary.py --only-eval | --only-cocoeval | --only-bboxeval | --only-boundaryeval
-                                  | --only-polygons | --only-lvis | --only-jpeg
+                                  | --only-polygons | --only-lvis | --only-jpeg | --only-png
 """
 import argparse
 import json
@@ -1096,6 +1096,87 @@ def jpeg_case(iters):
             **card()}), flush=True)
 
 
+def png_case(iters):
+    """Overlay PNG files encoded on the device (csrc/png.cu) against cv2.imencode on the host:
+    32 x 1024^2 and 16 x 2160x3840 overlays, and the tail of do_inference_batch that changed
+    (unmold + overlay + PNG files written) before (overlays downloaded, cv2.imwrite) and after
+    (encoded on the device, bytes written)."""
+    import tempfile
+    from concurrent.futures import ThreadPoolExecutor
+
+    import cv2
+
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, visualize
+
+    from torch.profiler import ProfilerActivity, profile
+
+    for name, batch, hw, n in [("32 x 1024x1024", 32, (1024, 1024), 100),
+                               ("configs[3] size: 16 x 2160x3840", 16, (2160, 3840), 50)]:
+        ims = synth.make_batch(5, 4, hw, n, num_classes=81)
+        items = [(ims[b % 4].detections, ims[b % 4].mrcnn_mask, ims[b % 4].original_image_shape,
+                  ims[b % 4].image_shape, ims[b % 4].window) for b in range(batch)]
+        rng = np.random.default_rng(3)
+        base = [synth.synth_rgb_image(rng, *hw) for _ in range(4)]
+        images = [base[b % 4] for b in range(batch)]
+        colors = visualize.random_colors(n)
+        overlays = [o[3] for o in api_utils.unmold_overlay_batch(items[:4], images[:4], colors)]
+        host = [overlays[b % 4] for b in range(batch)]
+        dev = [torch.from_numpy(h).cuda() for h in host]
+        files = api_utils.encode_png_batch(dev)
+        mb = sum(len(f) for f in files) / 1e6
+        api_utils.encode_png_batch(dev)
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(5):
+                api_utils.encode_png_batch(dev)
+            torch.cuda.synchronize()
+        kern = {}
+        for ev in prof.key_averages():
+            if "png_" in ev.key:
+                short = ev.key.split("png_")[1].split("_kernel")[0]
+                kern[short] = round(kern.get(short, 0) + ev.device_time_total / 1e3 / 5, 4)
+        enc_ms, _ = time_ms(lambda: api_utils.encode_png_batch(dev), iters)
+
+        def host_clock(fn, k):
+            fn()
+            ts = []
+            for _ in range(k):
+                t0 = time.perf_counter()
+                fn()
+                torch.cuda.synchronize()
+                ts.append((time.perf_counter() - t0) * 1e3)
+            return float(np.median(ts))
+
+        enc = lambda a: cv2.imencode(".png", a[:, :, ::-1])[1]     # noqa: E731
+        k = max(3, iters // 4)
+        one_ms = host_clock(lambda: [enc(a) for a in host], k)
+        with ThreadPoolExecutor(16) as pool:
+            pool_ms = host_clock(lambda: list(pool.map(enc, host)), k)
+        with tempfile.TemporaryDirectory() as tmp:
+            def before():
+                outs = api_utils.unmold_overlay_batch(items, images, colors)
+                for b, o in enumerate(outs):
+                    cv2.imwrite(os.path.join(tmp, f"{b}.png"), o[3][:, :, ::-1])
+
+            def after():
+                outs = api_utils._unmold_overlay_png_batch(items, images, colors)
+                for b, o in enumerate(outs):
+                    with open(os.path.join(tmp, f"{b}.png"), "wb") as f:
+                        f.write(o[3])
+
+            before_ms = host_clock(before, k)
+            after_ms = host_clock(after, k)
+        print(json.dumps({
+            "workload": f"PNG encode {name} overlays ({mb:.1f} MB of files)",
+            "kernel_ms": kern, "kernel_ms_total": round(sum(kern.values()), 3),
+            "api_utils_encode_png_batch_ms": round(enc_ms, 3),
+            "host_imencode_one_thread_ms": round(one_ms, 3),
+            "host_imencode_16_threads_ms": round(pool_ms, 3),
+            "do_inference_batch_tail_before_ms": round(before_ms, 3),
+            "do_inference_batch_tail_after_ms": round(after_ms, 3),
+            "host_threads": os.cpu_count(), **card()}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
@@ -1109,8 +1190,12 @@ def main():
                     "record")
     ap.add_argument("--only-lvis", action="store_true", help="only the LVIS mask AP record")
     ap.add_argument("--only-jpeg", action="store_true", help="only the JPEG decode record")
+    ap.add_argument("--only-png", action="store_true", help="only the PNG encode record")
     args = ap.parse_args()
     torch.cuda.set_device(0)
+    if args.only_png:
+        png_case(args.iters)
+        return
     if args.only_jpeg:
         jpeg_case(args.iters)
         return
