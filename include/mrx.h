@@ -28,7 +28,9 @@
  *   mrx_jpeg_coefficients / _pixels <- api_utils.load_img (cv2.imread)   serve.py:85-86
  *                             (extension: JPEG request bytes decoded on the device, as cv2.imdecode;
  *                             mrx_jpeg_progressive_coefficients for progressive files)
- *   mrx_png_encode         <- cv2.imwrite of the overlay PNG                 serve.py:168
+ *   mrx_png_decode         <- api_utils.load_img (cv2.imread)   serve.py:85-86
+ *                             (extension: PNG request bytes decoded on the device, as cv2.imdecode)
+ *   mrx_png_encode        <- cv2.imwrite of the overlay PNG                 serve.py:168
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
  *   mrx_device_alloc/_free (the canvas allocation: compressible device memory where offered)
  *
@@ -704,6 +706,68 @@ int mrx_png_encode(const long long *d_desc, int B, long long max_n, int max_bloc
                    unsigned char *d_stream, short *d_sym, int *d_stretch, long long *d_tiles,
                    int *d_blk_pos, int *d_blk_tab, long long *d_blk_info, unsigned int *d_zbuf,
                    long long *d_img_info, unsigned char *d_out, long long *d_sizes, void *stream);
+
+/* ---------------------------------------------------------------- PNG decode (load_img) */
+/* PNG files decoded bit for bit as cv2.imdecode(buf, IMREAD_COLOR) then BGR2RGB (libpng:
+ * strip_16, gray 1/2/4 expanded by bit replication, palette to RGB with indices past PLTE giving
+ * 0,0,0, gray to RGB, alpha dropped, Adam7; EXIF orientation; csrc/png_decode.cu).  The host
+ * (png.DecodePlan) parses every chunk but the image data and lays the batch out: the files at
+ * d_files, d_desc [B, 16] int64 words per image (png.py's DD_* indices: the image's zlib stream
+ * and filtered stream offsets and lengths, geometry, colour type, bit depth, interlace,
+ * orientation, palette length, block-list offset and capacity, window size, candidate tiles),
+ * d_chunks [n_chunks, 4] int64 words per IDAT chunk (image, file offset of its type, data
+ * length, offset in the image's zlib stream), d_plte [B, 768] (each image's palette).  Buffers,
+ * each sized by png.DecodePlan from the headers and file lengths alone:
+ *   d_z        uint8: each image's IDAT payloads, concatenated (its zlib stream)
+ *   d_tile_cnt int32 [total_tiles]: candidate block starts found per tile of
+ *              MRX_PNG_DEC_TILE_BITS stream bits (zeroed here first)
+ *   d_cand     int64 [total_tiles, K]: their bit positions (the first K of each tile)
+ *   d_meas     int64 [total_tiles, K, 4]: each candidate's end bit, bytes, reach before the
+ *              block, valid | BFINAL << 1
+ *   d_cells    int32: per filtered byte, a value or a reference to an earlier byte
+ *   d_filt     uint8: each image's filtered rows, exactly n = sum over passes of rows x (1 + row
+ *              bytes), unfiltered in place
+ *   d_blocks   int64 [blocks, 2]: per image, the first bit (in its zlib stream) and the output
+ *              offset of each block, up to the image's capacity (past it the image is expanded
+ *              by one warp, in order)
+ *   d_info     int64 [B, MRX_PNG_DEC_INFO_WORDS] (MRX_PNG_DEC_*), zeroed here first
+ *   d_status   int32 [B] (zeroed here first): MRX_PNG_ST_* bits; an image with a bit is not written
+ *   d_out      uint8 RGB [H', W', 3] at d_out + d_out_off[b]: the slots mrx_jpeg_pixels writes.
+ * K: candidate slots per tile, 0 to measure every block in the chain.  An error in the deflate
+ * stream is refused when libpng meets it before it has every row (a distance too far back:
+ * before it needs a byte past the rows); later ones end the stream, as libpng only warns there.
+ * The Adler-32 trailer is checked when the stream holds exactly the image's rows.  max_n,
+ * max_pixels, max_zlen, max_tiles, max_blocks: the batch's largest filtered length, pixel count,
+ * zlib length, tile count and block capacity.  Checks: null pointers, B outside
+ * [0, MRX_MAX_BATCH], n_chunks outside [B, 2^31], max_n outside [2, MRX_PNG_DEC_MAX_FILTERED],
+ * max_pixels outside [1, 2^30], max_zlen outside [2, MRX_PNG_DEC_MAX_FILE], K outside
+ * [0, MRX_PNG_DEC_MAX_SLOTS], a tile or block extent below 1: MRX_E_INVALID.  B = 0 returns MRX_OK
+ * without launching anything. */
+#define MRX_PNG_DEC_MAX_FILE     (1 << 27)   /* bytes per file: bit positions stay in int32 */
+#define MRX_PNG_DEC_MAX_FILTERED (1 << 30)   /* filtered bytes per image: positions in int32 */
+#define MRX_PNG_DEC_TILE_BITS    1024        /* stream bits per candidate tile */
+#define MRX_PNG_DEC_MAX_SLOTS    32          /* candidate slots per tile */
+#define MRX_PNG_ST_CRC    1    /* an IDAT chunk's CRC-32 */
+#define MRX_PNG_ST_TRUNC  2    /* the stream ends before the image's last row or its trailer */
+#define MRX_PNG_ST_CODE   4    /* an invalid block type, code set, code or stored length */
+#define MRX_PNG_ST_DIST   8    /* a distance past the stream start or the window */
+#define MRX_PNG_ST_ADLER  16   /* the Adler-32 trailer of a stream of exactly the image's rows */
+#define MRX_PNG_ST_FILTER 32   /* a filter type above 4 */
+#define MRX_PNG_DEC_NBLK    0   /* deflate blocks chained */
+#define MRX_PNG_DEC_SEQ     1   /* of them, measured by the chain itself */
+#define MRX_PNG_DEC_OUT     2   /* bytes the chained blocks describe */
+#define MRX_PNG_DEC_ADLER   3   /* the trailer when checked, else -1 */
+#define MRX_PNG_DEC_ADLER_A 4
+#define MRX_PNG_DEC_ADLER_B 5
+#define MRX_PNG_DEC_CAND    6   /* candidate block starts found */
+#define MRX_PNG_DEC_INFO_WORDS 8
+int mrx_png_decode(const unsigned char *d_files, const long long *d_desc,
+                   const long long *d_chunks, const unsigned char *d_plte, int B,
+                   long long n_chunks, long long max_n, long long max_pixels, long long max_zlen,
+                   long long max_tiles, long long total_tiles, long long max_blocks, int K,
+                   unsigned char *d_z, long long *d_cand, int *d_tile_cnt, long long *d_meas,
+                   int *d_cells, unsigned char *d_filt, long long *d_blocks, long long *d_info,
+                   int *d_status, unsigned char *d_out, const long long *d_out_off, void *stream);
 
 /* ---------------------------------------------------------------- multi-GPU gather (8e) */
 /* Peer-memory plumbing for the final gather of the canvases to rank 0 (one process per GPU).

@@ -13,8 +13,8 @@ serve.py:48): `unmold_detections_batch`, `unmold_detections_packed_batch`,
 `unmold_coco_results_batch` (upstream's `build_coco_results` of the unmolded detections),
 `unmold_compute_ap_batch` (upstream's `compute_ap` of them against ground truth) and
 `unmold_coco_eval_batch` (pycocotools' COCOeval "segm" of them, streamed batch by batch), and
-`decode_jpeg_batch` / `encode_png_batch` (request JPEG bytes in, response PNG bytes out, each as
-OpenCV would decode or write them).
+`decode_jpeg_batch` / `decode_png_batch` / `encode_png_batch` (request JPEG or PNG bytes in,
+response PNG bytes out, each as OpenCV would decode or write them).
 
 Numerical contract (checked by tests/ against the float64 oracle): N, boxes, class ids and
 scores are bit-exact.  The mask resize runs in float32 on exact integer source coordinates;
@@ -94,6 +94,22 @@ def decode_jpeg_batch(blobs):
         if m is None or m.config is not get_config():
             m = _state["molder"] = Molder(get_config())
         return m.decode_jpeg_batch(list(blobs))
+
+
+def decode_png_batch(blobs):
+    """PNG files (bytes, bytearray or memoryview) -> one uint8 [H, W, 3] RGB CUDA tensor each,
+    equal bit for bit to `load_img` of the same file (cv2.imdecode, BGR -> RGB), decoded on the
+    device (csrc/png_decode.cu): every colour type and bit depth, Adam7, EXIF orientation.  A file
+    the decoder does not accept raises ValueError naming its index and the reason before anything
+    is uploaded; corrupt image data (a CRC, code, distance, Adler-32 or filter error libpng would
+    refuse) raises ValueError after the decode."""
+    from .engine import Molder
+
+    with _jpeg_lock:     # the decoders share the Molder's buffers
+        m = _state.get("molder")
+        if m is None or m.config is not get_config():
+            m = _state["molder"] = Molder(get_config())
+        return m.decode_png_batch(list(blobs))
 
 
 def encode_png_batch(images):

@@ -16,6 +16,7 @@
 //   frame    one warp per block: block header, tree description, end-of-block code, LEN/NLEN
 //   file     one warp per IDAT chunk: chunk bytes and CRC-32; signature, IHDR and IEND
 #include "common.cuh"
+#include "deflate.cuh"
 
 namespace mrx {
 namespace {
@@ -24,14 +25,10 @@ constexpr int kThreads = 256;
 constexpr int kItems = 8;
 constexpr int kTile = kThreads * kItems;   // png.TILE
 constexpr int kSyms = 16383;               // symbols per block (zlib's lit_bufsize - 1)
-constexpr int kMaxMatch = 258;
-constexpr int kLCodes = 286, kDCodes = 30, kBLCodes = 19;
 constexpr int kHeap = 2 * kLCodes + 1;
-constexpr int kEndBlock = 256;
 constexpr int kTabWords = 654;             // per block: freq[287], code[287], header bits[80]
 constexpr int kFreq = 0, kCode = 287, kHdr = 574, kHdrWords = 80;
 constexpr int kIdat = 8192;
-constexpr unsigned kMod = 65521;
 
 // desc words per image (png.py D_*)
 enum {
@@ -42,18 +39,6 @@ enum {
 // per block int64 (MRX_PNG_BLK_*) and per image int64 (MRX_PNG_IMG_*)
 enum { BK_TYPE = 0, BK_LAST, BK_HDR_BITS, BK_DATA_BITS, BK_EOB, BK_BIT, BK_PBASE, BK_BITS };
 enum { IM_NSYM = 0, IM_NBLK, IM_ADLER_A, IM_ADLER_B, IM_BITS, IM_ZLEN, IM_CHUNKS, IM_FILE };
-
-__constant__ unsigned char c_extra_lbits[29] = {0, 0, 0, 0, 0, 0, 0, 0, 1, 1, 1, 1, 2, 2, 2,
-                                                2, 3, 3, 3, 3, 4, 4, 4, 4, 5, 5, 5, 5, 0};
-__constant__ unsigned char c_extra_dbits[30] = {0, 0, 0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 5, 5, 6,
-                                                6, 7, 7, 8, 8, 9, 9, 10, 10, 11, 11, 12, 12, 13, 13};
-__constant__ unsigned char c_extra_blbits[19] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0,
-                                                 0, 0, 0, 0, 0, 0, 2, 3, 7};
-__constant__ unsigned char c_bl_order[19] = {16, 17, 18, 0, 8, 7, 9, 6, 10, 5,
-                                             11, 4, 12, 3, 13, 2, 14, 1, 15};
-__constant__ unsigned char c_base_length[29] = {0,  1,  2,  3,  4,  5,   6,   7,   8,   10,
-                                                12, 14, 16, 20, 24, 28,  32,  40,  48,  56,
-                                                64, 80, 96, 112, 128, 160, 192, 224, 255};
 
 __device__ __forceinline__ int length_code(int lc) {   // zlib's _length_code[lc]
   int c = 28;
@@ -738,30 +723,6 @@ __global__ void __launch_bounds__(32) png_frame_kernel(const long long *__restri
 }
 
 // ------------------------------------------------------------------ file
-constexpr unsigned kPoly = 0xEDB88320u;
-
-__device__ unsigned multmodp(unsigned a, unsigned b) {   // a * b modulo the CRC polynomial
-  unsigned m = 1u << 31, p = 0;
-  for (;;) {
-    if (a & m) {
-      p ^= b;
-      if ((a & (m - 1)) == 0) break;
-    }
-    m >>= 1;
-    b = b & 1 ? (b >> 1) ^ kPoly : b >> 1;
-  }
-  return p;
-}
-
-// crc32(A || B) from crc32(A), crc32(B) and |B|; x2n[k] = x^(2^k) modulo the polynomial
-__device__ unsigned crc_combine(const unsigned *x2n, unsigned c1, unsigned c2, long long len2) {
-  unsigned p = 1u << 31;
-  int k = 3;
-  for (long long n = len2; n; n >>= 1, ++k)
-    if (n & 1) p = multmodp(x2n[k & 31], p);
-  return multmodp(p, c1) ^ c2;
-}
-
 constexpr int kFileWarps = 4;
 
 __global__ void __launch_bounds__(32 * kFileWarps) png_file_kernel(
@@ -769,16 +730,7 @@ __global__ void __launch_bounds__(32 * kFileWarps) png_file_kernel(
     const long long *__restrict__ img_info, unsigned char *__restrict__ out) {
   __shared__ unsigned table[256];
   __shared__ unsigned x2n[32];
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) {
-    unsigned c = unsigned(i);
-    for (int j = 0; j < 8; ++j) c = c & 1 ? (c >> 1) ^ kPoly : c >> 1;
-    table[i] = c;
-  }
-  if (threadIdx.x == 0) {
-    unsigned p = 1u << 30;   // x^1
-    x2n[0] = p;
-    for (int i = 1; i < 32; ++i) x2n[i] = p = multmodp(p, p);
-  }
+  crc_tables(table, x2n);
   __syncthreads();
   const int b = blockIdx.y, lane = threadIdx.x & 31;
   const long long c = (long long)blockIdx.x * kFileWarps + (threadIdx.x >> 5);
@@ -792,7 +744,7 @@ __global__ void __launch_bounds__(32 * kFileWarps) png_file_kernel(
   const unsigned adler = (bb << 16) | a;
   const unsigned char *zb = reinterpret_cast<const unsigned char *>(zbuf + D[D_ZBUF_OFF]);
   unsigned char *o = out + D[D_OUT_OFF];
-  auto crc_bytes = [&](unsigned crc, unsigned char v) { return table[(crc ^ v) & 0xFF] ^ (crc >> 8); };
+  auto crc_bytes = [&](unsigned crc, unsigned char v) { return crc_byte(table, crc, v); };
   if (c == 0 && lane == 0) {
     const unsigned char sig[8] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1A, '\n'};
     for (int i = 0; i < 8; ++i) o[i] = sig[i];

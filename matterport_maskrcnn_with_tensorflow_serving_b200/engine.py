@@ -1656,7 +1656,7 @@ class Molder:
     def jpeg_decode_into(self, plan, d_out, out_off, stream=None, d_status=None):
         """Enqueue the decode of every file of `plan` (a `jpeg.Plan` or `jpeg.ProgressivePlan`)
         into the uint8 slots d_out + out_off[b] (int64 byte offsets; image b is plan.shapes[b]).
-        Returns d_status [B] (device; `d_status` when given); call `jpeg_check` on it once the
+        Returns d_status [B] (device; `d_status` when given); call `files_check` on it once the
         work that reads the slots has been enqueued."""
         from . import jpeg
 
@@ -1677,64 +1677,129 @@ class Molder:
             "mrx_jpeg_pixels")
         return d_status
 
-    def jpeg_decode_files_into(self, plans, d_out, out_off, stream=None):
-        """Enqueue the decode of a batch split by `jpeg.plan_batch` ([(plan, positions)]) into the
-        slots d_out + out_off[position].  Every plan writes its part of one status buffer, in
-        plan order.  Returns (d_status, positions in that order) for `jpeg_check`."""
+    # ------------------------------------------------------------------ PNG (csrc/png_decode.cu)
+    def png_decode_into(self, plan, d_out, out_off, stream=None, d_status=None):
+        """Enqueue `mrx_png_decode` for a `png.DecodePlan` into the uint8 slots d_out + out_off[b]
+        (int64 byte offsets; image b is plan.shapes[b]).  Returns (d_status [B] int32, d_info
+        [B, 8] int64 (mrx.h MRX_PNG_DEC_*), d_blocks [blocks, 2] int64) on the device; call
+        `files_check` on the status once the work that reads the slots has been enqueued."""
+        from . import png
+
+        torch = _torch()
+        parts = [plan.desc.view(np.uint8).reshape(-1), plan.chunks.view(np.uint8).reshape(-1),
+                 np.ascontiguousarray(out_off, dtype=np.int64).view(np.uint8),
+                 plan.plte.reshape(-1), plan.files]
+        v = self._jpeg_upload_parts(parts, "png_")
+        d_desc, d_chunks, d_off = v[0].view(torch.int64), v[1].view(torch.int64), \
+            v[2].view(torch.int64)
+        d_plte, d_files = v[3], v[4]
+        d_z = self._jpeg_buffer("png_z", plan.z_bytes, torch.uint8)
+        slots = plan.total_tiles * max(plan.K, 1)
+        d_cand = self._jpeg_buffer("png_cand", slots, torch.int64)
+        d_tile_cnt = self._jpeg_buffer("png_tile_cnt", plan.total_tiles, torch.int32)
+        d_meas = self._jpeg_buffer("png_meas", 4 * slots, torch.int64)
+        d_cells = self._jpeg_buffer("png_cells", plan.filt_bytes, torch.int32)
+        d_filt = self._jpeg_buffer("png_filt", plan.filt_bytes, torch.uint8)
+        d_blocks = self._jpeg_buffer("png_blocks", plan.block_words, torch.int64)
+        d_info = self._jpeg_buffer("png_info", plan.B * png.DEC_INFO_WORDS, torch.int64)
+        if d_status is None:
+            d_status = self._jpeg_buffer("png_status", plan.B, torch.int32)
+        N.check(self.lib.mrx_png_decode(
+            d_files, d_desc, d_chunks, d_plte, plan.B, plan.n_chunks, plan.max_n,
+            plan.max_pixels, plan.max_zlen, plan.max_tiles, plan.total_tiles, plan.max_blocks,
+            plan.K, d_z, d_cand, d_tile_cnt, d_meas, d_cells, d_filt, d_blocks, d_info, d_status,
+            d_out, d_off, N.stream_ptr(stream)), "mrx_png_decode")
+        return (d_status[:plan.B], d_info[:plan.B * png.DEC_INFO_WORDS].view(plan.B, -1),
+                d_blocks[:plan.block_words].view(-1, 2))
+
+    # ------------------------------------------------------------------ files of either format
+    def decode_files_into(self, plans, d_out, out_off, stream=None):
+        """Enqueue the decode of a batch split by `imagefile.plan_batch` or `jpeg.plan_batch`
+        ([(plan, positions)]) into the slots d_out + out_off[position].  Every plan writes its
+        part of one status buffer, in plan order.  Returns (d_status, positions in that order,
+        their formats) for `files_check`."""
+        from . import png
+
         torch = _torch()
         n = sum(len(pos) for _, pos in plans)
         d_status = self._jpeg_buffer("status_all", n, torch.int32)[:n]
-        order, lo = [], 0
+        order, formats, lo = [], [], 0
         for plan, pos in plans:
-            self.jpeg_decode_into(plan, d_out, np.asarray(out_off)[pos], stream,
-                                  d_status[lo:lo + len(pos)])
+            st, off = d_status[lo:lo + len(pos)], np.asarray(out_off)[pos]
+            if isinstance(plan, png.DecodePlan):
+                self.png_decode_into(plan, d_out, off, stream, st)
+                formats += ["png"] * len(pos)
+            else:
+                self.jpeg_decode_into(plan, d_out, off, stream, st)
+                formats += ["jpeg"] * len(pos)
             order += list(pos)
             lo += len(pos)
-        return d_status, order
+        return d_status, order, formats
 
     @staticmethod
-    def jpeg_check(d_status, index=None):
+    def files_check(d_status, index, formats):
         """Download the status words (the one synchronisation) and raise ValueError naming the
-        first image whose entropy-coded data was corrupt.  index[b]: the caller's index of b."""
-        from . import jpeg
+        first image whose data was corrupt.  index[b]: the caller's index of b; formats[b]: its
+        format ("jpeg" or "png")."""
+        from . import jpeg, png
 
         st = d_status.cpu().numpy()
         for b in np.flatnonzero(st):
-            i = int(index[b]) if index is not None else int(b)
+            i = int(index[b])
+            if formats[b] == "png":
+                raise png.PngError(f"image {i}: corrupt PNG data ({png.status_reasons(st[b])})")
             raise jpeg.JpegError(f"image {i}: corrupt JPEG data ({jpeg.status_reasons(st[b])})")
+
+    def _decode_to_tensors(self, plans, shapes, stream):
+        torch = _torch()
+        if not shapes:
+            return []
+        sizes = np.asarray([h * w * 3 for h, w, _ in shapes], dtype=np.int64)
+        off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        out = torch.empty((int(off[-1]),), dtype=torch.uint8, device=self.device)
+        self.files_check(*self.decode_files_into(plans, out, off[:-1], stream))
+        return [out[int(off[b]):int(off[b + 1])].view(shapes[b]) for b in range(len(shapes))]
 
     def decode_jpeg_batch(self, blobs, S=None, stream=None):
         """uint8 [H, W, 3] RGB CUDA tensors, one per JPEG file: cv2.imdecode + BGR2RGB bit for
         bit.  The images share one buffer; equal sizes make them one contiguous [B, H, W, 3]."""
         from . import jpeg
 
-        torch = _torch()
         plans, shapes = jpeg.plan_batch(blobs, S=jpeg.DEFAULT_S if S is None else S)
-        if not shapes:
-            return []
-        sizes = np.asarray([h * w * 3 for h, w, _ in shapes], dtype=np.int64)
-        off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
-        out = torch.empty((int(off[-1]),), dtype=torch.uint8, device=self.device)
-        self.jpeg_check(*self.jpeg_decode_files_into(plans, out, off[:-1], stream))
-        return [out[int(off[b]):int(off[b + 1])].view(shapes[b]) for b in range(len(shapes))]
+        return self._decode_to_tensors(plans, shapes, stream)
+
+    def decode_png_batch(self, blobs, stream=None, slots=None):
+        """`decode_jpeg_batch` for PNG files (`png.DecodePlan`; slots: its candidate slots per
+        tile, 0 to measure every deflate block in the chain)."""
+        from . import png
+
+        plan = png.DecodePlan(list(blobs), slots=png.DEFAULT_SLOTS if slots is None else slots)
+        return self._decode_to_tensors([(plan, list(range(plan.B)))] if plan.B else [],
+                                       plan.shapes, stream)
+
+    def decode_files(self, blobs, stream=None):
+        """`decode_jpeg_batch` for JPEG and PNG files mixed, routed by their signature."""
+        from . import imagefile
+
+        plans, shapes, _ = imagefile.plan_batch(list(blobs))
+        return self._decode_to_tensors(plans, shapes, stream)
 
     # ------------------------------------------------------------------ batched (one launch each)
     def stage_images(self, images, align=16, stream=None):
         """Every image in its slot of one device buffer: uint8 HxWx3 NumPy images through one
-        pinned staging buffer and one H2D copy, JPEG files (bytes) decoded on the device into
-        their slots.  Returns (d_src, off [B+1] int64 slot offsets, shapes, d_status or None,
-        jidx: the indices of the JPEG items).  Call `jpeg_check(d_status, jidx)` once the work
-        that reads the slots has been enqueued."""
-        from . import jpeg
+        pinned staging buffer and one H2D copy, JPEG and PNG files (bytes) decoded on the device
+        into their slots.  Returns (d_src, off [B+1] int64 slot offsets, shapes, status, fidx: the
+        indices of the file items), status being None without files, else the arguments of
+        `files_check`: call it once the work that reads the slots has been enqueued."""
+        from . import imagefile
 
         torch = _torch()
         B = len(images)
-        is_jpeg = [isinstance(im, (bytes, bytearray, memoryview)) for im in images]
-        jidx = [b for b in range(B) if is_jpeg[b]]
-        plans, jshapes = jpeg.plan_batch([images[b] for b in jidx], index=jidx)
+        fidx = [b for b in range(B) if isinstance(images[b], (bytes, bytearray, memoryview))]
+        plans, fshapes, _ = imagefile.plan_batch([images[b] for b in fidx], index=fidx)
         shapes = [None] * B
-        for k, b in enumerate(jidx):
-            shapes[b] = jshapes[k]
+        for k, b in enumerate(fidx):
+            shapes[b] = fshapes[k]
         for b in range(B):
             if shapes[b] is None:
                 shapes[b] = tuple(int(v) for v in images[b].shape)
@@ -1744,27 +1809,28 @@ class Molder:
         if getattr(self, "_h_stage", None) is None or self._h_stage.numel() < total:
             self._h_stage = torch.empty((total,), dtype=torch.uint8).pin_memory()
         hs = self._h_stage.numpy()
+        is_file = set(fidx)
         for b, im in enumerate(images):
-            if not is_jpeg[b]:
+            if b not in is_file:
                 hs[int(off[b]):int(off[b]) + sizes[b]] = np.ascontiguousarray(im).reshape(-1)
         d_src = self._h_stage[:total].to(self.device, non_blocking=True)
-        d_status = None
-        if jidx:
-            d_status, order = self.jpeg_decode_files_into(plans, d_src, off[jidx], stream)
-            jidx = [jidx[k] for k in order]
-        return d_src, off, shapes, d_status, jidx
+        status = None
+        if fidx:
+            d_status, order, formats = self.decode_files_into(plans, d_src, off[fidx], stream)
+            status = (d_status, [fidx[k] for k in order], formats)
+        return d_src, off, shapes, status, fidx
 
     # ------------------------------------------------------------------ batched (one launch each)
     def cv2_resize_batch_device(self, images, size_hw, stream=None, return_sources=False):
         """`cv2.resize(img, (S, S))` for a list of images of ANY sizes in one launch: uint8 HxWx3
-        NumPy images or JPEG files as bytes, staged by `stage_images` (JPEG files decoded on the
+        NumPy images or JPEG / PNG files as bytes, staged by `stage_images` (files decoded on the
         device into their slots).  Returns uint8 [B, dh, dw, 3] on the device; with
-        return_sources also each image's pixels for later steps: the array itself, or for a JPEG
+        return_sources also each image's pixels for later steps: the array itself, or for a
         file its decoded slot (uint8 [H, W, 3] on the device)."""
         torch = _torch()
         B = len(images)
         dh, dw = int(size_hw[0]), int(size_hw[1])
-        d_src, off, shapes, d_status, jidx = self.stage_images(images, 16, stream)
+        d_src, off, shapes, status, fidx = self.stage_images(images, 16, stream)
         hw = np.asarray([sh[:2] for sh in shapes], dtype=np.int32).reshape(B, 2)
         d_off = torch.from_numpy(off[:B].copy()).to(self.device)
         d_hw = torch.from_numpy(hw).to(self.device)
@@ -1772,12 +1838,12 @@ class Molder:
         N.check(self.lib.mrx_cv2_resize_u8c3_batch(
             d_src, d_off, d_hw, out, B, dh, dw, N.stream_ptr(stream)),
             "mrx_cv2_resize_u8c3_batch")
-        if d_status is not None:
-            self.jpeg_check(d_status, jidx)
+        if status is not None:
+            self.files_check(*status)
         if not return_sources:
             return out
         sources = [d_src[int(off[b]):int(off[b]) + int(np.prod(shapes[b]))].view(shapes[b])
-                   if b in jidx else images[b] for b in range(B)]
+                   if b in fidx else images[b] for b in range(B)]
         return out, sources
 
     def mold_batch_device(self, d_imgs, out_dtype=np.float32, stream=None):

@@ -17,9 +17,9 @@ JWRN_BOGUS_PROGRESSION).  Anything else raises `JpegError` (a ValueError) naming
 """
 from __future__ import annotations
 
-import struct
-
 import numpy as np
+
+from . import exif
 
 # zig-zag index -> natural (row-major) index, with libjpeg's 16 guard entries for a corrupt run
 ZIGZAG = np.array([
@@ -116,27 +116,7 @@ def _exif_orientation(seg):
     """IFD0 tag 0x0112 of an APP1 Exif payload, or 1."""
     if len(seg) < 14 or seg[:6] != b"Exif\x00\x00":
         return None
-    t = seg[6:]
-    if t[:2] == b"II":
-        e = "<"
-    elif t[:2] == b"MM":
-        e = ">"
-    else:
-        return 1
-    try:
-        if struct.unpack(e + "H", t[2:4])[0] != 42:
-            return 1
-        ifd = struct.unpack(e + "I", t[4:8])[0]
-        n = struct.unpack(e + "H", t[ifd:ifd + 2])[0]
-        for i in range(n):
-            p = ifd + 2 + 12 * i
-            tag, typ, cnt = struct.unpack(e + "HHI", t[p:p + 8])
-            if tag == 0x0112 and typ == 3:
-                v = struct.unpack(e + "H", t[p + 8:p + 10])[0]
-                return v if 1 <= v <= 8 else 1
-    except struct.error:
-        return 1
-    return 1
+    return exif.orientation(seg[6:])
 
 
 class _Markers:

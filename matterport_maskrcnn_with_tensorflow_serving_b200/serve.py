@@ -24,9 +24,10 @@ pixels: the PNG file is encoded on the device, byte for byte what `cv2.imwrite` 
 (`api_utils.encode_png_batch`), and only its bytes are downloaded.  Boxes, captions and
 contour polygons are matplotlib artists in the reference and are not drawn (DESIGN.md 7).
 
-Wherever an image is accepted, a JPEG file's bytes (bytes, bytearray or memoryview) are accepted
-too: they are decoded on the device (`api_utils.decode_jpeg_batch`, bit for bit as `load_img`), so
-the decoded pixels never reach the host.  A `str` path still goes through `load_img`.
+Wherever an image is accepted, a JPEG or PNG file's bytes (bytes, bytearray or memoryview) are
+accepted too, told apart by their signature (`imagefile`): they are decoded on the device
+(`api_utils.decode_jpeg_batch`, `api_utils.decode_png_batch`, bit for bit as `load_img`), so the
+decoded pixels never reach the host.  A `str` path still goes through `load_img`.
 """
 from __future__ import annotations
 
@@ -38,7 +39,7 @@ import numpy as np
 
 from . import api_utils
 from . import configs as cf
-from . import wire
+from . import imagefile, wire
 from .engine import Molder
 
 _predict_fn = None
@@ -67,16 +68,17 @@ def _get_molder():
     return _molder
 
 
-def _is_jpeg(img):
+def _is_file(img):
     return isinstance(img, (bytes, bytearray, memoryview))
 
 
-def _check_image(img):
-    """An image argument: a path (loaded by `load_img`), JPEG bytes (kept for the device decoder)
-    or an HxWx3 uint8 array."""
+def _check_image(img, index=0):
+    """An image argument: a path (loaded by `load_img`), JPEG or PNG bytes (kept for the device
+    decoders; anything else raises ValueError) or an HxWx3 uint8 array."""
     if isinstance(img, str):
         img = api_utils.load_img(img)
-    if _is_jpeg(img):
+    if _is_file(img):
+        imagefile.kind(img, index)
         return img
     img = np.asarray(img)
     if img.dtype != np.uint8 or img.ndim != 3 or img.shape[2] != 3:
@@ -85,11 +87,9 @@ def _check_image(img):
 
 
 def _image_shape(img):
-    """(H, W, 3) of a checked image argument; for JPEG bytes from the header alone."""
-    if _is_jpeg(img):
-        from . import jpeg
-
-        return jpeg.parse(img).shape
+    """(H, W, 3) of a checked image argument; for a file from its headers alone."""
+    if _is_file(img):
+        return imagefile.shape(img)
     return tuple(img.shape)
 
 
@@ -103,8 +103,8 @@ def preprocess_input(img, img_size=640, molded_dtype=np.float64):
     img = _check_image(img)
     with _molder_lock:
         molder = _get_molder()
-        if _is_jpeg(img):
-            d_img, = molder.decode_jpeg_batch([img])
+        if _is_file(img):
+            d_img, = molder.decode_files([img])
         else:
             d_img = torch.from_numpy(np.ascontiguousarray(img)).to(molder.device)
         if img_size is not None:
@@ -128,13 +128,13 @@ def preprocess_input_batch(imgs, img_size=640, molded_dtype=np.float32):
     (molded_images [B,H,W,3], image_metas [B,M], anchors [A,4] (shared), windows: list of
     4-tuples) -- row b equals `preprocess_input(imgs[b], img_size, molded_dtype)`.
     Default dtype float32: what serve.py:117 puts on the wire."""
-    imgs = [_check_image(im) for im in imgs]
+    imgs = [_check_image(im, i) for i, im in enumerate(imgs)]
     return _preprocess_batch(imgs, img_size, molded_dtype)[:4]
 
 
 def _preprocess_batch(imgs, img_size, molded_dtype):
     """`preprocess_input_batch` of checked images, plus each image's pixels for the overlay: the
-    array itself, or for JPEG bytes its decoded slot of the buffer the resize read (uint8
+    array itself, or for file bytes its decoded slot of the buffer the resize read (uint8
     [H, W, 3] on the device, consumed in place)."""
     import torch
 
@@ -146,23 +146,23 @@ def _preprocess_batch(imgs, img_size, molded_dtype):
         if img_size is not None:
             d_imgs, sources = molder.cv2_resize_batch_device(imgs, (img_size, img_size),
                                                              return_sources=True)
-            d_status = None
+            status = None
         else:
             shapes = [_image_shape(im) for im in imgs]
             if any(sh != shapes[0] for sh in shapes):
                 raise ValueError("img_size=None needs equally sized images")
-            if not any(_is_jpeg(im) for im in imgs):
+            if not any(_is_file(im) for im in imgs):
                 d_imgs = torch.from_numpy(np.stack(imgs)).to(molder.device)
-                sources, d_status = list(imgs), None
+                sources, status = list(imgs), None
             else:
-                # one contiguous [B, H, W, 3] buffer: arrays staged, JPEG files decoded in place
-                d_src, off, _, d_status, jidx = molder.stage_images(imgs, align=1)
+                # one contiguous [B, H, W, 3] buffer: arrays staged, files decoded in place
+                d_src, off, _, status, fidx = molder.stage_images(imgs, align=1)
                 d_imgs = d_src[:int(off[-1])].view(len(imgs), *shapes[0])
-                sources = [d_imgs[b] if b in jidx else imgs[b] for b in range(len(imgs))]
+                sources = [d_imgs[b] if b in fidx else imgs[b] for b in range(len(imgs))]
         img_shape = tuple(d_imgs.shape[1:])
         d_molded, window, scale, _padding = molder.mold_batch_device(d_imgs, out_dtype=molded_dtype)
-        if d_status is not None:
-            molder.jpeg_check(d_status, jidx)
+        if status is not None:
+            molder.files_check(*status)
         molded = d_molded.cpu().numpy()
     meta = compose_image_meta(0, img_shape, molded.shape[1:], window, scale,
                               np.zeros([mcf.NUM_CLASSES], dtype=np.int32))
@@ -203,7 +203,7 @@ def grpc_inference_batch(imgs):
     """`grpc_inference` for a list of images: batched pre-processing, then one RPC per image
     (the served model's signature is batch 1, serve.py:48).  Returns a list of
     (mrcnn_detection, mrcnn_mask, molded_image_shape, window)."""
-    return _grpc_inference_batch([_check_image(im) for im in imgs])[0]
+    return _grpc_inference_batch([_check_image(im, i) for i, im in enumerate(imgs)])[0]
 
 
 def _grpc_inference_batch(imgs):
@@ -252,7 +252,7 @@ def do_inference(img, colors=None, media_dir=None):
 def do_inference_batch(imgs, colors=None, media_dir=None):
     """`do_inference` for a list of images: batched pre-processing, one RPC per image, ONE
     batched unmold + overlay on the device, one PNG per image.  Returns the list of paths."""
-    imgs = [_check_image(im) for im in imgs]
+    imgs = [_check_image(im, i) for i, im in enumerate(imgs)]
     if len(imgs) == 0:
         return []
     res, sources = _grpc_inference_batch(imgs)
@@ -273,7 +273,7 @@ def do_inference_coco_batch(imgs, image_ids, category_ids=None):
     per detected instance, its mask as a compressed RLE made on the device.  image_ids: one per
     image; category_ids: class id -> dataset category id (None: the class id itself).  Decode each
     `segmentation["counts"]` with `.decode("ascii")` before `json.dumps`."""
-    imgs = [_check_image(im) for im in imgs]
+    imgs = [_check_image(im, i) for i, im in enumerate(imgs)]
     if len(image_ids) != len(imgs):
         raise ValueError(f"{len(imgs)} images but {len(image_ids)} image ids")
     if len(imgs) == 0:

@@ -6,7 +6,7 @@ each unmold workload also names the GPU and its power limit.
   python tools/bench_secondary.py [--iters 20] [--cpu]     (--cpu also times the oracle)
   python tools/bench_secondary.py --only-eval | --only-cocoeval | --only-bboxeval | --only-boundaryeval
                                   | --only-polygons | --only-lvis | --only-jpeg | --only-png
-                                  | --only-jpeg-progressive
+                                  | --only-jpeg-progressive | --only-png-decode
 """
 import argparse
 import json
@@ -1251,6 +1251,98 @@ def png_case(iters):
             "host_threads": os.cpu_count(), **card()}), flush=True)
 
 
+def png_decode_case(iters):
+    """PNG request bytes decoded on the device (csrc/png_decode.cu) against cv2.imdecode on the host,
+    each followed by preprocess_input_batch: 32 x 1024^2 as cv2.imwrite writes them (level 1,
+    Z_RLE, Sub rows), the same images at zlib level 6 (most other encoders' default), and
+    16 x 2160x3840 as cv2.imwrite writes them.  Also the finder's candidates against the blocks
+    chained, and the blocks the chain had to measure itself."""
+    import zlib
+    from concurrent.futures import ThreadPoolExecutor
+
+    import cv2
+
+    from torch.profiler import ProfilerActivity, profile
+
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, png, serve
+
+    def level6(rgb):
+        raw = b"".join(b"\x01" + bytes(np.concatenate([r[:3], (r[3:].astype(np.int16) -
+                                                               r[:-3]).astype(np.uint8)]))
+                       for r in rgb.reshape(rgb.shape[0], -1))
+        h, w = rgb.shape[:2]
+        chunk = lambda t, d: (len(d).to_bytes(4, "big") + t + d +              # noqa: E731
+                              zlib.crc32(t + d).to_bytes(4, "big"))
+        ihdr = w.to_bytes(4, "big") + h.to_bytes(4, "big") + bytes([8, 2, 0, 0, 0])
+        return (png.SIGNATURE + chunk(b"IHDR", ihdr) + chunk(b"IDAT", zlib.compress(raw, 6)) +
+                chunk(b"IEND", b""))
+
+    rng = np.random.default_rng(13)
+    m = Molder(api_utils.get_config())
+    cv2_file = lambda a: cv2.imencode(".png", a[:, :, ::-1])[1].tobytes()   # noqa: E731
+    for name, batch, hw, write in [("32 x 1024x1024 cv2.imwrite", 32, (1024, 1024), cv2_file),
+                                   ("32 x 1024x1024 zlib level 6", 32, (1024, 1024), level6),
+                                   ("configs[3] size: 16 x 2160x3840 cv2.imwrite", 16,
+                                    (2160, 3840), cv2_file)]:
+        base = [synth.synth_rgb_image(rng, *hw) for _ in range(4)]
+        files = [write(a) for a in base]
+        blobs = [files[b % 4] for b in range(batch)]
+        mb = sum(len(b) for b in blobs) / 1e6
+        m.decode_png_batch(blobs)
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(5):
+                m.decode_png_batch(blobs)
+            torch.cuda.synchronize()
+        kern = {}
+        for ev in prof.key_averages():
+            if "png_" in ev.key:
+                short = ev.key.split("png_")[1].split("_kernel")[0]
+                kern[short] = round(kern.get(short, 0) + ev.device_time_total / 1e3 / 5, 4)
+        plan = png.DecodePlan(blobs)
+        sizes = [h * w * 3 for h, w, _ in plan.shapes]
+        off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        out = torch.empty(int(off[-1]), dtype=torch.uint8, device="cuda")
+        _, d_info, _ = m.png_decode_into(plan, out, off[:-1])
+        info = d_info.cpu().numpy()
+        nblk, seq, cand = info[:, 0], info[:, 1], info[:, 6]
+        dec_ms, _ = time_ms(lambda: api_utils.decode_png_batch(blobs), iters)
+        pre_ms, _ = time_ms(lambda: serve.preprocess_input_batch(blobs), iters)
+
+        def host(pool):
+            dec = (lambda b: cv2.cvtColor(cv2.imdecode(np.frombuffer(b, np.uint8), cv2.IMREAD_COLOR),
+                                          cv2.COLOR_BGR2RGB))
+            arrs = list(pool.map(dec, blobs)) if pool else [dec(b) for b in blobs]
+            return serve.preprocess_input_batch(arrs)
+
+        def host_clock(fn, n):
+            fn()
+            ts = []
+            for _ in range(n):
+                t0 = time.perf_counter()
+                fn()
+                torch.cuda.synchronize()
+                ts.append((time.perf_counter() - t0) * 1e3)
+            return float(np.median(ts))
+
+        one_ms = host_clock(lambda: host(None), max(3, iters // 4))
+        with ThreadPoolExecutor(os.cpu_count()) as pool:
+            pool_ms = host_clock(lambda: host(pool), max(3, iters // 4))
+        print(json.dumps({
+            "workload": f"PNG decode {name} ({mb:.1f} MB of files)",
+            "kernel_ms": kern, "kernel_ms_total": round(sum(kern.values()), 3),
+            "deflate_blocks_per_image_min_median_max": [int(nblk.min()), int(np.median(nblk)),
+                                                        int(nblk.max())],
+            "candidates_found_per_image_median": int(np.median(cand)),
+            "blocks_measured_by_the_chain_per_image_median": int(np.median(seq)),
+            "candidate_slots_per_tile": plan.K,
+            "api_utils_decode_png_batch_ms": round(dec_ms, 3),
+            "preprocess_input_batch_bytes_ms": round(pre_ms, 3),
+            "host_imdecode_one_thread_then_preprocess_ms": round(one_ms, 3),
+            "host_imdecode_pool_then_preprocess_ms": round(pool_ms, 3),
+            "host_threads": os.cpu_count(), **card()}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
@@ -1267,8 +1359,12 @@ def main():
     ap.add_argument("--only-png", action="store_true", help="only the PNG encode record")
     ap.add_argument("--only-jpeg-progressive", action="store_true",
                     help="only the progressive JPEG decode record")
+    ap.add_argument("--only-png-decode", action="store_true", help="only the PNG decode record")
     args = ap.parse_args()
     torch.cuda.set_device(0)
+    if args.only_png_decode:
+        png_decode_case(args.iters)
+        return
     if args.only_jpeg_progressive:
         jpeg_progressive_case(args.iters)
         return
