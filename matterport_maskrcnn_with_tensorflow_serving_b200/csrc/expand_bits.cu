@@ -188,7 +188,8 @@ mask_expand_bits_kernel(const BitsParams p) {
           // columns outside the box still run the shuffles: keep their lane index in range
           idx[c] = min(max(sx.i + 1, 0), 30);
           wx[c] = src_weight(sx.rem, invD);
-          thr[c] = colvalid ? 0.5f : __int_as_float(0x7f800000);
+          // NaN outside the box: no sample compares >= it, not even an infinite one
+          thr[c] = colvalid ? 0.5f : __int_as_float(0x7fc00000);
           // bytes of the block inside the row: lane 0 stores the word when rows are 4-byte
           // aligned (then all four are inside), else lane t < nbytes stores byte t
           const int nbytes = cb <= cb_last ? min(4, WB - (cb << 2)) : 0;

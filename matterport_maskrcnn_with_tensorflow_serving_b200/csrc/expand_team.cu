@@ -465,7 +465,9 @@ mask_expand_team_kernel(const ExpandParams p, const int buf_bytes) {
           if (3 < lim) r3 = __ldg(pr + 2 * mw);
           if (deep && 4 < lim) r4 = __ldg(pr + 3 * mw);
           if (deep && 5 < lim) r5 = __ldg(pr + 4 * mw);
-          const float thr = colvalid ? 0.5f : __int_as_float(0x7f800000);
+          // columns outside the box compare against NaN, which no sample reaches (an infinite
+          // one included: their lanes still interpolate whatever the shuffles bring)
+          const float thr = colvalid ? 0.5f : __int_as_float(0x7fc00000);
           float ht = hrow(r0, idx, wx), hb = hrow(r1, idx, wx), q2 = hrow(r2, idx, wx),
                 q3 = hrow(r3, idx, wx);
           float dh = hb - ht;

@@ -77,7 +77,9 @@ rle_walk_kernel(const RleParams p) {
   int idx;
   float wx;
   hcoord(x, idx, wx);
-  const float thr = colvalid ? 0.5f : __int_as_float(0x7f800000);
+  // NaN outside the box: no sample compares >= it, not even an infinite one, so such a lane
+  // never counts (or writes) a transition
+  const float thr = colvalid ? 0.5f : __int_as_float(0x7fc00000);
 
   const SrcPos first = src_floor(src_num(mh, bx.x, bx.x, bh), Dy, invDy);   // first box row
   int jcur = first.i, remy = first.rem;

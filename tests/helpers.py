@@ -1,4 +1,9 @@
-"""Shared helpers for the parity tests (oracle = checker, CUDA path = thing under test)."""
+"""Shared helpers for the parity tests (oracle = checker, CUDA path = thing under test).
+
+The mask expand is held to two claims.  Here, against upstream's float64 resize: every sample
+within MASK_VALUE_ATOL = 1e-6, and masks equal outside a +-1e-6 band around 0.5 (`check_values`,
+`compare_masks`).  In test_gpu_expand_exact.py, against its fp32 definition (csrc/expand.cuh,
+restated by expand_oracle.py): every kernel bit for bit, with no band."""
 import dataclasses
 
 import numpy as np

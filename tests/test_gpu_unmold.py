@@ -1,7 +1,9 @@
 """GPU parity of api_utils.unmold_detections (serve.py:147-154) against the oracle.
 
 Contract (SURVEY.md 8c): N, boxes, class_ids, scores bit-exact; binary masks equal
-wherever the oracle's float64 pre-threshold value is > 1e-6 away from 0.5.
+wherever the oracle's float64 pre-threshold value is > 1e-6 away from 0.5.  That is the claim
+against upstream's float64; the claim against the fp32 sample the kernels define
+(csrc/expand.cuh), bit for bit with no band, is test_gpu_expand_exact.py's.
 """
 import numpy as np
 import pytest
