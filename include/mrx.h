@@ -31,6 +31,8 @@
  *   mrx_png_decode         <- api_utils.load_img (cv2.imread)   serve.py:85-86
  *                             (extension: PNG request bytes decoded on the device, as cv2.imdecode)
  *   mrx_png_encode        <- cv2.imwrite of the overlay PNG                 serve.py:168
+ *   mrx_jpeg_encode       <- cv2.imwrite of the overlay                     serve.py:168
+ *                             (extension: the overlay as a JPEG file, as cv2.imencode('.jpg'))
  *   mrx_peer_*             (multi-GPU: the final gather of the masks to rank 0, SURVEY.md 8e)
  *   mrx_device_alloc/_free (the canvas allocation: compressible device memory where offered)
  *
@@ -706,6 +708,45 @@ int mrx_png_encode(const long long *d_desc, int B, long long max_n, int max_bloc
                    unsigned char *d_stream, short *d_sym, int *d_stretch, long long *d_tiles,
                    int *d_blk_pos, int *d_blk_tab, long long *d_blk_info, unsigned int *d_zbuf,
                    long long *d_img_info, unsigned char *d_out, long long *d_sizes, void *stream);
+
+/* ---------------------------------------------------------------- JPEG encode (cv2.imwrite) */
+/* uint8 RGB images encoded byte for byte as cv2.imencode('.jpg', rgb[..., ::-1],
+ * [IMWRITE_JPEG_QUALITY, quality, IMWRITE_JPEG_OPTIMIZE, optimize]) writes them (libjpeg-turbo:
+ * JFIF 1.01, jpeg_set_quality(quality, force_baseline), YCbCr 4:2:0, ISLOW FDCT, one interleaved
+ * baseline scan with the Annex K tables, or with optimize the K.2 optimal tables of the image, no
+ * restart markers; csrc/jpeg_encode.cu, tests/jpeg_encode_oracle.py).  The host
+ * (jpeg_encode.EncodePlan) lays the batch out: d_desc [B, 16] int64 words per image
+ * (jpeg_encode.py's D_* indices: the address of the image's contiguous H x W x 3 bytes, H, W, the
+ * MCU grid, the scan's block count nblk = 6 * MCUs, and the offset of the image's part of every
+ * buffer below).  Buffers, each sized by jpeg_encode.EncodePlan from H and W alone:
+ *   d_huff    uint8 [B, 4, 272]: bits[16] and vals of the tables DC0, AC0, DC1, AC1
+ *   d_codes   int32 [B, 4, 256]: code | length << 16 per symbol     d_hist int32 [B, 4, 256]
+ *   d_coef    int16 [blocks, 64]: each block's quantised coefficients in zigzag order, MCU order
+ *   d_blk_bit int32 [blocks]: each block's first bit within its tile of 256 blocks
+ *   d_tiles   int64 [blk_tiles + 1 + byte_tiles + 1]
+ *   d_words   uint32 [word_count] (zeroed here): each image's entropy-coded bits, big-endian
+ *   d_info    int64 [B, 8] (MRX_JPEG_ENC_*)
+ *   d_out     uint8: image b's file at its offset, at most jpeg_encode.file_bound(nblk) bytes
+ *   d_sizes   int64 [B]: the byte count of each file.
+ * min_side / max_side: the smallest and largest H or W of the batch; max_blocks, max_bytes: the
+ * largest nblk and entropy-coded byte bound.  Checks: null pointers, B outside [0, MRX_MAX_BATCH],
+ * quality outside [0, 100], optimize not 0 or 1, a max extent below 1: MRX_E_INVALID; a side
+ * outside [1, MRX_JPEG_ENC_MAX_SIDE]: MRX_E_UNSUPPORTED.  B = 0 returns MRX_OK without launching
+ * anything. */
+#define MRX_JPEG_ENC_MAX_SIDE 65535   /* the largest side a baseline frame header holds */
+#define MRX_JPEG_ENC_BITS     0   /* entropy-coded bits, padding excluded */
+#define MRX_JPEG_ENC_BYTES    1   /* entropy-coded bytes before stuffing */
+#define MRX_JPEG_ENC_FF       2   /* 0x00 bytes stuffed after 0xFF */
+#define MRX_JPEG_ENC_HDR      3   /* bytes from SOI to the end of SOS */
+#define MRX_JPEG_ENC_FILE     4
+#define MRX_JPEG_ENC_BLOCKS   5   /* blocks of the scan, dummy blocks included */
+#define MRX_JPEG_ENC_INFO_WORDS 8
+int mrx_jpeg_encode(const long long *d_desc, int B, int quality, int optimize, int min_side,
+                    int max_side, int max_blocks, long long max_bytes, long long blk_tiles,
+                    long long byte_tiles, long long word_count, unsigned char *d_huff,
+                    int *d_codes, int *d_hist, short *d_coef, int *d_blk_bit, long long *d_tiles,
+                    unsigned int *d_words, long long *d_info, unsigned char *d_out,
+                    long long *d_sizes, void *stream);
 
 /* ---------------------------------------------------------------- PNG decode (load_img) */
 /* PNG files decoded bit for bit as cv2.imdecode(buf, IMREAD_COLOR) then BGR2RGB (libpng:

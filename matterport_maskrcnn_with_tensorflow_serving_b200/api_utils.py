@@ -13,8 +13,8 @@ serve.py:48): `unmold_detections_batch`, `unmold_detections_packed_batch`,
 `unmold_coco_results_batch` (upstream's `build_coco_results` of the unmolded detections),
 `unmold_compute_ap_batch` (upstream's `compute_ap` of them against ground truth) and
 `unmold_coco_eval_batch` (pycocotools' COCOeval "segm" of them, streamed batch by batch), and
-`decode_jpeg_batch` / `decode_png_batch` / `encode_png_batch` (request JPEG or PNG bytes in,
-response PNG bytes out, each as OpenCV would decode or write them).
+`decode_jpeg_batch` / `decode_png_batch` / `encode_png_batch` / `encode_jpeg_batch` (request
+JPEG or PNG bytes in, response PNG or JPEG bytes out, each as OpenCV would decode or write them).
 
 Numerical contract (checked by tests/ against the float64 oracle): N, boxes, class ids and
 scores are bit-exact.  The mask resize runs in float32 on exact integer source coordinates;
@@ -120,6 +120,45 @@ def encode_png_batch(images):
     return _png_encode(images)[0]
 
 
+def _image_meta(images):
+    """(shape, dtype) of each image, CUDA tensor or array, for an encoder's plan."""
+    import torch
+
+    meta = []
+    for img in images:
+        if torch.is_tensor(img):
+            meta.append((tuple(img.shape), str(img.dtype).replace("torch.", "")))
+        else:
+            a = np.asarray(img)
+            meta.append((a.shape, a.dtype))
+    return meta
+
+
+def _device_images(images):
+    """(device, contiguous uint8 tensors on it): the images an encoder reads in place, on the
+    device of the first CUDA tensor among them, else the current one."""
+    import torch
+
+    dev = next((im.device for im in images if torch.is_tensor(im) and im.is_cuda),
+               torch.device("cuda", torch.cuda.current_device()))
+    srcs = []
+    for img in images:
+        t = img if torch.is_tensor(img) else torch.from_numpy(np.ascontiguousarray(img))
+        srcs.append(t.to(dev, non_blocking=True).contiguous())
+    return dev, srcs
+
+
+def _download_files(d_out, offs, d_sizes):
+    """The files at offsets offs of d_out, d_sizes[b] bytes each, as one copy to the host."""
+    import torch
+
+    sizes = d_sizes.cpu().numpy()
+    files = torch.cat([d_out[int(o):int(o) + int(s)] for o, s in zip(offs, sizes)]).cpu()
+    host = files.numpy().tobytes()
+    ends = np.cumsum(sizes)
+    return [host[int(e - s):int(e)] for s, e in zip(sizes, ends)]
+
+
 def _png_encode(images, stats=False):
     """`encode_png_batch`, plus (with stats) the device's per-image and per-block int64 tables
     (mrx.h MRX_PNG_IMG_* / MRX_PNG_BLK_*) and the plan."""
@@ -131,20 +170,8 @@ def _png_encode(images, stats=False):
     if len(images) == 0:
         return ([], None, None, None) if stats else ([],)
     N.require_cuda()
-    meta = []
-    for b, img in enumerate(images):
-        if torch.is_tensor(img):
-            meta.append((tuple(img.shape), str(img.dtype).replace("torch.", "")))
-        else:
-            a = np.asarray(img)
-            meta.append((a.shape, a.dtype))
-    plan = png.Plan(meta)
-    dev = next((im.device for im in images if torch.is_tensor(im) and im.is_cuda),
-               torch.device("cuda", torch.cuda.current_device()))
-    srcs = []
-    for img in images:
-        t = img if torch.is_tensor(img) else torch.from_numpy(np.ascontiguousarray(img))
-        srcs.append(t.to(dev, non_blocking=True).contiguous())
+    plan = png.Plan(_image_meta(images))
+    dev, srcs = _device_images(images)
     plan.set_sources([t.data_ptr() for t in srcs])
     lib = N.load()
 
@@ -167,16 +194,67 @@ def _png_encode(images, stats=False):
             d_desc, plan.B, plan.max_n, plan.max_blocks, plan.max_chunks, plan.total_tiles,
             plan.zbuf_words, d_stream, d_sym, d_stretch, d_tiles, d_blk_pos, d_blk_tab,
             d_blk_info, d_zbuf, d_img_info, d_out, d_sizes, N.stream_ptr(None)), "mrx_png_encode")
-        sizes = d_sizes.cpu().numpy()
-        offs = plan.desc[:, png.D_OUT_OFF]
-        files = torch.cat([d_out[int(o):int(o) + int(s)] for o, s in zip(offs, sizes)]).cpu()
-    host = files.numpy().tobytes()
-    ends = np.cumsum(sizes)
-    out = [host[int(e - s):int(e)] for s, e in zip(sizes, ends)]
+        out = _download_files(d_out, plan.desc[:, png.D_OUT_OFF], d_sizes)
     if not stats:
         return (out,)
     return out, d_img_info.view(plan.B, -1).cpu().numpy(), \
         d_blk_info.view(plan.blocks, -1).cpu().numpy(), plan
+
+
+def encode_jpeg_batch(images, quality=95, optimize=False):
+    """uint8 RGB [H, W, 3] images (CUDA tensors or arrays; sizes may differ) -> one JPEG file's
+    bytes each, equal byte for byte to `cv2.imencode('.jpg', img[..., ::-1],
+    [cv2.IMWRITE_JPEG_QUALITY, quality, cv2.IMWRITE_JPEG_OPTIMIZE, int(optimize)])[1].tobytes()`,
+    encoded on the device (csrc/jpeg_encode.cu): baseline, 4:2:0, the standard Huffman tables or
+    with `optimize` each image's optimal ones.  An image or quality the encoder does not accept
+    raises ValueError (naming the image's index) before anything runs.  Only the files travel to
+    the host."""
+    return _jpeg_encode(images, quality, optimize)[0]
+
+
+def _jpeg_encode(images, quality=95, optimize=False, stats=False):
+    """`encode_jpeg_batch`, plus (with stats) the device's per-image int64 table
+    (mrx.h MRX_JPEG_ENC_*), every block's quantised zigzag coefficients (int16 [blocks, 64], the
+    plan's D_BLK_OFF rows per image) and the plan."""
+    import torch
+
+    from . import jpeg_encode as je
+
+    images = list(images)
+    plan = je.EncodePlan(_image_meta(images), quality, optimize)
+    if len(images) == 0:
+        return ([], None, None, plan) if stats else ([],)
+    N.require_cuda()
+    dev, srcs = _device_images(images)
+    plan.set_sources([t.data_ptr() for t in srcs])
+    lib = N.load()
+
+    def buf(n, dtype):
+        return torch.empty(int(n), dtype=dtype, device=dev)
+
+    B = plan.B
+    d_desc = torch.from_numpy(plan.desc).to(dev)
+    d_huff = buf(B * 4 * je.TAB_BYTES, torch.uint8)
+    d_codes = buf(B * 4 * 256, torch.int32)
+    d_hist = buf(B * 4 * 256, torch.int32)
+    d_coef = buf(plan.blocks * 64, torch.int16)
+    d_blk_bit = buf(plan.blocks, torch.int32)
+    d_tiles = buf(plan.block_tiles + plan.byte_tiles + 2, torch.int64)
+    d_words = buf(plan.words, torch.int32)
+    d_info = buf(B * je.INFO_WORDS, torch.int64)
+    d_out = buf(plan.out_bytes, torch.uint8)
+    d_sizes = buf(B, torch.int64)
+    with torch.cuda.device(dev):
+        N.check(lib.mrx_jpeg_encode(
+            d_desc, B, plan.quality, int(plan.optimize), plan.min_side, plan.max_side,
+            plan.max_blocks, plan.max_bytes, plan.block_tiles, plan.byte_tiles, plan.words,
+            d_huff, d_codes, d_hist, d_coef, d_blk_bit, d_tiles, d_words, d_info, d_out,
+            d_sizes, N.stream_ptr(None)), "mrx_jpeg_encode")
+        out = _download_files(d_out, plan.desc[:, je.D_OUT_OFF], d_sizes)
+    if not stats:
+        return (out,)
+    return out, d_info.view(B, -1).cpu().numpy(), d_coef.view(plan.blocks, 64).cpu().numpy(), \
+        plan
 
 
 def get_anchors(image_shape):
@@ -645,13 +723,26 @@ def unmold_overlay_batch(items, images, colors=None, alpha=0.5):
     return [metas[b] + (host[b],) for b in range(st.n)]
 
 
-def _unmold_overlay_png_batch(items, images, colors=None, alpha=0.5):
+def _check_file_format(image_format, quality):
+    """Refuse a response format other than "png" or "jpeg", or a JPEG quality cv2 refuses."""
+    if image_format not in ("png", "jpeg"):
+        raise ValueError(f"image_format {image_format!r} (expected 'png' or 'jpeg')")
+    if image_format == "jpeg":
+        from .jpeg_encode import check_quality
+
+        check_quality(quality)
+
+
+def _unmold_overlay_file_batch(items, images, colors=None, alpha=0.5, image_format="png",
+                               quality=95):
     """`unmold_overlay_batch` that stops at the device overlays and encodes them there: returns
-    (boxes, class_ids, scores, png_bytes) per image, the file being what
+    (boxes, class_ids, scores, file_bytes) per image, the file being what
     `cv2.imencode('.png', overlay[..., ::-1])` gives for the overlay `unmold_overlay_batch`
-    returns.  Only the PNG bytes leave the device."""
+    returns, or with image_format "jpeg" `cv2.imencode('.jpg', ...)` at `quality`.  Only the
+    file bytes leave the device."""
     from . import visualize
 
+    _check_file_format(image_format, quality)
     if len(items) == 0:
         return []
     with _Staged(items) as st:
@@ -661,7 +752,10 @@ def _unmold_overlay_png_batch(items, images, colors=None, alpha=0.5):
             colors = visualize.random_colors(eng.R)
         overlays = visualize.composite_batch(eng, images, colors, alpha)
         counts, metas = st.meta()
-        files = encode_png_batch(overlays)
+        if image_format == "jpeg":
+            files = encode_jpeg_batch(overlays, quality)
+        else:
+            files = encode_png_batch(overlays)
     return [metas[b] + (files[b],) for b in range(st.n)]
 
 

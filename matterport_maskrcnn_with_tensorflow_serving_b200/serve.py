@@ -21,7 +21,9 @@ image and the picture is written to `media/mask-<uuid>.png`, whose path is retur
 blend runs on the device canvas the unmold kernels just wrote (`mrx_composite_masks`): the
 105 MB of masks per 1024x1024x100 image never travel to the host, and neither do the blended
 pixels: the PNG file is encoded on the device, byte for byte what `cv2.imwrite` writes
-(`api_utils.encode_png_batch`), and only its bytes are downloaded.  Boxes, captions and
+(`api_utils.encode_png_batch`), and only its bytes are downloaded.  `image_format="jpeg"` writes
+`media/mask-<uuid>.jpg` instead, the bytes `cv2.imencode('.jpg')` gives at `quality`
+(`api_utils.encode_jpeg_batch`), several times smaller than the PNG.  Boxes, captions and
 contour polygons are matplotlib artists in the reference and are not drawn (DESIGN.md 7).
 
 Wherever an image is accepted, a JPEG or PNG file's bytes (bytes, bytearray or memoryview) are
@@ -229,39 +231,46 @@ def do_inference_unmolded(img):
         mrcnn_detection, mrcnn_mask, _image_shape(img), molded_image.shape, window)
 
 
-def _save_png(png_bytes, media_dir=None):
-    """serve.py:156-158,168: media/mask-<uuid4>.png, the file's bytes encoded on the device (what
-    cv2.imwrite of the overlay writes)."""
+def _save_file(data, ext, media_dir=None):
+    """serve.py:156-158,168: media/mask-<uuid4>.<ext>, the file's bytes encoded on the device
+    (what cv2.imwrite of the overlay writes)."""
     media_dir = media_dir if media_dir is not None else getattr(cf, "MEDIA_DIR", "media")
     os.makedirs(media_dir, exist_ok=True)
-    save_path = os.path.join(media_dir, "mask-{}.png".format(str(uuid.uuid4())))
+    save_path = os.path.join(media_dir, "mask-{}.{}".format(str(uuid.uuid4()), ext))
     try:
         with open(save_path, "wb") as f:
-            f.write(png_bytes)
+            f.write(data)
     except OSError as e:
         raise IOError(f"could not write {save_path}") from e
     return save_path
 
 
-def do_inference(img, colors=None, media_dir=None):
+def do_inference(img, colors=None, media_dir=None, image_format="png", quality=95):
     """serve.py:141-173: inference, unmold, mask overlay, PNG -> `save_path`.  The masks stay
-    on the device between the unmold and the overlay (`api_utils.unmold_overlay_batch`)."""
-    return do_inference_batch([img], colors=colors, media_dir=media_dir)[0]
+    on the device between the unmold and the overlay (`api_utils.unmold_overlay_batch`).
+    image_format "jpeg" writes `media/mask-<uuid>.jpg` instead, the bytes of
+    `cv2.imencode('.jpg')` of the overlay at `quality`, encoded on the device."""
+    return do_inference_batch([img], colors=colors, media_dir=media_dir,
+                              image_format=image_format, quality=quality)[0]
 
 
-def do_inference_batch(imgs, colors=None, media_dir=None):
+def do_inference_batch(imgs, colors=None, media_dir=None, image_format="png", quality=95):
     """`do_inference` for a list of images: batched pre-processing, one RPC per image, ONE
-    batched unmold + overlay on the device, one PNG per image.  Returns the list of paths."""
+    batched unmold + overlay on the device, one PNG (or JPEG) per image.  Returns the list of
+    paths."""
+    api_utils._check_file_format(image_format, quality)
     imgs = [_check_image(im, i) for i, im in enumerate(imgs)]
     if len(imgs) == 0:
         return []
     res, sources = _grpc_inference_batch(imgs)
     items = [(det, msk, tuple(src.shape), mshape, window)
              for (det, msk, mshape, window), src in zip(res, sources)]
-    outs = api_utils._unmold_overlay_png_batch(items, sources, colors=colors)
+    outs = api_utils._unmold_overlay_file_batch(items, sources, colors=colors,
+                                                image_format=image_format, quality=quality)
+    ext = "jpg" if image_format == "jpeg" else "png"
     paths = []
-    for _boxes, _cls, _scores, png_bytes in outs:
-        paths.append(_save_png(png_bytes, media_dir))
+    for _boxes, _cls, _scores, data in outs:
+        paths.append(_save_file(data, ext, media_dir))
         print(">>> Save image: {}".format(paths[-1]))
     print(">>> Complete!")
     return paths

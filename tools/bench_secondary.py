@@ -6,7 +6,7 @@ each unmold workload also names the GPU and its power limit.
   python tools/bench_secondary.py [--iters 20] [--cpu]     (--cpu also times the oracle)
   python tools/bench_secondary.py --only-eval | --only-cocoeval | --only-bboxeval | --only-boundaryeval
                                   | --only-polygons | --only-lvis | --only-jpeg | --only-png
-                                  | --only-jpeg-progressive | --only-png-decode
+                                  | --only-jpeg-progressive | --only-png-decode | --only-jpeg-encode
 """
 import argparse
 import json
@@ -1233,7 +1233,7 @@ def png_case(iters):
                     cv2.imwrite(os.path.join(tmp, f"{b}.png"), o[3][:, :, ::-1])
 
             def after():
-                outs = api_utils._unmold_overlay_png_batch(items, images, colors)
+                outs = api_utils._unmold_overlay_file_batch(items, images, colors)
                 for b, o in enumerate(outs):
                     with open(os.path.join(tmp, f"{b}.png"), "wb") as f:
                         f.write(o[3])
@@ -1248,6 +1248,94 @@ def png_case(iters):
             "host_imencode_16_threads_ms": round(pool_ms, 3),
             "do_inference_batch_tail_before_ms": round(before_ms, 3),
             "do_inference_batch_tail_after_ms": round(after_ms, 3),
+            "host_threads": os.cpu_count(), **card()}), flush=True)
+
+
+def jpeg_encode_case(iters):
+    """Overlay JPEG files encoded on the device (csrc/jpeg_encode.cu) at cv2's defaults against
+    cv2.imencode('.jpg') on the host: 32 x 1024^2 and 16 x 2160x3840 overlays, their bytes
+    against the device PNG of the same overlays, and the tail of do_inference_batch (unmold +
+    overlay + files written) with image_format "jpeg" against "png"."""
+    import tempfile
+    from concurrent.futures import ThreadPoolExecutor
+
+    import cv2
+
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, visualize
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import jpeg_encode as je
+
+    from torch.profiler import ProfilerActivity, profile
+
+    for name, batch, hw, n in [("32 x 1024x1024", 32, (1024, 1024), 100),
+                               ("configs[3] size: 16 x 2160x3840", 16, (2160, 3840), 50)]:
+        ims = synth.make_batch(5, 4, hw, n, num_classes=81)
+        items = [(ims[b % 4].detections, ims[b % 4].mrcnn_mask, ims[b % 4].original_image_shape,
+                  ims[b % 4].image_shape, ims[b % 4].window) for b in range(batch)]
+        rng = np.random.default_rng(3)
+        base = [synth.synth_rgb_image(rng, *hw) for _ in range(4)]
+        images = [base[b % 4] for b in range(batch)]
+        colors = visualize.random_colors(n)
+        overlays = [o[3] for o in api_utils.unmold_overlay_batch(items[:4], images[:4], colors)]
+        host = [overlays[b % 4] for b in range(batch)]
+        dev = [torch.from_numpy(h).cuda() for h in host]
+        files = api_utils.encode_jpeg_batch(dev)
+        enc = lambda a: cv2.imencode(".jpg", a[:, :, ::-1])[1]     # noqa: E731
+        same = all(f == enc(h).tobytes() for f, h in zip(files[:4], host[:4]))
+        jpeg_mb = sum(len(f) for f in files) / 1e6
+        png_mb = sum(len(f) for f in api_utils.encode_png_batch(dev)) / 1e6
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(5):
+                api_utils.encode_jpeg_batch(dev)
+            torch.cuda.synchronize()
+        kern = {}
+        for ev in prof.key_averages():
+            if "jpeg_" in ev.key or "offsets_scan" in ev.key or "Memset" in ev.key:
+                short = ev.key.split("jpeg_")[1].split("_kernel")[0] if "jpeg_" in ev.key \
+                    else ev.key
+                kern[short] = round(kern.get(short, 0) + ev.device_time_total / 1e3 / 5, 4)
+        enc_ms, _ = time_ms(lambda: api_utils.encode_jpeg_batch(dev), iters)
+
+        def host_clock(fn, k):
+            fn()
+            ts = []
+            for _ in range(k):
+                t0 = time.perf_counter()
+                fn()
+                torch.cuda.synchronize()
+                ts.append((time.perf_counter() - t0) * 1e3)
+            return float(np.median(ts))
+
+        k = max(3, iters // 4)
+        plan_ms = host_clock(lambda: je.EncodePlan([(h.shape, h.dtype) for h in host]), k)
+        # the host part's largest piece: the files' bytes downloaded and made a bytes object
+        d_files = torch.empty(sum(len(f) for f in files), dtype=torch.uint8, device="cuda")
+        download_ms = host_clock(lambda: d_files.cpu().numpy().tobytes(), k)
+        one_ms = host_clock(lambda: [enc(a) for a in host], k)
+        with ThreadPoolExecutor(16) as pool:
+            pool_ms = host_clock(lambda: list(pool.map(enc, host)), k)
+        with tempfile.TemporaryDirectory() as tmp:
+            def tail(fmt):
+                outs = api_utils._unmold_overlay_file_batch(items, images, colors,
+                                                            image_format=fmt)
+                for b, o in enumerate(outs):
+                    with open(os.path.join(tmp, f"{b}.{fmt}"), "wb") as f:
+                        f.write(o[3])
+
+            png_tail_ms = host_clock(lambda: tail("png"), k)
+            jpeg_tail_ms = host_clock(lambda: tail("jpeg"), k)
+        print(json.dumps({
+            "workload": f"JPEG encode {name} overlays, quality 95 ({jpeg_mb:.1f} MB of files, "
+                        f"{png_mb:.1f} MB as PNG)",
+            "equal_to_cv2": same,
+            "kernel_ms": kern, "kernel_ms_total": round(sum(kern.values()), 3),
+            "api_utils_encode_jpeg_batch_ms": round(enc_ms, 3),
+            "host_plan_ms": round(plan_ms, 3),
+            "host_download_of_the_files_ms": round(download_ms, 3),
+            "host_imencode_one_thread_ms": round(one_ms, 3),
+            "host_imencode_16_threads_ms": round(pool_ms, 3),
+            "do_inference_batch_tail_png_ms": round(png_tail_ms, 3),
+            "do_inference_batch_tail_jpeg_ms": round(jpeg_tail_ms, 3),
             "host_threads": os.cpu_count(), **card()}), flush=True)
 
 
@@ -1360,10 +1448,14 @@ def main():
     ap.add_argument("--only-jpeg-progressive", action="store_true",
                     help="only the progressive JPEG decode record")
     ap.add_argument("--only-png-decode", action="store_true", help="only the PNG decode record")
+    ap.add_argument("--only-jpeg-encode", action="store_true", help="only the JPEG encode record")
     args = ap.parse_args()
     torch.cuda.set_device(0)
     if args.only_png_decode:
         png_decode_case(args.iters)
+        return
+    if args.only_jpeg_encode:
+        jpeg_encode_case(args.iters)
         return
     if args.only_jpeg_progressive:
         jpeg_progressive_case(args.iters)
