@@ -38,6 +38,68 @@ def rle_iou(d, g, iscrowd):
     return float(i) / float(u)
 
 
+# One-line departures of evaluateImg's loop below, each modelling a mutant of coco_match_kernel
+# (tools/mutate_eval.py): IoU ties to the earlier ground truth, a strict IoU threshold, a ground
+# truth at the lower area bound ignored, an unmatched detection at the upper bound ignored, and
+# crowd instances matched only once.
+MATCH_VARIANTS = ("tie_first", "thr_strict", "gt_lo_inclusive", "dt_hi_inclusive",
+                  "no_crowd_rematch")
+
+
+def match_image(ious, crowd, gt_area, dt_area, thresholds, area_rng, ignore=None,
+                rematch_crowd=True, variant=None):
+    """evaluateImg's matching loop for one (image, category, area range), line for line.
+
+    ious [D, G]: the detections in score order (already cut at maxDet) against the ground truth
+    in the caller's order; crowd [G] (iscrowd), gt_area [G], dt_area [D]; ignore [G]: the
+    annotations' `ignore` (COCOeval: iscrowd, the default).  rematch_crowd=False is LVISEval's
+    loop, which never matches an instance twice.  Returns (gtind, gtIg, dtm, gtm, dtIg): the
+    mergesort of the ground truth by _ignore, _ignore [G] in that order, dtm [T, D] the matched
+    position in that order or -1, gtm [T, G] the matching detection or -1, and dtIg [T, D] bool
+    (the matched instance's _ignore, or for an unmatched detection its area outside the
+    range)."""
+    lo, hi = area_rng
+    G, D, T = len(crowd), len(dt_area), len(thresholds)
+    ignore = crowd if ignore is None else ignore
+    gt_low = (lambda a: a <= lo) if variant == "gt_lo_inclusive" else (lambda a: a < lo)
+    ig = [1 if (ignore[g] or (gt_low(gt_area[g]) or gt_area[g] > hi)) else 0 for g in range(G)]
+    gtind = np.argsort(ig, kind="mergesort")
+    iscrowd = [int(crowd[g]) if rematch_crowd and variant != "no_crowd_rematch" else 0
+               for g in gtind]
+    ious = np.asarray(ious, np.float64).reshape(D, G)[:, gtind]
+    gtm = -np.ones((T, G), dtype=np.int64)
+    dtm = -np.ones((T, D), dtype=np.int64)
+    gtIg = np.array([ig[g] for g in gtind], dtype=np.int64)
+    dtIg = np.zeros((T, D))
+    if G and D:
+        for tind, t in enumerate(thresholds):
+            for dind in range(D):
+                iou = min([t, 1 - 1e-10])
+                m = -1
+                for gind in range(G):
+                    if gtm[tind, gind] > -1 and not iscrowd[gind]:
+                        continue
+                    if m > -1 and gtIg[m] == 0 and gtIg[gind] == 1:
+                        break
+                    if ious[dind, gind] < iou:
+                        continue
+                    if variant == "tie_first" and m > -1 and ious[dind, gind] == iou:
+                        continue
+                    if variant == "thr_strict" and ious[dind, gind] == min([t, 1 - 1e-10]):
+                        continue
+                    iou = ious[dind, gind]
+                    m = gind
+                if m == -1:
+                    continue
+                dtIg[tind, dind] = gtIg[m]
+                dtm[tind, dind] = m
+                gtm[tind, m] = dind
+    dt_high = (lambda a: a >= hi) if variant == "dt_hi_inclusive" else (lambda a: a > hi)
+    a = np.array([d < lo or dt_high(d) for d in dt_area], bool).reshape((1, D))
+    dtIg = np.logical_or(dtIg, np.logical_and(dtm == -1, np.repeat(a, T, 0)))
+    return gtind, gtIg, dtm, gtm, dtIg
+
+
 class COCOevalOracle:
     def __init__(self, gts, dts, params=None):
         self.params = params or Params()
@@ -92,48 +154,19 @@ class COCOevalOracle:
         return ious
 
     def evaluateImg(self, imgId, catId, aRng, maxDet):
-        p = self.params
         gt = self._gts[imgId, catId]
         dt = self._dts[imgId, catId]
         if len(gt) == 0 and len(dt) == 0:
             return None
-        for g in gt:
-            g["_ignore"] = 1 if (g["ignore"] or (g["area"] < aRng[0] or g["area"] > aRng[1])) else 0
-        gtind = np.argsort([g["_ignore"] for g in gt], kind="mergesort")
-        gt = [gt[i] for i in gtind]
         dtind = np.argsort([-d["score"] for d in dt], kind="mergesort")
         dt = [dt[i] for i in dtind[0:maxDet]]
-        iscrowd = [int(o["iscrowd"]) for o in gt]
-        ious = (self.ious[imgId, catId][:, gtind] if len(self.ious[imgId, catId]) > 0
-                else self.ious[imgId, catId])
-        T = len(p.iouThrs)
+        ious = self.ious[imgId, catId]
+        gtind, gtIg, dtm, gtm, dtIg = match_image(
+            ious if len(ious) else np.zeros((len(dt), len(gt))),
+            [g["iscrowd"] for g in gt], [g["area"] for g in gt], [d["area"] for d in dt],
+            self.params.iouThrs, aRng, ignore=[g["ignore"] for g in gt])
+        gt = [gt[i] for i in gtind]
         G = len(gt)
-        D = len(dt)
-        gtm = -np.ones((T, G), dtype=np.int64)
-        dtm = -np.ones((T, D), dtype=np.int64)
-        gtIg = np.array([g["_ignore"] for g in gt])
-        dtIg = np.zeros((T, D))
-        if not len(ious) == 0:
-            for tind, t in enumerate(p.iouThrs):
-                for dind, d in enumerate(dt):
-                    iou = min([t, 1 - 1e-10])
-                    m = -1
-                    for gind, g in enumerate(gt):
-                        if gtm[tind, gind] > -1 and not iscrowd[gind]:
-                            continue
-                        if m > -1 and gtIg[m] == 0 and gtIg[gind] == 1:
-                            break
-                        if ious[dind, gind] < iou:
-                            continue
-                        iou = ious[dind, gind]
-                        m = gind
-                    if m == -1:
-                        continue
-                    dtIg[tind, dind] = gtIg[m]
-                    dtm[tind, dind] = m
-                    gtm[tind, m] = dind
-        a = np.array([d["area"] < aRng[0] or d["area"] > aRng[1] for d in dt]).reshape((1, len(dt)))
-        dtIg = np.logical_or(dtIg, np.logical_and(dtm == -1, np.repeat(a, T, 0)))
         return {
             "image_id": imgId, "category_id": catId, "aRng": aRng, "maxDet": maxDet,
             "dtIds": [d["id"] for d in dt], "gtIds": [g["id"] for g in gt],

@@ -22,6 +22,7 @@ from collections import OrderedDict, defaultdict
 import numpy as np
 
 from bbox_cocoeval_oracle import bb_iou
+import cocoeval_oracle
 from cocoeval_oracle import rle_iou
 
 
@@ -42,13 +43,15 @@ class Params:
         self.iou_type = iou_type
 
 
-def limit_dets_per_image(dts, max_dets):
+def limit_dets_per_image(dts, max_dets, per_category=False):
     """LVISResults.limit_dets_per_image: per image, the first max_dets of the results sorted by
     descending score (stable: equal scores keep results order; NaN last).  Returns the kept
-    results, each with "id" its position in dts."""
+    results, each with "id" its position in dts.  per_category=True cuts each (image, category)
+    instead: a model of a mutant of the LVIS rank kernel (tools/mutate_eval.py)."""
     img_ann = defaultdict(list)
     for did, d in enumerate(dts):
-        img_ann[d["image_id"]].append(dict(d, id=did))
+        key = (d["image_id"], d["category_id"]) if per_category else d["image_id"]
+        img_ann[key].append(dict(d, id=did))
     for img_id, anns in img_ann.items():
         if len(anns) <= max_dets:
             continue
@@ -139,45 +142,19 @@ class LVISEvalOracle:
         gt, dt = self._gts[img_id, cat_id], self._dts[img_id, cat_id]
         if len(gt) == 0 and len(dt) == 0:
             return None
-        for g in gt:
-            g["_ignore"] = 1 if (g["ignore"] or g["area"] < area_rng[0]
-                                 or g["area"] > area_rng[1]) else 0
-        gt_idx = np.argsort([g["_ignore"] for g in gt], kind="mergesort")
-        gt = [gt[i] for i in gt_idx]
         dt_idx = np.argsort([-d["score"] for d in dt], kind="mergesort")
         dt = [dt[i] for i in dt_idx]
-        ious = (self.ious[img_id, cat_id][:, gt_idx] if len(self.ious[img_id, cat_id]) > 0
-                else self.ious[img_id, cat_id])
-        T, G, D = len(self.params.iou_thrs), len(gt), len(dt)
-        gt_m = -np.ones((T, G), np.int64)
-        dt_m = -np.ones((T, D), np.int64)
-        gt_ig = np.array([g["_ignore"] for g in gt])
-        dt_ig = np.zeros((T, D))
-        for t, thr in enumerate(self.params.iou_thrs):
-            if len(ious) == 0:
-                break
-            for di, d in enumerate(dt):
-                iou = min([thr, 1 - 1e-10])
-                m = -1
-                for gi, _ in enumerate(gt):
-                    if gt_m[t, gi] > -1:
-                        continue
-                    if m > -1 and gt_ig[m] == 0 and gt_ig[gi] == 1:
-                        break
-                    if ious[di, gi] < iou:
-                        continue
-                    iou = ious[di, gi]
-                    m = gi
-                if m == -1:
-                    continue
-                dt_ig[t, di] = gt_ig[m]
-                dt_m[t, di] = m
-                gt_m[t, m] = di
-        dt_ig_mask = np.array([d["area"] < area_rng[0] or d["area"] > area_rng[1]
-                               or d["category_id"] in self.img_nel[d["image_id"]]
-                               for d in dt]).reshape((1, D))
-        dt_ig_mask = np.repeat(dt_ig_mask, T, 0)
-        dt_ig = np.logical_or(dt_ig, np.logical_and(dt_m == -1, dt_ig_mask))
+        ious = self.ious[img_id, cat_id]
+        gt_idx, gt_ig, dt_m, gt_m, dt_ig = cocoeval_oracle.match_image(
+            ious if len(ious) else np.zeros((len(dt), len(gt))), [0] * len(gt),
+            [g["area"] for g in gt], [d["area"] for d in dt], self.params.iou_thrs, area_rng,
+            ignore=[g["ignore"] for g in gt], rematch_crowd=False)
+        gt = [gt[i] for i in gt_idx]
+        G, T = len(gt), len(self.params.iou_thrs)
+        # the not-exhaustive rule: an unmatched detection of such a category is ignored too
+        nel = np.array([d["category_id"] in self.img_nel[d["image_id"]] for d in dt],
+                       bool).reshape((1, len(dt)))
+        dt_ig = np.logical_or(dt_ig, np.logical_and(dt_m == -1, np.repeat(nel, T, 0)))
         return {
             "image_id": img_id, "category_id": cat_id, "area_rng": area_rng,
             "dt_ids": [d["id"] for d in dt], "gt_ids": [g["id"] for g in gt],

@@ -151,29 +151,9 @@ def test_closed_form_equals_the_loop(seed):
     ov = np.where(rng.random((n, m)) < 0.3, rng.random((n, m)).astype(np.float32), ov)
     pc, gc = rng.integers(1, 3, size=n), rng.integers(1, 3, size=m)
     for t, st in [(0.5, 0.0), (np.float64(0.7), 0.0), (0.7, 0.0), (0.25, 0.5), (np.float64(0.75), np.float64(0.3))]:
-        want = _loop_matches(ov, pc, gc, t, st)
+        want = eo.match_loop(ov, pc, gc, t, st)
         got = closed_form_matches(ov, pc, gc, t, st)
         assert np.array_equal(got[0], want[0]) and np.array_equal(got[1], want[1]), (t, st)
-
-
-def _loop_matches(overlaps, pred_cls, gt_cls, iou_threshold, score_threshold):
-    """The matching loop of eval_oracle.compute_matches on given overlaps (rows in rank order)."""
-    n, m = overlaps.shape
-    pred_match, gt_match = -np.ones(n), -np.ones(m)
-    for i in range(n):
-        sorted_ixs = np.argsort(overlaps[i], kind="stable")[::-1]
-        low = np.where(overlaps[i, sorted_ixs] < score_threshold)[0]
-        if low.size > 0:
-            sorted_ixs = sorted_ixs[:low[0]]
-        for j in sorted_ixs:
-            if gt_match[j] > -1:
-                continue
-            if overlaps[i, j] < iou_threshold:
-                break
-            if pred_cls[i] == gt_cls[j]:
-                gt_match[j], pred_match[i] = i, j
-                break
-    return gt_match, pred_match
 
 
 @pytest.mark.parametrize("t", [0.5, 0.7, 0.75, 0.95, 1, 0, np.float64(0.7), np.float32(0.7),
