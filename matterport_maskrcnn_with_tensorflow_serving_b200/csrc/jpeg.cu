@@ -162,6 +162,15 @@ __device__ int decode_span(const Ctx &c, uint32_t &p, int &cz, uint32_t end, uin
 // the subsequences of every unit.
 constexpr int kUnstuffPer = 16;
 
+// The byte after the run of 0xFF bytes at f[i] (f[i] is 0xFF): 0x00 makes the run one stuffed
+// 0xFF data byte, anything else is a marker, the run before it fill bytes (T.81 B.1.1.2;
+// libjpeg's fill_bit_buffer and next_marker skip them).  0xD9 past the end.
+__device__ __forceinline__ int after_ff(const unsigned char *f, long long i, long long len) {
+  ++i;
+  while (i < len && f[i] == 0xFF) ++i;
+  return i < len ? f[i] : 0xD9;
+}
+
 __global__ void __launch_bounds__(kThreads) jpeg_unstuff_kernel(
     const unsigned char *__restrict__ files, const long long *__restrict__ desc, int S,
     unsigned char *__restrict__ unst, int *__restrict__ work, int *__restrict__ status) {
@@ -191,7 +200,7 @@ __global__ void __launch_bounds__(kThreads) jpeg_unstuff_kernel(
     // the first marker that ends the scan in this thread's bytes
     for (long long i = lo; i < lo + kUnstuffPer && i < len; ++i) {
       if (f[i] == 0xFF && (i == s0 || f[i - 1] != 0xFF)) {
-        const int nx = i + 1 < len ? f[i + 1] : 0xD9;
+        const int nx = after_ff(f, i, len);
         if (nx != 0x00 && (nx < 0xD0 || nx > 0xD7)) {
           atomicMin(reinterpret_cast<unsigned long long *>(&s_end),
                     (unsigned long long)i);
@@ -205,7 +214,7 @@ __global__ void __launch_bounds__(kThreads) jpeg_unstuff_kernel(
     for (long long i = lo; i < lo + kUnstuffPer && i < end; ++i) {
       const bool second = i > s0 && f[i - 1] == 0xFF;
       if (second) continue;
-      if (f[i] == 0xFF && i + 1 < len && f[i + 1] != 0x00) ++rst;
+      if (f[i] == 0xFF && after_ff(f, i, len) != 0x00) ++rst;
       else ++keep;
     }
     unsigned long long tot;
@@ -215,9 +224,10 @@ __global__ void __launch_bounds__(kThreads) jpeg_unstuff_kernel(
     for (long long i = lo; i < lo + kUnstuffPer && i < end; ++i) {
       const bool second = i > s0 && f[i - 1] == 0xFF;
       if (second) continue;
-      if (f[i] == 0xFF && i + 1 < len && f[i + 1] != 0x00) {
+      const int nx = f[i] == 0xFF ? after_ff(f, i, len) : 0x00;
+      if (nx != 0x00) {
         const int k = int(at >> 32) + 1;        // the unit this RST starts
-        if (k >= n_units || f[i + 1] != 0xD0 + ((k - 1) & 7)) {
+        if (k >= n_units || nx != 0xD0 + ((k - 1) & 7)) {
           s_bad = 1;
         } else {
           unit_bit[k] = int(uint32_t(at) * 8u);
@@ -501,46 +511,37 @@ constexpr int FIX_0_298631336 = 2446, FIX_0_390180644 = 3196, FIX_0_541196100 = 
               FIX_2_053119869 = 16819, FIX_2_562915447 = 20995, FIX_3_072711026 = 25172;
 constexpr int CONST_BITS = 13, PASS1_BITS = 2;
 
-// jidctint.c's 1-D butterfly on x[0..8) (int64, as JLONG); out: the 8 undescaled results
-__device__ __forceinline__ void idct_1d(const long long *x, long long *o) {
-  long long z2 = x[2], z3 = x[6];
-  long long z1 = (z2 + z3) * FIX_0_541196100;
-  const long long tmp2 = z1 + z3 * -FIX_1_847759065;
-  const long long tmp3 = z1 + z2 * FIX_0_765366865;
-  const long long tmp0 = (x[0] + x[4]) * (1LL << CONST_BITS);
-  const long long tmp1 = (x[0] - x[4]) * (1LL << CONST_BITS);
-  const long long t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
-  long long t0 = x[7], t1 = x[5], t2 = x[3], t3 = x[1];
-  z1 = t0 + t3;
-  z2 = t1 + t2;
-  z3 = t0 + t2;
-  long long z4 = t1 + t3;
-  const long long z5 = (z3 + z4) * FIX_1_175875602;
-  t0 *= FIX_0_298631336;
-  t1 *= FIX_2_053119869;
-  t2 *= FIX_3_072711026;
-  t3 *= FIX_1_501321110;
-  z1 *= -FIX_0_899976223;
-  z2 *= -FIX_2_562915447;
-  z3 = z3 * -FIX_1_961570560 + z5;
-  z4 = z4 * -FIX_0_390180644 + z5;
-  t0 += z1 + z3;
-  t1 += z2 + z4;
-  t2 += z2 + z3;
-  t3 += z1 + z4;
-  o[0] = t10 + t3; o[7] = t10 - t3;
-  o[1] = t11 + t2; o[6] = t11 - t2;
-  o[2] = t12 + t1; o[5] = t12 - t1;
-  o[3] = t13 + t0; o[4] = t13 - t0;
+// libjpeg-turbo's x86 SIMD islow (jidctint-sse2.asm / jidctint-avx2.asm), which cv2.imdecode runs
+// on x86-64, not jidctint.c: the inputs are int16; in0 +- in4, in7 + in3 and in5 + in1 are 16-bit
+// adds that wrap; the products are pmaddwd pairs with the constants regrouped; the rest is int32.
+// No int32 sum can overflow: |in| <= 32768 bounds every output below 1.7e9.
+__device__ __forceinline__ void idct_1d(const int *x, int *o) {
+  const int tmp3 = x[2] * (FIX_0_541196100 + FIX_0_765366865) + x[6] * FIX_0_541196100;
+  const int tmp2 = x[2] * FIX_0_541196100 + x[6] * (FIX_0_541196100 - FIX_1_847759065);
+  const int tmp0 = int(short(x[0] + x[4])) * (1 << CONST_BITS);
+  const int tmp1 = int(short(x[0] - x[4])) * (1 << CONST_BITS);
+  const int t10 = tmp0 + tmp3, t13 = tmp0 - tmp3, t11 = tmp1 + tmp2, t12 = tmp1 - tmp2;
+  const int z3 = short(x[7] + x[3]), z4 = short(x[5] + x[1]);
+  const int z3p = z3 * (FIX_1_175875602 - FIX_1_961570560) + z4 * FIX_1_175875602;
+  const int z4p = z3 * FIX_1_175875602 + z4 * (FIX_1_175875602 - FIX_0_390180644);
+  const int o0 = x[7] * (FIX_0_298631336 - FIX_0_899976223) + x[1] * -FIX_0_899976223 + z3p;
+  const int o1 = x[5] * (FIX_2_053119869 - FIX_2_562915447) + x[3] * -FIX_2_562915447 + z4p;
+  const int o2 = x[5] * -FIX_2_562915447 + x[3] * (FIX_3_072711026 - FIX_2_562915447) + z3p;
+  const int o3 = x[7] * -FIX_0_899976223 + x[1] * (FIX_1_501321110 - FIX_0_899976223) + z4p;
+  o[0] = t10 + o3; o[7] = t10 - o3;
+  o[1] = t11 + o2; o[6] = t11 - o2;
+  o[2] = t12 + o1; o[5] = t12 - o1;
+  o[3] = t13 + o0; o[4] = t13 - o0;
 }
 
-// jdmaster.c's post-IDCT range-limit table, indexed by x & 1023 (not a clamp)
-__device__ __forceinline__ unsigned char range_limit(long long x) {
-  const int v = int(x & 1023);
-  return v < 128 ? v + 128 : v < 512 ? 255 : v < 896 ? 0 : v - 896;
-}
+__device__ __forceinline__ int sat16(int v) { return min(max(v, -32768), 32767); }   // packssdw
 
-// 8 threads per block: thread r runs column r, then row r, through shared memory.
+// 8 threads per block: thread r runs column r, then row r, through an int16 workspace in shared
+// memory.  Dequantisation is pmullw (the low 16 bits of coef * quant; the DQT value is held as a
+// signed 16-bit quantiser).  Pass 1 takes the asm's shortcut when rows 1-7 of the block's raw
+// coefficients are all zero: every workspace row is the dequantised row 0 << 2 as a 16-bit shift
+// that wraps (the full path would saturate).  Pass 2 has no shortcut and ends in packssdw,
+// packsswb and + 128: a clamp to [-128, 127], not jidctint.c's range-limit table.
 __global__ void __launch_bounds__(kThreads) jpeg_idct_kernel(
     const long long *__restrict__ desc, const unsigned char *__restrict__ tabs,
     const short *__restrict__ coef, unsigned char *__restrict__ planes,
@@ -552,12 +553,14 @@ __global__ void __launch_bounds__(kThreads) jpeg_idct_kernel(
   const long long blk = (long long)blockIdx.x * (kThreads / 8) + (threadIdx.x >> 3);
   if ((long long)blockIdx.x * (kThreads / 8) >= nblocks) return;
   const int r = threadIdx.x & 7;
-  __shared__ int ws[kThreads / 8][64];
-  int *w = ws[threadIdx.x >> 3];
+  __shared__ short ws[kThreads / 8][64];
+  short *w = ws[threadIdx.x >> 3];
   const bool active = blk < nblocks;
   const int bpm = int(D[D_BPM]);
   int ci = 0;
   long long bx = 0, by = 0;
+  int x[8], o[8];
+  bool ac = false;        // a nonzero raw coefficient in rows 1-7 of this column
   if (active) {
     const long long m = blk / bpm;
     const int c = int(blk - m * bpm);
@@ -568,24 +571,40 @@ __global__ void __launch_bounds__(kThreads) jpeg_idct_kernel(
     const int *q = reinterpret_cast<const int *>(tabs + size_t(b) * kTabBytes +
                                                  ci * kCompTabBytes);
     const short *in = coef + (D[D_COEF_OFF] + blk) * 64;
-    long long x[8], o[8];
 #pragma unroll
-    for (int k = 0; k < 8; ++k) x[k] = (long long)in[k * 8 + r] * q[k * 8 + r];
-    idct_1d(x, o);
-    const long long half = 1LL << (CONST_BITS - PASS1_BITS - 1);
+    for (int k = 0; k < 8; ++k) {
+      const int v = in[k * 8 + r];
+      x[k] = short(v * short(q[k * 8 + r]));
+      if (k) ac |= v != 0;
+    }
+  }
+  // the block's 8 columns are 8 adjacent lanes; every lane of the warp gets here (the returns
+  // above are uniform over the CTA)
+  const unsigned lane = threadIdx.x & 31;
+  const bool dc_only = ((__ballot_sync(0xFFFFFFFFu, ac) >> (lane & 24)) & 0xFFu) == 0;
+  if (active) {
+    if (dc_only) {
+      const short v = short(x[0] * (1 << PASS1_BITS));
 #pragma unroll
-    for (int k = 0; k < 8; ++k) w[k * 8 + r] = int((o[k] + half) >> (CONST_BITS - PASS1_BITS));
+      for (int k = 0; k < 8; ++k) w[k * 8 + r] = v;
+    } else {
+      idct_1d(x, o);
+      const int half = 1 << (CONST_BITS - PASS1_BITS - 1);
+#pragma unroll
+      for (int k = 0; k < 8; ++k)
+        w[k * 8 + r] = short(sat16((o[k] + half) >> (CONST_BITS - PASS1_BITS)));
+    }
   }
   __syncwarp();
   if (active) {
-    long long x[8], o[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) x[k] = w[r * 8 + k];
     idct_1d(x, o);
     const int sh = CONST_BITS + PASS1_BITS + 3;
     unsigned char px[8];
 #pragma unroll
-    for (int k = 0; k < 8; ++k) px[k] = range_limit((o[k] + (1LL << (sh - 1))) >> sh);
+    for (int k = 0; k < 8; ++k)
+      px[k] = (unsigned char)(min(max((o[k] + (1 << (sh - 1))) >> sh, -128), 127) + 128);
     const long long pw = D[D_PLANE_BW + ci] * 8;
     unsigned char *dst = planes + D[D_PLANE_OFF + ci] + (by * 8 + r) * pw + bx * 8;
     uint2 v;
@@ -725,8 +744,8 @@ __global__ void __launch_bounds__(kThreads) jpeg_prog_unstuff_kernel(
     const long long hi = min(lo + kUnstuffPer, len);
     unsigned int keep = 0, rst = 0;
     for (long long i = lo; i < hi; ++i) {
-      if (i > 0 && f[i - 1] == 0xFF) continue;        // the 0x00 or Dn after 0xFF
-      if (f[i] == 0xFF && i + 1 < len && f[i + 1] != 0x00) ++rst;
+      if (i > 0 && f[i - 1] == 0xFF) continue;        // fill, or the 0x00 or Dn after 0xFF
+      if (f[i] == 0xFF && after_ff(f, i, len) != 0x00) ++rst;
       else ++keep;
     }
     unsigned long long tot;
@@ -735,9 +754,10 @@ __global__ void __launch_bounds__(kThreads) jpeg_prog_unstuff_kernel(
     unsigned long long at = carry + ex;
     for (long long i = lo; i < hi; ++i) {
       if (i > 0 && f[i - 1] == 0xFF) continue;
-      if (f[i] == 0xFF && i + 1 < len && f[i + 1] != 0x00) {
+      const int nx = f[i] == 0xFF ? after_ff(f, i, len) : 0x00;
+      if (nx != 0x00) {
         const int k = int(at >> 32) + 1;        // the unit this RST starts
-        if (k >= n_units || f[i + 1] != 0xD0 + ((k - 1) & 7)) s_bad = 1;
+        if (k >= n_units || nx != 0xD0 + ((k - 1) & 7)) s_bad = 1;
         else unit_bit[k] = int(uint32_t(at) * 8u);
         at += 1ull << 32;
       } else {

@@ -483,12 +483,16 @@ class Scan:
 
 
 def _marker_starts(data):
-    """Every byte position holding 0xFF followed by neither 0x00 nor RSTn: the first one at or
-    after a scan's data is where the scan ends (the entropy-coded bytes are not read otherwise)."""
+    """The start of every run of 0xFF bytes followed by neither 0x00 nor RSTn (the 0xFF bytes
+    before a marker are fill bytes): the first one at or after a scan's data is where the scan
+    ends (the entropy-coded bytes are not read otherwise)."""
     a = np.frombuffer(data, dtype=np.uint8)
     ff = np.flatnonzero(a[:-1] == 0xFF)
-    nx = a[ff + 1]
-    return ff[(nx != 0x00) & ((nx < 0xD0) | (nx > 0xD7))]
+    head = ff[(ff == 0) | (a[ff - 1] != 0xFF)]
+    other = np.flatnonzero(a != 0xFF)
+    j = np.searchsorted(other, head)
+    nx = np.where(j < len(other), a[other[np.minimum(j, len(other) - 1)]], 0xD9)
+    return head[(nx != 0x00) & ((nx < 0xD0) | (nx > 0xD7))]
 
 
 def parse_progressive(blob, index=0):

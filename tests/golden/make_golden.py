@@ -4,7 +4,8 @@ vectors pin the ORACLE (parity unpinned w.r.t. the reference itself): they catch
 the restatement and give the GPU tests small cases whose expected output is a committed
 file rather than something recomputed at test time.
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py               # every file
+    python tests/golden/make_golden.py jpeg_edges    # one of CASES
 """
 import hashlib
 import os
@@ -79,9 +80,64 @@ def composite_case():
     print("composite_small", out.shape, "sha", hashlib.sha256(out.tobytes()).hexdigest()[:12])
 
 
-if __name__ == "__main__":
+def jpeg_edges_case():
+    """tests/jpeg_edge_inputs.py's files (baseline and progressive) with cv2.imdecode's decode of
+    each: the array when it is small, else its shape and SHA-256; plus the SHA-256 of the three
+    full 2048 x 2048 colour grids, and the cv2 / libjpeg-turbo versions and CPU that made them."""
+    import platform
+    import re
+
+    import cv2
+
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import jpeg_edge_inputs as E
+    import jpeg_inputs as JI
+
+    base = E.all_cases()
+    cases = base + E.progressive(base)
+    blobs = [c.blob for c in cases]
+    out = {"names": np.array([c.name for c in cases]),
+           "files": np.frombuffer(b"".join(blobs), dtype=np.uint8),
+           "file_off": np.cumsum([0] + [len(b) for b in blobs]).astype(np.int64),
+           "file_sha256": np.array([hashlib.sha256(b).hexdigest() for b in blobs])}
+    ok, shape, sha = [], [], []
+    for c in cases:
+        img = JI.cv2_decode(c.blob)
+        ok.append(img is not None)
+        shape.append(img.shape if img is not None else (0, 0, 0))
+        sha.append(hashlib.sha256(img.tobytes()).hexdigest() if img is not None else "")
+        if img is not None and img.size <= 3 * 64 * 64:
+            out["px_" + c.name] = img
+    out.update(cv2_ok=np.array(ok), shape=np.array(shape, dtype=np.int64), px_sha256=np.array(sha))
+    for c in E.colour_grids(step=1):
+        img = JI.cv2_decode(c.blob)
+        out["grid_sha256_" + c.name] = np.array(hashlib.sha256(img.tobytes()).hexdigest())
+    info = cv2.getBuildInformation()
+    turbo = re.search(r"JPEG:\s+\S+ \(ver ([^)]*)\)", info)
+    with open("/proc/cpuinfo") as f:
+        avx2 = " avx2" in f.read()
+    out.update(cv2_version=np.array(cv2.__version__),
+               libjpeg_turbo_version=np.array(turbo.group(1) if turbo else "unknown"),
+               cpu=np.array(platform.machine() + (" avx2" if avx2 else "")))
+    np.savez_compressed(os.path.join(HERE, "jpeg_edges.npz"), **out)
+    print("jpeg_edges", len(cases), "files,", int(out["file_off"][-1]), "bytes;",
+          str(out["cv2_version"]), str(out["libjpeg_turbo_version"]), str(out["cpu"]))
+
+
+CASES = {"unmold": lambda: (unmold_case("unmold_small", 101, (96, 128), 12, 5, 16,
+                                        zero_area_rows=(3,)),
+                            unmold_case("unmold_coco_shape", 102, (120, 200), 9, 4, 12)),
+         "anchors": anchors_case, "resize": resize_case, "composite": composite_case,
+         "jpeg_edges": jpeg_edges_case}
+
+
+if __name__ == "__main__" and len(sys.argv) > 1:    # python make_golden.py jpeg_edges ...
+    for name in sys.argv[1:]:
+        CASES[name]()
+elif __name__ == "__main__":
     unmold_case("unmold_small", 101, (96, 128), 12, 5, 16, zero_area_rows=(3,))
     unmold_case("unmold_coco_shape", 102, (120, 200), 9, 4, 12)
     anchors_case()
     resize_case()
     composite_case()
+    jpeg_edges_case()

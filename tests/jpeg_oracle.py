@@ -4,10 +4,12 @@
 Held bit for bit to cv2.imdecode by tests/test_jpeg_oracle.py, so it is pinned to the real library.
 The marker walk is the package's `jpeg.parse` (whose refusals test_host_jpeg.py covers); everything
 after it is restated here: jdhuff.c's decode_mcu (with the 16 guard entries of the natural-order
-table), the restart handling, jidctint.c's jpeg_idct_islow with the post-IDCT range-limit table,
-jdsample.c's upsamplers with the context rows of jdmainct.c, jdcolor.c's ycc_rgb_convert and
-OpenCV's EXIF orientation.  Corrupt entropy-coded data raises JpegError (libjpeg-turbo warns and
-substitutes zeros: a stated difference of the device decoder, which refuses the same files).
+table), the restart handling, the islow IDCT as libjpeg-turbo's x86 SIMD code computes it (16-bit
+dequantisation and sums, saturating packs: not jidctint.c's int64 arithmetic, which differs from
+it once coefficients leave the range an encoder writes from [0, 255] pixels), jdsample.c's
+upsamplers with the context rows of jdmainct.c, jdcolor.c's ycc_rgb_convert and OpenCV's EXIF
+orientation.  Corrupt entropy-coded data raises JpegError (libjpeg-turbo warns and substitutes
+zeros: a stated difference of the device decoder, which refuses the same files).
 """
 from __future__ import annotations
 
@@ -67,6 +69,8 @@ class _Bits:
         if self.marker is None:
             if self.pos + 1 >= len(d) or d[self.pos] != 0xFF:
                 raise J.JpegError("missing or out-of-order RST marker")
+            while self.pos + 2 < len(d) and d[self.pos + 1] == 0xFF:   # fill bytes (next_marker)
+                self.pos += 1
             self.marker = d[self.pos + 1]
             self.pos += 2
         else:
@@ -92,9 +96,12 @@ def _extend(r, s):
     return r - (1 << s) + 1 if r < (1 << (s - 1)) else r
 
 
-def coefficients(blob):
+def coefficients(blob, trace=None):
     """Quantised coefficients in decode order: int16 [MCUs * blocks_per_mcu, 64], natural order,
-    DC after the prediction (JCOEF), plus the parsed header."""
+    DC after the prediction (JCOEF), plus the parsed header.  A `trace` dict gathers what the
+    stored coefficients no longer show: "dc" (each block's DC sum before the int16 store),
+    "dc_cat" and "ac_cat" (symbol categories), "zrl_to_63" (ZRLs whose 16 zeros end at index 63,
+    the block's end without an EOB) and "run_past_63" (runs that end past 63: the guard entries)."""
     data = bytes(blob)
     hd = J.parse(data)
     mcus = hd.mcux * hd.mcuy
@@ -114,6 +121,9 @@ def coefficients(blob):
             s = _huff(bits, dct)
             diff = _extend(bits.bits(s), s) if s else 0
             dcv = last_dc[ci] + diff
+            if trace is not None:
+                trace.setdefault("dc", []).append(dcv)
+                trace.setdefault("dc_cat", []).append(s)
             if not -2 ** 31 <= dcv < 2 ** 31:
                 raise J.JpegError("DC coefficient overflows int32")
             last_dc[ci] = dcv
@@ -127,10 +137,16 @@ def coefficients(blob):
                     k += r
                     v = _extend(bits.bits(s), s)
                     blockv[J.ZIGZAG[k]] = v
+                    if trace is not None:
+                        trace.setdefault("ac_cat", []).append(s)
+                        trace["run_past_63"] = trace.get("run_past_63", 0) + (k > 63)
                 else:
                     if r != 15:
                         break
                     k += 15
+                    if trace is not None:
+                        trace["zrl_to_63"] = trace.get("zrl_to_63", 0) + (k == 63)
+                        trace["run_past_63"] = trace.get("run_past_63", 0) + (k > 63)
                 k += 1
             out[blk] = blockv
             blk += 1
@@ -144,8 +160,93 @@ def _range_limit():
                     ).astype(np.uint8)
 
 
-def idct_islow(coef, quant):
-    """jidctint.c jpeg_idct_islow over [N, 64] blocks -> uint8 [N, 8, 8] (vectorised, int64)."""
+def _w16(v):
+    """Two's-complement wrap to int16 (the SIMD word lanes)."""
+    return ((v + 32768) & 0xFFFF) - 32768
+
+
+def _w32(v):
+    """Two's-complement wrap to int32 (the SIMD dword lanes)."""
+    return ((v + (1 << 31)) & 0xFFFFFFFF) - (1 << 31)
+
+
+# One mistake each, for the tests to show that every one of them changes the expected pixels:
+MISTAKES = (
+    "c",                      # jidctint.c's arithmetic: int64, range-limit table at x & 1023
+    "unwrapped_product",      # dequantised value kept in 32 bits (signed quantiser)
+    "wide_sums",              # in0 +- in4, in7 + in3, in5 + in1 in 32 bits
+    "pass1_wraps",            # pass-1 results wrapped to int16 instead of saturated
+    "shortcut_dequantised",   # the all-zero-AC shortcut tested on dequantised coefficients
+    "shortcut_saturates",     # the shortcut's << 2 saturating instead of wrapping
+    "unsigned_quant",         # the quantiser read as unsigned 16 bits, product kept in 32 bits
+)
+
+
+def _one_d_simd(i0, i1, i2, i3, i4, i5, i6, i7, sum16):
+    """jidctint-sse2/avx2.asm's butterfly: 16-bit sums where the asm adds words, pmaddwd pairs
+    with the regrouped constants, 32-bit adds.  Inputs are int16 values (int64 arrays)."""
+    tmp3 = _w32(i2 * (FIX_0_541196100 + FIX_0_765366865) + i6 * FIX_0_541196100)
+    tmp2 = _w32(i2 * FIX_0_541196100 + i6 * (FIX_0_541196100 - FIX_1_847759065))
+    tmp0 = _w32(sum16(i0 + i4) << CONST_BITS)
+    tmp1 = _w32(sum16(i0 - i4) << CONST_BITS)
+    t10, t13 = _w32(tmp0 + tmp3), _w32(tmp0 - tmp3)
+    t11, t12 = _w32(tmp1 + tmp2), _w32(tmp1 - tmp2)
+    z3, z4 = sum16(i7 + i3), sum16(i5 + i1)
+    z3p = _w32(z3 * (FIX_1_175875602 - FIX_1_961570560) + z4 * FIX_1_175875602)
+    z4p = _w32(z3 * FIX_1_175875602 + z4 * (FIX_1_175875602 - FIX_0_390180644))
+    o0 = _w32(_w32(i7 * (FIX_0_298631336 - FIX_0_899976223) + i1 * -FIX_0_899976223) + z3p)
+    o3 = _w32(_w32(i7 * -FIX_0_899976223 + i1 * (FIX_1_501321110 - FIX_0_899976223)) + z4p)
+    o1 = _w32(_w32(i5 * (FIX_2_053119869 - FIX_2_562915447) + i3 * -FIX_2_562915447) + z4p)
+    o2 = _w32(_w32(i5 * -FIX_2_562915447 + i3 * (FIX_3_072711026 - FIX_2_562915447)) + z3p)
+    return [_w32(t10 + o3), _w32(t11 + o2), _w32(t12 + o1), _w32(t13 + o0),
+            _w32(t13 - o0), _w32(t12 - o1), _w32(t11 - o2), _w32(t10 - o3)]
+
+
+def idct_islow(coef, quant, mistake=None):
+    """libjpeg-turbo's x86 SIMD islow IDCT (jidctint-sse2.asm / jidctint-avx2.asm, the code
+    cv2.imdecode runs on x86-64) over [N, 64] blocks -> uint8 [N, 8, 8]:
+      - the quantiser is a signed 16-bit value and dequantisation is pmullw, the low 16 bits of
+        coef * quant;
+      - pass 1 takes a shortcut when rows 1-7 of the block's raw coefficients are all zero: every
+        row of the workspace is the dequantised row 0 << 2, a 16-bit shift that wraps;
+      - otherwise `_one_d_simd`, descaled and packed with saturation to int16 (packssdw);
+      - pass 2 has no shortcut: `_one_d_simd` on the workspace rows, descaled, packed with
+        saturation to int16 then int8 (packssdw, packsswb), then + 128.
+    `mistake` (one of MISTAKES) models one departure from it, for the sensitivity tests."""
+    if mistake == "c":
+        return _idct_c(coef, quant)
+    assert mistake is None or mistake in MISTAKES, mistake
+    c = coef.astype(np.int64).reshape(-1, 8, 8)
+    q = quant.astype(np.int64).reshape(1, 8, 8)
+    if mistake == "unsigned_quant":
+        x = _w32(c * (q & 0xFFFF))
+    elif mistake == "unwrapped_product":
+        x = _w32(c * _w16(q))
+    else:
+        x = _w16(c * q)
+    sum16 = (lambda v: v) if mistake == "wide_sums" else _w16
+    # pass 1: columns
+    cols = _one_d_simd(*[x[:, k, :] for k in range(8)], sum16=sum16)
+    half1 = 1 << (CONST_BITS - PASS1_BITS - 1)
+    pack1 = _w16 if mistake == "pass1_wraps" else (lambda v: np.clip(v, -32768, 32767))
+    ws = np.stack([pack1(_w32(v + half1) >> (CONST_BITS - PASS1_BITS)) for v in cols], axis=1)
+    test = _w16(c * q) if mistake == "shortcut_dequantised" else c
+    dc_only = ~test[:, 1:, :].any(axis=(1, 2))
+    if dc_only.any():
+        x0 = _w16(c[dc_only, 0, :] * q[:, 0, :])
+        s = np.clip(x0 << PASS1_BITS, -32768, 32767) if mistake == "shortcut_saturates" \
+            else _w16(x0 << PASS1_BITS)
+        ws[dc_only] = s[:, None, :]
+    # pass 2: rows
+    rows = _one_d_simd(*[ws[:, :, k] for k in range(8)], sum16=sum16)
+    sh = CONST_BITS + PASS1_BITS + 3
+    out = np.stack([_w32(v + (1 << (sh - 1))) >> sh for v in rows], axis=2)
+    return (np.clip(out, -128, 127) + 128).astype(np.uint8)
+
+
+def _idct_c(coef, quant):
+    """jidctint.c jpeg_idct_islow over [N, 64] blocks -> uint8 [N, 8, 8] (vectorised, int64):
+    what a libjpeg-turbo built without SIMD computes, and the "c" mistake of idct_islow."""
     x = coef.astype(np.int64).reshape(-1, 8, 8) * quant.astype(np.int64).reshape(1, 8, 8)
 
     def one_d(i0, i1, i2, i3, i4, i5, i6, i7):
@@ -177,7 +278,7 @@ def idct_islow(coef, quant):
     return _range_limit()[out & 1023]
 
 
-def planes(blob):
+def planes(blob, mistake=None):
     """IDCT output of every component at its full padded block size, plus the header."""
     coef, hd = coefficients(blob)
     res = []
@@ -186,7 +287,7 @@ def planes(blob):
     for ci, (h, v) in enumerate(hd.samp):
         q = hd.tables[ci][2]
         sel = blk[:, :, c0:c0 + h * v].reshape(-1, 64)
-        px = idct_islow(sel, q).reshape(hd.mcuy, hd.mcux, v, h, 8, 8)
+        px = idct_islow(sel, q, mistake).reshape(hd.mcuy, hd.mcux, v, h, 8, 8)
         res.append(px.transpose(0, 2, 4, 1, 3, 5).reshape(hd.mcuy * v * 8, hd.mcux * h * 8))
         c0 += h * v
     return res, hd
@@ -267,9 +368,10 @@ def orient(img, o):
     return img
 
 
-def decode(blob):
-    """uint8 [H, W, 3] RGB: what cv2.cvtColor(cv2.imdecode(...), COLOR_BGR2RGB) returns."""
-    pl, hd = planes(blob)
+def decode(blob, mistake=None):
+    """uint8 [H, W, 3] RGB: what cv2.cvtColor(cv2.imdecode(...), COLOR_BGR2RGB) returns;
+    `mistake` is passed to idct_islow."""
+    pl, hd = planes(blob, mistake)
     H, W = hd.height, hd.width
     ups = []
     for ci, (h, v) in enumerate(hd.samp):

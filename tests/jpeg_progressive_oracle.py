@@ -159,14 +159,15 @@ def coefficients(blob):
     return coef, hd
 
 
-def decode(blob):
-    """uint8 [H, W, 3] RGB through jpeg_oracle's pixel path: what cv2.imdecode + BGR2RGB gives."""
+def decode(blob, mistake=None):
+    """uint8 [H, W, 3] RGB through jpeg_oracle's pixel path: what cv2.imdecode + BGR2RGB gives;
+    `mistake` is passed to jpeg_oracle.idct_islow."""
     coef, hd = coefficients(blob)
     blk = coef.reshape(hd.mcuy, hd.mcux, hd.bpm, 64)
     c0, ups = 0, []
     for ci, (h, v) in enumerate(hd.samp):
         sel = blk[:, :, c0:c0 + h * v].reshape(-1, 64)
-        px = JO.idct_islow(sel, hd.tables[ci][2]).reshape(hd.mcuy, hd.mcux, v, h, 8, 8)
+        px = JO.idct_islow(sel, hd.tables[ci][2], mistake).reshape(hd.mcuy, hd.mcux, v, h, 8, 8)
         pl = px.transpose(0, 2, 4, 1, 3, 5).reshape(hd.mcuy * v * 8, hd.mcux * h * 8)
         c0 += h * v
         dw, dh = -(-hd.width * h // hd.hmax), -(-hd.height * v // hd.vmax)

@@ -47,10 +47,17 @@ def test_oracle_spliced_tables_and_colour_spaces():
         assert np.array_equal(O.decode(blob), JI.cv2_decode(blob))
 
 
-def test_oracle_range_limit_table():
-    t = O._range_limit()
-    assert t[0] == 128 and t[127] == 255 and t[128] == 255 and t[511] == 255
-    assert t[512] == 0 and t[895] == 0 and t[896] == 0 and t[1023] == 127
+def test_oracle_idct_saturates_where_jidctint_wraps():
+    """DC-only blocks (quantiser 1): pass 1's shortcut wraps at dequantised DC 8192 (8191 -> 255,
+    8192 -> 0, -8193 -> 255); pass 2 clamps where jidctint.c's x & 1023 table wraps (4100 -> 513
+    is 255, not 0; -4108 -> -513 is 0, not 255).  The C arithmetic is the "c" mistake."""
+    q = np.ones(64, dtype=np.int64)
+    for dc, want, c_want in ((8191, 255, 128), (8192, 0, 128), (-8193, 255, 128),
+                             (4100, 255, 0), (-4108, 0, 255), (4000, 255, 255)):
+        coef = np.zeros((1, 64), dtype=np.int64)
+        coef[0, 0] = dc
+        assert (O.idct_islow(coef, q) == want).all(), dc
+        assert (O.idct_islow(coef, q, "c") == c_want).all(), dc
 
 
 def test_oracle_refuses_corrupt_data():
