@@ -17,6 +17,11 @@ zlib's run parse and block coding are restated here step for step:
   fix), gen_codes, scan_tree / send_tree and the stored / static / dynamic choice.
 - the bit writer, Adler-32 (per-tile partial sums combined mod 65521), the zlib header with
   cv2's window bits, 8192-byte IDAT chunks with CRC-32, IHDR and IEND.
+
+`encode(img, variant=name)` computes the file with one mistake of VARIANTS made; with no variant
+the output is the file above.  Every block keeps the values its type was chosen from
+(`Block.opt_lenb` and the rest), and `block_trees(..., stats=...)` counts the heap ties and
+length-limit overflows it meets, for the census of tests/png_encode_edge_inputs.py.
 """
 from __future__ import annotations
 
@@ -84,6 +89,23 @@ def gen_codes(lens, max_code):
             next_code[ln] += 1
     return codes
 
+
+# one-mistake variants of the encoder (encode(img, variant=name)); the two marked equivalent
+# cannot change a file: after `if static_lenb <= opt_lenb: opt_lenb = static_lenb`, a tie leaves
+# opt_lenb equal to static_lenb either way, and opt_lenb <= static_lenb makes `<=` and `==` agree
+VARIANTS = {
+    "depth_lt": "smaller()'s depth tiebreak <= made <",
+    "overflow_keep_max": "the length-limit fix-up without bl_count[max_length] -= 1",
+    "overflow_from_max": "the fix-up's search for a shorter leaf starting at max_length",
+    "dummy_zero": "a dummy node of a tree with fewer than two codes always 0",
+    "stored_lt": "the stored pick stored_len + 4 <= opt_lenb made <",
+    "static_min_lt": "static_lenb <= opt_lenb made < (equivalent)",
+    "static_pick_le": "the static pick static_lenb == opt_lenb made <= (equivalent)",
+    "static_tie_dynamic": "a byte tie of static and dynamic coding picks dynamic",
+    "min_count_3": "scan_tree / send_tree's min_count of 4 made 3",
+    "remainder_gt3": "a stretch's remainder r matched only when r > 3",
+}
+EQUIVALENT_VARIANTS = {"static_min_lt", "static_pick_le"}
 
 STATIC_LLEN = [8] * 144 + [9] * 112 + [7] * 24 + [8] * 8
 STATIC_LCODE = gen_codes(STATIC_LLEN, 287)
@@ -158,7 +180,7 @@ def ihdr(h, w):
 
 
 # ----------------------------------------------------------------------------- parse
-def parse(stream):
+def parse(stream, variant=None):
     """Per-position symbol code (the device's sym array): -1, 0..255 literal, 256 + len - 3."""
     s = np.asarray(stream, dtype=np.uint8)
     n = len(s)
@@ -178,7 +200,8 @@ def parse(stream):
     full = (L // MAX_MATCH) * MAX_MATCH
     r = L - full
     code = s[idx].astype(np.int16)                         # the r < 3 tail: literals
-    code = np.where((j >= full) & (r >= 3), np.where(j == full, 256 + r - 3, -1), code)
+    r_min = 4 if variant == "remainder_gt3" else 3
+    code = np.where((j >= full) & (r >= r_min), np.where(j == full, 256 + r - 3, -1), code)
     code = np.where(j < full, np.where(j % MAX_MATCH == 0, 256 + MAX_MATCH - 3, -1), code)
     sym[idx] = code
     return sym
@@ -234,17 +257,21 @@ def stored_ok(sym, bstart, bend, last, w, rowlen):
 
 
 # ----------------------------------------------------------------------------- trees
-def _smaller(freq, depth, n, m):
-    return freq[n] < freq[m] or (freq[n] == freq[m] and depth[n] <= depth[m])
+def _smaller(freq, depth, n, m, variant, stats):
+    if freq[n] != freq[m]:
+        return freq[n] < freq[m]
+    if stats is not None:      # the depth decides; with equal depths the `<=` itself does
+        stats["depth_tie" if depth[n] != depth[m] else "full_tie"] += 1
+    return depth[n] < depth[m] if variant == "depth_lt" else depth[n] <= depth[m]
 
 
-def _downheap(heap, heap_len, freq, depth, k):
+def _downheap(heap, heap_len, freq, depth, k, variant=None, stats=None):
     v = heap[k]
     j = k << 1
     while j <= heap_len:
-        if j < heap_len and _smaller(freq, depth, heap[j + 1], heap[j]):
+        if j < heap_len and _smaller(freq, depth, heap[j + 1], heap[j], variant, stats):
             j += 1
-        if _smaller(freq, depth, v, heap[j]):
+        if _smaller(freq, depth, v, heap[j], variant, stats):
             break
         heap[k] = heap[j]
         k = j
@@ -252,9 +279,10 @@ def _downheap(heap, heap_len, freq, depth, k):
     heap[k] = v
 
 
-def build_tree(freq_in, elems, slen, extra, base, max_length, acc):
+def build_tree(freq_in, elems, slen, extra, base, max_length, acc, variant=None, stats=None):
     """trees.c build_tree + gen_bitlen + gen_codes for one tree.  acc: [opt_len, static_len],
-    updated in place.  Returns (lens[elems], codes[elems], max_code)."""
+    updated in place.  Returns (lens[elems], codes[elems], max_code).  stats (a Counter): heap
+    ties (`depth_tie`, `full_tie`), `overflow` (nodes deeper than max_length) and `dummies`."""
     freq = [0] * HEAP_SIZE
     freq[:elems] = list(freq_in)
     depth = [0] * HEAP_SIZE
@@ -267,11 +295,13 @@ def build_tree(freq_in, elems, slen, extra, base, max_length, acc):
             heap_len += 1
             heap[heap_len] = max_code = n
     while heap_len < 2:
-        if max_code < 2:
+        if max_code < 2 and variant != "dummy_zero":
             max_code += 1
             node = max_code
         else:
             node = 0
+        if stats is not None:
+            stats["dummies"] += 1
         heap_len += 1
         heap[heap_len] = node
         freq[node] = 1
@@ -280,13 +310,13 @@ def build_tree(freq_in, elems, slen, extra, base, max_length, acc):
         if slen is not None:
             acc[1] -= slen[node]
     for n in range(heap_len // 2, 0, -1):
-        _downheap(heap, heap_len, freq, depth, n)
+        _downheap(heap, heap_len, freq, depth, n, variant, stats)
     node = elems
     while True:
         n = heap[1]
         heap[1] = heap[heap_len]
         heap_len -= 1
-        _downheap(heap, heap_len, freq, depth, 1)
+        _downheap(heap, heap_len, freq, depth, 1, variant, stats)
         m = heap[1]
         heap_max -= 1
         heap[heap_max] = n
@@ -297,13 +327,13 @@ def build_tree(freq_in, elems, slen, extra, base, max_length, acc):
         dad[n] = dad[m] = node
         heap[1] = node
         node += 1
-        _downheap(heap, heap_len, freq, depth, 1)
+        _downheap(heap, heap_len, freq, depth, 1, variant, stats)
         if heap_len < 2:
             break
     heap_max -= 1
     heap[heap_max] = heap[1]
     # gen_bitlen
-    bl_count = [0] * 16
+    bl_count = [0] * 17          # [16]: where the overflow_from_max variant moves two leaves
     ln[heap[heap_max]] = 0
     overflow = 0
     for h in range(heap_max + 1, HEAP_SIZE):
@@ -319,21 +349,23 @@ def build_tree(freq_in, elems, slen, extra, base, max_length, acc):
         acc[0] += freq[n] * (bits + xbits)
         if slen is not None:
             acc[1] += freq[n] * (slen[n] + xbits)
+    if stats is not None:
+        stats["overflow"] += overflow
     if overflow:
         while True:
-            bits = max_length - 1
+            bits = max_length - (variant != "overflow_from_max")
             while bl_count[bits] == 0:
                 bits -= 1
             bl_count[bits] -= 1
             bl_count[bits + 1] += 2
-            bl_count[max_length] -= 1
+            bl_count[max_length] -= variant != "overflow_keep_max"
             overflow -= 2
             if overflow <= 0:
                 break
         h = HEAP_SIZE
         for bits in range(max_length, 0, -1):
             n = bl_count[bits]
-            while n:
+            while n and h > heap_max + 1:      # the bound holds unless a variant overcounts
                 h -= 1
                 m = heap[h]
                 if m > max_code:
@@ -346,11 +378,12 @@ def build_tree(freq_in, elems, slen, extra, base, max_length, acc):
     return lens, gen_codes(lens, max_code), max_code
 
 
-def _scan_runs(lens, max_code):
+def _scan_runs(lens, max_code, variant=None):
     """The (symbol, extra value, extra bits) sequence scan_tree counts and send_tree sends."""
+    four = 3 if variant == "min_count_3" else 4
     out = []
     prevlen, nextlen, count = -1, lens[0], 0
-    max_count, min_count = (138, 3) if nextlen == 0 else (7, 4)
+    max_count, min_count = (138, 3) if nextlen == 0 else (7, four)
     for n in range(max_code + 1):
         curlen = nextlen
         nextlen = lens[n + 1] if n + 1 <= max_code else 0xFFFF
@@ -363,7 +396,7 @@ def _scan_runs(lens, max_code):
             if curlen != prevlen:
                 out.append((curlen, 0, 0))
                 count -= 1
-            out.append((16, count - 3, 2))
+            out.append((16, (count - 3) & 3, 2))
         elif count <= 10:
             out.append((17, count - 3, 3))
         else:
@@ -374,51 +407,68 @@ def _scan_runs(lens, max_code):
         elif curlen == nextlen:
             max_count, min_count = 6, 3
         else:
-            max_count, min_count = 7, 4
+            max_count, min_count = 7, four
     return out
 
 
 class Block:
-    """One deflate block: its symbol range, trees, type and bits."""
+    """One deflate block: its symbol range, trees, type and bits, and what the type was chosen
+    from: the frequencies, stored_len, can_store, dyn_lenb, static_lenb and opt_lenb."""
 
 
-def block_trees(lfreq, dfreq, stored_len, can_store):
-    """trees.c _tr_flush_block's decision for one block's frequencies (END_BLOCK counted)."""
+def block_trees(lfreq, dfreq, stored_len, can_store, variant=None, stats=None):
+    """trees.c _tr_flush_block's decision for one block's frequencies (END_BLOCK counted).
+    stats: None, or a dict that receives one Counter per tree ("lit", "dist", "bl")."""
+    from collections import Counter
+
+    st = {k: Counter() for k in ("lit", "dist", "bl")} if stats is not None else {}
     acc = [0, 0]
-    llen, lcode, lmax = build_tree(lfreq, L_CODES, STATIC_LLEN, EXTRA_LBITS, 257, 15, acc)
-    dlen, dcode, dmax = build_tree(dfreq, D_CODES, STATIC_DLEN, EXTRA_DBITS, 0, 15, acc)
-    runs = _scan_runs(llen, lmax) + _scan_runs(dlen, dmax)
+    llen, lcode, lmax = build_tree(lfreq, L_CODES, STATIC_LLEN, EXTRA_LBITS, 257, 15, acc,
+                                   variant, st.get("lit"))
+    dlen, dcode, dmax = build_tree(dfreq, D_CODES, STATIC_DLEN, EXTRA_DBITS, 0, 15, acc,
+                                   variant, st.get("dist"))
+    runs = _scan_runs(llen, lmax, variant) + _scan_runs(dlen, dmax, variant)
     blfreq = [0] * BL_CODES
     for sym, _, _ in runs:
         blfreq[sym] += 1
     blacc = [0, 0]
-    bllen, blcode, _ = build_tree(blfreq, BL_CODES, None, EXTRA_BLBITS, 0, 7, blacc)
+    bllen, blcode, _ = build_tree(blfreq, BL_CODES, None, EXTRA_BLBITS, 0, 7, blacc, variant,
+                                  st.get("bl"))
+    if stats is not None:
+        stats.update(st)
     acc[0] += blacc[0]
     max_blindex = BL_CODES - 1
     while max_blindex >= 3 and bllen[BL_ORDER[max_blindex]] == 0:
         max_blindex -= 1
     acc[0] += 3 * (max_blindex + 1) + 5 + 5 + 4
-    opt_lenb = (acc[0] + 3 + 7) >> 3
+    opt_lenb = dyn_lenb = (acc[0] + 3 + 7) >> 3
     static_lenb = (acc[1] + 3 + 7) >> 3
-    if static_lenb <= opt_lenb:
+    if static_lenb < opt_lenb if variant == "static_min_lt" else static_lenb <= opt_lenb:
         opt_lenb = static_lenb
     b = Block()
     b.opt_len, b.static_len = acc
-    if stored_len + 4 <= opt_lenb and can_store:
+    b.lfreq, b.dfreq, b.stored_len, b.can_store = list(lfreq), list(dfreq), stored_len, can_store
+    b.dyn_lenb, b.static_lenb, b.opt_lenb, b.blfreq = dyn_lenb, static_lenb, opt_lenb, blfreq
+    b.hdr_bits = 0
+    if variant == "stored_lt" and stored_len + 4 < opt_lenb and can_store or \
+            variant != "stored_lt" and stored_len + 4 <= opt_lenb and can_store:
         b.type = STORED
-    elif static_lenb == opt_lenb:
+    elif static_lenb <= opt_lenb if variant == "static_pick_le" else \
+            static_lenb < dyn_lenb if variant == "static_tie_dynamic" else \
+            static_lenb == opt_lenb:
         b.type = STATIC
         llen, lcode, dlen, dcode = STATIC_LLEN[:L_CODES], STATIC_LCODE[:L_CODES], STATIC_DLEN, \
             STATIC_DCODE
     else:
         b.type = DYNAMIC
-        hdr = [(lmax + 1 - 257, 5), (dmax + 1 - 1, 5), (max_blindex + 1 - 4, 4)]
+        hdr = [(lmax + 1 - 257, 5), ((dmax + 1 - 1) & 31, 5), (max_blindex + 1 - 4, 4)]
         hdr += [(bllen[BL_ORDER[r]], 3) for r in range(max_blindex + 1)]
         for sym, xv, xb in runs:
             hdr.append((blcode[sym], bllen[sym]))
             if xb:
                 hdr.append((xv, xb))
         b.hdr = hdr
+        b.hdr_bits = sum(nb for _, nb in hdr)
     b.llen, b.lcode, b.dlen, b.dcode = llen, lcode, dlen, dcode
     return b
 
@@ -465,13 +515,13 @@ class Encoded:
     """encode()'s result: the file and the intermediates the device also reports."""
 
 
-def deflate(stream, rowlen):
+def deflate(stream, rowlen, variant=None):
     """The raw deflate stream of zlib level 1 / Z_RLE over `stream`, plus its blocks."""
     s = np.asarray(stream, dtype=np.uint8)
     n = len(s)
     _, zbits = window_bits(n)
     w = 1 << zbits
-    sym = parse(s)
+    sym = parse(s, variant)
     pos = symbol_starts(sym)
     nsym = len(pos)
     nblocks = nsym // SYMS_PER_BLOCK + 1
@@ -491,7 +541,7 @@ def deflate(stream, rowlen):
         dfreq = np.zeros(D_CODES, dtype=np.int64)
         dfreq[0] = int(is_match.sum())
         b = block_trees([int(x) for x in lfreq], [int(x) for x in dfreq], bend - bstart,
-                        stored_ok(sym, bstart, bend, last, w, rowlen))
+                        stored_ok(sym, bstart, bend, last, w, rowlen), variant)
         b.start, b.end, b.nsym, b.bit_start = bstart, bend, z - a, bw.bits
         bw.put([(b.type << 1) | int(last)], [3])
         if b.type == STORED:
@@ -521,12 +571,14 @@ def deflate(stream, rowlen):
     return bw.tobytes(), sym, nsym, blocks
 
 
-def encode(img):
-    """uint8 [H, W, 3] RGB -> (PNG bytes equal to cv2.imencode('.png', img[..., ::-1]), Encoded)."""
+def encode(img, variant=None):
+    """uint8 [H, W, 3] RGB -> (PNG bytes equal to cv2.imencode('.png', img[..., ::-1]), Encoded);
+    with a variant (a key of VARIANTS), the file that mistake writes."""
+    assert variant is None or variant in VARIANTS, variant
     img = np.asarray(img)
     H, W, _ = img.shape
     stream = filter_rows(img)
-    body, sym, nsym, blocks = deflate(stream, 3 * W + 1)
+    body, sym, nsym, blocks = deflate(stream, 3 * W + 1, variant)
     z = zlib_header(len(stream)) + body + struct.pack(">I", adler32(stream))
     out = bytearray(b"\x89PNG\r\n\x1a\n" + ihdr(H, W))
     for c in range(0, len(z), IDAT_BYTES):
@@ -534,4 +586,5 @@ def encode(img):
     out += chunk(b"IEND", b"")
     e = Encoded()
     e.stream, e.sym, e.nsym, e.blocks, e.body, e.zstream = stream, sym, nsym, blocks, body, z
+    e.rowlen = 3 * W + 1
     return bytes(out), e
