@@ -18,6 +18,7 @@
  *   mrx_rle_count / _write (extension: the same masks as COCO run-length encodings)
  *   mrx_rle_strings        (extension: those encodings as COCO compressed RLE strings)
  *   mrx_contours_count / _write <- visualize.display_instances (contour polygons) serve.py:160-169
+ *   mrx_annotate_draw / _resolve <- visualize.display_instances (boxes, outlines, captions) serve.py:160-169
  *   mrx_mask_extents / _overlaps / _matches (extension: mrcnn.utils.compute_overlaps_masks and
  *                             compute_matches, scoring the masks against ground truth)
  *   mrx_rle_parse / _decode (extension: ground truth given as COCO RLE, decoded to packed planes)
@@ -342,6 +343,43 @@ int mrx_contours_write(const unsigned char *d_packed, const long long *d_packed_
                        long long max_inst_segments, void *d_scratch, float *d_vertices,
                        long long *d_contour_off, long long *d_inst_contour_off, int B, int R,
                        int max_h, void *stream);
+
+/* EXTENSION: the boxes, contour outlines and captions visualize.display_instances draws over the
+ * overlay (serve.py:160-169), as these OpenCV calls draw them at the image's own resolution
+ * (annotate.cu; DESIGN.md section 3.25): for every kept instance k whose box is not all zeros, in
+ * order, cv2.rectangle(img, (x1, y1), (x2, y2), col_k, 1, LINE_8) when show_bbox, and
+ * cv2.polylines(img, [int32(2 v)], False, col_k, 1, LINE_8, shift=1) for each of its contours v;
+ * then every caption, cv2.putText in white.  Two calls:
+ *   mrx_annotate_draw:    d_keys: int32 key planes, image b's [H_b, W_b] at d_keys + d_key_off[b]
+ *                         (int64, in elements); they are zeroed, then every pixel instance k draws
+ *                         does atomicMax(key, k + 1), so a later instance wins.  Box edges are
+ *                         clipped to the image.  A contour segment sets its two end points rounded
+ *                         half up, ((2x + 1) >> 1, (2y + 1) >> 1), where they lie in the image (what
+ *                         LINE_8 with shift=1 draws for every step between edge midpoints).  d_boxes
+ *                         [B,R,4] int32 (y1, x1, y2, x2); the contours as mrx_contours_write leaves
+ *                         them: d_vertices [n_vertices, 2], d_contour_off, d_inst_contour_off
+ *                         [B*R + 1] (instance i = b*R + k); n_vertices = 0 draws no outline (the
+ *                         three pointers may then be NULL).
+ *   mrx_annotate_resolve: the uint8 [H_b, W_b, 3] images at d_images + d_image_off[b] (int64 bytes)
+ *                         in place: a pixel with key k + 1 becomes d_rgb8[b][k] (uint8 [B,R,3]);
+ *                         then the P caption patches are set to 255 where their stencil bit is
+ *                         set: record p is d_patches[6p .. 6p+5] = (image, y0, x0, h, w, byte
+ *                         offset) int64, and patch pixel (y, x) is bit 7 - (j & 7) of
+ *                         d_stencils[offset + (j >> 3)], j = y*w + x.  Patch pixels outside their
+ *                         image, and records of an image outside [0, B), are not written.
+ * max_pixels: the extent of "Output slots".  Checks: null pointers, B outside [0, MRX_MAX_BATCH], R
+ * outside [1, 65534], max_pixels outside [0, 2^31 - 1), n_vertices or P below 0: MRX_E_INVALID.
+ * B = 0 or max_pixels = 0 returns MRX_OK without launching anything. */
+int mrx_annotate_draw(const int *d_counts, const int *d_geom, const int *d_boxes,
+                      const float *d_vertices, const long long *d_contour_off,
+                      const long long *d_inst_contour_off, long long n_vertices, int show_bbox,
+                      int *d_keys, const long long *d_key_off, int B, int R, long long max_pixels,
+                      void *stream);
+int mrx_annotate_resolve(const int *d_geom, const int *d_keys, const long long *d_key_off,
+                         const unsigned char *d_rgb8, unsigned char *d_images,
+                         const long long *d_image_off, const unsigned char *d_stencils,
+                         const long long *d_patches, int P, int B, int R, long long max_pixels,
+                         void *stream);
 
 /* ---------------------------------------------------------------- mask IoU and matches */
 /* EXTENSION: upstream mrcnn.utils.compute_overlaps_masks and the matching loop of compute_matches

@@ -700,16 +700,24 @@ def unmold_detections_contours_batch(items):
     return [metas[b] + (contours[b],) for b in range(st.n)]
 
 
-def unmold_overlay_batch(items, images, colors=None, alpha=0.5):
+def _check_annotate(annotate, class_names):
+    if annotate and class_names is None:
+        raise ValueError("annotate=True needs class_names for the captions")
+
+
+def unmold_overlay_batch(items, images, colors=None, alpha=0.5, annotate=False, class_names=None):
     """`unmold_detections` followed by the mask overlay of `visualize.display_instances`
     (serve.py:147-169) without moving the masks to the host: the [H,W,N] canvases stay on
     the device, only boxes, class ids, scores and the blended uint8 images come back.
 
     items as for `unmold_detections_batch`; images: the original uint8 HxWx3 images;
     colors: RGB triples (shared list, or one list per image; default: `random_colors(R)`).
+    annotate=True also draws each instance's box, contour outlines and caption
+    "<class_names[class_id]> <score:.3f>" as OpenCV draws them (`visualize.composite_batch`).
     Returns a list of (boxes, class_ids, scores, overlay_uint8)."""
     from . import visualize
 
+    _check_annotate(annotate, class_names)
     if len(items) == 0:
         return []
     with _Staged(items) as st:
@@ -717,7 +725,8 @@ def unmold_overlay_batch(items, images, colors=None, alpha=0.5):
         eng.enqueue(st.d_det, st.d_msk)
         if colors is None:
             colors = visualize.random_colors(eng.R)
-        overlays = visualize.composite_batch(eng, images, colors, alpha)
+        overlays = visualize.composite_batch(eng, images, colors, alpha, annotate=annotate,
+                                             class_names=class_names)
         counts, metas = st.meta()
         host = [o.cpu().numpy() for o in overlays]
     return [metas[b] + (host[b],) for b in range(st.n)]
@@ -734,15 +743,16 @@ def _check_file_format(image_format, quality):
 
 
 def _unmold_overlay_file_batch(items, images, colors=None, alpha=0.5, image_format="png",
-                               quality=95):
+                               quality=95, annotate=False, class_names=None):
     """`unmold_overlay_batch` that stops at the device overlays and encodes them there: returns
     (boxes, class_ids, scores, file_bytes) per image, the file being what
     `cv2.imencode('.png', overlay[..., ::-1])` gives for the overlay `unmold_overlay_batch`
-    returns, or with image_format "jpeg" `cv2.imencode('.jpg', ...)` at `quality`.  Only the
-    file bytes leave the device."""
+    returns (with the same `annotate` and `class_names`), or with image_format "jpeg"
+    `cv2.imencode('.jpg', ...)` at `quality`.  Only the file bytes leave the device."""
     from . import visualize
 
     _check_file_format(image_format, quality)
+    _check_annotate(annotate, class_names)
     if len(items) == 0:
         return []
     with _Staged(items) as st:
@@ -750,7 +760,8 @@ def _unmold_overlay_file_batch(items, images, colors=None, alpha=0.5, image_form
         eng.enqueue(st.d_det, st.d_msk)
         if colors is None:
             colors = visualize.random_colors(eng.R)
-        overlays = visualize.composite_batch(eng, images, colors, alpha)
+        overlays = visualize.composite_batch(eng, images, colors, alpha, annotate=annotate,
+                                             class_names=class_names)
         counts, metas = st.meta()
         if image_format == "jpeg":
             files = encode_jpeg_batch(overlays, quality)

@@ -24,7 +24,7 @@ LIB_DIR = os.path.join(PKG_DIR, "lib")
 SOURCES = ["capi.cu", "anchors.cu", "unmold.cu", "expand_team.cu", "expand_bits.cu", "mold.cu",
            "composite.cu", "pack.cu", "rle.cu", "contours.cu", "overlaps.cu", "rle_decode.cu", "cocoeval.cu",
            "boundary.cu", "polygons.cu", "peer.cu", "alloc.cu", "jpeg.cu", "png.cu", "png_decode.cu",
-           "jpeg_encode.cu"]
+           "jpeg_encode.cu", "annotate.cu"]
 HEADERS = [os.path.join(CSRC, "common.cuh"), os.path.join(CSRC, "expand.cuh"),
            os.path.join(CSRC, "planes.cuh"), os.path.join(CSRC, "deflate.cuh"),
            os.path.join(os.path.dirname(PKG_DIR), "include", "mrx.h")]

@@ -442,6 +442,27 @@ class UnmoldEngine:
             verts, coff = _download_contours(d_vert, d_coff)
         return contours_to_lists(verts, coff, icoff, counts, self.layout)
 
+    def annotate(self, d_images, d_image_off, rgb8, patches, show_bbox=True, stream=None):
+        """EXTENSION: draw the boxes, contour outlines and captions of `display_instances` on the
+        planned batch's overlays (after `enqueue` and the composite), in place, as OpenCV draws
+        them (DESIGN.md section 3.25): the byte canvas packed (`pack_masks`), the contours traced
+        inside each box (`trace_contours`, one host read), then mrx_annotate_draw and
+        mrx_annotate_resolve.  d_images: uint8 device tensor, image b's [H_b, W_b, 3] at byte
+        offset d_image_off[b] (int64 device tensor [n]); rgb8 [n, R, 3] uint8
+        (`visualize.color_table`); patches: the caption stencils (`visualize.caption_stencils`).
+        The trace and key buffers live in `_contour_bufs`."""
+        if self.layout is None or self.d_canvas is None:
+            raise RuntimeError("annotate needs the byte canvas: call plan() and enqueue() first")
+        n = self._n_images
+        with _stream_ctx(stream):
+            self.pack_masks()
+            d_vert, d_coff, _ = self.trace_contours()
+            d_icoff = self._contour_bufs["inst_contour_off"][:n * self.R + 1]
+            annotate_overlays(self.lib, self.device, self.d_counts, self.d_geom, self.d_boxes,
+                              (d_vert, d_coff, d_icoff), d_images, d_image_off,
+                              [self.layout.hw(b) for b in range(n)], self.R, rgb8, patches,
+                              show_bbox, bufs=self._contour_bufs)
+
     # ------------------------------------------------------------------ scoring against ground truth
     def ground_truth(self, class_ids, masks, stream=None):
         """A `MaskBatch` of ground truth for the planned images: class_ids[b] [M_b] and bool
@@ -1426,6 +1447,35 @@ def _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom
     n_contours = int(icoff[-1])
     # every contour repeats its first vertex: V = S + C
     return d_vert[:2 * (S + n_contours)].view(-1, 2), d_coff[:n_contours + 1], icoff
+
+
+def annotate_overlays(lib, dev, d_counts, d_geom, d_boxes, trace, d_images, d_image_off, hws, R,
+                    rgb8, patches, show_bbox, stream=None, bufs=None):
+    """mrx_annotate_draw then mrx_annotate_resolve on the overlays at `d_images` (image b at byte
+    offset d_image_off[b]), in place.  trace: (d_vertices, d_contour_off, d_inst_contour_off) of
+    the batch's contours; rgb8 [B, R, 3] uint8 (`visualize.color_table`); patches: `visualize.caption_stencils`;
+    bufs: keeps the key planes between calls."""
+    torch = _torch()
+    B = len(hws)
+    pixels = np.array([H * W for H, W in hws], dtype=np.int64)
+    key_off = np.zeros(B + 1, dtype=np.int64)
+    np.cumsum(pixels, out=key_off[1:])
+    d_keys = _buffer({} if bufs is None else bufs, "keys", max(int(key_off[-1]), 1), torch.int32,
+                     dev)
+    d_key_off = torch.from_numpy(key_off[:B].copy()).to(dev)
+    d_vert, d_coff, d_icoff = trace
+    max_px = int(pixels.max(initial=0))
+    st = N.stream_ptr(stream)
+    N.check(lib.mrx_annotate_draw(d_counts, d_geom, d_boxes, d_vert, d_coff, d_icoff,
+                                  d_vert.shape[0], int(bool(show_bbox)), d_keys, d_key_off, B, R,
+                                  max_px, st), "mrx_annotate_draw")
+    recs, bits = patches
+    d_rgb8 = torch.from_numpy(np.ascontiguousarray(rgb8, dtype=np.uint8)).to(dev)
+    d_recs = torch.from_numpy(recs).to(dev) if len(recs) else None
+    d_bits = torch.from_numpy(bits).to(dev) if len(recs) else None
+    N.check(lib.mrx_annotate_resolve(d_geom, d_keys, d_key_off, d_rgb8, d_images, d_image_off,
+                                     d_bits, d_recs, len(recs), B, R, max_px, st),
+            "mrx_annotate_resolve")
 
 
 def _download_contours(d_vert, d_coff):

@@ -24,7 +24,10 @@ pixels: the PNG file is encoded on the device, byte for byte what `cv2.imwrite` 
 (`api_utils.encode_png_batch`), and only its bytes are downloaded.  `image_format="jpeg"` writes
 `media/mask-<uuid>.jpg` instead, the bytes `cv2.imencode('.jpg')` gives at `quality`
 (`api_utils.encode_jpeg_batch`), several times smaller than the PNG.  Boxes, captions and
-contour polygons are matplotlib artists in the reference and are not drawn (DESIGN.md 7).
+contour polygons are matplotlib artists in the reference; by default they are not drawn.
+`annotate=True` draws them on the device as OpenCV draws them (DESIGN.md 3.25), the captions
+naming the classes `["BG", *cf.DAMAGE_CLASSES]` as serve.py:165 does; matplotlib's own styling
+stays out of scope (DESIGN.md 7).
 
 Wherever an image is accepted, a JPEG or PNG file's bytes (bytes, bytearray or memoryview) are
 accepted too, told apart by their signature (`imagefile`): they are decoded on the device
@@ -245,16 +248,19 @@ def _save_file(data, ext, media_dir=None):
     return save_path
 
 
-def do_inference(img, colors=None, media_dir=None, image_format="png", quality=95):
+def do_inference(img, colors=None, media_dir=None, image_format="png", quality=95,
+                 annotate=False):
     """serve.py:141-173: inference, unmold, mask overlay, PNG -> `save_path`.  The masks stay
     on the device between the unmold and the overlay (`api_utils.unmold_overlay_batch`).
     image_format "jpeg" writes `media/mask-<uuid>.jpg` instead, the bytes of
-    `cv2.imencode('.jpg')` of the overlay at `quality`, encoded on the device."""
+    `cv2.imencode('.jpg')` of the overlay at `quality`, encoded on the device.  annotate=True
+    also draws the boxes, contour outlines and captions (module docstring)."""
     return do_inference_batch([img], colors=colors, media_dir=media_dir,
-                              image_format=image_format, quality=quality)[0]
+                              image_format=image_format, quality=quality, annotate=annotate)[0]
 
 
-def do_inference_batch(imgs, colors=None, media_dir=None, image_format="png", quality=95):
+def do_inference_batch(imgs, colors=None, media_dir=None, image_format="png", quality=95,
+                       annotate=False):
     """`do_inference` for a list of images: batched pre-processing, one RPC per image, ONE
     batched unmold + overlay on the device, one PNG (or JPEG) per image.  Returns the list of
     paths."""
@@ -265,8 +271,9 @@ def do_inference_batch(imgs, colors=None, media_dir=None, image_format="png", qu
     res, sources = _grpc_inference_batch(imgs)
     items = [(det, msk, tuple(src.shape), mshape, window)
              for (det, msk, mshape, window), src in zip(res, sources)]
-    outs = api_utils._unmold_overlay_file_batch(items, sources, colors=colors,
-                                                image_format=image_format, quality=quality)
+    outs = api_utils._unmold_overlay_file_batch(
+        items, sources, colors=colors, image_format=image_format, quality=quality,
+        annotate=annotate, class_names=["BG", *cf.DAMAGE_CLASSES] if annotate else None)
     ext = "jpg" if image_format == "jpeg" else "png"
     paths = []
     for _boxes, _cls, _scores, data in outs:

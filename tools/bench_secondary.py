@@ -7,6 +7,7 @@ each unmold workload also names the GPU and its power limit.
   python tools/bench_secondary.py --only-eval | --only-cocoeval | --only-bboxeval | --only-boundaryeval
                                   | --only-polygons | --only-lvis | --only-jpeg | --only-png
                                   | --only-jpeg-progressive | --only-png-decode | --only-jpeg-encode
+                                  | --only-annotate
 """
 import argparse
 import json
@@ -1339,6 +1340,97 @@ def jpeg_encode_case(iters):
             "host_threads": os.cpu_count(), **card()}), flush=True)
 
 
+def annotate_case(iters):
+    """The boxes, contour outlines and captions of display_instances drawn on the overlay
+    (csrc/annotate.cu, DESIGN.md section 3.25) on 32 x 1024^2 x 100 and 16 x 2160x3840 x 50
+    synthetic batches: the kernels of `UnmoldEngine.annotate` (pack, contour trace, draw,
+    resolve) from a profile, the host caption stencils, and the tail of do_inference_batch (unmold
+    + overlay + files written) with and without annotate, for PNG and JPEG.  The synthetic masks
+    are thresholded noise: their outlines have thousands of segments each, far more than a real
+    mask's."""
+    import random
+    import tempfile
+
+    from torch.profiler import ProfilerActivity, profile
+
+    from matterport_maskrcnn_with_tensorflow_serving_b200 import api_utils, visualize
+
+    names = ["BG"] + ["class_%d" % i for i in range(1, 81)]
+    for name, batch, hw, n in [("configs[1] 32 x 1024x1024 x 100", 32, (1024, 1024), 100),
+                               ("configs[3] size: 16 x 2160x3840 x 50", 16, (2160, 3840), 50)]:
+        ims = synth.make_batch(5, 4, hw, n, num_classes=81, max_instances=n)
+        items = [(ims[b % 4].detections, ims[b % 4].mrcnn_mask, ims[b % 4].original_image_shape,
+                  ims[b % 4].image_shape, ims[b % 4].window) for b in range(batch)]
+        rng = np.random.default_rng(3)
+        base = [synth.synth_rgb_image(rng, *hw) for _ in range(4)]
+        images = [torch.from_numpy(base[b % 4]).cuda() for b in range(batch)]
+        colors = visualize.random_colors(n, rng=random.Random(0))
+        eng = UnmoldEngine(batch, n, (28, 28), 81)
+        eng.plan([make_geom(*it[2:]) for it in items])
+        d_det = torch.from_numpy(np.stack([it[0] for it in items])).cuda()
+        d_msk = torch.from_numpy(np.stack([it[1] for it in items])).cuda()
+        eng.enqueue(d_det, d_msk)
+        stage = visualize.CompositeStage(eng, images, colors)
+        stage.run()
+        counts, boxes, ids, scs = eng.fetch_meta()
+        boxes = [boxes[b, :int(counts[b])].copy() for b in range(batch)]
+        ids = [ids[b, :int(counts[b])].copy() for b in range(batch)]
+        scs = [scs[b, :int(counts[b])].copy() for b in range(batch)]
+        hws = [hw] * batch
+
+        def host_clock(fn, k):
+            fn()
+            ts = []
+            for _ in range(k):
+                t0 = time.perf_counter()
+                fn()
+                torch.cuda.synchronize()
+                ts.append((time.perf_counter() - t0) * 1e3)
+            return float(np.median(ts))
+
+        k = max(3, iters // 4)
+        caption_ms = host_clock(lambda: visualize.caption_stencils(boxes, hws, ids, names, scs), k)
+        patches = visualize.caption_stencils(boxes, hws, ids, names, scs)
+        rgb8 = np.stack([visualize.color_table(colors, n)] * batch)
+        annotate = lambda: eng.annotate(stage.d_out, stage.d_off, rgb8, patches)   # noqa: E731
+        annotate()
+        d_vert, _, icoff = eng.trace_contours()
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(3):
+                annotate()
+            torch.cuda.synchronize()
+        kern = {}
+        for ev in prof.key_averages():
+            for part, keys in (("pack", ("pack_",)), ("trace", ("contour_", "offsets_scan")),
+                               ("draw", ("annotate_zero", "annotate_box", "annotate_vertex")),
+                               ("resolve", ("annotate_resolve", "annotate_caption"))):
+                if any(key in ev.key for key in keys):
+                    kern[part] = round(kern.get(part, 0) + ev.device_time_total / 1e3 / 3, 4)
+        step_ms = host_clock(annotate, k)
+        with tempfile.TemporaryDirectory() as tmp:
+            def tail(fmt, ann):
+                outs = api_utils._unmold_overlay_file_batch(
+                    items, images, colors, image_format=fmt, annotate=ann,
+                    class_names=names if ann else None)
+                for b, o in enumerate(outs):
+                    with open(os.path.join(tmp, f"{b}.{fmt}"), "wb") as f:
+                        f.write(o[3])
+
+            tails = {f"do_inference_batch_tail_{fmt}{'_annotated' if ann else ''}_ms":
+                     round(host_clock(lambda: tail(fmt, ann), k), 3)
+                     for fmt in ("png", "jpeg") for ann in (False, True)}
+        n_vert, n_contours = int(d_vert.shape[0]), int(icoff[-1])
+        print(json.dumps({
+            "workload": f"annotate {name} (synthetic noise masks)",
+            "instances": int(sum(counts)), "contour_segments": n_vert - n_contours,
+            "caption_patches": int(patches[0].shape[0]),
+            "kernel_ms": kern, "annotate_step_ms_incl_host_reads": round(step_ms, 3),
+            "host_caption_stencils_ms": round(caption_ms, 3), **tails, **card()}), flush=True)
+        del eng, stage, d_det, d_msk
+        torch.cuda.empty_cache()
+
+
 def png_decode_case(iters):
     """PNG request bytes decoded on the device (csrc/png_decode.cu) against cv2.imdecode on the host,
     each followed by preprocess_input_batch: 32 x 1024^2 as cv2.imwrite writes them (level 1,
@@ -1449,8 +1541,13 @@ def main():
                     help="only the progressive JPEG decode record")
     ap.add_argument("--only-png-decode", action="store_true", help="only the PNG decode record")
     ap.add_argument("--only-jpeg-encode", action="store_true", help="only the JPEG encode record")
+    ap.add_argument("--only-annotate", action="store_true",
+                    help="only the annotated overlay record")
     args = ap.parse_args()
     torch.cuda.set_device(0)
+    if args.only_annotate:
+        annotate_case(args.iters)
+        return
     if args.only_png_decode:
         png_decode_case(args.iters)
         return
