@@ -321,7 +321,7 @@ int mrx_rle_strings(const unsigned int *d_run_lengths, const long long *d_inst_o
  *                        instances before i = b*R + k, d_inst_off[B*R] = their total S.  The
  *                        caller reads them and allocates, from S alone:
  *                          d_scratch          MRX_CONTOUR_SCRATCH_BYTES(S) bytes
- *                          d_vertices         float32 [S + S/4, 2]   (every contour has >= 4 segments)
+ *                          d_vertices         float64 [S + S/4, 2]   (every contour has >= 4 segments)
  *                          d_contour_off      int64 [S/4 + 1]
  *                          d_inst_contour_off int64 [B*R + 1]
  *   mrx_contours_write:  total_segments = S, max_inst_segments = the largest d_inst_off[i+1] -
@@ -329,7 +329,8 @@ int mrx_rle_strings(const unsigned int *d_run_lengths, const long long *d_inst_o
  *                        contours are c in [d_inst_contour_off[i], d_inst_contour_off[i+1]), in
  *                        find_contours' order; contour c's vertices are
  *                        d_vertices[d_contour_off[c] .. d_contour_off[c+1]) as (x, y) pairs, the
- *                        first repeated at the end.  The values are exact (integers and halves).
+ *                        first repeated at the end.  The values are exact (integers and halves,
+ *                        float64 for every side below 2^30; float32 would round halves past 2^23).
  * S above MRX_MAX_CONTOUR_SEGMENTS: MRX_E_UNSUPPORTED (split the batch). */
 #define MRX_MAX_CONTOUR_SEGMENTS (1 << 30)
 #define MRX_CONTOUR_SCRATCH_BYTES(S) (48LL * (S) + 256)
@@ -340,7 +341,7 @@ int mrx_contours_count(const unsigned char *d_packed, const long long *d_packed_
 int mrx_contours_write(const unsigned char *d_packed, const long long *d_packed_off,
                        const int *d_counts, const int *d_geom, const int *d_regions,
                        const int *d_row_off, const long long *d_inst_off, long long total_segments,
-                       long long max_inst_segments, void *d_scratch, float *d_vertices,
+                       long long max_inst_segments, void *d_scratch, double *d_vertices,
                        long long *d_contour_off, long long *d_inst_contour_off, int B, int R,
                        int max_h, void *stream);
 
@@ -357,7 +358,7 @@ int mrx_contours_write(const unsigned char *d_packed, const long long *d_packed_
  *                         half up, ((2x + 1) >> 1, (2y + 1) >> 1), where they lie in the image (what
  *                         LINE_8 with shift=1 draws for every step between edge midpoints).  d_boxes
  *                         [B,R,4] int32 (y1, x1, y2, x2); the contours as mrx_contours_write leaves
- *                         them: d_vertices [n_vertices, 2], d_contour_off, d_inst_contour_off
+ *                         them: d_vertices float64 [n_vertices, 2], d_contour_off, d_inst_contour_off
  *                         [B*R + 1] (instance i = b*R + k); n_vertices = 0 draws no outline (the
  *                         three pointers may then be NULL).
  *   mrx_annotate_resolve: the uint8 [H_b, W_b, 3] images at d_images + d_image_off[b] (int64 bytes)
@@ -371,7 +372,7 @@ int mrx_contours_write(const unsigned char *d_packed, const long long *d_packed_
  * outside [1, 65534], max_pixels outside [0, 2^31 - 1), n_vertices or P below 0: MRX_E_INVALID.
  * B = 0 or max_pixels = 0 returns MRX_OK without launching anything. */
 int mrx_annotate_draw(const int *d_counts, const int *d_geom, const int *d_boxes,
-                      const float *d_vertices, const long long *d_contour_off,
+                      const double *d_vertices, const long long *d_contour_off,
                       const long long *d_inst_contour_off, long long n_vertices, int show_bbox,
                       int *d_keys, const long long *d_key_off, int B, int R, long long max_pixels,
                       void *stream);

@@ -77,13 +77,13 @@ __device__ __forceinline__ int last_at_most(const long long *__restrict__ off, i
 }
 
 // a half-pixel coordinate u (2u an integer) rounded half up: floor((2u + 1) / 2)
-__device__ __forceinline__ int round_half_up(float u) {
-  return (__float2int_rn(2.0f * u) + 1) >> 1;
+__device__ __forceinline__ int round_half_up(double u) {
+  return (__double2int_rn(2.0 * u) + 1) >> 1;
 }
 
 __global__ void __launch_bounds__(kThreads)
 annotate_vertex_kernel(const int *__restrict__ counts, const int *__restrict__ geom,
-                       const int4 *__restrict__ boxes, const float2 *__restrict__ verts,
+                       const int4 *__restrict__ boxes, const double2 *__restrict__ verts,
                        const long long *__restrict__ contour_off,
                        const long long *__restrict__ inst_contour_off, long long n_vertices,
                        int *__restrict__ keys, const long long *__restrict__ key_off, int B, int R) {
@@ -99,7 +99,7 @@ annotate_vertex_kernel(const int *__restrict__ counts, const int *__restrict__ g
     const int b = i / R, k = i - b * R;
     if (k >= counts[b] || box_is_zero(boxes[i])) continue;
     const int H = geom[b * MRX_GEOM_INTS + 0], W = geom[b * MRX_GEOM_INTS + 1];
-    const float2 p = verts[v];
+    const double2 p = verts[v];
     const int x = round_half_up(p.x), y = round_half_up(p.y);
     if (x < 0 || x >= W || y < 0 || y >= H) continue;
     atomicMax(keys + key_off[b] + static_cast<long long>(y) * W + x, k + 1);
@@ -171,7 +171,7 @@ static int check_batch(const char *fn, int B, int R, long long max_pixels) {
 }
 
 extern "C" int mrx_annotate_draw(const int *d_counts, const int *d_geom, const int *d_boxes,
-                                 const float *d_vertices, const long long *d_contour_off,
+                                 const double *d_vertices, const long long *d_contour_off,
                                  const long long *d_inst_contour_off, long long n_vertices,
                                  int show_bbox, int *d_keys, const long long *d_key_off, int B,
                                  int R, long long max_pixels, void *stream) {
@@ -196,7 +196,7 @@ extern "C" int mrx_annotate_draw(const int *d_counts, const int *d_geom, const i
   if (n_vertices > 0) {
     const long long blocks = min((n_vertices + kThreads - 1) / kThreads, static_cast<long long>(dev.sms) * 16);
     annotate_vertex_kernel<<<static_cast<unsigned>(blocks), kThreads, 0, st>>>(
-        d_counts, d_geom, boxes, reinterpret_cast<const float2 *>(d_vertices), d_contour_off,
+        d_counts, d_geom, boxes, reinterpret_cast<const double2 *>(d_vertices), d_contour_off,
         d_inst_contour_off, n_vertices, d_keys, d_key_off, B, R);
     MRX_LAUNCH_CHECK("annotate_vertex_kernel");
   }

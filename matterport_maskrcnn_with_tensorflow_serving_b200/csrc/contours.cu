@@ -24,12 +24,17 @@
 //                         offsets
 //   --- one host read of the total S and of the longest instance ---
 //   contour_link_kernel   the same walk over three cell rows: each segment's raster number, its
-//                         to-vertex, and its successor's number (row offset + popcount prefix)
+//                         to-vertex in half pixels, and its successor's number (row offset +
+//                         popcount prefix)
 //   contour_jump_kernel   ceil(log2(max S_i)) rounds of pointer jumping: each segment learns the
 //                         smallest and largest number of its cycle and its distance to the largest
 //   contour_head / scan / write kernels   contour lengths, an exclusive scan over the segments
 //                         (contours and vertices before each cycle head; the tile sums by
 //                         offsets_scan_kernel), the vertex stores
+//
+// Vertices are edge midpoints, integers and halves up to 2^30 (the largest side).  float32 holds
+// a half exactly only below 2^23 and an integer only up to 2^24, so the link pass keeps each
+// to-point as int32 half-units (2x, 2y: at most 2^31 - 1) and the write pass stores float64.
 //
 // Pointer jumping reads one 16-byte record per segment and round at a random address: the cost is
 // about ceil(log2(max S_i)) x 48 bytes of traffic per segment, far above the counting walk.
@@ -78,7 +83,7 @@ struct Params {
   int R, row_pitch;
   // link pass
   int *succ;                     // [S]
-  float2 *to;                    // [S]
+  int2 *to;                      // [S] to-points in half pixels (2x, 2y)
   int4 *jump;                    // [S] (jump pointer, min, max, distance to max)
 };
 
@@ -132,6 +137,10 @@ __device__ __forceinline__ uint64_t pixel_bits(const Inst &in, int y, int x) {
   v = __brevll(v << (x & 7));
   return v & span_mask(in.g.x1 - x, in.g.x2 - x);
 }
+
+// the midpoint of pixel coordinates a and b in half pixels, a + b: an edge between two pixels of
+// the image and its ring, so a, b < 2^30 and the sum fits
+__device__ __forceinline__ int half_units(int a, int b) { return a + b; }
 
 // the cases of the 34 cells c0 - 1 + j of cell row r, as corner bit masks over j
 struct CellRow {
@@ -233,26 +242,26 @@ contour_link_kernel(const Params p) {
       for (int t = 0; t < nseg; ++t) {
         const int to = t == 0 ? static_cast<int>((kToTab >> (2 * q)) & 3u) : (q == 6 ? kBottom : kRight);
         int next;
-        float2 v;
+        int2 v;   // (2x, 2y) = the to-edge's two pixel coordinates summed
         switch (to) {
           case kTop:      // enters the cell above through its bottom edge (case 9's second segment)
             next = wu + up.before(jj) + static_cast<int>((up.s9 >> jj) & 1ull);
-            v = make_float2(c - 0.5f, static_cast<float>(r - 1));
+            v = make_int2(half_units(c - 1, c), half_units(r - 1, r - 1));
             break;
           case kBottom:   // enters the cell below through its top edge
             next = wd + dn.before(jj);
-            v = make_float2(c - 0.5f, static_cast<float>(r));
+            v = make_int2(half_units(c - 1, c), half_units(r, r));
             break;
           case kLeft: {   // enters the cell to the left through its right edge
             const int jl = jj - 1;
             next = jl == 0 ? wc - 1 - static_cast<int>((sad_c & 1ull) != 0) : wc + cr.before(jl);
-            v = make_float2(static_cast<float>(c - 1), r - 0.5f);
+            v = make_int2(half_units(c - 1, c - 1), half_units(r - 1, r));
             break;
           }
           default: {      // right: enters the cell to the right through its left edge
             const int jr = jj + 1;   // (case 6's second segment)
             next = wc + cr.before(jr) + static_cast<int>((cr.s6 >> jr) & 1ull);
-            v = make_float2(static_cast<float>(c), r - 0.5f);
+            v = make_int2(half_units(c, c), half_units(r - 1, r));
             break;
           }
         }
@@ -341,18 +350,20 @@ contour_scan_apply_kernel(unsigned long long *v, const unsigned long long *__res
 }
 
 // Vertex j (1..L) of a contour is the to-point of the segment j steps after its largest one; the
-// largest segment also stores vertex 0.  Cycle heads store their contour's vertex offset.
+// largest segment also stores vertex 0.  Cycle heads store their contour's vertex offset.  The
+// half-units convert to float64 exactly.
 __global__ void __launch_bounds__(256)
 contour_write_kernel(const int4 *__restrict__ f, const int *__restrict__ len,
-                     const unsigned long long *__restrict__ pre, const float2 *__restrict__ to,
-                     float2 *__restrict__ verts, long long *__restrict__ contour_off, int S) {
+                     const unsigned long long *__restrict__ pre, const int2 *__restrict__ to,
+                     double2 *__restrict__ verts, long long *__restrict__ contour_off, int S) {
   for (int s = blockIdx.x * blockDim.x + threadIdx.x; s < S; s += gridDim.x * blockDim.x) {
     const int4 r = f[s];
     const int m = r.y;
     const unsigned long long pm = pre[m];
     const unsigned base = static_cast<unsigned>(pm);
     const int L = len[m];
-    const float2 v = to[s];
+    const int2 h = to[s];
+    const double2 v = make_double2(0.5 * h.x, 0.5 * h.y);
     verts[base + static_cast<unsigned>(L - r.w)] = v;
     if (r.w == 0) verts[base] = v;
     if (m == s) contour_off[pm >> 32] = static_cast<long long>(base);
@@ -424,7 +435,7 @@ extern "C" int mrx_contours_write(const unsigned char *d_packed, const long long
                                   const int *d_counts, const int *d_geom, const int *d_regions,
                                   const int *d_row_off, const long long *d_inst_off,
                                   long long total_segments, long long max_inst_segments,
-                                  void *d_scratch, float *d_vertices, long long *d_contour_off,
+                                  void *d_scratch, double *d_vertices, long long *d_contour_off,
                                   long long *d_inst_contour_off, int B, int R, int max_h,
                                   void *stream) {
   using namespace contours;
@@ -448,10 +459,10 @@ extern "C" int mrx_contours_write(const unsigned char *d_packed, const long long
   if (int rc = current_device_info(&dev)) return rc;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int ntiles = (S + kScanTile - 1) / kScanTile;
-  // scratch: two jump records, to-points and successors per segment, then the tile sums
+  // scratch: two jump records, to-points (int2) and successors per segment, then the tile sums
   unsigned char *base = static_cast<unsigned char *>(d_scratch);
   int4 *jump[2] = {reinterpret_cast<int4 *>(base), reinterpret_cast<int4 *>(base + 16ll * S)};
-  prm.to = reinterpret_cast<float2 *>(base + 32ll * S);
+  prm.to = reinterpret_cast<int2 *>(base + 32ll * S);
   prm.succ = reinterpret_cast<int *>(base + 40ll * S);
   unsigned long long *bsum = reinterpret_cast<unsigned long long *>(base + ((44ll * S + 15) & ~15ll));
   prm.jump = jump[0];
@@ -479,7 +490,7 @@ extern "C" int mrx_contours_write(const unsigned char *d_packed, const long long
     contour_scan_apply_kernel<<<ntiles, kScanThreads, 0, st>>>(scan, bsum, S);
     MRX_LAUNCH_CHECK("contour_scan_apply_kernel");
     contour_write_kernel<<<grid, 256, 0, st>>>(jump[cur], len, scan, prm.to,
-                                               reinterpret_cast<float2 *>(d_vertices),
+                                               reinterpret_cast<double2 *>(d_vertices),
                                                d_contour_off, S);
     MRX_LAUNCH_CHECK("contour_write_kernel");
     contour_finish_kernel<<<(B * R + 256) / 256, 256, 0, st>>>(d_inst_off, scan, bsum + ntiles,

@@ -423,7 +423,7 @@ class UnmoldEngine:
         """EXTENSION: the contour polygons of `visualize.display_instances` for every kept
         instance of the planned batch, traced on the device from the packed planes (after
         `enqueue_expand_packed` or `pack_masks`) inside each instance's box.  Synchronises to size
-        the output.  Returns (d_vertices float32 [V, 2] device tensor, d_contour_off int64 device
+        the output.  Returns (d_vertices float64 [V, 2] device tensor, d_contour_off int64 device
         tensor [C + 1], inst_contour_off int64 ndarray [n*R + 1]); see `contours_to_lists`."""
         if self.layout is None or self.d_packed is None:
             raise RuntimeError("trace_contours needs the packed planes: call enqueue_expand_packed "
@@ -1406,7 +1406,7 @@ def trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom,
                           stream=None, bufs=None):
     """mrx_contours_count, one host read of the segment counts, mrx_contours_write, over the planes
     of a BatchLayout as mrx_pack_masks writes them; d_regions [n,R,4] int32 pixel rectangles; `bufs`
-    keeps the work and output buffers between calls.  Returns (d_vertices [V,2] float32,
+    keeps the work and output buffers between calls.  Returns (d_vertices [V,2] float64,
     d_contour_off [C+1] int64, inst_contour_off int64 ndarray [n*R+1])."""
     with _stream_ctx(stream):
         return _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom,
@@ -1437,7 +1437,7 @@ def _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom
         raise N.MrxError(f"{S} contour segments in one batch (limit {N.MRX_MAX_CONTOUR_SEGMENTS}); "
                          "split the batch")
     d_scr = _buffer(bufs, "scratch", N.contour_scratch_bytes(S), torch.uint8, device)
-    d_vert = _buffer(bufs, "vertices", 2 * (S + S // 4), torch.float32, device)
+    d_vert = _buffer(bufs, "vertices", 2 * (S + S // 4), torch.float64, device)
     d_coff = _buffer(bufs, "contour_off", S // 4 + 1, torch.int64, device)
     d_icoff = _buffer(bufs, "inst_contour_off", ni + 1, torch.int64, device)
     N.check(lib.mrx_contours_write(*args, S, smax, d_scr, d_vert, d_coff, d_icoff, n, R, max_h,
@@ -1480,7 +1480,7 @@ def annotate_overlays(lib, dev, d_counts, d_geom, d_boxes, trace, d_images, d_im
 
 def _download_contours(d_vert, d_coff):
     """Host copies (float64 vertices [V, 2], int64 contour offsets) of a trace's output."""
-    return d_vert.cpu().numpy().astype(np.float64), d_coff.cpu().numpy()
+    return d_vert.cpu().numpy(), d_coff.cpu().numpy()
 
 
 def contours_to_lists(verts, contour_off, inst_contour_off, counts, layout):

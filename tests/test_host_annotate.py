@@ -176,8 +176,8 @@ def _i64(*shape):
 
 
 def _draw(**replace):
-    args = [_i32(1), _i32(1, 8), _i32(1, 2, 4), torch.zeros(4, 2), _i64(2), _i64(3), 4, 1,
-            _i32(16), _i64(1), 0, 2, 16, None]
+    args = [_i32(1), _i32(1, 8), _i32(1, 2, 4), torch.zeros(4, 2, dtype=torch.float64), _i64(2),
+            _i64(3), 4, 1, _i32(16), _i64(1), 0, 2, 16, None]
     for k, v in replace.items():
         args[int(k[1:])] = v
     return N.load().mrx_annotate_draw(*args)
@@ -203,10 +203,17 @@ def _resolve(**replace):
     ({"a11": 0}, "MRX_E_INVALID"), ({"a11": 65535}, "MRX_E_INVALID"),
     ({"a12": -1}, "MRX_E_INVALID"), ({"a12": (1 << 31) - 1}, "MRX_E_INVALID"),
 ])
-def test_draw_refusals(replace, status):
+def test_draw_refusals_with_float64_vertices(replace, status):
     assert _draw(**replace) == getattr(N, status)
     if status != "MRX_OK":
         assert N.load().mrx_last_error().decode().startswith("mrx_annotate_draw")
+
+
+def test_draw_binding_refuses_float32_vertices():
+    """The vertices are float64 (mrx.h, mrx_contours_write): float32 rounds halves past 2^23, and
+    a float32 buffer read as float64 would draw garbage, so the binding refuses it."""
+    with pytest.raises(Exception, match=r"double \* parameter: got a torch.float32 tensor"):
+        _draw(a3=torch.zeros(4, 2))
 
 
 @pytest.mark.parametrize("replace, status", [

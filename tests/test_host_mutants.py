@@ -14,7 +14,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 
 import mutants  # noqa: E402
 
-SUITES = ["expand", "eval", "preprocess", "polygons", "jpeg", "png_decode", "png_encode"]
+SUITES = ["expand", "eval", "preprocess", "polygons", "jpeg", "png_decode", "png_encode", "contours"]
 
 
 def check_table(suite, root):

@@ -75,7 +75,7 @@ def unmold_case(name, batch, hw, n, classes, R, iters, base_images=4, seed=7, co
     pct_ms, _ = time_ms(lambda: (eng.enqueue_expand_packed(), eng.trace_contours()), max(3, iters // 4))
     d_vert, d_coff, icoff = eng.trace_contours()
     n_vert, n_contours = int(d_vert.shape[0]), int(icoff[-1])
-    contour_bytes = n_vert * 8 + (n_contours + 1) * 8 + icoff.size * 8
+    contour_bytes = n_vert * 16 + (n_contours + 1) * 8 + icoff.size * 8
     if composite:
         import random
 

@@ -27,7 +27,7 @@ MUTANTS = [
     (2, "box: right edge at x2 - 1", [
         (A, "xb = max(bx.y, bx.w);", "xb = max(bx.y, bx.w - 1);", 1)]),
     (3, "segment rule: end points rounded half down", [
-        (A, "return (__float2int_rn(2.0f * u) + 1) >> 1;", "return __float2int_rn(2.0f * u) >> 1;",
+        (A, "return (__double2int_rn(2.0 * u) + 1) >> 1;", "return __double2int_rn(2.0 * u) >> 1;",
          1)]),
     (4, "segment clip ignored: end points outside the image clamped onto its border", [
         (A, "const int x = round_half_up(p.x), y = round_half_up(p.y);\n"
