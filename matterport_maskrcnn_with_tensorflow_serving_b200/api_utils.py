@@ -193,7 +193,7 @@ def _png_encode(images, stats=False):
         N.check(lib.mrx_png_encode(
             d_desc, plan.B, plan.max_n, plan.max_blocks, plan.max_chunks, plan.total_tiles,
             plan.zbuf_words, d_stream, d_sym, d_stretch, d_tiles, d_blk_pos, d_blk_tab,
-            d_blk_info, d_zbuf, d_img_info, d_out, d_sizes, N.stream_ptr(None)), "mrx_png_encode")
+            d_blk_info, d_zbuf, d_img_info, d_out, d_sizes, N.stream_ptr()), "mrx_png_encode")
         out = _download_files(d_out, plan.desc[:, png.D_OUT_OFF], d_sizes)
     if not stats:
         return (out,)
@@ -249,7 +249,7 @@ def _jpeg_encode(images, quality=95, optimize=False, stats=False):
             d_desc, B, plan.quality, int(plan.optimize), plan.min_side, plan.max_side,
             plan.max_blocks, plan.max_bytes, plan.block_tiles, plan.byte_tiles, plan.words,
             d_huff, d_codes, d_hist, d_coef, d_blk_bit, d_tiles, d_words, d_info, d_out,
-            d_sizes, N.stream_ptr(None)), "mrx_jpeg_encode")
+            d_sizes, N.stream_ptr()), "mrx_jpeg_encode")
         out = _download_files(d_out, plan.desc[:, je.D_OUT_OFF], d_sizes)
     if not stats:
         return (out,)

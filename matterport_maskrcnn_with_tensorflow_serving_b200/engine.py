@@ -3,6 +3,12 @@
 PyTorch tensors are used only as owners of device / pinned-host memory and for streams;
 every computation on the path is a libmrx kernel launched through ctypes.
 
+Every libmrx launch, and every torch allocation or copy feeding it, goes on the current CUDA
+stream, as torch's own ops do.  To run elsewhere, the caller writes `with torch.cuda.stream(s):`.
+The pipeline launches that streaming and sharding drive on explicit streams
+(`UnmoldEngine.enqueue`, `enqueue_expand`, `enqueue_expand_packed`, `enqueue_packed`) keep a
+`stream` argument as shorthand for exactly that.
+
   UnmoldEngine     batched `unmold_detections` (serve.py:147-154): prologue -> class-tile
                    gather -> fused mask expand, all stream-ordered, no host sync
   MaskBatch        caller-held masks (ground truth) as packed planes, from bool arrays, COCO
@@ -242,7 +248,7 @@ class UnmoldEngine:
 
     # ------------------------------------------------------------------ launch
     def enqueue(self, d_detections, d_mrcnn_mask, stream=None, expand=True):
-        """Enqueue the three kernels for the planned batch on `stream` (no host sync).
+        """Enqueue the three kernels for the planned batch (no host sync).
         d_detections [n,R,6] and d_mrcnn_mask [n,R,mh,mw,C] are device tensors of the
         dtypes given at construction (d_mrcnn_mask may also be PINNED HOST memory: the class
         gather then reads the wanted elements over PCIe instead of the whole tensor being
@@ -262,17 +268,17 @@ class UnmoldEngine:
                              f"{d_mrcnn_mask.dtype}")
         if not (d_detections.is_contiguous() and d_mrcnn_mask.is_contiguous()):
             raise ValueError("inputs must be contiguous")
-        st = N.stream_ptr(stream)
-        # steps 1-6 and the class-tile gather in one launch; tiles are stored by detection row
-        # and found through d_src_index by the expand kernels
-        N.check(self.lib.mrx_unmold_prepare(
-            d_detections, _dtype_code(self.det_dtype), d_mrcnn_mask, _dtype_code(self.mask_dtype),
-            n, self.R, self.mh, self.mw, self.C, self.d_geom, self.d_boxes, self.d_class_ids,
-            self.d_scores, self.d_src_index, self.d_counts, self.d_status, self.d_tiles,
-            self.d_sched, st),
-            "mrx_unmold_prepare")
-        if expand:
-            self.enqueue_expand(stream)
+        with N.on_stream(stream):
+            # steps 1-6 and the class-tile gather in one launch; tiles are stored by detection
+            # row and found through d_src_index by the expand kernels
+            N.check(self.lib.mrx_unmold_prepare(
+                d_detections, _dtype_code(self.det_dtype), d_mrcnn_mask,
+                _dtype_code(self.mask_dtype), n, self.R, self.mh, self.mw, self.C, self.d_geom,
+                self.d_boxes, self.d_class_ids, self.d_scores, self.d_src_index, self.d_counts,
+                self.d_status, self.d_tiles, self.d_sched, N.stream_ptr()),
+                "mrx_unmold_prepare")
+            if expand:
+                self.enqueue_expand()
 
     def enqueue_expand(self, stream=None, canvas_ptr=None, images=None):
         """Only the mask-expand kernel (boxes / tiles / counts already on the device).
@@ -284,13 +290,14 @@ class UnmoldEngine:
         if b1 <= b0:
             return
         base = self.d_canvas if canvas_ptr is None else int(canvas_ptr)
-        N.check(self.lib.mrx_mask_expand(
-            self.d_tiles[b0:], self.d_src_index[b0:], self.d_boxes[b0:], self.d_counts[b0:],
-            self.d_geom[b0:], self.d_canvas_off[b0:], base, b1 - b0, self.R, self.mh, self.mw,
-            self.chunk_bytes, self.ctas_per_sm, self.d_sched,
-            N.stream_ptr(stream)), "mrx_mask_expand")
+        with N.on_stream(stream):
+            N.check(self.lib.mrx_mask_expand(
+                self.d_tiles[b0:], self.d_src_index[b0:], self.d_boxes[b0:], self.d_counts[b0:],
+                self.d_geom[b0:], self.d_canvas_off[b0:], base, b1 - b0, self.R, self.mh,
+                self.mw, self.chunk_bytes, self.ctas_per_sm, self.d_sched,
+                N.stream_ptr()), "mrx_mask_expand")
 
-    def enqueue_expand_values(self, d_values, stream=None):
+    def enqueue_expand_values(self, d_values):
         """Parity instrumentation: the same kernel (second instantiation of its template) also
         stores every pre-threshold sample into d_values (float32, indexed like the canvas)."""
         n = self._n_images
@@ -299,8 +306,7 @@ class UnmoldEngine:
         N.check(self.lib.mrx_mask_expand_values(
             self.d_tiles, self.d_src_index, self.d_boxes, self.d_counts, self.d_geom,
             self.d_canvas_off, self.d_canvas, d_values, n, self.R, self.mh, self.mw, self.d_sched,
-            N.stream_ptr(stream)),
-            "mrx_mask_expand_values")
+            N.stream_ptr()), "mrx_mask_expand_values")
 
     # ------------------------------------------------------------------ packed output
     def packed_layout(self):
@@ -328,18 +334,19 @@ class UnmoldEngine:
         Returns (d_packed, offsets).  packed_ptr: another base address (peer memory);
         images=(b0, b1): only that range of the planned batch."""
         b0, b1 = (0, self._n_images) if images is None else images
-        if packed_ptr is None:
-            off = self._packed_buffer()
-            base = self.d_packed
-        else:
-            off, _ = self.packed_layout()
-            base = int(packed_ptr)
-        if b1 > b0:
-            N.check(self.lib.mrx_mask_expand_packed(
-                self.d_tiles[b0:], self.d_src_index[b0:], self.d_boxes[b0:], self.d_counts[b0:],
-                self.d_geom[b0:], self.d_packed_off[b0:], base, b1 - b0, self.R, self.mh,
-                self.mw, self.layout.max_w, self.d_sched, N.stream_ptr(stream)),
-                "mrx_mask_expand_packed")
+        with N.on_stream(stream):
+            if packed_ptr is None:
+                off = self._packed_buffer()
+                base = self.d_packed
+            else:
+                off, _ = self.packed_layout()
+                base = int(packed_ptr)
+            if b1 > b0:
+                N.check(self.lib.mrx_mask_expand_packed(
+                    self.d_tiles[b0:], self.d_src_index[b0:], self.d_boxes[b0:],
+                    self.d_counts[b0:], self.d_geom[b0:], self.d_packed_off[b0:], base, b1 - b0,
+                    self.R, self.mh, self.mw, self.layout.max_w, self.d_sched, N.stream_ptr()),
+                    "mrx_mask_expand_packed")
         return self.d_packed, off
 
     def enqueue_packed(self, d_detections, d_mrcnn_mask, stream=None, direct=True):
@@ -348,13 +355,14 @@ class UnmoldEngine:
         canvas is written) when the tiles are at most MRX_MAX_LANE_MASK_W columns wide.
         Otherwise, and for direct=False: byte canvas, then mrx_pack_masks.  Both give identical
         bytes."""
-        if direct and self.mw <= N.MRX_MAX_LANE_MASK_W:
-            self.enqueue(d_detections, d_mrcnn_mask, stream, expand=False)
-            return self.enqueue_expand_packed(stream)
-        if self.layout is not None:     # (a plan made with canvas=False has no canvas)
-            self.plan(self.layout.geom, canvas=True)
-        self.enqueue(d_detections, d_mrcnn_mask, stream)
-        return self.pack_masks(stream)
+        with N.on_stream(stream):
+            if direct and self.mw <= N.MRX_MAX_LANE_MASK_W:
+                self.enqueue(d_detections, d_mrcnn_mask, expand=False)
+                return self.enqueue_expand_packed()
+            if self.layout is not None:     # (a plan made with canvas=False has no canvas)
+                self.plan(self.layout.geom, canvas=True)
+            self.enqueue(d_detections, d_mrcnn_mask)
+            return self.pack_masks()
 
     # ------------------------------------------------------------------ results
     def canvas_bytes(self, counts):
@@ -370,25 +378,23 @@ class UnmoldEngine:
         lo, hi = self.layout.packed_span(b, n_kept)
         return self.d_packed[lo:hi].view(self.layout.packed_shape(b, n_kept))
 
-    def enqueue_rle(self, stream=None):
+    def enqueue_rle(self):
         """EXTENSION: COCO run-length encodings of the planned batch's masks, from the tiles
         (after `enqueue(..., expand=False)`; no mask is materialised).  Synchronises once to
         size the output.  Returns (d_run_lengths uint32 tensor, inst_off int64 ndarray [n*R+1]):
         instance i = b*R + k owns d_run_lengths[inst_off[i] + i : inst_off[i+1] + i + 1]."""
-        with _stream_ctx(stream):
-            d_runs, _, off = self._enqueue_rle()
+        d_runs, _, off = self._enqueue_rle()
         return d_runs, off
 
     def _enqueue_rle(self):
-        """`enqueue_rle` on the current stream, also returning the device copy of inst_off:
-        (d_runs, d_off, off)."""
+        """`enqueue_rle`, also returning the device copy of inst_off: (d_runs, d_off, off)."""
         torch = _torch()
         n = self._n_images
         max_w = self.layout.max_w
         dev = self.device
         d_col = torch.empty((n * self.R * max_w,), dtype=torch.int32, device=dev)
         d_off = torch.empty((n * self.R + 1,), dtype=torch.int64, device=dev)
-        st = N.stream_ptr(None)
+        st = N.stream_ptr()
         args = (self.d_tiles, self.d_src_index, self.d_boxes, self.d_counts, self.d_geom, d_col,
                 d_off)
         N.check(self.lib.mrx_rle_count(*args, n, self.R, self.mh, self.mw, max_w, st),
@@ -401,25 +407,23 @@ class UnmoldEngine:
                                        self.mw, max_w, st), "mrx_rle_write")
         return d_runs, d_off, off
 
-    def enqueue_rle_strings(self, stream=None):
+    def enqueue_rle_strings(self):
         """EXTENSION: pycocotools' compressed RLE (the "counts" string of `mask.encode`) of every
         mask of the planned batch: `enqueue_rle` (and its one synchronisation), then
-        mrx_rle_strings, on `stream`.  Returns (d_str uint8, d_str_off int64 [n*R+1]) device
-        tensors: instance i = b*R + k's string is d_str[d_str_off[i]:d_str_off[i+1]] (empty for
+        mrx_rle_strings.  Returns (d_str uint8, d_str_off int64 [n*R+1]) device tensors:
+        instance i = b*R + k's string is d_str[d_str_off[i]:d_str_off[i+1]] (empty for
         k >= N_b), d_str_off[n*R] the total."""
         torch = _torch()
         ni = self._n_images * self.R
-        with _stream_ctx(stream):
-            d_runs, d_off, off = self._enqueue_rle()
-            d_str = torch.empty((max(N.rle_string_bound(off[-1], ni), 1),), dtype=torch.uint8,
-                                device=self.device)
-            d_str_off = torch.empty((ni + 1,), dtype=torch.int64, device=self.device)
-            N.check(self.lib.mrx_rle_strings(d_runs, d_off, self.d_counts,
-                                             self._n_images, self.R, d_str_off, d_str,
-                                             N.stream_ptr(None)), "mrx_rle_strings")
+        d_runs, d_off, off = self._enqueue_rle()
+        d_str = torch.empty((max(N.rle_string_bound(off[-1], ni), 1),), dtype=torch.uint8,
+                            device=self.device)
+        d_str_off = torch.empty((ni + 1,), dtype=torch.int64, device=self.device)
+        N.check(self.lib.mrx_rle_strings(d_runs, d_off, self.d_counts, self._n_images, self.R,
+                                         d_str_off, d_str, N.stream_ptr()), "mrx_rle_strings")
         return d_str, d_str_off
 
-    def trace_contours(self, stream=None):
+    def trace_contours(self):
         """EXTENSION: the contour polygons of `visualize.display_instances` for every kept
         instance of the planned batch, traced on the device from the packed planes (after
         `enqueue_expand_packed` or `pack_masks`) inside each instance's box.  Synchronises to size
@@ -430,19 +434,17 @@ class UnmoldEngine:
                                "or pack_masks first")
         return trace_packed_contours(self.lib, self.device, self.d_packed, self.d_packed_off,
                                      self.d_counts, self.d_geom, self.d_boxes, self.layout,
-                                     stream, self._contour_bufs)
+                                     bufs=self._contour_bufs)
 
-    def enqueue_contours(self, stream=None):
+    def enqueue_contours(self):
         """`trace_contours` with the result on the host: per planned image, per kept instance, the
         list of float64 [V, 2] (x, y) polygons `display_instances` draws for it."""
-        d_vert, d_coff, icoff = self.trace_contours(stream)
-        n = self._n_images
-        with _stream_ctx(stream):
-            counts = self.d_counts[:n].cpu().numpy()
-            verts, coff = _download_contours(d_vert, d_coff)
+        d_vert, d_coff, icoff = self.trace_contours()
+        counts = self.d_counts[:self._n_images].cpu().numpy()
+        verts, coff = _download_contours(d_vert, d_coff)
         return contours_to_lists(verts, coff, icoff, counts, self.layout)
 
-    def annotate(self, d_images, d_image_off, rgb8, patches, show_bbox=True, stream=None):
+    def annotate(self, d_images, d_image_off, rgb8, patches, show_bbox=True):
         """EXTENSION: draw the boxes, contour outlines and captions of `display_instances` on the
         planned batch's overlays (after `enqueue` and the composite), in place, as OpenCV draws
         them (DESIGN.md section 3.25): the byte canvas packed (`pack_masks`), the contours traced
@@ -454,52 +456,50 @@ class UnmoldEngine:
         if self.layout is None or self.d_canvas is None:
             raise RuntimeError("annotate needs the byte canvas: call plan() and enqueue() first")
         n = self._n_images
-        with _stream_ctx(stream):
-            self.pack_masks()
-            d_vert, d_coff, _ = self.trace_contours()
-            d_icoff = self._contour_bufs["inst_contour_off"][:n * self.R + 1]
-            annotate_overlays(self.lib, self.device, self.d_counts, self.d_geom, self.d_boxes,
-                              (d_vert, d_coff, d_icoff), d_images, d_image_off,
-                              [self.layout.hw(b) for b in range(n)], self.R, rgb8, patches,
-                              show_bbox, bufs=self._contour_bufs)
+        self.pack_masks()
+        d_vert, d_coff, _ = self.trace_contours()
+        d_icoff = self._contour_bufs["inst_contour_off"][:n * self.R + 1]
+        annotate_overlays(self.lib, self.device, self.d_counts, self.d_geom, self.d_boxes,
+                          (d_vert, d_coff, d_icoff), d_images, d_image_off,
+                          [self.layout.hw(b) for b in range(n)], self.R, rgb8, patches,
+                          show_bbox, bufs=self._contour_bufs)
 
     # ------------------------------------------------------------------ scoring against ground truth
-    def ground_truth(self, class_ids, masks, stream=None):
+    def ground_truth(self, class_ids, masks):
         """A `MaskBatch` of ground truth for the planned images: class_ids[b] [M_b] and bool
         masks[b] [H_b, W_b, M_b] in the plan's image shapes."""
         if self.layout is None:
             raise RuntimeError("plan() first")
-        return MaskBatch(self.lib, self.device, self.layout.geom, class_ids, masks, stream)
+        return MaskBatch(self.lib, self.device, self.layout.geom, class_ids, masks)
 
-    def ground_truth_rle(self, class_ids, rles, stream=None):
+    def ground_truth_rle(self, class_ids, rles):
         """`ground_truth` from COCO RLE: class_ids[b] [M_b] and rles[b], a list of M_b dicts
         {'size': [H_b, W_b], 'counts': ...} (see `MaskBatch.from_rle`, which also states what
         raises), decoded on the device."""
         if self.layout is None:
             raise RuntimeError("plan() first")
-        return MaskBatch.from_rle(self.lib, self.device, self.layout.geom, class_ids, rles, stream)
+        return MaskBatch.from_rle(self.lib, self.device, self.layout.geom, class_ids, rles)
 
-    def ground_truth_coco(self, class_ids, segms, stream=None):
+    def ground_truth_coco(self, class_ids, segms):
         """`ground_truth` from COCO `segmentation` values: class_ids[b] [M_b] and segms[b], a
         list of M_b polygon lists, box lists or RLE dicts (see `MaskBatch.from_coco`, which also
         states what raises), rasterised and decoded on the device."""
         if self.layout is None:
             raise RuntimeError("plan() first")
-        return MaskBatch.from_coco(self.lib, self.device, self.layout.geom, class_ids, segms,
-                                   stream)
+        return MaskBatch.from_coco(self.lib, self.device, self.layout.geom, class_ids, segms)
 
-    def enqueue_overlaps(self, gt, stream=None):
+    def enqueue_overlaps(self, gt):
         """EXTENSION: upstream `compute_overlaps_masks(pred_masks, gt_masks)` of every planned image
         against `gt` (a `MaskBatch` from `ground_truth`), on the packed planes (after
         `enqueue_expand_packed` or `pack_masks`); each prediction is read only inside its box.
         Returns the float32 device tensor [n, R, gt.R]: element (b, i, j) for i < N_b, j < M_b is
         the IoU of kept instance i and ground-truth instance j."""
-        pred = self._prediction_planes(gt, "enqueue_overlaps", stream)
+        pred = self._prediction_planes(gt, "enqueue_overlaps")
         self._overlaps = (gt, mask_overlaps(self.lib, pred, gt.planes, self.d_geom,
-                                            self._n_images, stream))
+                                            self._n_images))
         return self._overlaps[1]
 
-    def enqueue_matches(self, gt, thresholds, score_threshold=0.0, stream=None):
+    def enqueue_matches(self, gt, thresholds, score_threshold=0.0):
         """EXTENSION: the matching of upstream `compute_matches` for each IoU threshold, on the
         overlaps of the last `enqueue_overlaps(gt)`.  Thresholds compare as upstream's do
         (`comparison_threshold`).  Returns device tensors (order [n, R]: rank -> kept instance,
@@ -509,23 +509,23 @@ class UnmoldEngine:
         if last is None or last[0] is not gt:
             raise RuntimeError("enqueue_overlaps(gt) first")
         return mask_matches(self.lib, last[1], self.d_counts, self.d_class_ids, self.d_scores,
-                            _dtype_code(self.det_dtype), gt, thresholds, score_threshold, stream)
+                            _dtype_code(self.det_dtype), gt, thresholds, score_threshold)
 
-    def predictions(self, gt=None, stream=None):
+    def predictions(self, gt=None):
         """EXTENSION: the planned batch's kept predictions as the scorers read them
         (`coco_evaluate_batch`, `coco_boundary_evaluate_batch`, `coco_box_evaluate_batch`), after
         `enqueue`: its counts, class ids, scores and boxes.  With `gt` (a `MaskBatch` of the same
         plan, e.g. from `ground_truth_rle`) also their `Planes` on the packed planes (after
         `enqueue_expand_packed` or `pack_masks`), each prediction counted only inside its box;
         without it no mask is read, as box scoring after `enqueue(..., expand=False)` needs."""
-        planes = None if gt is None else self._prediction_planes(gt, "predictions", stream)
+        planes = None if gt is None else self._prediction_planes(gt, "predictions")
         n = self._n_images
         if n == 0:
             raise RuntimeError("call plan() and enqueue() first")
         return Predictions(self.d_counts[:n], self.d_class_ids[:n], self.d_scores[:n],
                            self.d_boxes[:n], planes)
 
-    def boundary_planes(self, dilation_ratio=0.02, stream=None):
+    def boundary_planes(self, dilation_ratio=0.02):
         """EXTENSION: `Planes` of the boundaries of the planned batch's kept masks (after
         `enqueue_expand_packed` or `pack_masks`), as boundary_iou_api's mask_to_boundary computes
         them for `dilation_ratio`: mrx_mask_boundary inside each kept box, then mrx_mask_extents
@@ -536,14 +536,12 @@ class UnmoldEngine:
             raise RuntimeError("boundary_planes needs the packed planes: call "
                                "enqueue_expand_packed or pack_masks first")
         d = boundary_dilation(self.layout.geom, dilation_ratio)
-        with _stream_ctx(stream):
-            d_dil = _torch().from_numpy(d).to(self.device)
-            pred = Planes(self.d_packed, self.d_packed_off, self.d_counts, None, None, self.R)
-            return mask_boundary_planes(self.lib, pred, self.d_geom, self.d_boxes, d_dil,
-                                        self._n_images, self.layout.max_w, self._eval_bufs,
-                                        stream)
+        d_dil = _torch().from_numpy(d).to(self.device)
+        pred = Planes(self.d_packed, self.d_packed_off, self.d_counts, None, None, self.R)
+        return mask_boundary_planes(self.lib, pred, self.d_geom, self.d_boxes, d_dil,
+                                    self._n_images, self.layout.max_w, self._eval_bufs)
 
-    def _prediction_planes(self, gt, fn, stream):
+    def _prediction_planes(self, gt, fn):
         """`Planes` of the planned batch's kept instances to score against `gt` (a `MaskBatch` of
         the same plan), each counted only inside its box (mrx_mask_extents into `_eval_bufs`)."""
         if self.layout is None or self.d_packed is None:
@@ -558,11 +556,11 @@ class UnmoldEngine:
         d_ext = _buffer(bufs, "extents", n * self.R * 4, torch.int32, self.device)
         N.check(self.lib.mrx_mask_extents(
             self.d_packed, self.d_packed_off, self.d_counts, self.d_geom, self.d_boxes, d_areas,
-            d_ext, n, self.R, N.stream_ptr(stream)),
+            d_ext, n, self.R, N.stream_ptr()),
             "mrx_mask_extents")
         return Planes(self.d_packed, self.d_packed_off, self.d_counts, d_areas, d_ext, self.R)
 
-    def pack_masks(self, stream=None):
+    def pack_masks(self):
         """EXTENSION: bit-pack the byte canvases already written for the planned batch
         (mrx_pack_masks; same output layout as `enqueue_expand_packed`).  Returns
         (d_packed, offsets)."""
@@ -571,10 +569,10 @@ class UnmoldEngine:
         N.check(self.lib.mrx_pack_masks(
             self.d_canvas, self.d_canvas_off, self.d_counts, self.d_geom, self.d_packed,
             self.d_packed_off, n, self.R,
-            self.layout.max_h, self.layout.max_w, N.stream_ptr(stream)), "mrx_pack_masks")
+            self.layout.max_h, self.layout.max_w, N.stream_ptr()), "mrx_pack_masks")
         return self.d_packed, off
 
-    def fetch_meta(self, stream=None):
+    def fetch_meta(self):
         """Copy counts/status/boxes/class_ids/scores of the planned batch to the host
         (one batch of async copies into cached pinned memory, one synchronisation).
         Raises like numpy would on bad inputs.  The returned arrays are views of the
@@ -588,14 +586,12 @@ class UnmoldEngine:
                             pin((B, R, 4), torch.int32), pin((B, R), torch.int32),
                             pin((B, R), _torch_dtype(self.det_dtype)))
         hc, hs, hb, hk, hsc = self._h_meta
-        st = stream or torch.cuda.current_stream(self.device)
-        with torch.cuda.stream(st):
-            hc[:n].copy_(self.d_counts[:n], non_blocking=True)
-            hs[:n].copy_(self.d_status[:n], non_blocking=True)
-            hb[:n].copy_(self.d_boxes[:n], non_blocking=True)
-            hk[:n].copy_(self.d_class_ids[:n], non_blocking=True)
-            hsc[:n].copy_(self.d_scores[:n], non_blocking=True)
-        st.synchronize()
+        hc[:n].copy_(self.d_counts[:n], non_blocking=True)
+        hs[:n].copy_(self.d_status[:n], non_blocking=True)
+        hb[:n].copy_(self.d_boxes[:n], non_blocking=True)
+        hk[:n].copy_(self.d_class_ids[:n], non_blocking=True)
+        hsc[:n].copy_(self.d_scores[:n], non_blocking=True)
+        torch.cuda.current_stream(self.device).synchronize()
         counts, status = hc[:n].numpy(), hs[:n].numpy()
         if (status & N.MRX_ST_CLASS_RANGE).any():
             b = int(np.nonzero(status & N.MRX_ST_CLASS_RANGE)[0][0])
@@ -667,7 +663,7 @@ class MaskBatch:
     into its slot by mrx_pack_masks, so device memory holds one image's bytes plus the packed
     planes.  M_b above what mrx_pack_masks takes raises ValueError."""
 
-    def __init__(self, lib, device, geoms, class_ids, masks, stream=None):
+    def __init__(self, lib, device, geoms, class_ids, masks):
         torch = _torch()
         g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
         n = g.shape[0]
@@ -696,15 +692,15 @@ class MaskBatch:
                 H, W = layout.hw(b)
                 rc = lib.mrx_pack_masks(canvas, d_zero, self.d_counts[b:],
                                         self.d_geom[b:], d_packed, d_off[b:],
-                                        1, layout.R, H, W, N.stream_ptr(stream))
+                                        1, layout.R, H, W, N.stream_ptr())
                 if rc == N.MRX_E_UNSUPPORTED:
                     raise ValueError(lib.mrx_last_error().decode())
                 N.check(rc, "mrx_pack_masks")
 
-        self._stage(lib, device, g, class_ids, counts, [np.zeros(1, np.int64)], fill, stream)
+        self._stage(lib, device, g, class_ids, counts, [np.zeros(1, np.int64)], fill)
 
     @classmethod
-    def from_rle(cls, lib, device, geoms, class_ids, rles, stream=None):
+    def from_rle(cls, lib, device, geoms, class_ids, rles):
         """The same batch from COCO RLE: rles[b] is a list of M_b dicts {'size': [H_b, W_b],
         'counts': c} with c pycocotools' compressed string (`bytes`, or an ASCII `str`) or its
         uncompressed runs (a 1-D sequence of integers in [0, 2^32), column-major, starting with
@@ -721,10 +717,10 @@ class MaskBatch:
         count that is negative or does not fit in uint32, or counts that do not sum to H*W.
         pycocotools decodes such input without a check; this raises instead."""
         g = np.asarray(geoms, dtype=np.int32).reshape(-1, N.MRX_GEOM_INTS)
-        return cls._decoded(lib, device, g, class_ids, pack_rle(g, class_ids, rles), None, stream)
+        return cls._decoded(lib, device, g, class_ids, pack_rle(g, class_ids, rles), None)
 
     @classmethod
-    def from_coco(cls, lib, device, geoms, class_ids, segms, stream=None):
+    def from_coco(cls, lib, device, geoms, class_ids, segms):
         """The same batch from COCO `segmentation` values as a COCO instances file holds them:
         segms[b] is a list of M_b of them, each a polygon list [[x0, y0, x1, y1, ...], ...], a
         box list [[x, y, w, h], ...] or an RLE dict (as for `from_rle`); kinds may mix, as crowd
@@ -749,10 +745,10 @@ class MaskBatch:
                                                     "counts": b""} for seg in inst]
                 for b, inst in enumerate(segms)]
         pk = pack_rle(g, class_ids, rles)   # a polygon instance: an empty string, not parsed
-        return cls._decoded(lib, device, g, class_ids, pk, pp, stream)
+        return cls._decoded(lib, device, g, class_ids, pk, pp)
 
     @classmethod
-    def _decoded(cls, lib, device, g, class_ids, pk, pp, stream):
+    def _decoded(cls, lib, device, g, class_ids, pk, pp):
         """`from_rle` (pp None) and `from_coco`: the RLE tables of `pack_rle` and the polygon
         tables of `pack_polygons` in one upload; the RLE kernels write the planes of the RLE
         instances (all of them for `from_rle`), mrx_poly_decode those of the polygon ones."""
@@ -771,7 +767,7 @@ class MaskBatch:
 
         def fill(layout, d_packed, d_off, d_status, d_str_off, d_run_off, d_run_count,
                  d_uploaded_runs, d_str, *d_poly):
-            st = N.stream_ptr(stream)
+            st = N.stream_ptr()
             max_h, max_w = max(layout.max_h, 1), max(layout.max_w, 1)
             if run_rle:
                 d_runs = torch.empty((max(S + pk["runs"].size, 1),), dtype=torch.int32,
@@ -798,10 +794,9 @@ class MaskBatch:
                     max_h, max_w, st), "mrx_poly_decode")
 
         d_status, *_ = self._stage(lib, device, g, class_ids, pk["counts"],
-                                   rle_extra + poly_extra, fill, stream)
-        with _stream_ctx(stream):
-            status = d_status.cpu().numpy().reshape(n, R)     # the one synchronisation
-            self.extents = self.planes.d_extents.cpu().numpy()
+                                   rle_extra + poly_extra, fill)
+        status = d_status.cpu().numpy().reshape(n, R)     # the one synchronisation
+        self.extents = self.planes.d_extents.cpu().numpy()
         if pp is not None:
             status = np.where(pp["poly"].reshape(n, R), 0, status)
         for b, k in zip(*np.nonzero(status)):
@@ -810,7 +805,7 @@ class MaskBatch:
             raise ValueError(f"image {b}, instance {k}: " + "; ".join(what).format(hw=hw))
         return self
 
-    def _stage(self, lib, device, geoms, class_ids, counts, extra, fill, stream):
+    def _stage(self, lib, device, geoms, class_ids, counts, extra, fill):
         """The one staging step of both constructors, once they have checked their input: the
         layout and the class-id table, one upload of every table (the fill's own arrays `extra`
         last), the packed slots, fill(layout, d_packed, d_off, *device views of extra) writing
@@ -824,41 +819,36 @@ class MaskBatch:
         regions[:, :, 2:] = layout.geom[:, None, :2]
         tables = [layout.packed_off[:-1], counts, _class_id_table(class_ids, n, R), layout.geom,
                   regions, *extra]
-        with _stream_ctx(stream):
-            d_off, self.d_counts, self.d_class_ids, self.d_geom, d_regions, *d_extra = \
-                _upload_parts(tables, device)
-            d_packed = torch.empty((max(int(layout.packed_off[-1]), 1),), dtype=torch.uint8,
-                                   device=device)
-            fill(layout, d_packed, d_off, *d_extra)
-            d_areas = torch.empty((n, R), dtype=torch.int64, device=device)
-            d_ext = torch.empty((n, R, 4), dtype=torch.int32, device=device)
-            N.check(lib.mrx_mask_extents(d_packed, d_off, self.d_counts,
-                                         self.d_geom, d_regions, d_areas,
-                                         d_ext, n, R, N.stream_ptr(stream)),
-                    "mrx_mask_extents")
+        d_off, self.d_counts, self.d_class_ids, self.d_geom, d_regions, *d_extra = \
+            _upload_parts(tables, device)
+        d_packed = torch.empty((max(int(layout.packed_off[-1]), 1),), dtype=torch.uint8,
+                               device=device)
+        fill(layout, d_packed, d_off, *d_extra)
+        d_areas = torch.empty((n, R), dtype=torch.int64, device=device)
+        d_ext = torch.empty((n, R, 4), dtype=torch.int32, device=device)
+        N.check(lib.mrx_mask_extents(d_packed, d_off, self.d_counts, self.d_geom, d_regions,
+                                     d_areas, d_ext, n, R, N.stream_ptr()), "mrx_mask_extents")
         self.planes = Planes(d_packed, d_off, self.d_counts, d_areas, d_ext, R)
         self.d_regions = d_regions
         return d_extra
 
-    def boundary_planes(self, dilation_ratio=0.02, stream=None):
+    def boundary_planes(self, dilation_ratio=0.02):
         """EXTENSION: `Planes` of the boundaries of this batch's masks, as boundary_iou_api's
         mask_to_boundary computes them for `dilation_ratio` (`boundary_dilation`), each over its
         whole image (mrx_mask_boundary, then mrx_mask_extents for the areas; the extents are the
         masks')."""
         d = boundary_dilation(self.geom, dilation_ratio)
-        with _stream_ctx(stream):
-            d_dil = _torch().from_numpy(d).to(self.d_geom.device)
-            return mask_boundary_planes(N.load(), self.planes, self.d_geom, self.d_regions, d_dil,
-                                        self.n, int(self.geom[:, 1].max(initial=1)), {}, stream)
+        d_dil = _torch().from_numpy(d).to(self.d_geom.device)
+        return mask_boundary_planes(N.load(), self.planes, self.d_geom, self.d_regions, d_dil,
+                                    self.n, int(self.geom[:, 1].max(initial=1)), {})
 
-    def set_counts(self, counts, stream=None):
+    def set_counts(self, counts):
         """Keep only the first counts[b] instances of each image (counts[b] <= M_b), as upstream
         cuts the ground truth to the rows `trim_zeros` leaves of its boxes."""
         counts = np.asarray(counts, dtype=np.int32).reshape(self.n)
         if (counts < 0).any() or (counts > self.counts).any():
             raise ValueError("counts must lie within the batch's instances")
-        with _stream_ctx(stream):
-            self.d_counts.copy_(_torch().from_numpy(counts))
+        self.d_counts.copy_(_torch().from_numpy(counts))
         self.counts = counts
 
 
@@ -1077,7 +1067,7 @@ def pack_polygons(geoms, class_ids, segms):
             "inst_part": inst_part.astype(np.int32), "part_col": part_col, "part_tog": tog_off}
 
 
-def mask_overlaps(lib, p1, p2, d_geom, n, stream=None):
+def mask_overlaps(lib, p1, p2, d_geom, n):
     """mrx_mask_overlaps of two `Planes` of the same n images (d_geom [n, 8]): float32 device
     tensor [n, p1.R, p2.R], element (b, i, j) the IoU of mask i of p1 and mask j of p2 for i, j
     below the image's counts (the rest is not written)."""
@@ -1085,7 +1075,7 @@ def mask_overlaps(lib, p1, p2, d_geom, n, stream=None):
     N.check(lib.mrx_mask_overlaps(
         p1.d_packed, p1.d_packed_off, p1.d_counts, p1.d_areas, p1.d_extents, p1.R, p2.d_packed,
         p2.d_packed_off, p2.d_counts, p2.d_areas, p2.d_extents, p2.R, d_geom, d_out, n,
-        N.stream_ptr(stream)), "mrx_mask_overlaps")
+        N.stream_ptr()), "mrx_mask_overlaps")
     return d_out
 
 
@@ -1101,7 +1091,7 @@ def comparison_threshold(t):
 
 
 def mask_matches(lib, d_overlaps, d_pred_counts, d_pred_class_ids, d_scores, score_code, gt,
-                 thresholds, score_threshold=0.0, stream=None):
+                 thresholds, score_threshold=0.0):
     """mrx_mask_matches on overlaps [n, R1, gt.R] (see `mask_overlaps`), thresholds in launches of
     at most MRX_MAX_IOU_THRESHOLDS.  Returns device tensors (order [n, R1], pred_match
     [T, n, R1], gt_match [T, n, gt.R]) int32."""
@@ -1120,7 +1110,7 @@ def mask_matches(lib, d_overlaps, d_pred_counts, d_pred_class_ids, d_scores, sco
             d_overlaps, d_pred_counts, d_pred_class_ids, d_scores, score_code, gt.d_counts,
             gt.d_class_ids, N.double_array(chunk), len(chunk),
             comparison_threshold(score_threshold), d_order, d_pm[t0], d_gm[t0], n, R1, R2,
-            N.stream_ptr(stream)), "mrx_mask_matches")
+            N.stream_ptr()), "mrx_mask_matches")
     return d_order, d_pm, d_gm
 
 
@@ -1152,7 +1142,7 @@ def _device_params(iou_thrs, area_rng, max_det, max_det_name):
 
 
 def coco_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt_area, class_map,
-                        params, stream=None, status=None):
+                        params, *, status=None):
     """The per-image half of COCOeval (iouType "segm") for one batch: mrx_coco_ranks,
     mrx_coco_ious and mrx_coco_match, then one download and one synchronisation.  With `status`
     it is lvis-api's LVISEval (iouType "segm"): mrx_lvis_ranks (the per-image cut at
@@ -1177,23 +1167,23 @@ def coco_evaluate_batch(lib, pred, pred_class_ids, pred_scores, gt, gt_crowd, gt
     the caller's); and `d_iou`, the float64 device tensor [n, pred.R, gt.R] of mrx_coco_ious."""
     n, R1, R2 = gt.n, int(pred.R), int(gt.R)
     class_map = _coco_class_map(class_map)
-    with _stream_ctx(stream):
-        d_crowd, d_area, d_map, *d_status = _upload_parts(
-            [np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
-             np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map]
-            + _status_part(status, n), gt.d_geom.device)
+    d_crowd, d_area, d_map, *d_status = _upload_parts(
+        [np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
+         np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map]
+        + _status_part(status, n), gt.d_geom.device)
 
-        def ious(v, d_iou, st):
-            v["area"].copy_(pred.d_areas.view(-1)[:n * R1].view(n, R1))
-            N.check(lib.mrx_coco_ious(
-                pred.d_packed, pred.d_packed_off, pred.d_counts, pred.d_areas, pred.d_extents,
-                v["cat"], v["keep"], R1, gt.planes.d_packed, gt.planes.d_packed_off,
-                gt.planes.d_counts, gt.planes.d_areas, gt.planes.d_extents, gt.d_class_ids,
-                d_crowd, R2, gt.d_geom, d_iou, n, st), "mrx_coco_ious")
+    def ious(v, d_iou, st):
+        v["area"].copy_(pred.d_areas.view(-1)[:n * R1].view(n, R1))
+        N.check(lib.mrx_coco_ious(
+            pred.d_packed, pred.d_packed_off, pred.d_counts, pred.d_areas, pred.d_extents,
+            v["cat"], v["keep"], R1, gt.planes.d_packed, gt.planes.d_packed_off,
+            gt.planes.d_counts, gt.planes.d_areas, gt.planes.d_extents, gt.d_class_ids,
+            d_crowd, R2, gt.d_geom, d_iou, n, st), "mrx_coco_ious")
 
-        return _coco_evaluate(lib, n, R1, R2, pred.d_counts, pred_class_ids, pred_scores,
-                              gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map,
-                              _scorer_params(params, status), np.int64, ious, stream, *d_status)
+    return _coco_evaluate(lib, n, R1, R2, pred.d_counts, pred_class_ids, pred_scores,
+                          gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map,
+                          _scorer_params(params, status), np.int64, ious,
+                          d_status=d_status[0] if d_status else None)
 
 
 def _scorer_params(params, status):
@@ -1213,7 +1203,7 @@ def _status_part(status, n):
 
 
 def coco_box_evaluate_batch(lib, pred_boxes, pred_counts, pred_class_ids, pred_scores, gt_counts,
-                            gt_cat, gt_boxes, gt_crowd, gt_area, class_map, params, stream=None,
+                            gt_cat, gt_boxes, gt_crowd, gt_area, class_map, params, *,
                             status=None):
     """The per-image half of COCOeval (iouType "bbox") for one batch of n images: mrx_coco_ranks
     (mrx_lvis_ranks with `status`: LVISEval "bbox"), mrx_coco_box_ious and
@@ -1243,25 +1233,22 @@ def coco_box_evaluate_batch(lib, pred_boxes, pred_counts, pred_class_ids, pred_s
              np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map]
     parts += _status_part(status, n)
     on_host = [k for k, x in enumerate(pred) if isinstance(x, np.ndarray)]
-    with _stream_ctx(stream):
-        up = _upload_parts(parts + [np.ascontiguousarray(pred[k]) for k in on_host], dev)
-        d_counts, d_cat, d_boxes, d_crowd, d_area, d_map = up[:6]
-        d_status = up[6:len(parts)]
-        for k, t in zip(on_host, up[len(parts):]):
-            pred[k] = t
-        pred_boxes, pred_counts, pred_class_ids, pred_scores = pred
-        form = {torch.int32: N.MRX_BOX_YXYX_I32, torch.float64: N.MRX_BOX_XYWH_F64}[
-            pred_boxes.dtype]
+    up = _upload_parts(parts + [np.ascontiguousarray(pred[k]) for k in on_host], dev)
+    d_counts, d_cat, d_boxes, d_crowd, d_area, d_map = up[:6]
+    d_status = up[6:len(parts)]
+    for k, t in zip(on_host, up[len(parts):]):
+        pred[k] = t
+    pred_boxes, pred_counts, pred_class_ids, pred_scores = pred
+    form = {torch.int32: N.MRX_BOX_YXYX_I32, torch.float64: N.MRX_BOX_XYWH_F64}[pred_boxes.dtype]
 
-        def ious(v, d_iou, st):
-            N.check(lib.mrx_coco_box_ious(
-                pred_boxes, form, pred_counts, v["cat"], v["keep"], R1, d_boxes, d_counts, d_cat,
-                d_crowd, R2, v["area"], d_iou, n, st), "mrx_coco_box_ious")
+    def ious(v, d_iou, st):
+        N.check(lib.mrx_coco_box_ious(
+            pred_boxes, form, pred_counts, v["cat"], v["keep"], R1, d_boxes, d_counts, d_cat,
+            d_crowd, R2, v["area"], d_iou, n, st), "mrx_coco_box_ious")
 
-        return _coco_evaluate(lib, n, R1, R2, pred_counts, pred_class_ids, pred_scores, d_counts,
-                              d_cat, d_crowd, d_area, d_map, _scorer_params(params, status),
-                              np.float64, ious, stream,
-                              *d_status)
+    return _coco_evaluate(lib, n, R1, R2, pred_counts, pred_class_ids, pred_scores, d_counts,
+                          d_cat, d_crowd, d_area, d_map, _scorer_params(params, status),
+                          np.float64, ious, d_status=d_status[0] if d_status else None)
 
 
 def check_dilation_ratio(dilation_ratio):
@@ -1284,7 +1271,7 @@ def boundary_dilation(geoms, dilation_ratio):
                      for H, W in g[:, :2]], dtype=np.int32).reshape(-1)
 
 
-def mask_boundary_planes(lib, planes, d_geom, d_regions, d_dilation, n, max_w, bufs, stream=None,
+def mask_boundary_planes(lib, planes, d_geom, d_regions, d_dilation, n, max_w, bufs, *,
                          name="boundary"):
     """`Planes` of the boundaries of `planes` (n images, d_geom [n, 8]): mrx_mask_boundary with
     regions d_regions [n, planes.R, 4] and dilations d_dilation [n] int32 into a buffer of the
@@ -1295,7 +1282,7 @@ def mask_boundary_planes(lib, planes, d_geom, d_regions, d_dilation, n, max_w, b
     d_bnd = _buffer(bufs, name + "_packed", planes.d_packed.numel(), torch.uint8, dev)
     d_areas = _buffer(bufs, name + "_areas", n * R, torch.int64, dev)
     d_ext = _buffer(bufs, name + "_extents", n * R * 4, torch.int32, dev)
-    st = N.stream_ptr(stream)
+    st = N.stream_ptr()
     N.check(lib.mrx_mask_boundary(
         planes.d_packed, planes.d_packed_off, planes.d_counts, d_geom, d_regions, d_dilation,
         d_bnd, n, R, max(int(max_w), 1), st),
@@ -1308,8 +1295,8 @@ def mask_boundary_planes(lib, planes, d_geom, d_regions, d_dilation, n, max_w, b
 
 
 def coco_boundary_evaluate_batch(lib, pred, pred_regions, pred_class_ids, pred_scores, gt,
-                                 gt_crowd, gt_area, class_map, params, dilation_ratio=0.02,
-                                 stream=None, bufs=None):
+                                 gt_crowd, gt_area, class_map, params, dilation_ratio=0.02, *,
+                                 bufs=None):
     """The per-image half of COCOeval for iouType "boundary" (boundary_iou_api) for one batch:
     mrx_coco_ranks, the boundaries of both sides (`mask_boundary_planes`: the predictions inside
     pred_regions [n, pred.R, 4] int32, e.g. their boxes, the ground truth over its whole images),
@@ -1322,28 +1309,27 @@ def coco_boundary_evaluate_batch(lib, pred, pred_regions, pred_class_ids, pred_s
     dil = boundary_dilation(gt.geom, dilation_ratio)
     max_w = int(gt.geom[:, 1].max(initial=1))
     bufs = {} if bufs is None else bufs
-    with _stream_ctx(stream):
-        d_crowd, d_area, d_map, d_dil = _upload_parts(
-            [np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
-             np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map, dil],
-            gt.d_geom.device)
+    d_crowd, d_area, d_map, d_dil = _upload_parts(
+        [np.ascontiguousarray(gt_crowd, dtype=np.uint8).reshape(n, R2),
+         np.ascontiguousarray(gt_area, dtype=np.float64).reshape(n, R2), class_map, dil],
+        gt.d_geom.device)
 
-        def ious(v, d_iou, st):
-            v["area"].copy_(pred.d_areas.view(-1)[:n * R1].view(n, R1))
-            bp = mask_boundary_planes(lib, pred, gt.d_geom, pred_regions, d_dil, n, max_w, bufs,
-                                      stream, "pred_boundary")
-            bg = mask_boundary_planes(lib, gt.planes, gt.d_geom, gt.d_regions, d_dil, n, max_w,
-                                      bufs, stream, "gt_boundary")
-            N.check(lib.mrx_coco_boundary_ious(
-                pred.d_packed, pred.d_packed_off, pred.d_counts, pred.d_areas, pred.d_extents,
-                bp.d_packed, bp.d_areas, v["cat"], v["keep"], R1, gt.planes.d_packed,
-                gt.planes.d_packed_off, gt.planes.d_counts, gt.planes.d_areas,
-                gt.planes.d_extents, bg.d_packed, bg.d_areas, gt.d_class_ids, d_crowd, R2,
-                gt.d_geom, d_iou, n, st), "mrx_coco_boundary_ious")
+    def ious(v, d_iou, st):
+        v["area"].copy_(pred.d_areas.view(-1)[:n * R1].view(n, R1))
+        bp = mask_boundary_planes(lib, pred, gt.d_geom, pred_regions, d_dil, n, max_w, bufs,
+                                  name="pred_boundary")
+        bg = mask_boundary_planes(lib, gt.planes, gt.d_geom, gt.d_regions, d_dil, n, max_w, bufs,
+                                  name="gt_boundary")
+        N.check(lib.mrx_coco_boundary_ious(
+            pred.d_packed, pred.d_packed_off, pred.d_counts, pred.d_areas, pred.d_extents,
+            bp.d_packed, bp.d_areas, v["cat"], v["keep"], R1, gt.planes.d_packed,
+            gt.planes.d_packed_off, gt.planes.d_counts, gt.planes.d_areas, gt.planes.d_extents,
+            bg.d_packed, bg.d_areas, gt.d_class_ids, d_crowd, R2, gt.d_geom, d_iou, n, st),
+            "mrx_coco_boundary_ious")
 
-        return _coco_evaluate(lib, n, R1, R2, pred.d_counts, pred_class_ids, pred_scores,
-                              gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map,
-                              coco_device_params(params), np.int64, ious, stream)
+    return _coco_evaluate(lib, n, R1, R2, pred.d_counts, pred_class_ids, pred_scores,
+                          gt.d_counts, gt.d_class_ids, d_crowd, d_area, d_map,
+                          coco_device_params(params), np.int64, ious)
 
 
 def _coco_class_map(class_map):
@@ -1352,9 +1338,9 @@ def _coco_class_map(class_map):
 
 
 def _coco_evaluate(lib, n, R1, R2, d_pred_counts, pred_class_ids, pred_scores, d_gt_counts,
-                   d_gt_cat, d_crowd, d_area, d_map, dparams, area_dtype, ious, stream,
+                   d_gt_cat, d_crowd, d_area, d_map, dparams, area_dtype, ious, *,
                    d_status=None):
-    """What every IoU type shares, on the current stream: the rank step (mrx_coco_ranks, or
+    """What every IoU type shares: the rank step (mrx_coco_ranks, or
     mrx_lvis_ranks with the [n, K] status table d_status), `ious(v, d_iou, st)` (fills d_iou
     [n, R1, R2] and the predictions' `area` in the output views v), the match kernel for
     area_dtype (int64 mask pixels or float64 box areas), then the one download of the output
@@ -1365,7 +1351,7 @@ def _coco_evaluate(lib, n, R1, R2, d_pred_counts, pred_class_ids, pred_scores, d
     T, A = len(thr), len(rng) // 2
     dev = d_map.device
     score_code = {torch.float32: N.MRX_F32, torch.float64: N.MRX_F64}[pred_scores.dtype]
-    st = N.stream_ptr(stream)
+    st = N.stream_ptr()
     # everything that comes back lives in one device buffer laid out by _part_offsets
     parts = {"counts": ((n,), np.int32), "cat": ((n, R1), np.int32), "rank": ((n, R1), np.int32),
              "keep": ((n, R1), np.uint8), "area": ((n, R1), area_dtype),
@@ -1403,27 +1389,14 @@ def _coco_evaluate(lib, n, R1, R2, d_pred_counts, pred_class_ids, pred_scores, d
 
 
 def trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom, d_regions, layout,
-                          stream=None, bufs=None):
+                          *, bufs=None):
     """mrx_contours_count, one host read of the segment counts, mrx_contours_write, over the planes
     of a BatchLayout as mrx_pack_masks writes them; d_regions [n,R,4] int32 pixel rectangles; `bufs`
     keeps the work and output buffers between calls.  Returns (d_vertices [V,2] float64,
     d_contour_off [C+1] int64, inst_contour_off int64 ndarray [n*R+1])."""
-    with _stream_ctx(stream):
-        return _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom,
-                                      d_regions, layout, stream, {} if bufs is None else bufs)
-
-
-def _stream_ctx(stream):
-    """Make `stream` current (host reads then wait for the work queued on it)."""
-    import contextlib
-
-    return contextlib.nullcontext() if stream is None else _torch().cuda.stream(stream)
-
-
-def _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom, d_regions,
-                           layout, stream, bufs):
     torch = _torch()
-    st = N.stream_ptr(stream)
+    bufs = {} if bufs is None else bufs
+    st = N.stream_ptr()
     n, R, max_h = layout.n, layout.R, layout.max_h
     ni = n * R
     d_rows = _buffer(bufs, "rows", ni * (max_h + 1), torch.int32, device)
@@ -1450,7 +1423,7 @@ def _trace_packed_contours(lib, device, d_packed, d_packed_off, d_counts, d_geom
 
 
 def annotate_overlays(lib, dev, d_counts, d_geom, d_boxes, trace, d_images, d_image_off, hws, R,
-                    rgb8, patches, show_bbox, stream=None, bufs=None):
+                    rgb8, patches, show_bbox, *, bufs=None):
     """mrx_annotate_draw then mrx_annotate_resolve on the overlays at `d_images` (image b at byte
     offset d_image_off[b]), in place.  trace: (d_vertices, d_contour_off, d_inst_contour_off) of
     the batch's contours; rgb8 [B, R, 3] uint8 (`visualize.color_table`); patches: `visualize.caption_stencils`;
@@ -1465,7 +1438,7 @@ def annotate_overlays(lib, dev, d_counts, d_geom, d_boxes, trace, d_images, d_im
     d_key_off = torch.from_numpy(key_off[:B].copy()).to(dev)
     d_vert, d_coff, d_icoff = trace
     max_px = int(pixels.max(initial=0))
-    st = N.stream_ptr(stream)
+    st = N.stream_ptr()
     N.check(lib.mrx_annotate_draw(d_counts, d_geom, d_boxes, d_vert, d_coff, d_icoff,
                                   d_vert.shape[0], int(bool(show_bbox)), d_keys, d_key_off, B, R,
                                   max_px, st), "mrx_annotate_draw")
@@ -1519,7 +1492,7 @@ class AnchorGenerator:
             "mrx_anchor_count")
         return int(out.value)
 
-    def generate_device(self, image_shape, out=None, stream=None):
+    def generate_device(self, image_shape, out=None):
         """[A,4] float32 device tensor (not cached)."""
         torch = _torch()
         A = self.count(image_shape)
@@ -1529,7 +1502,7 @@ class AnchorGenerator:
             out, int(image_shape[0]), int(image_shape[1]),
             N.double_array(self.scales), N.double_array(self.ratios),
             N.int_array(self.strides), len(self.strides), len(self.ratios),
-            self.anchor_stride, N.stream_ptr(stream)), "mrx_anchors")
+            self.anchor_stride, N.stream_ptr()), "mrx_anchors")
         return out
 
     def get_anchors(self, image_shape):
@@ -1596,16 +1569,16 @@ class Molder:
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None \
             else torch.device(device)
 
-    def cv2_resize_device(self, d_img, size_hw, stream=None):
+    def cv2_resize_device(self, d_img, size_hw):
         torch = _torch()
         sh, sw = int(d_img.shape[0]), int(d_img.shape[1])
         dh, dw = int(size_hw[0]), int(size_hw[1])
         out = torch.empty((dh, dw, 3), dtype=torch.uint8, device=self.device)
-        N.check(self.lib.mrx_cv2_resize_u8c3(d_img, sh, sw, out, dh, dw,
-                                             N.stream_ptr(stream)), "mrx_cv2_resize_u8c3")
+        N.check(self.lib.mrx_cv2_resize_u8c3(d_img, sh, sw, out, dh, dw, N.stream_ptr()),
+                "mrx_cv2_resize_u8c3")
         return out
 
-    def mold_device(self, d_img, out_dtype=np.float32, want_u8=False, stream=None):
+    def mold_device(self, d_img, out_dtype=np.float32, want_u8=False):
         """resize_image + mold_image for a uint8 HxWx3 device image.
         Returns (molded, molded_u8|None, window, scale, padding)."""
         torch = _torch()
@@ -1620,8 +1593,7 @@ class Molder:
         mean = [float(v) for v in np.asarray(cfg.MEAN_PIXEL, dtype=np.float64)]
         N.check(self.lib.mrx_mold_image(
             d_img, h, w, nh, nw, top, left, oh, ow, N.double_array(mean),
-            _dtype_code(out_dtype), out, u8, N.stream_ptr(stream)),
-            "mrx_mold_image")
+            _dtype_code(out_dtype), out, u8, N.stream_ptr()), "mrx_mold_image")
         return out, u8, window, scale, padding
 
 
@@ -1663,7 +1635,7 @@ class Molder:
         d[:total].copy_(h[:total], non_blocking=True)
         return [d[int(o):int(o) + p.size] for p, o in zip(parts, off[:-1])]
 
-    def jpeg_coefficients(self, plan, stream=None, d_status=None):
+    def jpeg_coefficients(self, plan, *, d_status=None):
         """Enqueue `mrx_jpeg_coefficients` for a `jpeg.Plan`: returns (d_coef int16 [blocks, 64]
         in decode order, d_status [B] int32, the device upload).  Nothing is synchronised."""
         torch = _torch()
@@ -1676,10 +1648,10 @@ class Molder:
         N.check(self.lib.mrx_jpeg_coefficients(
             d_files, d_desc, d_tabs, d_unit_img, plan.B,
             max(plan.units, 1), plan.S, plan.max_subs, d_unst, d_work, d_coef,
-            plan.coef_blocks, d_status, N.stream_ptr(stream)), "mrx_jpeg_coefficients")
+            plan.coef_blocks, d_status, N.stream_ptr()), "mrx_jpeg_coefficients")
         return d_coef[:plan.coef_blocks * 64].view(-1, 64), d_status[:plan.B], up
 
-    def jpeg_progressive_coefficients(self, plan, stream=None, d_status=None):
+    def jpeg_progressive_coefficients(self, plan, *, d_status=None):
         """Enqueue `mrx_jpeg_progressive_coefficients` for a `jpeg.ProgressivePlan`: returns
         (d_coef int16 [blocks, 64] in MCU decode order, as `jpeg_coefficients` writes it, d_status
         [B] int32, (d_desc, d_tabs) for `mrx_jpeg_pixels`).  Nothing is synchronised."""
@@ -1699,11 +1671,10 @@ class Molder:
         N.check(self.lib.mrx_jpeg_progressive_coefficients(
             d_files, d_desc, d_scans, d_scan_tabs, d_unit_scan, d_round_off, plan.B,
             plan.n_scans, plan.rounds, plan.max_round_units, d_unst, d_unit_bit, d_coef,
-            plan.coef_blocks, d_status, N.stream_ptr(stream)),
-            "mrx_jpeg_progressive_coefficients")
+            plan.coef_blocks, d_status, N.stream_ptr()), "mrx_jpeg_progressive_coefficients")
         return d_coef[:plan.coef_blocks * 64].view(-1, 64), d_status[:plan.B], (d_desc, d_tabs)
 
-    def jpeg_decode_into(self, plan, d_out, out_off, stream=None, d_status=None):
+    def jpeg_decode_into(self, plan, d_out, out_off, *, d_status=None):
         """Enqueue the decode of every file of `plan` (a `jpeg.Plan` or `jpeg.ProgressivePlan`)
         into the uint8 slots d_out + out_off[b] (int64 byte offsets; image b is plan.shapes[b]).
         Returns d_status [B] (device; `d_status` when given); call `files_check` on it once the
@@ -1713,22 +1684,21 @@ class Molder:
         torch = _torch()
         if isinstance(plan, jpeg.ProgressivePlan):
             d_coef, d_status, (d_desc, d_tabs) = self.jpeg_progressive_coefficients(
-                plan, stream, d_status)
+                plan, d_status=d_status)
             d_planes = self._jpeg_buffer("p_planes", plan.plane_bytes, torch.uint8)
         else:
             d_coef, d_status, (d_desc, _, d_tabs, _) = self.jpeg_coefficients(
-                plan, stream, d_status)
+                plan, d_status=d_status)
             d_planes = self._jpeg_buffer("planes", plan.plane_bytes, torch.uint8)
         d_off = torch.from_numpy(np.ascontiguousarray(out_off, dtype=np.int64)).to(
             self.device, non_blocking=True)
         N.check(self.lib.mrx_jpeg_pixels(
             d_desc, d_tabs, d_coef, d_status, plan.B, plan.max_blocks,
-            plan.max_pixels, d_planes, d_out, d_off, N.stream_ptr(stream)),
-            "mrx_jpeg_pixels")
+            plan.max_pixels, d_planes, d_out, d_off, N.stream_ptr()), "mrx_jpeg_pixels")
         return d_status
 
     # ------------------------------------------------------------------ PNG (csrc/png_decode.cu)
-    def png_decode_into(self, plan, d_out, out_off, stream=None, d_status=None):
+    def png_decode_into(self, plan, d_out, out_off, *, d_status=None):
         """Enqueue `mrx_png_decode` for a `png.DecodePlan` into the uint8 slots d_out + out_off[b]
         (int64 byte offsets; image b is plan.shapes[b]).  Returns (d_status [B] int32, d_info
         [B, 8] int64 (mrx.h MRX_PNG_DEC_*), d_blocks [blocks, 2] int64) on the device; call
@@ -1758,12 +1728,12 @@ class Molder:
             d_files, d_desc, d_chunks, d_plte, plan.B, plan.n_chunks, plan.max_n,
             plan.max_pixels, plan.max_zlen, plan.max_tiles, plan.total_tiles, plan.max_blocks,
             plan.K, d_z, d_cand, d_tile_cnt, d_meas, d_cells, d_filt, d_blocks, d_info, d_status,
-            d_out, d_off, N.stream_ptr(stream)), "mrx_png_decode")
+            d_out, d_off, N.stream_ptr()), "mrx_png_decode")
         return (d_status[:plan.B], d_info[:plan.B * png.DEC_INFO_WORDS].view(plan.B, -1),
                 d_blocks[:plan.block_words].view(-1, 2))
 
     # ------------------------------------------------------------------ files of either format
-    def decode_files_into(self, plans, d_out, out_off, stream=None):
+    def decode_files_into(self, plans, d_out, out_off):
         """Enqueue the decode of a batch split by `imagefile.plan_batch` or `jpeg.plan_batch`
         ([(plan, positions)]) into the slots d_out + out_off[position].  Every plan writes its
         part of one status buffer, in plan order.  Returns (d_status, positions in that order,
@@ -1777,10 +1747,10 @@ class Molder:
         for plan, pos in plans:
             st, off = d_status[lo:lo + len(pos)], np.asarray(out_off)[pos]
             if isinstance(plan, png.DecodePlan):
-                self.png_decode_into(plan, d_out, off, stream, st)
+                self.png_decode_into(plan, d_out, off, d_status=st)
                 formats += ["png"] * len(pos)
             else:
-                self.jpeg_decode_into(plan, d_out, off, stream, st)
+                self.jpeg_decode_into(plan, d_out, off, d_status=st)
                 formats += ["jpeg"] * len(pos)
             order += list(pos)
             lo += len(pos)
@@ -1800,42 +1770,42 @@ class Molder:
                 raise png.PngError(f"image {i}: corrupt PNG data ({png.status_reasons(st[b])})")
             raise jpeg.JpegError(f"image {i}: corrupt JPEG data ({jpeg.status_reasons(st[b])})")
 
-    def _decode_to_tensors(self, plans, shapes, stream):
+    def _decode_to_tensors(self, plans, shapes):
         torch = _torch()
         if not shapes:
             return []
         sizes = np.asarray([h * w * 3 for h, w, _ in shapes], dtype=np.int64)
         off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
         out = torch.empty((int(off[-1]),), dtype=torch.uint8, device=self.device)
-        self.files_check(*self.decode_files_into(plans, out, off[:-1], stream))
+        self.files_check(*self.decode_files_into(plans, out, off[:-1]))
         return [out[int(off[b]):int(off[b + 1])].view(shapes[b]) for b in range(len(shapes))]
 
-    def decode_jpeg_batch(self, blobs, S=None, stream=None):
+    def decode_jpeg_batch(self, blobs, S=None):
         """uint8 [H, W, 3] RGB CUDA tensors, one per JPEG file: cv2.imdecode + BGR2RGB bit for
         bit.  The images share one buffer; equal sizes make them one contiguous [B, H, W, 3]."""
         from . import jpeg
 
         plans, shapes = jpeg.plan_batch(blobs, S=jpeg.DEFAULT_S if S is None else S)
-        return self._decode_to_tensors(plans, shapes, stream)
+        return self._decode_to_tensors(plans, shapes)
 
-    def decode_png_batch(self, blobs, stream=None, slots=None):
+    def decode_png_batch(self, blobs, *, slots=None):
         """`decode_jpeg_batch` for PNG files (`png.DecodePlan`; slots: its candidate slots per
         tile, 0 to measure every deflate block in the chain)."""
         from . import png
 
         plan = png.DecodePlan(list(blobs), slots=png.DEFAULT_SLOTS if slots is None else slots)
         return self._decode_to_tensors([(plan, list(range(plan.B)))] if plan.B else [],
-                                       plan.shapes, stream)
+                                       plan.shapes)
 
-    def decode_files(self, blobs, stream=None):
+    def decode_files(self, blobs):
         """`decode_jpeg_batch` for JPEG and PNG files mixed, routed by their signature."""
         from . import imagefile
 
         plans, shapes, _ = imagefile.plan_batch(list(blobs))
-        return self._decode_to_tensors(plans, shapes, stream)
+        return self._decode_to_tensors(plans, shapes)
 
     # ------------------------------------------------------------------ batched (one launch each)
-    def stage_images(self, images, align=16, stream=None):
+    def stage_images(self, images, align=16):
         """Every image in its slot of one device buffer: uint8 HxWx3 NumPy images through one
         pinned staging buffer and one H2D copy, JPEG and PNG files (bytes) decoded on the device
         into their slots.  Returns (d_src, off [B+1] int64 slot offsets, shapes, status, fidx: the
@@ -1866,12 +1836,12 @@ class Molder:
         d_src = self._h_stage[:total].to(self.device, non_blocking=True)
         status = None
         if fidx:
-            d_status, order, formats = self.decode_files_into(plans, d_src, off[fidx], stream)
+            d_status, order, formats = self.decode_files_into(plans, d_src, off[fidx])
             status = (d_status, [fidx[k] for k in order], formats)
         return d_src, off, shapes, status, fidx
 
     # ------------------------------------------------------------------ batched (one launch each)
-    def cv2_resize_batch_device(self, images, size_hw, stream=None, return_sources=False):
+    def cv2_resize_batch_device(self, images, size_hw, *, return_sources=False):
         """`cv2.resize(img, (S, S))` for a list of images of ANY sizes in one launch: uint8 HxWx3
         NumPy images or JPEG / PNG files as bytes, staged by `stage_images` (files decoded on the
         device into their slots).  Returns uint8 [B, dh, dw, 3] on the device; with
@@ -1880,14 +1850,13 @@ class Molder:
         torch = _torch()
         B = len(images)
         dh, dw = int(size_hw[0]), int(size_hw[1])
-        d_src, off, shapes, status, fidx = self.stage_images(images, 16, stream)
+        d_src, off, shapes, status, fidx = self.stage_images(images, 16)
         hw = np.asarray([sh[:2] for sh in shapes], dtype=np.int32).reshape(B, 2)
         d_off = torch.from_numpy(off[:B].copy()).to(self.device)
         d_hw = torch.from_numpy(hw).to(self.device)
         out = torch.empty((B, dh, dw, 3), dtype=torch.uint8, device=self.device)
         N.check(self.lib.mrx_cv2_resize_u8c3_batch(
-            d_src, d_off, d_hw, out, B, dh, dw, N.stream_ptr(stream)),
-            "mrx_cv2_resize_u8c3_batch")
+            d_src, d_off, d_hw, out, B, dh, dw, N.stream_ptr()), "mrx_cv2_resize_u8c3_batch")
         if status is not None:
             self.files_check(*status)
         if not return_sources:
@@ -1896,7 +1865,7 @@ class Molder:
                    if b in fidx else images[b] for b in range(B)]
         return out, sources
 
-    def mold_batch_device(self, d_imgs, out_dtype=np.float32, stream=None):
+    def mold_batch_device(self, d_imgs, out_dtype=np.float32):
         """resize_image + mold_image for uint8 [B,h,w,3] device images of one size, one launch.
         Returns (molded [B,oh,ow,3], window, scale, padding)."""
         torch = _torch()
@@ -1909,8 +1878,7 @@ class Molder:
         mean = [float(v) for v in np.asarray(cfg.MEAN_PIXEL, dtype=np.float64)]
         N.check(self.lib.mrx_mold_image_batch(
             d_imgs, B, h, w, nh, nw, top, left, oh, ow, N.double_array(mean),
-            _dtype_code(out_dtype), out, None, N.stream_ptr(stream)),
-            "mrx_mold_image_batch")
+            _dtype_code(out_dtype), out, None, N.stream_ptr()), "mrx_mold_image_batch")
         return out, window, scale, padding
 
 

@@ -26,6 +26,9 @@ import ctypes as C
 import os
 
 import numpy as np
+import torch
+
+from . import _native as N
 
 
 def partition_images(costs, world_size):
@@ -77,7 +80,6 @@ def gather_bytes_to_root(local, sizes, dst=0, group=None):
     local: 1-D uint8 tensor of this rank's bytes (device or CPU).
     sizes: list of byte counts per rank (known to all ranks; derived from the partition).
     Returns on dst a list of tensors (one per rank, rank order); None elsewhere."""
-    import torch
     import torch.distributed as dist
 
     rank = dist.get_rank(group)
@@ -126,7 +128,6 @@ class RootGather:
     current stream and runs on NCCL's own stream, so later kernels overlap it."""
 
     def __init__(self, sizes, device, dst=0, group=None):
-        import torch
         import torch.distributed as dist
 
         self.dist = dist
@@ -208,12 +209,8 @@ class PeerGather:
     HEADER = 4096     # flags live in front of the data (one uint32 per rank)
 
     def __init__(self, sizes, device, dst=0, group=None):
-        import torch
         import torch.distributed as dist
 
-        from . import _native as N
-
-        self.N = N
         self.lib = N.load()
         self.group = group
         self.rank = dist.get_rank(group)
@@ -287,21 +284,19 @@ class PeerGather:
 
     def signal(self, stream=None):
         """After everything queued on `stream`: tell dst that this rank's bytes have landed."""
-        N = self.N
-        N.check(self.lib.mrx_peer_signal(self.base + 4 * self.rank, self.epoch,
-                                         N.stream_ptr(stream)), "mrx_peer_signal")
+        with N.on_stream(stream):
+            N.check(self.lib.mrx_peer_signal(self.base + 4 * self.rank, self.epoch,
+                                             N.stream_ptr()), "mrx_peer_signal")
 
     def wait(self, stream=None):
         """dst only: `stream` proceeds once every rank has signalled the current epoch."""
         if not self._owner:
             return
-        N = self.N
-        N.check(self.lib.mrx_peer_wait(self.base, self.world, self.epoch, N.stream_ptr(stream)),
-                "mrx_peer_wait")
+        with N.on_stream(stream):
+            N.check(self.lib.mrx_peer_wait(self.base, self.world, self.epoch, N.stream_ptr()),
+                    "mrx_peer_wait")
 
     def close(self):
-        import torch
-
         torch.cuda.synchronize()
         self.dist_barrier()
         if not self._owner:          # mappings go first, the allocation last

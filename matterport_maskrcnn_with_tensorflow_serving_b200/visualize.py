@@ -191,13 +191,13 @@ class CompositeStage:
         self.d_off = torch.from_numpy(offs[:B].copy()).to(dev)
         self.max_px = max(H * W for H, W in hw)
 
-    def run(self, stream=None):
+    def run(self):
         eng = self.engine
         B = eng.layout.n
         N.check(self.lib.mrx_composite_masks(
             eng.d_canvas, eng.d_canvas_off, eng.d_counts, eng.d_geom, eng.d_boxes, self.d_in,
             self.d_off, self.d_tab, 1 - self.alpha, self.d_out, B, eng.R, self.max_px,
-            N.stream_ptr(stream)), "mrx_composite_masks")
+            N.stream_ptr()), "mrx_composite_masks")
         return self.outputs()
 
     def outputs(self):
@@ -206,13 +206,13 @@ class CompositeStage:
                 for b in range(self.layout.n)]
 
     def annotate(self, class_names=None, class_ids=None, scores=None, captions=None,
-                 show_bbox=True, stream=None):
+                 show_bbox=True):
         """Draw the boxes, outlines and captions on the overlays `run()` wrote (`composite_batch`
         with annotate=True).  The boxes, and the class ids and scores not given, are read from
         the engine (`fetch_meta`, one synchronisation)."""
         eng = self.engine
         B = self.layout.n
-        counts, boxes, ids, scs = eng.fetch_meta(stream)
+        counts, boxes, ids, scs = eng.fetch_meta()
         boxes = [boxes[b, :int(counts[b])] for b in range(B)]
         class_ids = class_ids if class_ids is not None else \
             [ids[b, :int(counts[b])] for b in range(B)]
@@ -220,12 +220,12 @@ class CompositeStage:
         hws = [self.layout.hw(b) for b in range(B)]
         patches = caption_stencils(boxes, hws, class_ids, class_names, scores, captions)
         rgb8 = np.stack([color_table(c, eng.R) for c in self.colors])
-        eng.annotate(self.d_out, self.d_off, rgb8, patches, show_bbox, stream)
+        eng.annotate(self.d_out, self.d_off, rgb8, patches, show_bbox)
         return self.outputs()
 
 
-def composite_batch(engine, images, colors, alpha=0.5, stream=None, annotate=False,
-                    class_names=None, class_ids=None, scores=None, captions=None, show_bbox=True):
+def composite_batch(engine, images, colors, alpha=0.5, *, annotate=False, class_names=None,
+                    class_ids=None, scores=None, captions=None, show_bbox=True):
     """Overlay the masks an `UnmoldEngine` holds on its device canvas (after `enqueue`).
 
     images: list of uint8 HxWx3 arrays (NumPy or CUDA tensors), one per planned image, each
@@ -238,9 +238,9 @@ def composite_batch(engine, images, colors, alpha=0.5, stream=None, annotate=Fal
     "<class_names[id]> <score:.3f>"); class_names is needed unless captions are given.
     """
     stage = CompositeStage(engine, images, colors, alpha)
-    out = stage.run(stream)
+    out = stage.run()
     if annotate:
-        out = stage.annotate(class_names, class_ids, scores, captions, show_bbox, stream)
+        out = stage.annotate(class_names, class_ids, scores, captions, show_bbox)
     return out
 
 
@@ -287,7 +287,7 @@ def apply_masks(image, boxes, masks, colors, alpha=0.5):
     d_tab = torch.from_numpy(blend_table(colors, alpha, n)).to(dev)
     N.check(lib.mrx_composite_masks(
         d_canvas, d_off, d_counts, d_geom, d_boxes, d_img, d_off, d_tab, 1 - alpha, d_out, 1, n,
-        H * W, N.stream_ptr(None)), "mrx_composite_masks")
+        H * W, N.stream_ptr()), "mrx_composite_masks")
     return d_out.cpu().numpy()
 
 
@@ -304,7 +304,7 @@ def _trace_masks(boxes, masks, bufs):
         np.ascontiguousarray(masks).astype(np.bool_, copy=False).view(np.uint8), H, W, n)
     d_packed = torch.empty(int(layout.packed_off[-1]), dtype=torch.uint8, device=dev)
     N.check(lib.mrx_pack_masks(d_canvas, d_off, d_counts, d_geom, d_packed, d_off, 1, n, H, W,
-                               N.stream_ptr(None)), "mrx_pack_masks")
+                               N.stream_ptr()), "mrx_pack_masks")
     # the whole image, or nothing for an all-zero box (display_instances skips those)
     regions = np.zeros((n, 4), dtype=np.int32)
     regions[boxes.reshape(n, -1).any(axis=1)] = (0, 0, H, W)
